@@ -2,6 +2,7 @@
 """bench.py -- NNConv edge-applications/s on synthetic Darcy-2D radius graphs (BASELINE.json metric).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--workload darcy241|darcy85]
+                    [--dump-outputs DIR]
 
 One "step" = one KernelNN conv stack (T applications of the shared NNConv, graph-neural-operator/
 UAI1_full_resolution.py:29-30) over ONE graph sample per GPU: the x-independent edge features are
@@ -47,11 +48,13 @@ def peaks():
         d = json.load(open(p))
         return dict(hbm_gbs=d['hbm_gbs'], tf_burst=d['bf16_tflops'], tf_sustained=d.get('bf16_tflops_sustained',
                     d['bf16_tflops']), source='measured')
-    return dict(hbm_gbs=6650.0, tf_burst=1590.0, tf_sustained=1400.0, source='fallback')
+    # NVIDIA H100 SXM data sheet (700 W card): HBM3 3.35 TB/s, dense bf16 989 TFLOP/s.  Upper bounds, not measured
+    # rates; a power-limited card reaches less.
+    return dict(hbm_gbs=3350.0, tf_burst=989.0, tf_sustained=989.0, source='H100 SXM data sheet (not measured)')
 
 
 class ClockSampler(object):
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
 
     def __init__(self, index):
         self.rows = []
@@ -105,10 +108,10 @@ REF_SAMPLE_SOURCES = 192     # fixed, so that reference-arm numbers are comparab
 
 def cpu_reference_rate(cfg, steps=1, warmup=0, n_src=REF_SAMPLE_SOURCES):
     """The reference's CPU path on a bounded, FIXED sample: out-edges of the first n_src source nodes of the
-    workload graph, T applications of one NNConv.  Runs the reference's OWN files (baseline/_ref, vendored
-    unmodified by oracle/vendor_ref.py; kind 'reference') over oracle/pyg_stub, exactly as the reference runs them
-    (one shot over all edges of the sample, torch CPU fp32); falls back to the oracle port (kind 'port') only when
-    the vendored copy is absent.  Returns (edge_apps_per_s, cores, kind, sample_description, ms_per_step)."""
+    workload graph, T applications of one NNConv, torch CPU fp32.  Times the oracle port (kind 'port'); only when a
+    copy of the reference's own files has been placed in baseline/_ref by hand (oracle/vendor_ref.py, never run by
+    the build) are those timed instead over oracle/pyg_stub (kind 'reference', one shot over all edges of the sample).
+    Returns (edge_apps_per_s, cores, kind, sample_description, ms_per_step)."""
     from graph_pde_b200 import graphs
     from oracle import nnconv_oracle as O
     from oracle import vendor_ref
@@ -440,7 +443,7 @@ def run_strip_children(args, rank):
     """Every rank of the main bench spawns its own child (same RANK / WORLD_SIZE / LOCAL_RANK, MASTER_PORT + 23);
     rank 0 returns the child's JSON object (or an error record)."""
     # the children rendezvous among themselves: not through the elastic agent's store of the parent job (with
-    # TORCHELASTIC_USE_AGENT_STORE every rank is a CLIENT of MASTER_PORT and nobody would serve the new port: run r2h)
+    # TORCHELASTIC_USE_AGENT_STORE every rank is a CLIENT of MASTER_PORT and nobody would serve the new port)
     env = {k: v for k, v in os.environ.items() if not k.startswith('TORCHELASTIC_')}
     env['MASTER_PORT'] = str(int(env.get('MASTER_PORT', '29500')) + 23)
     env.setdefault('MASTER_ADDR', '127.0.0.1')
@@ -472,7 +475,11 @@ def main():
     ap.add_argument('--no-other-configs', action='store_true', help='skip BASELINE configs 2, 4, 5')
     ap.add_argument('--no-strip', action='store_true', help='skip the single-mesh strip-partition measurement (N > 1)')
     ap.add_argument('--strip-only', action='store_true', help=argparse.SUPPRESS)
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='after the timed steps, write what the last timed step computed to DIR/<name>.npy (float32)')
     args = ap.parse_args()
+    if args.dump_outputs and args.impl == 'reference':
+        ap.error('--dump-outputs writes the outputs of the CUDA arm; it does not apply to --impl reference')
     if args.strip_only:
         return strip_child_main(args)
     cfg = WORKLOADS[args.workload]
@@ -500,7 +507,7 @@ def main():
         print(json.dumps(line))
         return 0
 
-    # ------------------------------------------------------------------------------------ B200 arm
+    # ------------------------------------------------------------------------------------ CUDA arm
     import torch.distributed as dist
     from graph_pde_b200 import _lib, graphs, nn_conv
     from graph_pde_b200.models import KernelNN
@@ -570,6 +577,8 @@ def main():
             dist.barrier()
         torch.cuda.synchronize()
 
+    last = {}
+
     def timed(fn, steps, warmup, pre=None):
         for i in range(warmup):
             fn(i)
@@ -579,7 +588,7 @@ def main():
         a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         a.record()
         for i in range(steps):
-            fn(warmup + i)
+            last[fn.__name__] = fn(warmup + i)
         b.record()
         barrier()
         ms = torch.tensor([a.elapsed_time(b)], device=dev)
@@ -603,6 +612,13 @@ def main():
 
     ms_e2e = timed(step_e2e, args.steps, 1, pre=e2e_reset)
     e2e_value = world * E * T * args.steps / (ms_e2e * 1e-3)
+    if args.dump_outputs and rank == 0:
+        # the arrays a caller of each timed path receives from its last timed step: the conv-stack activations
+        # [N, width] (device-resident inputs) and the model output [N, 1] (end-to-end path); ~15 MB at 241^2
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, 'conv_stack_out.npy'),
+                last['step_resident'].detach().float().cpu().numpy())
+        np.save(os.path.join(args.dump_outputs, 'model_out.npy'), last['step_e2e'].detach().float().cpu().numpy().copy())
     h2d = host_x[0].numel() * 4 + host_ea[0].numel() * 4
     d2h = host_out.numel() * 4
 
@@ -655,7 +671,7 @@ def main():
                      note='one 241^2-class graph per rank per step, L1 loss, Adam; gradients sum-reduced with one flat '
                           'all-reduce per step' if world > 1 else 'one graph per step, L1 loss, Adam')
         tmodel.conv1.invalidate()                 # the closure above still references the model: drop its 2 KB/edge
-        tmodel.conv1._tstate = None               # buffers (edge features + kept activations, ~94 GB at 241^2) explicitly
+        tmodel.conv1._tstate = None               # buffers (edge features + kept activations) explicitly
         del step_train, tmodel, opt
         import gc
         gc.collect()
@@ -677,7 +693,12 @@ def main():
                       config='%s, full graph (E=%d), all T=%d applications, metric max|out-ref|/max|ref| of the final '
                              'node features' % (args.workload, E, T))
         del got
-        if args.precision == 'f16':
+        # f16x2 keeps every edge feature as an fp16 (hi, lo) pair: 4 bytes per edge and hidden unit
+        x2_bytes = E * kw * 4
+        if args.precision == 'f16' and x2_bytes > 0.8 * torch.cuda.mem_get_info(dev)[0]:
+            fp32_grade = dict(precision='f16x2', value=None, skipped='edge features of %.1f GB do not fit this GPU'
+                              % (x2_bytes / 1e9))
+        elif args.precision == 'f16':
             m2 = KernelNN(w, kw, T, 6, in_width=6, precision='f16x2').to(dev).eval()
             m2.load_state_dict(model.state_dict())
 
@@ -745,11 +766,6 @@ def main():
         for rf in (rf_conv, rf_gemm):
             rf['frac'] = (rf['achieved'] / rf['peak']) if rf['achieved'] else None
             rf['peak_source'] = pk['source']
-        if fused and args.workload == 'darcy241' and args.precision == 'f16':
-            # dram__bytes_read.sum + dram__bytes_write.sum of ONE k_apply_tc launch, ncu --set full capture of this
-            # command (profiles/r2r_k_apply_tc_full.md); algorithmic bytes per launch = E * 2052 B
-            rf_conv['traffic'] = 56.86e9
-            rf_conv['traffic_source'] = 'profiles/r2r_k_apply_tc_full.md (per launch: 52.50 GB read + 4.36 GB written; algorithmic %.2f GB per launch)' % (E * (Kp * es + 4) / 1e9)
         dominant = rf_conv if conv_ms >= gemm_ms else rf_gemm
         f_alg = 2.0 * (6 * kw + kw * kw + kw * w * w + w * w)    # SURVEY 8(d), reference formulation A
         b_alg = 16 + 24 + 4.0 * 2 * w * N / E
@@ -779,7 +795,7 @@ def main():
     if world > 1:
         dist.barrier()
         dist.destroy_process_group()
-    if rank == 0 and fp32_grade is not None and not fp32_grade['parity']['ok']:
+    if rank == 0 and fp32_grade is not None and 'parity' in fp32_grade and not fp32_grade['parity']['ok']:
         sys.stderr.write('bench.py: fp32-grade (f16x2) line outside its tolerance: %s\n' % fp32_grade['parity'])
     if rank == 0 and parity is not None and not parity['ok']:      # the benchmarked precision itself: hard failure
         sys.stderr.write('bench.py: PARITY FAILED: %s\n' % parity)

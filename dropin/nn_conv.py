@@ -1,5 +1,5 @@
 """Drop-in for graph-neural-operator/nn_conv.py: put this directory FIRST on sys.path (or PYTHONPATH) and the
-reference scripts' ``from nn_conv import NNConv_old`` (UAI1_full_resolution.py:9) resolves to the B200 op.
+reference scripts' ``from nn_conv import NNConv_old`` (UAI1_full_resolution.py:9) resolves to this library's op.
 Whole-module checkpoints pickled by the reference bind to the class path ``nn_conv.NNConv_old`` -- kept."""
 import os
 import sys

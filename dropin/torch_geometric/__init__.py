@@ -1,5 +1,5 @@
 """Minimal stand-in for the parts of torch_geometric the reference scripts import, with NNConv backed by the
-B200 library.  Put the parent directory first on sys.path:
+H100 library.  Put the parent directory first on sys.path:
 
     from torch_geometric.nn import NNConv            (MGKN_general_darcy2d.py:8)
     from torch_geometric.data import Data, DataLoader (UAI1_full_resolution.py:6)

@@ -1,4 +1,4 @@
-"""graph_pde_b200 -- B200-native (sm_100a) implementation of the NNConv hot path of
+"""graph_pde_b200 -- H100-native (sm_90a) implementation of the NNConv hot path of
 neuraloperator/graph-pde: the edge-conditioned convolution iterated inside KernelNN and the MGKN
 V-cycle.  Public surface mirrors the reference's operator API:
 

@@ -1,7 +1,7 @@
 """ctypes binding of libnnconv_b200.so (C ABI declared in include/nnconv_b200.h).
 
-The product path has NO fallback: if the shared library is missing or the device is not sm_100-class,
-importing / calling raises.  `build()` compiles the library in-tree with nvcc (sm_100a only).
+The product path has NO fallback: if the shared library is missing or the device is not an sm_90 GPU (H100),
+importing / calling raises.  `build()` compiles the library in-tree with nvcc (sm_90a only).
 """
 import ctypes
 import os
@@ -42,7 +42,7 @@ class NNConvLibraryError(RuntimeError):
 
 
 def build(verbose=False):
-    """Compile libnnconv_b200.so for sm_100a (nvcc cross-compiles without a GPU)."""
+    """Compile libnnconv_b200.so for sm_90a (nvcc cross-compiles without a GPU)."""
     cmd = ['make', '-C', CSRC, '-j', str(min(8, os.cpu_count() or 1))]
     res = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if verbose or res.returncode != 0:

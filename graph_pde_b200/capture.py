@@ -10,8 +10,6 @@ the torch caching allocator, tensor maps are encoded on the host, no call synchr
     data.x.copy_(new_x)                    # inputs are STATIC tensors: refresh them in place
     out = g.replay()                       # same tensor object every time
 
-Measured on B200 (scripts/mgkn_bench.py, 5-level 241^2 sampling, width 64, ker_width 256, depth 4):
-eager 3.9 ms, replay 2.3 ms, reference-equivalent torch path 71 ms per forward.
 Inference only (the autograd graph is not captured); parameters and edge attributes must not change between
 replays -- re-create the object after an optimiser step or a new mesh."""
 import torch

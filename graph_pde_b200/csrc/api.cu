@@ -333,10 +333,10 @@ int edge_features(const Plan* P, const Weights* W, const float* edge_attr, void*
 
 // ------------------------------------------------------------------------------------------------
 // formulation B (SURVEY 8(d)): per-edge kernel matrices, for graphs whose sources have only a few out-edges.
-// Formulation C spends one [out, Kp] matrix per SOURCE (128 KB at out=64, Kp=1024) and a 128-row UMMA tile per
+// Formulation C spends one [out, Kp] matrix per SOURCE (128 KB at out=64, Kp=1024) and a 128-row wgmma tile per
 // source; with 2-4 out-edges per node (the 1-D multipole hierarchy of config 5) that is as expensive as one kernel
 // matrix per EDGE and the tiles are 97 % empty.  K_e = W_L h_e + b_L is x-independent like h: it is built once per
-// (edge_attr, parameters) by the tcgen05 GEMM and every application is one bandwidth-bound pass over it.
+// (edge_attr, parameters) by the wgmma GEMM and every application is one bandwidth-bound pass over it.
 // ------------------------------------------------------------------------------------------------
 bool edge_kernels_supported(const Weights* W) {
   return (W->prec == PREC_F16 || W->prec == PREC_BF16) && W->W3n != nullptr && (W->cin * W->cout) % 64 == 0 &&
@@ -423,7 +423,7 @@ int apply(const Plan* P, const Weights* W, const void* h, const float* x, const 
   // fused persistent kernel (below): its batch geometry is needed here because the node-prep launch also clears its flags
   const bool no_fuse_env = opt.no_fuse != 0 && !W->split;      // measurement / debugging knob
   bool fused = W->prec != PREC_FP32 && !no_fuse_env && apply_fused_supported(W);
-  int ring = opt.ring;   // measured (run22): with dynamic unit scheduling 3 x 128 sources (48 MB at out=64, Kp=1024) is best
+  int ring = opt.ring;   // with dynamic unit scheduling 3 x 128 sources (48 MB at out=64, Kp=1024) is best
   int64_t nb = 0;
   if (fused) {
     if (opt.ring_deep && nodes_cap / 128 > ring) ring = nodes_cap / 128 < 16 ? static_cast<int>(nodes_cap / 128) : 16;
@@ -864,7 +864,7 @@ int nnconv_halo_push(const float* out, int relu, int64_t n_local, int channels, 
 // library allocates device memory itself: a CUDA IPC handle can only be taken of a whole cudaMalloc allocation, and
 // the importing side must open it with ITS device current (cudaIpcMemLazyEnablePeerAccess then maps the memory for
 // kernels of that device) -- memory imported through torch's tensor sharing is opened under the exporter's device and
-// faulted when a kernel of the importing rank's device stored into it (run r2g).
+// faulted when a kernel of the importing rank's device stored into it.
 int nnconv_ipc_alloc(size_t bytes, void** dev_ptr, unsigned char* handle64) {
   NNC_REQUIRE(dev_ptr && handle64 && bytes > 0, NNCONV_ERR_ARG, "ipc_alloc: bad arguments");
   static_assert(sizeof(cudaIpcMemHandle_t) == 64, "cudaIpcMemHandle_t is 64 bytes");

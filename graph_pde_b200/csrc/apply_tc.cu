@@ -2,19 +2,20 @@
 // contraction + scatter run CONCURRENTLY inside every CTA as two independent warp-specialised pipelines,
 // coupled only through completion flags in global memory and a ring of Y batches that lives in L2.
 //
-// Why (measured, profiles/r1c_trace_*.md): with one launch per batch of sources (the batch must be small for
+// Why: with one launch per batch of sources (the batch must be small for
 // Y to stay L2 resident) every CTA streamed only ~3 tiles per launch and spent as long ramping up / draining
 // as streaming; PDL overlapped the launches but not the per-CTA ramps.  Here a CTA never drains: its
 // contraction pipeline walks batch after batch (its share of each batch's tiles), while its Y pipeline
 // produces the batches ahead.
 //
-//   roles (12 warps):  0 conv TMA producer | 1 conv MMA issuer (+TMEM owner) | 2-5 conv epilogue (scatter)
-//                      6 Y   TMA producer | 7 Y   MMA issuer               | 8-11 Y epilogue (fp16 stores)
-//   TMEM (512 cols):   [0,256) contraction accumulators 2 stages x kTU tiles x out | [256,512) Y 2 x 128
-//   flags per batch b: okY[b]  raised when all 4*grid Y-epilogue warps finished batch b   (conv waits)
+//   roles (14 warps):  0-3 / 4-7 conv warpgroups (tile 0 / tile 1 of every unit: wgmma into registers, scatter)
+//                      8-11 Y warpgroup (wgmma into registers, fp16 stores) | 12 conv TMA producer | 13 Y TMA producer
+//   flags per batch b: okY[b]  raised when all 4*grid Y warps finished batch b                (conv waits)
 //                      okC[b]  raised when all grid CTAs consumed batch b                 (Y waits okC[b-ring])
 //
 // Math and data movement of the two pipelines are those of conv_tc.cu and gemm_tc.cu.
+#include <type_traits>
+
 #include "kernels.h"
 #include "options.h"
 #include "tc05.cuh"
@@ -33,10 +34,12 @@ constexpr int kMaxAStages = 10;
 constexpr int kTU = 2;
 constexpr int kATileBytes = 128 * 64 * 2;
 constexpr int kYStages = 2;
-constexpr int kThreads = 384;
-constexpr int kQueue = 8;                  // unit queue between the scheduler and the MMA / epilogue warps
-constexpr int kScatterPitch = 272;         // bytes per staged edge row (64 fp32 + 16 B: bank-conflict-free v4 stores)
-constexpr int kScatterBytes = 4 * 32 * kScatterPitch;
+constexpr int kThreads = 14 * 32;
+constexpr int kConvProducer = 12, kYProducer = 13;
+constexpr int kQueue = 8;                  // unit queue between the scheduler and the conv warpgroups
+constexpr int kScatterPitch = 272;         // bytes per staged edge row (64 fp32 + 16 B)
+constexpr int kScatterBytes = 8 * 32 * kScatterPitch;
+constexpr int kYScratchBytes = 4 * acc_scratch_bytes<16>();
 
 struct ApplyArgs {
   // plan
@@ -53,7 +56,7 @@ struct ApplyArgs {
   const float* xs;        // [S] power-of-two row scale of the Y operand (see k_src_prep)
   float* out;             // [N, cout]
   int n_src, nb, n_batches, ring;
-  int cout, nb_slots, passes, a_stages, e_pad;
+  int nb_slots, passes, a_stages, e_pad;
   // PREC_F16X2 (plan.h): split_nk = Kp/64 > 0 -> h holds 2*split_nk chunk panels [hi | lo], a Y ring row is
   // [cout][hi(Kp) | lo(Kp)], and contraction step j = 3q + r pairs (A, B) = (hi_q, Yhi_q), (hi_q, Ylo_q), (lo_q, Yhi_q)
   int split_nk;
@@ -87,14 +90,14 @@ __device__ __forceinline__ void raise_when_all(int* cnt, int* ok, int target) {
   }
 }
 
-template <int FMT, int kYBlockN>
+template <int FMT, int kYBlockN, int NC>
 __global__ void __launch_bounds__(kThreads, 1)
 k_apply_tc(const __grid_constant__ HMaps tmH, const __grid_constant__ CUtensorMap tmY,
            const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmW, ApplyArgs a) {
   constexpr int kYStageBytes = kATileBytes + kYBlockN * 64 * 2;   // Xc tile + W3p tile
   extern __shared__ __align__(1024) uint8_t smem[];
   if ((smem_u32(smem) & 1023u) != 0) __trap();
-  const int b_chunk_bytes = a.cout * 128;
+  const int b_chunk_bytes = NC * 128;
   const int b_stride = (b_chunk_bytes + 1023) & ~1023;
   uint8_t* smem_b = smem;
   uint8_t* smem_a = smem_b + a.nb_slots * b_stride;
@@ -104,72 +107,56 @@ k_apply_tc(const __grid_constant__ HMaps tmH, const __grid_constant__ CUtensorMa
   uint64_t* a_empty = a_full + kMaxAStages;
   uint64_t* b_full = a_empty + kMaxAStages;
   uint64_t* b_empty = b_full + kMaxSlots;
-  uint64_t* tfull = b_empty + kMaxSlots;
-  uint64_t* tempty = tfull + 2;
-  uint64_t* y_full = tempty + 2;
+  uint64_t* y_full = b_empty + kMaxSlots;
   uint64_t* y_empty = y_full + kYStages;
-  uint64_t* yt_full = y_empty + kYStages;
-  uint64_t* yt_empty = yt_full + 2;
-  uint64_t* q_full = yt_empty + 2;       // [kQueue] 1 arrival (scheduler)
-  uint64_t* q_empty = q_full + kQueue;   // [kQueue] 5 arrivals (MMA issuer + 4 epilogue warps)
+  uint64_t* q_full = y_empty + kYStages;   // [kQueue] 1 arrival (scheduler)
+  uint64_t* q_empty = q_full + kQueue;   // [kQueue] 8 arrivals (the conv warps)
   int4* q_ent = reinterpret_cast<int4*>(q_empty + kQueue);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(q_ent + kQueue);
-  // scatter staging (scatter_mode 1): 4 epilogue warps x 32 rows x kScatterPitch bytes, after the 1 KB barrier block
-  uint8_t* smem_sc = reinterpret_cast<uint8_t*>(bars) + 1024;
+  // Y transposes (4 warps), then the scatter staging (scatter_mode 1: 8 conv warps x 32 rows x kScatterPitch bytes),
+  // after the 1 KB barrier block
+  float* y_scratch = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(bars) + 1024);
+  uint8_t* smem_sc = reinterpret_cast<uint8_t*>(bars) + 1024 + kYScratchBytes;
 
   // shfl: the warp index is warp-uniform for the compiler (see tc05::elect_one)
   const int warp = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x / 32), 0), lane = threadIdx.x % 32;
   const unsigned long long tr0 = a.trace.rec ? gtime() : 0ull;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == kConvProducer && lane == 0) {
     for (int i = 0; i < 8; ++i) prefetch_tmap(&tmH.m[i]);
     prefetch_tmap(&tmY);
     prefetch_tmap(&tmX);
     prefetch_tmap(&tmW);
     for (int s = 0; s < a.a_stages; ++s) {
       mbar_init(&a_full[s], 1);
-      mbar_init(&a_empty[s], 1);
+      mbar_init(&a_empty[s], 4);          // the 4 warps of the tile's warpgroup
     }
     for (int j = 0; j < a.nb_slots; ++j) {
       mbar_init(&b_full[j], 1);
-      mbar_init(&b_empty[j], 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&tfull[s], 1);
-      mbar_init(&tempty[s], 4);
-      mbar_init(&yt_full[s], 1);
-      mbar_init(&yt_empty[s], 4);
+      mbar_init(&b_empty[j], 8);          // both conv warpgroups
     }
     for (int s = 0; s < kYStages; ++s) {
       mbar_init(&y_full[s], 1);
-      mbar_init(&y_empty[s], 1);
+      mbar_init(&y_empty[s], 4);
     }
     for (int s = 0; s < kQueue; ++s) {
       mbar_init(&q_full[s], 1);
-      mbar_init(&q_empty[s], 5);
+      mbar_init(&q_empty[s], 8);
     }
     fence_barrier_init();
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, 512);
-    tmem_relinquish();
-  }
-  fence_before_sync();
   __syncthreads();
-  fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tmem_y = tmem_base + 256;
 
   // ---- contraction work distribution: units (<= 2 tiles of one source) of batch b are handed out
-  // dynamically (atomic counter per batch) to whichever CTA is ready.  With a static equal split the period of
-  // every batch was set by its slowest CTA and fast CTAs idled 17-29 % (profiles/r1e_trace_fused_flags.md).
-  // The producer thread grabs units and publishes them to the MMA / epilogue warps through a small
+  // dynamically (atomic counter per batch) to whichever CTA is ready, so that the period of a batch is not set by
+  // its slowest CTA (as with a static equal split).
+  // The producer thread grabs units and publishes them to the conv warpgroups through a small
   // shared-memory queue: entry = {first tile, #tiles (0 = end of this CTA's share of batch b, -1 = done), c, b}.
-  if (warp == 0) {
+  if (warp == kConvProducer) {
     // ============================================================== contraction: TMA producer + scheduler
     // (whole warp runs the loops; the elected lane issues -- see tc05::elect_one)
-    int stage = 0;
-    uint32_t phase = 0;
+    ARing ring[kTU];
+#pragma unroll
+    for (int ti = 0; ti < kTU; ++ti) ring[ti].init(ti, a.a_stages);
     int bs = 0;               // B slot ring (one slot per K chunk of the current unit's Y slice)
     uint32_t bph = 0;
     const int num_kc = a.passes * a.nb_slots;
@@ -220,8 +207,8 @@ k_apply_tc(const __grid_constant__ HMaps tmH, const __grid_constant__ CUtensorMa
         tbox[ti] = ti < uu ? (__shfl_sync(0xffffffffu, __ldg(a.tile_cnt + ut + ti), 0) + 15) >> 4 : 1;
       }
       // K chunk outer, tile inner: the B slot of chunk j is released after the unit's LAST tile and needed again
-      // only nb_slots chunks later, i.e. 2*nb_slots - 1 MMA blocks for a 2-tile unit (with a pass-major order it
-      // was nb_slots - 1 and the MMA warp spent 20% of its time waiting for B, ncu r1g)
+      // only nb_slots chunks later, i.e. 2*nb_slots - 1 MMA blocks for a 2-tile unit (a pass-major order leaves only
+      // nb_slots - 1)
       for (int j = 0; j < num_kc; ++j) {
         int ja = j, jb = j;
         if (a.split_nk > 0) {
@@ -232,7 +219,7 @@ k_apply_tc(const __grid_constant__ HMaps tmH, const __grid_constant__ CUtensorMa
         mbar_wait(&b_empty[bs], bph ^ 1u);
         if (elect_one()) {
           mbar_arrive_expect_tx(&b_full[bs], b_chunk_bytes);
-          tma_load_2d(smem_b + bs * b_stride, &tmY, &b_full[bs], jb * 64, (ring_row0 + uc) * a.cout, kEvictLast);
+          tma_load_2d(smem_b + bs * b_stride, &tmY, &b_full[bs], jb * 64, (ring_row0 + uc) * NC, kEvictLast);
         }
         __syncwarp();
         if (++bs == a.nb_slots) { bs = 0; bph ^= 1u; }
@@ -241,160 +228,132 @@ k_apply_tc(const __grid_constant__ HMaps tmH, const __grid_constant__ CUtensorMa
           if (ti < uu) {
             const CUtensorMap* mh = &tmH.m[tbox[ti] - 1];
             const uint32_t a_bytes = static_cast<uint32_t>(tbox[ti]) * 16u * 128u;
-            mbar_wait(&a_empty[stage], phase ^ 1u);
+            const int stage = ring[ti].stage;
+            mbar_wait(&a_empty[stage], ring[ti].phase ^ 1u);
             if (elect_one()) {
               mbar_arrive_expect_tx(&a_full[stage], a_bytes);
               tma_load_2d(smem_a + stage * kATileBytes, mh, &a_full[stage], 0, ja * a.e_pad + te0[ti], a.a_policy);
             }
             __syncwarp();
-            if (++stage == a.a_stages) { stage = 0; phase ^= 1u; }
+            ring[ti].next();
           }
         }
       }
     }
     publish(0, -1, 0, 0);
-  } else if (warp == 1) {
-    // ============================================================== contraction: MMA issuer (whole warp, elected lane)
-    const uint32_t idesc = idesc_f16(FMT, 128, static_cast<uint32_t>(a.cout));
-    int stage = 0;
-    uint32_t phase = 0;
+  } else if (warp < 8) {
+    // ============================================================== contraction: warpgroup g = tile g of every unit
+    const int g = warp / 4, quarter = warp % 4;
+    Acc<NC> acc;
+    ARing ring;
+    ring.init(g, a.a_stages);
     int bs = 0;
     uint32_t bph = 0;
     const int num_kc = a.passes * a.nb_slots;
-    int it = 0;
     int qi = 0;
     uint32_t qph = 0;
+    // fragment rows of this thread (acc_row numbering: lane L of the warp stands for row acc_row(quarter, L))
+    const int fr = lane >> 2, fc = (lane & 3) * 2;
+    const uint32_t my_rows = smem_u32(smem_sc) + static_cast<uint32_t>(warp * 32 * kScatterPitch);
     for (;;) {
       mbar_wait(&q_full[qi], qph);
-      const int4 en0 = q_ent[qi];
-      const int en_y = __shfl_sync(0xffffffffu, en0.y, 0);
-      __syncwarp();
-      if (elect_one()) mbar_arrive(&q_empty[qi]);
-      if (++qi == kQueue) { qi = 0; qph ^= 1u; }
-      if (en_y < 0) break;
-      if (en_y == 0) continue;
-      const int as = it & 1;
-      mbar_wait(&tempty[as], ((it >> 1) & 1) ^ 1u);
-      fence_after_sync();
-      for (int j = 0; j < num_kc; ++j) {
-        mbar_wait(&b_full[bs], bph);
-        const uint64_t bdesc = smem_desc_sw128(smem_u32(smem_b + bs * b_stride));
-#pragma unroll
-        for (int ti = 0; ti < kTU; ++ti) {
-          if (ti < en_y) {
-            const uint32_t d_tmem = tmem_base + (as * kTU + ti) * a.cout;
-            mbar_wait(&a_full[stage], phase);
-            fence_after_sync();
-            const uint64_t adesc = smem_desc_sw128(smem_u32(smem_a + stage * kATileBytes));
-            if (elect_one()) {
-#pragma unroll
-              for (int k = 0; k < 4; ++k) umma_f16(d_tmem, adesc + 2 * k, bdesc + 2 * k, idesc, (j | k) != 0);
-              umma_commit(&a_empty[stage]);
-              if (ti == en_y - 1) umma_commit(&b_empty[bs]);    // B is re-loaded for every unit
-            }
-            __syncwarp();
-            if (++stage == a.a_stages) { stage = 0; phase ^= 1u; }
-          }
-        }
-        if (++bs == a.nb_slots) { bs = 0; bph ^= 1u; }
-      }
-      if (elect_one()) umma_commit(&tfull[as]);
-      __syncwarp();
-      ++it;
-    }
-  } else if (warp < 6) {
-    // ================================================================ contraction: epilogue warps 2..5
-    const int quarter = warp % 4;
-    int it = 0;
-    int qi = 0;
-    uint32_t qph = 0;
-    for (;;) {
-      mbar_wait(&q_full[qi], qph);
-      const int4 en = q_ent[qi];
+      int4 en = q_ent[qi];
+      en.y = __shfl_sync(0xffffffffu, en.y, 0);          // warp-uniform: wgmma sits under `g < en.y`
       __syncwarp();
       if (lane == 0) mbar_arrive(&q_empty[qi]);
       if (++qi == kQueue) { qi = 0; qph ^= 1u; }
       if (en.y < 0) break;
       if (en.y == 0) continue;
-      const int as = it & 1;
-      const int r = quarter * 32 + lane;
-      int d[kTU];
-      float sc[kTU];
-      bool ok[kTU];
-#pragma unroll
-      for (int ti = 0; ti < kTU; ++ti) {
-        ok[ti] = ti < en.y && r < a.tile_cnt[en.x + ti];
-        d[ti] = 0;
-        sc[ti] = 1.f;
-        if (ok[ti]) {
-          d[ti] = __ldg(a.dst_sorted + a.tile_e0[en.x + ti] + r);
-          if (a.inv_deg) sc[ti] = __ldg(a.inv_deg + d[ti]);
+      for (int j = 0; j < num_kc; ++j) {
+        mbar_wait(&b_full[bs], bph);
+        const uint64_t bdesc = smem_desc_sw128(smem_u32(smem_b + bs * b_stride));
+        if (g < en.y) {
+          mbar_wait(&a_full[ring.stage], ring.phase);
+          const uint64_t adesc = smem_desc_sw128(smem_u32(smem_a + ring.stage * kATileBytes));
+          mma_block<NC, FMT>(acc, adesc, bdesc, 512, 2, 4, j != 0);
+          wgmma_wait<0>();
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&a_empty[ring.stage]);
+          ring.next();
         }
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&b_empty[bs]);          // B is re-loaded for every unit
+        if (++bs == a.nb_slots) { bs = 0; bph ^= 1u; }
       }
-      const float* cv = a.cvec + static_cast<int64_t>(en.z) * a.cout;
-      const float xsc = __ldg(a.xs + en.z);
-      const uint32_t my_row = smem_u32(smem_sc) + static_cast<uint32_t>(((warp - 2) * 32 + lane) * kScatterPitch);
-      mbar_wait(&tfull[as], (it >> 1) & 1);
-      fence_after_sync();
-      if (warp == 2 && lane == 0) {
-        // every MMA that read this unit's Y slice has completed: count the unit; the last unit of batch b
-        // frees the ring slot for the Y pipeline
+      // every MMA that read this unit's Y slice has completed: count the unit; the last unit of batch b frees the
+      // ring slot for the Y pipeline
+      named_bar_sync(1, 256);
+      if (warp == 0 && lane == 0) {
         const int c0 = en.w * a.nb;
         const int target = __ldg(a.unit_ptr + min(c0 + a.nb, a.n_src)) - __ldg(a.unit_ptr + c0);
         raise_when_all(a.cntC + en.w, a.okC + en.w, target);
       }
+      if (g >= en.y) continue;
+      // ---- scatter of tile g straight from the accumulator fragments: thread (lane) holds rows
+      // L = fr, fr + 8 (first m64 half) and 16 + fr, 24 + fr (second half) of the warp, columns 8 jj + fc, + 1
+      const int r = acc_row(quarter, lane);
+      const bool ok = r < a.tile_cnt[en.x + g];
+      int d = 0;
+      float sc = 1.f;
+      if (ok) {
+        d = __ldg(a.dst_sorted + a.tile_e0[en.x + g] + r);
+        if (a.inv_deg) sc = __ldg(a.inv_deg + d);
+      }
+      const float* cv = a.cvec + static_cast<int64_t>(en.z) * NC;
+      const float xsc = __ldg(a.xs + en.z);
+      float* orow = a.out + static_cast<int64_t>(d) * NC;
+      int fd[4];
+      float fsc[4];
+      bool fok[4];
 #pragma unroll
-      for (int ti = 0; ti < kTU; ++ti) {
-        if (ti < en.y) {
-          float* orow = a.out + static_cast<int64_t>(d[ti]) * a.cout;
-          if (a.scatter_mode == 1) bulk_wait_read0();     // this lane's previous row has left its staging slot
-#pragma unroll 1
-          for (int cc = 0; cc < a.cout; cc += 16) {
-            uint32_t v[16];
-            tmem_ld16(tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + (as * kTU + ti) * a.cout + cc, v);
-            tmem_ld_wait();
-            if (a.scatter_mode == 1) {
-              // the lane's own row: 4 x 16 B into its staging slot (pitch 272 B: conflict-free 8-lane phases)
+      for (int i = 0; i < 4; ++i) {
+        const int L = fr + 8 * i;
+        fd[i] = __shfl_sync(0xffffffffu, d, L);
+        fsc[i] = __shfl_sync(0xffffffffu, sc, L);
+        fok[i] = __shfl_sync(0xffffffffu, ok ? 1 : 0, L) != 0;
+      }
+      if (a.scatter_mode == 1) {
+        // rows staged in shared memory, then one bulk reduction per row (its lane issues it)
+        bulk_wait_read0();                                 // this lane's previous row has left its staging slot
+        __syncwarp();
 #pragma unroll
-              for (int q = 0; q < 4; ++q) {
-                const float4 cq = __ldg(reinterpret_cast<const float4*>(cv + cc) + q);
-                st_shared_v4(my_row + static_cast<uint32_t>((cc + 4 * q) * 4),
-                             __float_as_uint(fmaf(__uint_as_float(v[4 * q + 0]), xsc, cq.x) * sc[ti]),
-                             __float_as_uint(fmaf(__uint_as_float(v[4 * q + 1]), xsc, cq.y) * sc[ti]),
-                             __float_as_uint(fmaf(__uint_as_float(v[4 * q + 2]), xsc, cq.z) * sc[ti]),
-                             __float_as_uint(fmaf(__uint_as_float(v[4 * q + 3]), xsc, cq.w) * sc[ti]));
-              }
-            } else if (ok[ti] && a.debug_scatter == 2) {
+        for (int jj = 0; jj < NC / 8; ++jj) {
+          const float2 cq = __ldg(reinterpret_cast<const float2*>(cv + 8 * jj + fc));
 #pragma unroll
-              for (int q = 0; q < 4; ++q)
-                *reinterpret_cast<float4*>(orow + cc + 4 * q) =
-                    make_float4(__uint_as_float(v[4 * q]), __uint_as_float(v[4 * q + 1]), __uint_as_float(v[4 * q + 2]),
-                                __uint_as_float(v[4 * q + 3]));
-            } else if (ok[ti] && a.debug_scatter == 0) {
-#pragma unroll
-              for (int q = 0; q < 4; ++q) {
-                const float4 cq = __ldg(reinterpret_cast<const float4*>(cv + cc) + q);
-                red_add_v4(orow + cc + 4 * q, fmaf(__uint_as_float(v[4 * q + 0]), xsc, cq.x) * sc[ti],
-                           fmaf(__uint_as_float(v[4 * q + 1]), xsc, cq.y) * sc[ti],
-                           fmaf(__uint_as_float(v[4 * q + 2]), xsc, cq.z) * sc[ti],
-                           fmaf(__uint_as_float(v[4 * q + 3]), xsc, cq.w) * sc[ti]);
-              }
-            }
+          for (int i = 0; i < 4; ++i) {
+            const float* dv = acc.d[i >> 1] + 4 * jj + 2 * (i & 1);
+            const uint32_t addr = my_rows + static_cast<uint32_t>((fr + 8 * i) * kScatterPitch + (8 * jj + fc) * 4);
+            asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(fmaf(dv[0], xsc, cq.x) * fsc[i]),
+                         "f"(fmaf(dv[1], xsc, cq.y) * fsc[i])
+                         : "memory");
           }
-          if (a.scatter_mode == 1) {
-            fence_proxy_async_smem();                       // generic-proxy writes of this lane -> async proxy
-            if (ok[ti]) bulk_reduce_add_f32(orow, my_row, static_cast<uint32_t>(a.cout) * 4u);
-            bulk_commit();
+        }
+        fence_proxy_async_smem();                         // generic-proxy writes of the warp -> async proxy
+        __syncwarp();
+        if (ok) bulk_reduce_add_f32(orow, my_rows + static_cast<uint32_t>(lane * kScatterPitch), static_cast<uint32_t>(NC) * 4u);
+        bulk_commit();
+      } else if (a.debug_scatter != 1) {
+#pragma unroll
+        for (int jj = 0; jj < NC / 8; ++jj) {
+          const float2 cq = __ldg(reinterpret_cast<const float2*>(cv + 8 * jj + fc));
+#pragma unroll
+          for (int i = 0; i < 4; ++i) {
+            if (!fok[i]) continue;
+            const float* dv = acc.d[i >> 1] + 4 * jj + 2 * (i & 1);
+            float* dst = a.out + static_cast<int64_t>(fd[i]) * NC + 8 * jj + fc;
+            if (a.debug_scatter == 2) {
+              *reinterpret_cast<float2*>(dst) = make_float2(dv[0], dv[1]);
+            } else {
+              asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(dst), "f"(fmaf(dv[0], xsc, cq.x) * fsc[i]),
+                           "f"(fmaf(dv[1], xsc, cq.y) * fsc[i])
+                           : "memory");
+            }
           }
         }
       }
-      fence_before_sync();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty[as]);
-      ++it;
     }
     if (a.scatter_mode == 1) bulk_wait0();                  // every row has been added before the CTA retires
-  } else if (warp == 6) {
+  } else if (warp == kYProducer) {
     // ============================================================== Y GEMM: TMA producer (whole warp, elected lane)
     const int n_blocks = a.NY / kYBlockN;
     int stage = 0;
@@ -418,51 +377,22 @@ k_apply_tc(const __grid_constant__ HMaps tmH, const __grid_constant__ CUtensorMa
         }
       }
     }
-  } else if (warp == 7) {
-    // ============================================================== Y GEMM: MMA issuer (whole warp, elected lane)
-    constexpr uint32_t idesc = idesc_f16(FMT, 128, kYBlockN);
-    const int n_blocks = a.NY / kYBlockN;
-    int stage = 0;
-    uint32_t phase = 0;
-    int it = 0;
-    for (int b = 0; b < a.n_batches; ++b) {
-      const int c0 = b * a.nb;
-      const int rows = min(a.nb, a.n_src - c0);
-      const int tiles = ((rows + 127) / 128) * n_blocks;
-      for (int i = static_cast<int>((blockIdx.x + 7u * b) % gridDim.x); i < tiles; i += gridDim.x, ++it) {
-        const int ys = it & 1;
-        mbar_wait(&yt_empty[ys], ((it >> 1) & 1) ^ 1u);
-        fence_after_sync();
-        for (int kx = 0; kx < a.num_kx; ++kx) {
-          mbar_wait(&y_full[stage], phase);
-          fence_after_sync();
-          uint8_t* st = smem_y + stage * kYStageBytes;
-          const uint64_t adesc = smem_desc_sw128(smem_u32(st));
-          const uint64_t bdesc = smem_desc_sw128(smem_u32(st + kATileBytes));
-          if (elect_one()) {
-#pragma unroll
-            for (int k = 0; k < 4; ++k) umma_f16(tmem_y + ys * kYBlockN, adesc + 2 * k, bdesc + 2 * k, idesc, (kx | k) != 0);
-            umma_commit(&y_empty[stage]);
-            if (kx == a.num_kx - 1) umma_commit(&yt_full[ys]);
-          }
-          __syncwarp();
-          if (++stage == kYStages) { stage = 0; phase ^= 1u; }
-        }
-      }
-    }
   } else {
-    // ================================================================ Y GEMM: epilogue warps 8..11
+    // ================================================================ Y GEMM: warpgroup of warps 8..11
     const int quarter = warp % 4;
     const int n_blocks = a.NY / kYBlockN;
-    int it = 0;
+    float* wb = y_scratch + quarter * (acc_scratch_bytes<16>() / 4);
+    Acc<kYBlockN> acc;
+    int stage = 0;
+    uint32_t phase = 0;
     for (int b = 0; b < a.n_batches; ++b) {
       const int c0 = b * a.nb;
       const int rows = min(a.nb, a.n_src - c0);
       const int tiles = ((rows + 127) / 128) * n_blocks;
       const unsigned long long ty0 = a.trace.rec ? gtime() : 0ull;
       if (b >= a.ring) {                         // the ring slot must have been consumed by every CTA
-        // ONE slow poller per CTA (the Y pipeline runs ring-1 batches ahead, so this wait is long -- 20-35 us per
-        // batch -- and never urgent); the other three epilogue warps park on a named barrier
+        // ONE slow poller per CTA (the Y pipeline runs ring-1 batches ahead, so this wait is long and never
+        // urgent); the other three warps of the Y warpgroup park on a named barrier
         if (warp == 8 && lane == 0) flag_wait(a.okC + (b - a.ring), 500);
         named_bar_sync(2, 128);
       }
@@ -470,28 +400,31 @@ k_apply_tc(const __grid_constant__ HMaps tmH, const __grid_constant__ CUtensorMa
       const int ymul = a.split_nk > 0 ? 2 : 1;
       const float ysc = a.y_scale != nullptr ? __ldg(a.y_scale) : 1.f;
       uint16_t* ybase = reinterpret_cast<uint16_t*>(a.Yring) + static_cast<int64_t>(b % a.ring) * a.nb * a.NY * ymul;
-      for (int i = static_cast<int>((blockIdx.x + 7u * b) % gridDim.x); i < tiles; i += gridDim.x, ++it) {
+      for (int i = static_cast<int>((blockIdx.x + 7u * b) % gridDim.x); i < tiles; i += gridDim.x) {
         const int mb = i / n_blocks, nbk = i % n_blocks;
-        const int ys = it & 1;
-        mbar_wait(&yt_full[ys], (it >> 1) & 1);
-        fence_after_sync();
-        const int row = mb * 128 + quarter * 32 + lane;
+        for (int kx = 0; kx < a.num_kx; ++kx) {
+          mbar_wait(&y_full[stage], phase);
+          uint8_t* st = smem_y + stage * kYStageBytes;
+          mma_block<kYBlockN, FMT>(acc, smem_desc_sw128(smem_u32(st)), smem_desc_sw128(smem_u32(st + kATileBytes)), 512, 2,
+                                   4, kx != 0);
+          wgmma_wait<0>();
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&y_empty[stage]);
+          if (++stage == kYStages) { stage = 0; phase ^= 1u; }
+        }
+        const int row = mb * 128 + acc_row(quarter, lane);
         const bool row_ok = row < rows;
         // column n = o * Kp + k of the source's matrix; with split rows of 2*Kp: offset n + o * Kp
         const int n0 = nbk * kYBlockN;
         uint16_t* yrow0 = ybase + static_cast<int64_t>(row) * a.NY * ymul;
-        const uint32_t tb = tmem_y + (static_cast<uint32_t>(quarter * 32) << 16) + ys * kYBlockN;
-        uint32_t v[2][32];
-        tmem_ld32(tb, v[0]);
-        tmem_ld_wait();
 #pragma unroll
-        for (int cc = 0; cc < kYBlockN / 32; ++cc) {
-          if (cc + 1 < kYBlockN / 32) tmem_ld32(tb + (cc + 1) * 32, v[(cc + 1) & 1]);
+        for (int cc = 0; cc < kYBlockN / 16; ++cc) {
+          uint32_t vv[16];
+          acc_rows<kYBlockN, 16>(acc, cc * 16, wb, vv);
           if (row_ok) {
-            const uint32_t* vv = v[cc & 1];
-            uint32_t packed[16], packed_lo[16];
+            uint32_t packed[8], packed_lo[8];
 #pragma unroll
-            for (int j = 0; j < 16; ++j) {
+            for (int j = 0; j < 8; ++j) {
               float f0 = __uint_as_float(vv[2 * j]), f1 = __uint_as_float(vv[2 * j + 1]);
               if (FMT == 0 && a.split_nk > 0) { f0 *= ysc; f1 *= ysc; }
               if (FMT == 0) {
@@ -507,20 +440,12 @@ k_apply_tc(const __grid_constant__ HMaps tmH, const __grid_constant__ CUtensorMa
                 packed[j] = *reinterpret_cast<uint32_t*>(&hh);
               }
             }
-            const int n = n0 + cc * 32;
+            const int n = n0 + cc * 16;
             uint16_t* yrow = yrow0 + n + (a.split_nk > 0 ? (n / a.Kp) * a.Kp : 0);
-            st_global_v8_hint(yrow, packed, a.y_store_policy);
-            st_global_v8_hint(yrow + 16, packed + 8, a.y_store_policy);
-            if (FMT == 0 && a.split_nk > 0) {
-              st_global_v8_hint(yrow + a.Kp, packed_lo, a.y_store_policy);
-              st_global_v8_hint(yrow + a.Kp + 16, packed_lo + 8, a.y_store_policy);
-            }
+            st_global_32b_hint(yrow, packed, a.y_store_policy);
+            if (FMT == 0 && a.split_nk > 0) st_global_32b_hint(yrow + a.Kp, packed_lo, a.y_store_policy);
           }
-          if (cc + 1 < kYBlockN / 32) tmem_ld_wait();
         }
-        fence_before_sync();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&yt_empty[ys]);
       }
       // this warp's stores of batch b are out: 4 warps x grid arrivals complete the batch
       __threadfence();
@@ -530,12 +455,7 @@ k_apply_tc(const __grid_constant__ HMaps tmH, const __grid_constant__ CUtensorMa
         trace_write(a.trace, 302u | (static_cast<unsigned>(b) << 12), ty0, ty1, gtime());
     }
   }
-  fence_before_sync();
   __syncthreads();
-  if (warp == 1) {
-    fence_after_sync();
-    tmem_dealloc(tmem_base, 512);
-  }
   if (threadIdx.x == 0) trace_write(a.trace, 300u, tr0, tr0, a.trace.rec ? gtime() : 0ull);
 }
 
@@ -545,10 +465,10 @@ struct ApplyShape {
 
 bool apply_shape(int cout, int Kp, int ybn, ApplyShape* as) {
   const int kYStageBytes = kATileBytes + ybn * 64 * 2;
-  if (cout % 16 != 0 || cout < 16 || 2 * kTU * cout > 256 || Kp % 64 != 0) return false;
+  if (cout % 16 != 0 || cout < 16 || cout > 64 || Kp % 64 != 0) return false;
   const int num_kc = Kp / 64;
   const int b_stride = (cout * 128 + 1023) & ~1023;
-  const int bar_bytes = 1024 + (options().scatter_mode == 1 ? kScatterBytes : 0);
+  const int bar_bytes = 1024 + kYScratchBytes + (options().scatter_mode == 1 ? kScatterBytes : 0);
   const int budget = 227 * 1024 - bar_bytes - kYStages * kYStageBytes;
   // fewest passes that leave >= 7 A stages (the h stream needs the bytes in flight), else >= 5, else >= 3
   const int forced = options().apply_passes;
@@ -575,11 +495,9 @@ bool apply_shape(int cout, int Kp, int ybn, ApplyShape* as) {
 
 }  // namespace
 
-static int y_block_n() {
-  // N tile of the Y pipeline: 64 (default: smaller stage -> 7 instead of 6 A stages for the h stream, measured
-  // 72.6 vs 74.1 ms per step at 241^2, run27) or 128
-  return options().y_block_n == 128 ? 128 : 64;
-}
+// N tile of the Y pipeline: 64 columns = 64 accumulator registers per thread of the Y warpgroup, which shares the SM's
+// register file with the two conv warpgroups (a 128-column tile spills and serialises its wgmma on sm_90)
+constexpr int kYBN = 64;
 
 static int eff_kp(const Weights* W) { return W->split ? 3 * W->Kp : W->Kp; }
 
@@ -587,21 +505,21 @@ bool apply_fused_supported(const Weights* W) {
   if (W->prec != PREC_F16 && W->prec != PREC_BF16 && W->prec != PREC_F16X2) return false;
   if ((W->cout * W->Kp) % 128 != 0) return false;
   ApplyShape as;
-  return apply_shape(W->cout, eff_kp(W), y_block_n(), &as);
+  return apply_shape(W->cout, eff_kp(W), kYBN, &as);
 }
 
 namespace {
-template <int FMT, int YBN>
+template <int FMT, int YBN, int NC>
 int launch_variant(int grid, int smem_bytes, bool coop, cudaStream_t st, const HMaps& tmH, const CUtensorMap& tmY,
                    const CUtensorMap& tmX, const CUtensorMap& tmW, const ApplyArgs& a) {
   static bool attr_set = false;
   static int blocks_per_sm = -1;
   if (!attr_set) {
-    NNC_CHECK_CUDA(cudaFuncSetAttribute(k_apply_tc<FMT, YBN>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    NNC_CHECK_CUDA(cudaFuncSetAttribute(k_apply_tc<FMT, YBN, NC>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     attr_set = true;
   }
   if (blocks_per_sm < 0)
-    NNC_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks_per_sm, k_apply_tc<FMT, YBN>, kThreads,
+    NNC_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks_per_sm, k_apply_tc<FMT, YBN, NC>, kThreads,
                                                                  smem_bytes));
   NNC_REQUIRE(blocks_per_sm >= 1, NNCONV_ERR_UNSUPPORTED, "apply_tc: the persistent kernel does not fit one SM");
   cudaLaunchConfig_t cfg{};
@@ -619,7 +537,7 @@ int launch_variant(int grid, int smem_bytes, bool coop, cudaStream_t st, const H
   attr[0].val.cooperative = 1;
   cfg.attrs = attr;
   cfg.numAttrs = coop ? 1 : 0;
-  cudaError_t e = cudaLaunchKernelEx(&cfg, k_apply_tc<FMT, YBN>, tmH, tmY, tmX, tmW, a);
+  cudaError_t e = cudaLaunchKernelEx(&cfg, k_apply_tc<FMT, YBN, NC>, tmH, tmY, tmX, tmW, a);
   if (e == cudaErrorCooperativeLaunchTooLarge) {
     cudaGetLastError();
     return kApplyCannotCoSchedule;   // handled by apply(): per-batch kernels instead
@@ -637,7 +555,7 @@ int launch_apply_tc(int prec, const Plan* P, const Weights* W, const void* h, co
   const Options& opt = options();
   const int bf = prec == PREC_BF16;
   const int split = W->split ? 1 : 0;
-  const int ybn = y_block_n();
+  const int ybn = kYBN;
   ApplyShape as;
   NNC_REQUIRE(apply_shape(W->cout, eff_kp(W), ybn, &as), NNCONV_ERR_UNSUPPORTED, "apply_tc: unsupported shape");
   if (opt.apply_stages >= 2 && opt.apply_stages < as.a_stages) as.a_stages = opt.apply_stages;
@@ -667,7 +585,7 @@ int launch_apply_tc(int prec, const Plan* P, const Weights* W, const void* h, co
   a.unit_ptr = P->unit_ptr; a.unit_t = P->unit_t; a.unit_u = P->unit_u;
   a.dst_sorted = P->dst_sorted; a.inv_deg = aggr_mean ? P->inv_deg : nullptr; a.cvec = cvec; a.xs = xs; a.out = out;
   a.n_src = P->n_src; a.nb = nb; a.n_batches = n_batches; a.ring = ring;
-  a.cout = W->cout; a.nb_slots = as.nb_slots; a.passes = as.passes; a.a_stages = as.a_stages;
+  a.nb_slots = as.nb_slots; a.passes = as.passes; a.a_stages = as.a_stages;
   a.e_pad = static_cast<int>(e_pad);
   a.split_nk = split ? W->Kp / 64 : 0;
   a.Kp = W->Kp;
@@ -712,10 +630,19 @@ int launch_apply_tc(int prec, const Plan* P, const Weights* W, const void* h, co
   // exactly one CTA per SM, never more than #SMs (see launch_variant about co-residency)
   const int grid = tc_num_sms();
   const bool coop = opt.no_coop == 0;
-  if (ybn == 64) s = bf ? launch_variant<1, 64>(grid, as.smem_bytes, coop, st, tmH, tmY, tmX, tmW, a)
-                        : launch_variant<0, 64>(grid, as.smem_bytes, coop, st, tmH, tmY, tmX, tmW, a);
-  else s = bf ? launch_variant<1, 128>(grid, as.smem_bytes, coop, st, tmH, tmY, tmX, tmW, a)
-              : launch_variant<0, 128>(grid, as.smem_bytes, coop, st, tmH, tmY, tmX, tmW, a);
+  auto go = [&](auto fmt, auto nc) -> int {
+    return launch_variant<decltype(fmt)::value, kYBN, decltype(nc)::value>(grid, as.smem_bytes, coop, st,
+                                                                                           tmH, tmY, tmX, tmW, a);
+  };
+  auto by_cout = [&](auto fmt) -> int {
+    switch (W->cout) {
+      case 16: return go(fmt, std::integral_constant<int, 16>());
+      case 32: return go(fmt, std::integral_constant<int, 32>());
+      case 48: return go(fmt, std::integral_constant<int, 48>());
+      default: return go(fmt, std::integral_constant<int, 64>());
+    }
+  };
+  s = bf ? by_cout(std::integral_constant<int, 1>()) : by_cout(std::integral_constant<int, 0>());
   if (window_set) {
     cudaStreamAttrValue v{};
     v.accessPolicyWindow.num_bytes = 0;

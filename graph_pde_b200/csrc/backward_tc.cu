@@ -6,7 +6,7 @@
 // G_e = g[dst_e] / max(deg_in(dst_e),1) (mean) or g[dst_e] (add), g = dL/dout.
 //
 //   per APPLICATION (backward_apply_tc, needs g of that application):
-//     dY_c[k,o]  = sum_{e in c} h_e[k] G_e[o]            k_dy:   per-source reduction over edges, MN-major UMMA
+//     dY_c[k,o]  = sum_{e in c} h_e[k] G_e[o]            k_dy:   per-source reduction over edges, MN-major wgmma
 //     dx_c       = dY_c : W_L + B_L Gs_c                  k_gemm_tc (K = Kp*out) + scatter
 //     dW_L      += x_c (x) dY_c                           k_gemm_tn over sources
 //     droot, dbias, dx += g root^T, dB_L                  CUDA cores (N x in x out, negligible)
@@ -47,16 +47,6 @@ __device__ __forceinline__ uint32_t pack2(float a, float b) {
     __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
     return *reinterpret_cast<uint32_t*>(&h);
   }
-}
-
-__device__ __forceinline__ uint64_t desc_mn_sw128(uint32_t smem_addr, uint32_t lbo_bytes) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);
-  d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;
-  d |= static_cast<uint64_t>(1024 >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
-  return d;
 }
 
 struct Maps8 {
@@ -332,15 +322,14 @@ __global__ void k_max_f(const float* __restrict__ v, int n, float* __restrict__ 
 
 // =====================================================================================================
 // k_dy: dY_c^T[k, o] = sum_{e in c} h_e[k] G_e[o] for the sources [c0, c1)   (out = 64)
-//   UMMA M = 128 k's (two 64-column chunk panels of h, MN-major A), N = 64 (G tile, MN-major B), K = edges.
-//   One source at a time per CTA; its ceil(Kp/128) accumulators of 64 columns sit side by side in TMEM.
-//   roles: warp 0 TMA producer | warp 1 MMA issuer | warps 2..5 epilogue (TMEM -> 16-bit -> dY[c, k*64 + o])
+//   wgmma M = 128 k's (two 64-column chunk panels of h, MN-major A), N = 64 (G tile, MN-major B), K = edges.
+//   One (source, 128-k block) at a time per CTA, its [128 x 64] accumulator in the registers of the warpgroup; a
+//   stage holds the k block's two h boxes and the G box of one tile of the source.
+//   roles: warps 0..3 consumer warpgroup (wgmma, then 16-bit -> dY[c, k*64 + o]) | warp 4 TMA producer
 // =====================================================================================================
-constexpr int kDyAStage = 32 * 1024;   // two [<=128 rows x 128 B] boxes
-constexpr int kDyBStage = 16 * 1024;
-constexpr int kDyAStages = 5;
-constexpr int kDyBStages = 2;
-constexpr int kDySmem = kDyAStages * kDyAStage + kDyBStages * kDyBStage + 1024;
+constexpr int kDyStage = 48 * 1024;    // two [<=128 rows x 128 B] h boxes + one G box
+constexpr int kDyStages = 4;
+constexpr int kDySmem = kDyStages * kDyStage + 4 * acc_scratch_bytes<32>() + 1024;
 
 struct DyArgs {
   const int* tile_ptr;
@@ -349,154 +338,99 @@ struct DyArgs {
   int c0, c1;
   int e_pad, nk;            // nk = Kp / 64 chunk panels
   int num_mt;               // ceil(nk / 2)
-  int nbuf;                 // 2 when two sources' accumulators fit TMEM, else 1
   int Kp;
   uint16_t* dY;             // [c1 - c0, Kp * 64]
 };
 
 template <int FMT>
-__global__ void __launch_bounds__(192, 1)
+__global__ void __launch_bounds__(160, 1)
 k_dy(const __grid_constant__ Maps8 tmH, const __grid_constant__ Maps8 tmG, DyArgs a) {
   extern __shared__ __align__(1024) uint8_t smem[];
   if ((smem_u32(smem) & 1023u) != 0) __trap();
-  uint8_t* smem_a = smem;
-  uint8_t* smem_b = smem + kDyAStages * kDyAStage;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem_b + kDyBStages * kDyBStage);
-  uint64_t* a_full = bars;
-  uint64_t* a_empty = a_full + kDyAStages;
-  uint64_t* b_full = a_empty + kDyAStages;
-  uint64_t* b_empty = b_full + kDyBStages;
-  uint64_t* tfull = b_empty + kDyBStages;
-  uint64_t* tempty = tfull + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
+  float* scratch = reinterpret_cast<float*>(smem + kDyStages * kDyStage);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kDyStages * kDyStage + 4 * acc_scratch_bytes<32>());
+  uint64_t* full = bars;
+  uint64_t* empty = full + kDyStages;
   const int warp = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x / 32), 0), lane = threadIdx.x % 32;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == 4 && lane == 0) {
     for (int i = 0; i < 8; ++i) { prefetch_tmap(&tmH.m[i]); prefetch_tmap(&tmG.m[i]); }
-    for (int s = 0; s < kDyAStages; ++s) { mbar_init(&a_full[s], 1); mbar_init(&a_empty[s], 1); }
-    for (int s = 0; s < kDyBStages; ++s) { mbar_init(&b_full[s], 1); mbar_init(&b_empty[s], 1); }
-    for (int s = 0; s < 2; ++s) { mbar_init(&tfull[s], 1); mbar_init(&tempty[s], 4); }
+    for (int s = 0; s < kDyStages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 4); }
     fence_barrier_init();
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, 512);
-    tmem_relinquish();
-  }
-  fence_before_sync();
   __syncthreads();
-  fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
-  const int acc_cols = a.num_mt * 64;
 
-  if (warp == 0) {
-    int stage = 0, bs = 0;
-    uint32_t phase = 0, bph = 0;
+  if (warp == 4) {
+    int stage = 0;
+    uint32_t phase = 0;
     for (int c = a.c0 + blockIdx.x; c < a.c1; c += gridDim.x) {
       const int t0 = __ldg(a.tile_ptr + c), t1 = __ldg(a.tile_ptr + c + 1);
-      for (int t = t0; t < t1; ++t) {
-        const int e0 = __ldg(a.tile_e0 + t);
-        const int box = (__ldg(a.tile_cnt + t) + 15) >> 4;       // 16-row units, 1..8
-        const uint32_t box_bytes = static_cast<uint32_t>(box) * 16u * 128u;
-        mbar_wait(&b_empty[bs], bph ^ 1u);
-        if (elect_one()) {
-          mbar_arrive_expect_tx(&b_full[bs], box_bytes);
-          tma_load_2d(smem_b + bs * kDyBStage, &tmG.m[box - 1], &b_full[bs], 0, t * 128, kEvictFirst);
-        }
-        __syncwarp();
-        if (++bs == kDyBStages) { bs = 0; bph ^= 1u; }
-        for (int m = 0; m < a.num_mt; ++m) {
-          const bool two = 2 * m + 1 < a.nk;
-          mbar_wait(&a_empty[stage], phase ^ 1u);
+      for (int m = 0; m < a.num_mt; ++m) {
+        const bool two = 2 * m + 1 < a.nk;
+        for (int t = t0; t < t1; ++t) {
+          const int e0 = __ldg(a.tile_e0 + t);
+          const int box = (__ldg(a.tile_cnt + t) + 15) >> 4;       // 16-row units, 1..8
+          const uint32_t box_bytes = static_cast<uint32_t>(box) * 16u * 128u;
+          mbar_wait(&empty[stage], phase ^ 1u);
           if (elect_one()) {
-            mbar_arrive_expect_tx(&a_full[stage], two ? 2u * box_bytes : box_bytes);
-            uint8_t* st = smem_a + stage * kDyAStage;
-            tma_load_2d(st, &tmH.m[box - 1], &a_full[stage], 0, (2 * m) * a.e_pad + e0, kEvictFirst);
-            if (two) tma_load_2d(st + 16384, &tmH.m[box - 1], &a_full[stage], 0, (2 * m + 1) * a.e_pad + e0, kEvictFirst);
+            uint8_t* st = smem + stage * kDyStage;
+            mbar_arrive_expect_tx(&full[stage], (two ? 3u : 2u) * box_bytes);
+            tma_load_2d(st, &tmH.m[box - 1], &full[stage], 0, (2 * m) * a.e_pad + e0, kEvictFirst);
+            if (two) tma_load_2d(st + 16384, &tmH.m[box - 1], &full[stage], 0, (2 * m + 1) * a.e_pad + e0, kEvictFirst);
+            tma_load_2d(st + 32768, &tmG.m[box - 1], &full[stage], 0, t * 128, kEvictFirst);
           }
           __syncwarp();
-          if (++stage == kDyAStages) { stage = 0; phase ^= 1u; }
+          if (++stage == kDyStages) { stage = 0; phase ^= 1u; }
         }
       }
-    }
-  } else if (warp == 1) {
-    constexpr uint32_t idesc = idesc_f16(FMT, 128, 64) | (1u << 15) | (1u << 16);
-    int stage = 0, bs = 0;
-    uint32_t phase = 0, bph = 0;
-    int it = 0;
-    for (int c = a.c0 + blockIdx.x; c < a.c1; c += gridDim.x, ++it) {
-      const int buf = a.nbuf == 2 ? (it & 1) : 0;
-      const int use = a.nbuf == 2 ? (it >> 1) : it;
-      mbar_wait(&tempty[buf], (use & 1) ^ 1u);
-      fence_after_sync();
-      const int t0 = __ldg(a.tile_ptr + c), t1 = __ldg(a.tile_ptr + c + 1);
-      for (int t = t0; t < t1; ++t) {
-        const int ksteps = (__ldg(a.tile_cnt + t) + 15) >> 4;
-        mbar_wait(&b_full[bs], bph);
-        const uint64_t bdesc = desc_mn_sw128(smem_u32(smem_b + bs * kDyBStage), 16384);
-        for (int m = 0; m < a.num_mt; ++m) {
-          mbar_wait(&a_full[stage], phase);
-          fence_after_sync();
-          const uint64_t adesc = desc_mn_sw128(smem_u32(smem_a + stage * kDyAStage), 16384);
-          const uint32_t d = tmem_base + buf * acc_cols + m * 64;
-          if (elect_one()) {
-            for (int k = 0; k < ksteps; ++k) umma_f16(d, adesc + 128 * k, bdesc + 128 * k, idesc, (t != t0 || k != 0));
-            umma_commit(&a_empty[stage]);
-            if (m == a.num_mt - 1) umma_commit(&b_empty[bs]);
-          }
-          __syncwarp();
-          if (++stage == kDyAStages) { stage = 0; phase ^= 1u; }
-        }
-        if (++bs == kDyBStages) { bs = 0; bph ^= 1u; }
-      }
-      if (elect_one()) umma_commit(&tfull[buf]);
-      __syncwarp();
     }
   } else {
-    const int quarter = warp % 4;
-    int it = 0;
-    for (int c = a.c0 + blockIdx.x; c < a.c1; c += gridDim.x, ++it) {
-      const int buf = a.nbuf == 2 ? (it & 1) : 0;
-      const int use = a.nbuf == 2 ? (it >> 1) : it;
-      mbar_wait(&tfull[buf], use & 1);
-      fence_after_sync();
+    const int quarter = warp;
+    float* wb = scratch + warp * (acc_scratch_bytes<32>() / 4);
+    Acc<64> acc;
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int c = a.c0 + blockIdx.x; c < a.c1; c += gridDim.x) {
+      const int t0 = __ldg(a.tile_ptr + c), t1 = __ldg(a.tile_ptr + c + 1);
       uint16_t* yrow = a.dY + static_cast<int64_t>(c - a.c0) * a.Kp * 64;
       for (int m = 0; m < a.num_mt; ++m) {
-        const int k = m * 128 + quarter * 32 + lane;
-        const uint32_t tb = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + buf * acc_cols + m * 64;
+        for (int t = t0; t < t1; ++t) {
+          const int ksteps = (__ldg(a.tile_cnt + t) + 15) >> 4;
+          mbar_wait(&full[stage], phase);
+          const uint32_t st = smem_u32(smem + stage * kDyStage);
+          // second m64 half = the second h box (+16 KB); 16 edges = two 8-row groups of 1024 B (+128 units)
+          mma_block<64, FMT, 1, 1>(acc, smem_desc_mn_sw128(st, 16384), smem_desc_mn_sw128(st + 32768, 16384), 16384 >> 4,
+                                   128, ksteps, t != t0);
+          wgmma_wait<0>();
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&empty[stage]);
+          if (++stage == kDyStages) { stage = 0; phase ^= 1u; }
+        }
+        const int k = m * 128 + acc_row(quarter, lane);
 #pragma unroll
         for (int cc = 0; cc < 64; cc += 32) {
           uint32_t v[32];
-          tmem_ld32(tb + cc, v);
-          tmem_ld_wait();
+          acc_rows<64, 32>(acc, cc, wb, v);
           if (k < a.Kp) {
             uint32_t pk[16];
 #pragma unroll
             for (int j = 0; j < 16; ++j) pk[j] = pack2<FMT>(__uint_as_float(v[2 * j]), __uint_as_float(v[2 * j + 1]));
             uint16_t* dst = yrow + static_cast<int64_t>(k) * 64 + cc;
-            st_global_v8(dst, pk);
-            st_global_v8(dst + 16, pk + 8);
+            st_global_32b(dst, pk);
+            st_global_32b(dst + 16, pk + 8);
           }
         }
       }
-      fence_before_sync();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty[buf]);
     }
-  }
-  fence_before_sync();
-  __syncthreads();
-  if (warp == 1) {
-    fence_after_sync();
-    tmem_dealloc(tmem_base, 512);
   }
 }
 
 // =====================================================================================================
 // k_dh: dz[e, k] = [h_e[k] > 0] * sum_{t<T} sum_o Ghat[e, t*64 + o] * Yt[(t, c(e), k), o]     for the tiles of a batch
-//   UMMA M = 128 edges (A = Ghat tile, K-major, resident for the tile: T chunks of 64),
-//        N = BN k's  (B = rows (t, c, k) of the per-application Y^T matrices, K-major [BN x 64] boxes),
-//        K = T * 64.  Two accumulators of BN columns alternate so the epilogue of one k block overlaps the
-//   MMAs of the next.  Epilogue: TMEM -> ReLU mask from the chunk-major h -> 16-bit -> dz[e - e_base, k].
+//   wgmma M = 128 edges (A = Ghat tile, K-major, resident for the tile: T chunks of 64),
+//         N = BN k's  (B = rows (t, c, k) of the per-application Y^T matrices, K-major [BN x 64] boxes),
+//         K = T * 64; the accumulator lives in the registers of the consumer warpgroup (warps 0..3, warp 4 = TMA
+//   producer), which runs the epilogue: ReLU mask from the chunk-major h -> 16-bit -> dz[e - e_base, k].
 // =====================================================================================================
 constexpr int kDhAChunk = 16 * 1024;
 constexpr int kDhBStages = 3;
@@ -509,7 +443,7 @@ struct DhArgs {
   int c0, Sb;               // batch of sources [c0, c0 + Sb)
   int e_base;               // first sorted edge of the batch
   int e_pad;
-  int T, Kp, BN, n_nb;      // n_nb = Kp / BN
+  int T, Kp, n_nb;          // n_nb = Kp / BN
   const uint16_t* h;        // chunk-major edge features (the ReLU mask)
   uint16_t* dz;             // [batch edges, Kp] row-major
   // optional fused bias gradient: colsum[k * colsum_stride] += sum over the batch's edges of dz[e, k] (fp32, unscaled by
@@ -519,12 +453,14 @@ struct DhArgs {
   int colsum_stride;
 };
 
-template <int FMT>
-__global__ void __launch_bounds__(192, 1)
+constexpr int kDhScratch = 4 * acc_scratch_bytes<32>();
+
+template <int FMT, int BN>
+__global__ void __launch_bounds__(160, 1)
 k_dh(const __grid_constant__ Maps8 tmA, const __grid_constant__ CUtensorMap tmB, DhArgs a) {
   extern __shared__ __align__(1024) uint8_t smem[];
   if ((smem_u32(smem) & 1023u) != 0) __trap();
-  const int b_stage_bytes = a.BN * 128;
+  const int b_stage_bytes = BN * 128;
   uint8_t* smem_a = smem;                                   // [kMaxApps? T] chunks of 16 KB
   uint8_t* smem_b = smem + a.T * kDhAChunk;
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem_b + kDhBStages * b_stage_bytes);
@@ -532,31 +468,21 @@ k_dh(const __grid_constant__ Maps8 tmA, const __grid_constant__ CUtensorMap tmB,
   uint64_t* a_empty = a_full + kMaxApps;
   uint64_t* b_full = a_empty + kMaxApps;
   uint64_t* b_empty = b_full + kDhBStages;
-  uint64_t* tfull = b_empty + kDhBStages;
-  uint64_t* tempty = tfull + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
-  float* s_tr = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(bars) + 1024);     // [4][32][33]  (colsum only)
+  float* scratch = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(bars) + 1024);  // [4] accumulator transposes
+  float* s_tr = scratch + kDhScratch / 4;                                               // [4][32][33]  (colsum only)
   float* s_cs = s_tr + 4 * 32 * 33;                                                     // [4][Kp]
   const int warp = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x / 32), 0), lane = threadIdx.x % 32;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == 4 && lane == 0) {
     for (int i = 0; i < 8; ++i) prefetch_tmap(&tmA.m[i]);
     prefetch_tmap(&tmB);
-    for (int s = 0; s < kMaxApps; ++s) { mbar_init(&a_full[s], 1); mbar_init(&a_empty[s], 1); }
-    for (int s = 0; s < kDhBStages; ++s) { mbar_init(&b_full[s], 1); mbar_init(&b_empty[s], 1); }
-    for (int s = 0; s < 2; ++s) { mbar_init(&tfull[s], 1); mbar_init(&tempty[s], 4); }
+    for (int s = 0; s < kMaxApps; ++s) { mbar_init(&a_full[s], 1); mbar_init(&a_empty[s], 4); }
+    for (int s = 0; s < kDhBStages; ++s) { mbar_init(&b_full[s], 1); mbar_init(&b_empty[s], 4); }
     fence_barrier_init();
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, 512);
-    tmem_relinquish();
-  }
-  fence_before_sync();
   __syncthreads();
-  fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp == 4) {
     int bs = 0;
     uint32_t bph = 0, aph = 0;
     for (int t = a.tile0 + blockIdx.x; t < a.tile1; t += gridDim.x, aph ^= 1u) {
@@ -576,35 +502,7 @@ k_dh(const __grid_constant__ Maps8 tmA, const __grid_constant__ CUtensorMap tmB,
           mbar_wait(&b_empty[bs], bph ^ 1u);
           if (elect_one()) {
             mbar_arrive_expect_tx(&b_full[bs], static_cast<uint32_t>(b_stage_bytes));
-            tma_load_2d(smem_b + bs * b_stage_bytes, &tmB, &b_full[bs], 0, (j * a.Sb + cl) * a.Kp + nb * a.BN, kEvictLast);
-          }
-          __syncwarp();
-          if (++bs == kDhBStages) { bs = 0; bph ^= 1u; }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    const uint32_t idesc = idesc_f16(FMT, 128, static_cast<uint32_t>(a.BN));
-    int bs = 0;
-    uint32_t bph = 0, aph = 0;
-    int it = 0;                                              // accumulator uses
-    for (int t = a.tile0 + blockIdx.x; t < a.tile1; t += gridDim.x, aph ^= 1u) {
-      for (int nb = 0; nb < a.n_nb; ++nb, ++it) {
-        const int as = it & 1;
-        mbar_wait(&tempty[as], ((it >> 1) & 1) ^ 1u);
-        fence_after_sync();
-        for (int j = 0; j < a.T; ++j) {
-          if (nb == 0) mbar_wait(&a_full[j], aph);
-          mbar_wait(&b_full[bs], bph);
-          fence_after_sync();
-          const uint64_t adesc = smem_desc_sw128(smem_u32(smem_a + j * kDhAChunk));
-          const uint64_t bdesc = smem_desc_sw128(smem_u32(smem_b + bs * b_stage_bytes));
-          if (elect_one()) {
-#pragma unroll
-            for (int k = 0; k < 4; ++k) umma_f16(tmem_base + as * 256, adesc + 2 * k, bdesc + 2 * k, idesc, (j | k) != 0);
-            umma_commit(&b_empty[bs]);
-            if (nb == a.n_nb - 1) umma_commit(&a_empty[j]);
-            if (j == a.T - 1) umma_commit(&tfull[as]);
+            tma_load_2d(smem_b + bs * b_stage_bytes, &tmB, &b_full[bs], 0, (j * a.Sb + cl) * a.Kp + nb * BN, kEvictLast);
           }
           __syncwarp();
           if (++bs == kDhBStages) { bs = 0; bph ^= 1u; }
@@ -618,21 +516,33 @@ k_dh(const __grid_constant__ Maps8 tmA, const __grid_constant__ CUtensorMap tmB,
     if (a.colsum != nullptr)
       for (int k = lane; k < a.Kp; k += 32) my_cs[k] = 0.f;
     __syncwarp();
-    int it = 0;
-    for (int t = a.tile0 + blockIdx.x; t < a.tile1; t += gridDim.x) {
+    float* wb = scratch + quarter * (acc_scratch_bytes<32>() / 4);
+    Acc<BN> acc;
+    int bs = 0;
+    uint32_t bph = 0, aph = 0;
+    for (int t = a.tile0 + blockIdx.x; t < a.tile1; t += gridDim.x, aph ^= 1u) {
       const int e0 = __ldg(a.tile_e0 + t), cnt = __ldg(a.tile_cnt + t);
-      const int r = quarter * 32 + lane;
+      const int r = acc_row(quarter, lane);
       const bool ok = r < cnt;
-      for (int nb = 0; nb < a.n_nb; ++nb, ++it) {
-        const int as = it & 1;
-        mbar_wait(&tfull[as], (it >> 1) & 1);
-        fence_after_sync();
-        const uint32_t tb = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + as * 256;
-        for (int cc = 0; cc < a.BN; cc += 32) {
+      for (int nb = 0; nb < a.n_nb; ++nb) {
+        for (int j = 0; j < a.T; ++j) {
+          if (nb == 0) mbar_wait(&a_full[j], aph);
+          mbar_wait(&b_full[bs], bph);
+          mma_block<BN, FMT>(acc, smem_desc_sw128(smem_u32(smem_a + j * kDhAChunk)),
+                             smem_desc_sw128(smem_u32(smem_b + bs * b_stage_bytes)), 512, 2, 4, j != 0);
+          wgmma_wait<0>();
+          __syncwarp();
+          if (lane == 0) {
+            mbar_arrive(&b_empty[bs]);
+            if (nb == a.n_nb - 1) mbar_arrive(&a_empty[j]);
+          }
+          if (++bs == kDhBStages) { bs = 0; bph ^= 1u; }
+        }
+#pragma unroll
+        for (int cc = 0; cc < BN; cc += 32) {
           uint32_t v[32];
-          tmem_ld32(tb + cc, v);
-          tmem_ld_wait();
-          const int k0 = nb * a.BN + cc;
+          acc_rows<BN, 32>(acc, cc, wb, v);
+          const int k0 = nb * BN + cc;
           if (ok) {
             const uint16_t* hp = a.h + (static_cast<int64_t>(k0 >> 6) * a.e_pad + e0 + r) * 64 + (k0 & 63);
             uint32_t pk[16];
@@ -650,8 +560,8 @@ k_dh(const __grid_constant__ Maps8 tmA, const __grid_constant__ CUtensorMap tmB,
               }
             }
             uint16_t* dst = a.dz + static_cast<int64_t>(e0 - a.e_base + r) * a.Kp + k0;
-            st_global_v8(dst, pk);
-            st_global_v8(dst + 16, pk + 8);
+            st_global_32b(dst, pk);
+            st_global_32b(dst + 16, pk + 8);
           }
           if (a.colsum != nullptr) {          // column sums of this warp's [32 rows x 32 columns] piece
 #pragma unroll
@@ -664,9 +574,6 @@ k_dh(const __grid_constant__ Maps8 tmA, const __grid_constant__ CUtensorMap tmB,
             __syncwarp();
           }
         }
-        fence_before_sync();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&tempty[as]);
       }
     }
     if (a.colsum != nullptr) {
@@ -676,12 +583,6 @@ k_dh(const __grid_constant__ Maps8 tmA, const __grid_constant__ CUtensorMap tmB,
         if (v != 0.f) atomicAdd(a.colsum + static_cast<int64_t>(k) * a.colsum_stride, v);
       }
     }
-  }
-  fence_before_sync();
-  __syncthreads();
-  if (warp == 1) {
-    fence_after_sync();
-    tmem_dealloc(tmem_base, 512);
   }
 }
 
@@ -694,7 +595,6 @@ bool backward_tc_supported(const Weights* W) {
   if (W->prec != PREC_F16 && W->prec != PREC_BF16) return false;
   if (W->cout != 64 || W->cin > 64 || W->n_layers < 2 || W->W1aug == nullptr) return false;
   if (W->W3q == nullptr || W->W3t == nullptr) return false;
-  if ((W->Kp + 127) / 128 * 64 > 512) return false;                  // k_dy accumulators
   for (int l = 2; l <= W->n_layers - 1; ++l)
     if (W->WhT[l] == nullptr) return false;
   return true;
@@ -827,11 +727,10 @@ int backward_apply_tc(const Plan* P, const Weights* W, const void* h, const floa
     a.tile_ptr = P->tile_ptr; a.tile_e0 = P->tile_e0; a.tile_cnt = P->tile_cnt;
     a.c0 = static_cast<int>(c0); a.c1 = static_cast<int>(c0) + nb;
     a.e_pad = static_cast<int>(e_pad); a.nk = Kp / 64; a.num_mt = (a.nk + 1) / 2;
-    a.nbuf = a.num_mt * 64 * 2 <= 512 ? 2 : 1;
     a.Kp = Kp; a.dY = dY;
     const int grid = nb < tc_num_sms() ? nb : tc_num_sms();
-    if (bf) k_dy<1><<<grid, 192, kDySmem, st>>>(tmH, tmG, a);
-    else k_dy<0><<<grid, 192, kDySmem, st>>>(tmH, tmG, a);
+    if (bf) k_dy<1><<<grid, 160, kDySmem, st>>>(tmH, tmG, a);
+    else k_dy<0><<<grid, 160, kDySmem, st>>>(tmH, tmG, a);
     NNC_CHECK_LAUNCH();
     // dxp[c, i] = sum_n dY[c, n] W3t[i, n]      (fp32 out)
     s = launch_gemm_tc(W->prec, dY, nb, 0, nb, NY, W->W3t, cin_p, nullptr, 0, dxp, cin_p, st, nullptr, 0, 0, 0, nullptr,
@@ -947,16 +846,18 @@ int backward_mlp_tc(const Plan* P, const Weights* W, const float* edge_attr, con
   const int* htp = P->h_tile_ptr;
   const size_t avail = ws_bytes - L.fixed - (1 << 16);
   const int64_t e_pad = round_up64(P->E, 128);
-  const int BN = Kp % 256 == 0 ? 256 : Kp % 128 == 0 ? 128 : 64;   // k block of k_dh (Kp is a multiple of 64)
+  const int BN = Kp % 128 == 0 ? 128 : 64;   // k block of k_dh (Kp is a multiple of 64; <= 128 accumulator registers)
   int maxkp = 0;
   for (int l = 1; l <= nl - 1; ++l) maxkp = W->kp[l] > maxkp ? W->kp[l] : maxkp;
   static bool attr_set = false;
   if (!attr_set) {
-    NNC_CHECK_CUDA(cudaFuncSetAttribute(k_dh<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    NNC_CHECK_CUDA(cudaFuncSetAttribute(k_dh<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    NNC_CHECK_CUDA(cudaFuncSetAttribute(k_dh<0, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    NNC_CHECK_CUDA(cudaFuncSetAttribute(k_dh<1, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    NNC_CHECK_CUDA(cudaFuncSetAttribute(k_dh<0, 128>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    NNC_CHECK_CUDA(cudaFuncSetAttribute(k_dh<1, 128>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     attr_set = true;
   }
-  int dh_smem = T * kDhAChunk + kDhBStages * BN * 128 + 1024;
+  int dh_smem = T * kDhAChunk + kDhBStages * BN * 128 + 1024 + kDhScratch;
   NNC_REQUIRE(dh_smem <= 227 * 1024, NNCONV_ERR_UNSUPPORTED, "backward_mlp: T=%d applications do not fit shared memory", T);
   // bias gradient of the top hidden layer fused into k_dh (one pass over dz_{L-1} saved) when the transpose + column
   // accumulators fit next to the operand stages; layer 1 (nl == 2) needs the full dz^T A1 product anyway
@@ -1020,14 +921,19 @@ int backward_mlp_tc(const Plan* P, const Weights* W, const float* edge_attr, con
       DhArgs a;
       a.tile_c = P->tile_c; a.tile_e0 = P->tile_e0; a.tile_cnt = P->tile_cnt;
       a.tile0 = htp[c0]; a.tile1 = htp[c1]; a.c0 = c0; a.Sb = nb; a.e_base = e_base; a.e_pad = static_cast<int>(e_pad);
-      a.T = T; a.Kp = Kp; a.BN = BN; a.n_nb = Kp / BN;
+      a.T = T; a.Kp = Kp; a.n_nb = Kp / BN;
       a.h = static_cast<const uint16_t*>(h); a.dz = dzA;
       a.colsum = fuse_colsum ? reinterpret_cast<float*>(base + L.off_D[nl - 1]) + 3 * k_in : nullptr;
       a.colsum_stride = 64;
       const int tiles = a.tile1 - a.tile0;
       const int grid = tiles < tc_num_sms() ? tiles : tc_num_sms();
-      if (bf) k_dh<1><<<grid, 192, dh_smem, st>>>(tmA, tmB, a);
-      else k_dh<0><<<grid, 192, dh_smem, st>>>(tmA, tmB, a);
+      if (BN == 128) {
+        if (bf) k_dh<1, 128><<<grid, 160, dh_smem, st>>>(tmA, tmB, a);
+        else k_dh<0, 128><<<grid, 160, dh_smem, st>>>(tmA, tmB, a);
+      } else {
+        if (bf) k_dh<1, 64><<<grid, 160, dh_smem, st>>>(tmA, tmB, a);
+        else k_dh<0, 64><<<grid, 160, dh_smem, st>>>(tmA, tmB, a);
+      }
       NNC_CHECK_LAUNCH();
     }
     // ---- recompute the hidden activations h_1 .. h_{L-2} of the batch (16-bit, row-major) and A1

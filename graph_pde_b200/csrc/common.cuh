@@ -51,7 +51,7 @@ struct Carver {
   bool ok() const { return off <= cap; }
 };
 
-constexpr int kTileEdges = 128;
+constexpr int kTileEdges = 128;   // edges per contraction tile (two m64 wgmma halves)
 
 // Optional per-kernel-class timing with CUDA events (bench.py roofline numbers); off by default.
 enum ProfKind : int { PK_LAYER1 = 0, PK_HIDDEN_GEMM = 1, PK_NODE_PREP = 2, PK_Y_GEMM = 3, PK_CONV = 4, PK_APPLY_FUSED = 5, PK_COUNT = 6 };
@@ -63,6 +63,6 @@ struct ProfScope {
   bool on;
   ProfScope(int k, cudaStream_t s) : kind(k), st(s), on(prof_enabled()) { if (on) prof_mark(kind, st, true); }
   ~ProfScope() { if (on) prof_mark(kind, st, false); }
-};   // edges per contraction tile (= UMMA M)
+};
 
 }  // namespace nnc

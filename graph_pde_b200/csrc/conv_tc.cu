@@ -10,8 +10,9 @@
 // its edges form a dense GEMM  M[cnt, out] = H[cnt, Kp] * Y_src[out, Kp]^T  with the SAME B operand.
 //
 // Work decomposition
-//   tile  = <= 128 consecutive edges of one source (UMMA M = 128)
-//   unit  = <= kTU consecutive tiles of one source; a unit keeps one TMEM accumulator per tile
+//   tile  = <= 128 consecutive edges of one source (one warpgroup, two m64 wgmma halves)
+//   unit  = <= kTU consecutive tiles of one source; tile ti of a unit is accumulated (in registers) and scattered
+//           by consumer warpgroup ti
 //   pass  = a slice of nb_slots K-chunks (64 columns each) of Y_src that is resident in shared memory.
 //           For Kp = 1024, out = 64 the whole Y_src (128 KB) would leave room for only one CTA per SM;
 //           splitting K in two passes (64 KB resident) lets TWO CTAs share an SM, so that consecutive
@@ -23,10 +24,11 @@
 //     rounded up to 16 -- this stream is the kernel's HBM roofline (Kp * 2 bytes per edge-application);
 //   * B slots: TMA from the L2-resident per-batch Y buffer, one full/empty mbarrier pair per slot, so the
 //     next pass / next source is fetched slot by slot as soon as the last tile has consumed it;
-//   * 4 epilogue warps: TMEM -> registers (thread = edge row) -> + c_src, * 1/deg(dst) ->
-//     red.global.add.v4.f32 into out[dst] (fp32, L2 resident).
+//   * epilogue (the tile's warpgroup): registers -> per-warp transpose (thread = edge row) -> + c_src, * 1/deg(dst)
+//     -> red.global.add.v4.f32 into out[dst] (fp32, L2 resident).
 // Persistent: each CTA owns a contiguous range of tiles.
 #include <cstdlib>
+#include <type_traits>
 
 #include "kernels.h"
 #include "options.h"
@@ -43,7 +45,9 @@ using namespace tc05;
 
 constexpr int kMaxSlots = 16;
 constexpr int kMaxAStages = 8;
-constexpr int kTU = 2;                     // tiles per unit (TMEM: 2 stages x kTU x out columns)
+constexpr int kTU = 2;                     // tiles per unit = consumer warpgroups
+constexpr int kThreads = 32 * (4 * kTU + 1);   // consumer warpgroups, then the TMA producer warp
+constexpr int kScratchBytes = 4 * kTU * acc_scratch_bytes<16>();
 constexpr int kATileBytes = 128 * 64 * 2;
 constexpr int kSmemTwoPerSm = 115200;      // dynamic smem per CTA that still lets two CTAs share one SM
 
@@ -58,7 +62,6 @@ struct ConvTcArgs {
   float* out;             // [N, cout]
   int tile_begin, tile_end;
   int c0;                 // compact source index of Y row block 0
-  int cout;
   int nb_slots;           // resident K chunks per pass
   int passes;             // nb_slots * passes == Kp / 64
   int a_stages;
@@ -94,66 +97,53 @@ __device__ __forceinline__ bool next_unit(const ConvTcArgs& a, int t1, int& t, U
   return true;
 }
 
-template <int FMT>
-__global__ void __launch_bounds__(192, 2)
+template <int FMT, int NC>
+__global__ void __launch_bounds__(kThreads, NC <= 64 ? 2 : 1)
 k_conv_tc(const __grid_constant__ HMaps tmH, const __grid_constant__ CUtensorMap tmY, ConvTcArgs a) {
   extern __shared__ __align__(1024) uint8_t smem[];
   if ((smem_u32(smem) & 1023u) != 0) __trap();            // SWIZZLE_128B tiles need 1024 B alignment
-  const int b_chunk_bytes = a.cout * 128;                 // [cout rows x 64 k] 16-bit
+  const int b_chunk_bytes = NC * 128;                 // [cout rows x 64 k] 16-bit
   const int b_stride = (b_chunk_bytes + 1023) & ~1023;
   uint8_t* smem_b = smem;
   uint8_t* smem_a = smem + a.nb_slots * b_stride;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem_a + a.a_stages * kATileBytes);
+  float* scratch = reinterpret_cast<float*>(smem_a + a.a_stages * kATileBytes);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem_a + a.a_stages * kATileBytes + kScratchBytes);
   uint64_t* a_full = bars;
   uint64_t* a_empty = bars + kMaxAStages;
   uint64_t* b_full = bars + 2 * kMaxAStages;
   uint64_t* b_empty = b_full + kMaxSlots;
-  uint64_t* tfull = b_empty + kMaxSlots;
-  uint64_t* tempty = tfull + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
 
-  const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
+  // shfl: warp-uniform role index (wgmma under a branch the compiler cannot prove uniform is serialised)
+  const int warp = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x / 32), 0), lane = threadIdx.x % 32;
   const int total = a.tile_end - a.tile_begin;
   const int t0 = a.tile_begin + static_cast<int>((static_cast<int64_t>(total) * blockIdx.x) / gridDim.x);
   const int t1 = a.tile_begin + static_cast<int>((static_cast<int64_t>(total) * (blockIdx.x + 1)) / gridDim.x);
-  const int acc_cols = 2 * kTU * a.cout;
-  const uint32_t tmem_cols = acc_cols <= 32 ? 32 : acc_cols <= 64 ? 64 : acc_cols <= 128 ? 128 : acc_cols <= 256 ? 256 : 512;
+  constexpr int kProducer = 4 * kTU;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == kProducer && lane == 0) {
     for (int i = 0; i < 8; ++i) prefetch_tmap(&tmH.m[i]);
     prefetch_tmap(&tmY);
     for (int s = 0; s < a.a_stages; ++s) {
       mbar_init(&a_full[s], 1);
-      mbar_init(&a_empty[s], 1);
+      mbar_init(&a_empty[s], 4);                // the 4 warps of the tile's warpgroup
     }
     for (int j = 0; j < a.nb_slots; ++j) {
       mbar_init(&b_full[j], 1);
-      mbar_init(&b_empty[j], 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&tfull[s], 1);
-      mbar_init(&tempty[s], 4);
+      mbar_init(&b_empty[j], 4 * kTU);          // every consumer warp
     }
     fence_barrier_init();
-  }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, tmem_cols);
-    tmem_relinquish();
   }
   const unsigned long long tr0 = a.trace.rec ? gtime() : 0ull;
   pdl_launch_dependents();
   if (a.wait_ok != nullptr && threadIdx.x == 0) flag_wait(a.wait_ok);
   const unsigned long long tr1 = a.trace.rec ? gtime() : 0ull;
-  fence_before_sync();
   __syncthreads();
-  fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp == kProducer) {
     if (lane == 0) {
       // ------------------------------------------------------------ TMA producer
-      int stage = 0;
-      uint32_t phase = 0;
+      ARing ring[kTU];
+      for (int ti = 0; ti < kTU; ++ti) ring[ti].init(ti, a.a_stages);
       int prev_c = -1;
       uint32_t ld = 0;                              // B load events so far
       int t = t0;
@@ -171,124 +161,99 @@ k_conv_tc(const __grid_constant__ HMaps tmH, const __grid_constant__ CUtensorMap
               if (need && ti == 0) {
                 mbar_wait(&b_empty[s], (ld & 1u) ^ 1u);
                 mbar_arrive_expect_tx(&b_full[s], b_chunk_bytes);
-                tma_load_2d(smem_b + s * b_stride, &tmY, &b_full[s], j * 64, (un.c - a.c0) * a.cout, kEvictLast);
+                tma_load_2d(smem_b + s * b_stride, &tmY, &b_full[s], j * 64, (un.c - a.c0) * NC, kEvictLast);
               }
-              mbar_wait(&a_empty[stage], phase ^ 1u);
+              const int stage = ring[ti].stage;
+              mbar_wait(&a_empty[stage], ring[ti].phase ^ 1u);
               mbar_arrive_expect_tx(&a_full[stage], a_bytes);
               tma_load_2d(smem_a + stage * kATileBytes, mh, &a_full[stage], 0, j * a.e_pad + e0, kEvictFirst);
-              if (++stage == a.a_stages) { stage = 0; phase ^= 1u; }
+              ring[ti].next();
             }
           }
           if (need) ++ld;
         }
         prev_c = un.c;
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      // ------------------------------------------------------------ MMA issuer
-      const uint32_t idesc = idesc_f16(FMT, 128, static_cast<uint32_t>(a.cout));
-      int stage = 0;
-      uint32_t phase = 0;
-      int prev_c = -1;
-      uint32_t ld = 0;
-      int it = 0;
-      int t = t0;
-      Unit un;
-      while (next_unit(a, t1, t, un)) {
-        const int as = it & 1;
-        mbar_wait(&tempty[as], ((it >> 1) & 1) ^ 1u);
-        fence_after_sync();
-        const bool has_next = t < t1;
-        const bool next_same = has_next && a.tile_c[t] == un.c;
-        for (int p = 0; p < a.passes; ++p) {
-          const bool need = a.passes > 1 || un.c != prev_c;
-          // the resident slots are released (for re-filling) iff the next (unit, pass) loads B again
-          const bool release = (p + 1 < a.passes) || !has_next || a.passes > 1 || !next_same;
-          for (int ti = 0; ti < un.u; ++ti) {
-            const uint32_t d_tmem = tmem_base + (as * kTU + ti) * a.cout;
-            for (int s = 0; s < a.nb_slots; ++s) {
-              if (need && ti == 0) mbar_wait(&b_full[s], ld & 1u);
-              mbar_wait(&a_full[stage], phase);
-              fence_after_sync();
-              const uint64_t adesc = smem_desc_sw128(smem_u32(smem_a + stage * kATileBytes));
-              const uint64_t bdesc = smem_desc_sw128(smem_u32(smem_b + s * b_stride));
-#pragma unroll
-              for (int k = 0; k < 4; ++k) umma_f16(d_tmem, adesc + 2 * k, bdesc + 2 * k, idesc, (p | s | k) != 0);
-              umma_commit(&a_empty[stage]);
-              if (release && ti == un.u - 1) umma_commit(&b_empty[s]);
-              if (++stage == a.a_stages) { stage = 0; phase ^= 1u; }
-            }
-          }
-          if (need) ++ld;
-        }
-        umma_commit(&tfull[as]);
-        prev_c = un.c;
-        ++it;
       }
     }
   } else {
-    // ---------------------------------------------------------------- epilogue warps 2..5
-    const int quarter = warp % 4;
-    int it = 0;
+    // ---------------------------------------------------------------- consumer warpgroup g = tile g of every unit
+    const int g = warp / 4, quarter = warp % 4;
+    float* wb = scratch + warp * (acc_scratch_bytes<16>() / 4);
+    Acc<NC> acc;
+    ARing ring;
+    ring.init(g, a.a_stages);
+    int prev_c = -1;
+    uint32_t ld = 0;
     int t = t0;
     Unit un;
     while (next_unit(a, t1, t, un)) {
-      const int as = it & 1;
-      const int r = quarter * 32 + lane;
-      int d[kTU];
-      float sc[kTU];
-      bool ok[kTU];
-#pragma unroll
-      for (int ti = 0; ti < kTU; ++ti) {
-        ok[ti] = ti < un.u && r < a.tile_cnt[un.t + ti];
-        d[ti] = 0;
-        sc[ti] = 1.f;
-        if (ok[ti]) {
-          d[ti] = __ldg(a.dst_sorted + a.tile_e0[un.t + ti] + r);
-          if (a.inv_deg) sc[ti] = __ldg(a.inv_deg + d[ti]);
-        }
-      }
-      const float* cv = a.cvec + static_cast<int64_t>(un.c) * a.cout;
-      const float xsc = __ldg(a.xs + un.c);
-      mbar_wait(&tfull[as], (it >> 1) & 1);
-      fence_after_sync();
-#pragma unroll
-      for (int ti = 0; ti < kTU; ++ti) {
-        if (ti < un.u) {
-          float* orow = a.out + static_cast<int64_t>(d[ti]) * a.cout;
-#pragma unroll 1
-          for (int cc = 0; cc < a.cout; cc += 16) {
-            uint32_t v[16];
-            tmem_ld16(tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + (as * kTU + ti) * a.cout + cc, v);
-            tmem_ld_wait();
-            if (ok[ti] && !(a.debug & 1)) {
-#pragma unroll
-              for (int q = 0; q < 4; ++q) {
-                const float4 cq = __ldg(reinterpret_cast<const float4*>(cv + cc) + q);
-                red_add_v4(orow + cc + 4 * q, fmaf(__uint_as_float(v[4 * q + 0]), xsc, cq.x) * sc[ti],
-                           fmaf(__uint_as_float(v[4 * q + 1]), xsc, cq.y) * sc[ti],
-                           fmaf(__uint_as_float(v[4 * q + 2]), xsc, cq.z) * sc[ti],
-                           fmaf(__uint_as_float(v[4 * q + 3]), xsc, cq.w) * sc[ti]);
-              }
+      un.u = __shfl_sync(0xffffffffu, un.u, 0);       // warp-uniform (see above)
+      un.c = __shfl_sync(0xffffffffu, un.c, 0);
+      const bool has_next = t < t1;
+      const bool next_same = has_next && a.tile_c[t] == un.c;
+      for (int p = 0; p < a.passes; ++p) {
+        const bool need = a.passes > 1 || un.c != prev_c;
+        if (need) ++ld;
+        // the resident slots are released (for re-filling) iff the next (unit, pass) loads B again
+        const bool release = (p + 1 < a.passes) || !has_next || a.passes > 1 || !next_same;
+        for (int ti = 0; ti < un.u; ++ti) {
+          for (int s = 0; s < a.nb_slots; ++s) {
+            if (ti == g) {
+              mbar_wait(&b_full[s], (ld - 1) & 1u);
+              mbar_wait(&a_full[ring.stage], ring.phase);
+              const uint64_t adesc = smem_desc_sw128(smem_u32(smem_a + ring.stage * kATileBytes));
+              const uint64_t bdesc = smem_desc_sw128(smem_u32(smem_b + s * b_stride));
+              mma_block<NC, FMT>(acc, adesc, bdesc, 512, 2, 4, (p | s) != 0);
+              wgmma_wait<0>();
+              __syncwarp();
+              if (lane == 0) mbar_arrive(&a_empty[ring.stage]);
+              ring.next();
             }
           }
         }
+        if (release) {
+          // every consumer warp releases the slots, after the load it releases has landed (never a phase ahead)
+          for (int s = 0; s < a.nb_slots; ++s) {
+            mbar_wait(&b_full[s], (ld - 1) & 1u);
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&b_empty[s]);
+          }
+        }
       }
-      fence_before_sync();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty[as]);
-      ++it;
+      prev_c = un.c;
+      if (g >= un.u) continue;
+      // ---- epilogue of tile g
+      const int r = acc_row(quarter, lane);
+      const bool ok = r < a.tile_cnt[un.t + g];
+      int d = 0;
+      float sc = 1.f;
+      if (ok) {
+        d = __ldg(a.dst_sorted + a.tile_e0[un.t + g] + r);
+        if (a.inv_deg) sc = __ldg(a.inv_deg + d);
+      }
+      const float* cv = a.cvec + static_cast<int64_t>(un.c) * NC;
+      const float xsc = __ldg(a.xs + un.c);
+      float* orow = a.out + static_cast<int64_t>(d) * NC;
+#pragma unroll
+      for (int cc = 0; cc < NC; cc += 16) {
+        uint32_t v[16];
+        acc_rows<NC, 16>(acc, cc, wb, v);
+        if (ok && !(a.debug & 1)) {
+#pragma unroll
+          for (int q = 0; q < 4; ++q) {
+            const float4 cq = __ldg(reinterpret_cast<const float4*>(cv + cc) + q);
+            red_add_v4(orow + cc + 4 * q, fmaf(__uint_as_float(v[4 * q + 0]), xsc, cq.x) * sc,
+                       fmaf(__uint_as_float(v[4 * q + 1]), xsc, cq.y) * sc,
+                       fmaf(__uint_as_float(v[4 * q + 2]), xsc, cq.z) * sc,
+                       fmaf(__uint_as_float(v[4 * q + 3]), xsc, cq.w) * sc);
+          }
+        }
+      }
     }
   }
-  fence_before_sync();
   if (a.done_cnt != nullptr) signal_done(a.done_cnt, a.done_ok);   // includes __syncthreads
   else __syncthreads();
   if (threadIdx.x == 0) trace_write(a.trace, 200u | (a.trace_seq << 12), tr0, tr1, a.trace.rec ? gtime() : 0ull);
-  if (warp == 1) {
-    fence_after_sync();
-    tmem_dealloc(tmem_base, tmem_cols);
-  }
   if (a.join_ok != nullptr && blockIdx.x == 0 && threadIdx.x == 0) {
     for (int i = 0; i < a.join_n; ++i) flag_wait(a.join_ok + i);
   }
@@ -299,17 +264,16 @@ struct ConvShape {
 };
 
 // Choose the K split: prefer a configuration in which two CTAs fit one SM (smem <= kSmemTwoPerSm and
-// TMEM <= 256 columns) with >= 3 A stages; otherwise one CTA per SM with everything resident.
+// out <= 64, i.e. <= 64 accumulator registers per thread) with >= 3 A stages; otherwise one CTA per SM with
+// everything resident.  out <= 128: a warpgroup holds its [128 x out] fp32 tile in registers.
 bool conv_shape(int cout, int Kp, ConvShape* cs) {
-  if (cout % 16 != 0 || cout < 16 || cout > 256 || Kp % 64 != 0) return false;
+  if (cout % 16 != 0 || cout < 16 || cout > 128 || Kp % 64 != 0) return false;
   const int num_kc = Kp / 64;
   const int b_stride = (cout * 128 + 1023) & ~1023;
-  const int bar_bytes = 512;
-  const int acc_cols = 2 * kTU * cout;
-  if (acc_cols > 512) return false;
+  const int bar_bytes = 512 + kScratchBytes;
   const bool one_per_sm = options().conv_one_per_sm != 0;   // measurement knob
   for (int two = one_per_sm ? 0 : 1; two >= 0; --two) {
-    if (two && acc_cols > 256) continue;
+    if (two && cout > 64) continue;
     const int budget = two ? kSmemTwoPerSm : 227 * 1024;
     for (int passes = 1; passes <= num_kc; ++passes) {
       if (num_kc % passes) continue;
@@ -359,20 +323,14 @@ int launch_conv_tc(int prec, const Plan* P, const void* h, int Kp, const void* Y
   }
   s = make_tmap_2d_16b(&tmY, bf, Y, static_cast<uint64_t>(y_nodes) * cout, static_cast<uint64_t>(Kp), cout);
   if (s != NNCONV_OK) return s;
-  ConvTcArgs a;
+  ConvTcArgs a{};
   a.e_pad = static_cast<int>(e_pad);
   a.tile_c = P->tile_c; a.tile_e0 = P->tile_e0; a.tile_cnt = P->tile_cnt; a.dst_sorted = P->dst_sorted;
   a.inv_deg = aggr_mean ? P->inv_deg : nullptr; a.cvec = cvec; a.xs = xs; a.out = out;
-  a.tile_begin = tile_begin; a.tile_end = tile_end; a.c0 = c0; a.cout = cout;
+  a.tile_begin = tile_begin; a.tile_end = tile_end; a.c0 = c0;
   a.nb_slots = cs.nb_slots; a.passes = cs.passes; a.a_stages = cs.a_stages;
   { const int v = options().conv_stages; if (v >= 2 && v < a.a_stages) a.a_stages = v; }
   a.debug = options().conv_debug;
-  static int attr_set[2] = {0, 0};
-  if (!attr_set[bf]) {
-    if (bf) NNC_CHECK_CUDA(cudaFuncSetAttribute(k_conv_tc<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    else NNC_CHECK_CUDA(cudaFuncSetAttribute(k_conv_tc<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    attr_set[bf] = 1;
-  }
   {
     TraceHandle th = trace_get();
     static unsigned int launch_seq = 0;
@@ -389,7 +347,7 @@ int launch_conv_tc(int prec, const Plan* P, const void* h, int Kp, const void* Y
   const int grid = tiles < max_ctas ? tiles : max_ctas;
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3(grid);
-  cfg.blockDim = dim3(192);
+  cfg.blockDim = dim3(kThreads);
   cfg.dynamicSmemBytes = cs.smem_bytes;
   cfg.stream = st;
   cudaLaunchAttribute attr[1];
@@ -397,9 +355,29 @@ int launch_conv_tc(int prec, const Plan* P, const void* h, int Kp, const void* Y
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = (pf && pf->pdl) ? 1 : 0;
-  if (bf) NNC_CHECK_CUDA(cudaLaunchKernelEx(&cfg, k_conv_tc<1>, tmH, tmY, a));
-  else NNC_CHECK_CUDA(cudaLaunchKernelEx(&cfg, k_conv_tc<0>, tmH, tmY, a));
-  return NNCONV_OK;
+  auto go = [&](auto fmt, auto nc) -> int {
+    constexpr int F = decltype(fmt)::value, C = decltype(nc)::value;
+    static bool attr_set = false;
+    if (!attr_set) {
+      NNC_CHECK_CUDA(cudaFuncSetAttribute(k_conv_tc<F, C>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+      attr_set = true;
+    }
+    NNC_CHECK_CUDA(cudaLaunchKernelEx(&cfg, k_conv_tc<F, C>, tmH, tmY, a));
+    return NNCONV_OK;
+  };
+  auto by_cout = [&](auto fmt) -> int {
+    switch (cout) {
+      case 16: return go(fmt, std::integral_constant<int, 16>());
+      case 32: return go(fmt, std::integral_constant<int, 32>());
+      case 48: return go(fmt, std::integral_constant<int, 48>());
+      case 64: return go(fmt, std::integral_constant<int, 64>());
+      case 80: return go(fmt, std::integral_constant<int, 80>());
+      case 96: return go(fmt, std::integral_constant<int, 96>());
+      case 112: return go(fmt, std::integral_constant<int, 112>());
+      default: return go(fmt, std::integral_constant<int, 128>());
+    }
+  };
+  return bf ? by_cout(std::integral_constant<int, 1>()) : by_cout(std::integral_constant<int, 0>());
 }
 
 }  // namespace nnc

@@ -1,14 +1,14 @@
-// tcgen05 GEMM for the dense stages of the NNConv path (sm_100a only):
-//     C[M, N] (fp16/bf16) = act( A[M, K] * B[N, K]^T + bias )          fp32 accumulation in TMEM
+// wgmma GEMM for the dense stages of the NNConv path (sm_90a):
+//     C[M, N] (fp16/bf16) = act( A[M, K] * B[N, K]^T + bias )          fp32 accumulation in registers
 // used for (a) the hidden layers of the edge MLP (graph-neural-operator/utilities.py:223-227,
 // Linear + ReLU) over a chunk of edges and (b) the per-source matrices
 // Y[c, (o,k)] = sum_i x[c, i] * W_L[i*out + o, k]  (the last Linear reassociated, nn_conv.py:274-275).
 //
-// Structure: persistent CTAs (grid = #SMs), 10 warps: warp 0 = TMA producer (one lane), warp 1 = MMA
-// issuer (one lane) + TMEM allocator, warps 2..9 = epilogue (TMEM -> registers -> bias/ReLU -> 16-bit
-// -> per-warp swizzled smem piece -> TMA store; direct 32-byte stores for pipelined / small launches).  Operands are K-major 128B-swizzled tiles [128 x 64] / [BLOCK_N x 64] staged by TMA in a
-// ring of kStages; accumulators are double buffered in TMEM (2 x BLOCK_N columns) so the epilogue of
-// tile i overlaps the MMAs of tile i+1.
+// Structure: persistent CTAs (grid = #SMs), 9 warps: warps 0..7 = two consumer warpgroups, each owning half of
+// the BLOCK_N columns of the tile (wgmma into registers, then the epilogue: bias/ReLU -> 16-bit -> per-warp
+// swizzled smem piece -> TMA store; direct 32-byte stores for pipelined / small launches), warp 8 = TMA producer.
+// Operands are K-major 128B-swizzled tiles [128 x 64] / [BLOCK_N x 64] staged by TMA in a ring of kStages, so the
+// producer runs ahead into the next tile while the warpgroups run the epilogue of this one.
 #include "kernels.h"
 #include "options.h"
 #include "tc05.cuh"
@@ -37,9 +37,8 @@ struct GemmTcArgs {
   int* done_cnt;
   int* done_ok;
   // 1: every epilogue warp stages its [32 rows x 32 cols] piece in its own double-buffered 2 KB of shared
-  // memory (64-byte swizzle) and lane 0 writes it with TMA (tmC): no global stores on the LSU data pipe, which
-  // ncu r1f showed at 85% in the K = 64 first-layer GEMM (TMEM loads + stores touching 32 lines per instruction),
-  // no block-level barrier, and the store of piece i drains while piece i+1 is converted.
+  // memory (64-byte swizzle) and one lane writes it with TMA (tmC, two [16 x 32] panels): no global stores on the
+  // LSU data pipe, no block-level barrier, and the store of piece i drains while piece i+1 is converted.
   int tma_store;
   int bias_v4;         // bias is 16-byte aligned: float4 loads
   // PREC_F16X2 (see plan.h): a_split_nk = K/3/64 > 0 -> A holds [hi | lo] (2K/3 columns) and K block kb reads
@@ -62,7 +61,7 @@ struct GemmTcArgs {
   unsigned int trace_seq;
 };
 
-// SMALL = 1: a 3-stage, BLOCK_N = 128 footprint (97 KB smem, 256 TMEM columns) that can share an SM with a
+// SMALL = 1: a 2-stage, BLOCK_N = 128 footprint (~101 KB smem) that can share an SM with a
 // contraction CTA or a second GEMM CTA -- used for the per-source Y GEMM, which is store bound and runs
 // concurrently with the contraction of the previous batch.
 template <int BLOCK_N, int SMALL = 0>
@@ -72,22 +71,23 @@ struct GemmCfg {
   static constexpr int kABytes = kBlockM * kBlockK * 2;
   static constexpr int kBBytes = BLOCK_N * kBlockK * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr int kStages = SMALL ? 3 : ((196608 / kStageBytes) > 8 ? 8 : (196608 / kStageBytes));
-  static constexpr int kTmemCols = 2 * BLOCK_N;   // power of two >= 32 for BLOCK_N in {64,128,256}
+  static constexpr int kStages = SMALL ? 2 : ((155648 / kStageBytes) > 8 ? 8 : (155648 / kStageBytes));
   // output staging for the TMA-store epilogue: 8 warps x 2 buffers x [32 x 32] 16-bit pieces
   static constexpr int kStoreBytes = SMALL ? 0 : 8 * 2 * 2048;
-  static constexpr int kSmemBytes = kStages * kStageBytes + kStoreBytes + 1024 /*align slack*/ + 256 /*barriers*/;
+  static constexpr int kScratchBytes = 8 * acc_scratch_bytes<32>();   // per-warp accumulator transposes
+  static constexpr int kSmemBytes =
+      kStages * kStageBytes + kStoreBytes + kScratchBytes + 1024 /*align slack*/ + 256 /*barriers*/;
 };
 
 // EPI selects the epilogue at COMPILE time (runtime flags inside the 32-column inner loop cut it into dozens of
-// tiny basic blocks and the K = 64 first-layer GEMM, which is epilogue bound, ran 2.4x slower: run r2b):
+// tiny basic blocks, and the K = 64 first-layer GEMM is epilogue bound):
 //   EPI_PLAIN bias / ReLU / 16-bit store     EPI_SPLIT the same, written as (hi, lo) fp16 pairs (PREC_F16X2)
 //   EPI_MASK  ReLU-derivative mask from a stored activation (backward)     EPI_F32 fp32 output, plain stores
 //   EPI_NOCHECK = EPI_PLAIN without the fp16 range tracking (bf16 outputs, option overflow_check = 0, test hooks)
 enum { EPI_PLAIN = 0, EPI_SPLIT = 1, EPI_MASK = 2, EPI_F32 = 3, EPI_NOCHECK = 4 };
 
 template <int BLOCK_N, int FMT, int SMALL, int EPI>
-__global__ void __launch_bounds__(320, SMALL ? 2 : 1)
+__global__ void __launch_bounds__(288, SMALL ? 2 : 1)
 k_gemm_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
           const __grid_constant__ CUtensorMap tmC, GemmTcArgs a) {
   using Cfg = GemmCfg<BLOCK_N, SMALL>;
@@ -97,12 +97,10 @@ k_gemm_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
   uint8_t* smem_a = smem;
   uint8_t* smem_b = smem + Cfg::kStages * Cfg::kABytes;
   uint8_t* smem_c = smem + Cfg::kStages * Cfg::kStageBytes;     // 1024-aligned (stage sizes are multiples of 8 KB)
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem_c + Cfg::kStoreBytes);
+  float* scratch = reinterpret_cast<float*>(smem_c + Cfg::kStoreBytes);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem_c + Cfg::kStoreBytes + Cfg::kScratchBytes);
   uint64_t* full = bars;
   uint64_t* empty = bars + Cfg::kStages;
-  uint64_t* tfull = bars + 2 * Cfg::kStages;
-  uint64_t* tempty = tfull + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
 
   // shfl: the warp index is warp-uniform for the compiler (role branches converge, operands stay in uniform registers)
   const int warp = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x / 32), 0), lane = threadIdx.x % 32;
@@ -111,34 +109,23 @@ k_gemm_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
   const int num_tiles = m_blocks * n_blocks;
   const int num_kb = a.K / Cfg::kBlockK;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == 8 && lane == 0) {
     prefetch_tmap(&tmA);
     prefetch_tmap(&tmB);
     if (a.tma_store) prefetch_tmap(&tmC);
     for (int s = 0; s < Cfg::kStages; ++s) {
       mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&tfull[s], 1);
-      mbar_init(&tempty[s], 8);   // one arrive per epilogue warp
+      mbar_init(&empty[s], 8);   // one arrive per consumer warp
     }
     fence_barrier_init();
-  }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, Cfg::kTmemCols);
-    tmem_relinquish();
   }
   const unsigned long long tr0 = a.trace.rec ? gtime() : 0ull;
   pdl_launch_dependents();
   if (a.wait_ok != nullptr && threadIdx.x == 0) flag_wait(a.wait_ok);
   const unsigned long long tr1 = a.trace.rec ? gtime() : 0ull;
-  fence_before_sync();
   __syncthreads();
-  fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp == 8) {
     // -------------------------------------------------------------- TMA producer (whole warp, elected lane issues)
     int stage = 0;
     uint32_t phase = 0;
@@ -162,71 +149,54 @@ k_gemm_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
         if (++stage == Cfg::kStages) { stage = 0; phase ^= 1u; }
       }
     }
-  } else if (warp == 1) {
-    // -------------------------------------------------------------- MMA issuer (whole warp, elected lane issues)
-    constexpr uint32_t idesc = idesc_f16(FMT, Cfg::kBlockM, BLOCK_N);
+  } else {
+    // ---------------------------------------------------------------- consumer warpgroups (warps 0..7)
+    // warpgroup `half` computes columns [half * BLOCK_N / 2, (half + 1) * BLOCK_N / 2) of the tile, then stores them;
+    // warp `quarter` of it owns tile rows acc_row(quarter, lane) in the epilogue
+    const int quarter = warp % 4;
+    const int half = warp / 4;
+    constexpr int kChunks = BLOCK_N / 64;          // 32-column chunks per half
+    float* wb = scratch + warp * (acc_scratch_bytes<32>() / 4);
     int stage = 0;
     uint32_t phase = 0;
-    int it = 0;
-    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x, ++it) {
-      const int as = it & 1;
-      mbar_wait(&tempty[as], ((it >> 1) & 1) ^ 1u);
-      fence_after_sync();
-      const uint32_t d_tmem = tmem_base + as * BLOCK_N;
+    uint32_t piece = 0;   // TMA-store pieces issued by this warp (selects the staging buffer)
+    Acc<BLOCK_N / 2> acc;
+    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
+      const int mb = t / n_blocks, nb = t % n_blocks;
+      int prev = stage;
       for (int kb = 0; kb < num_kb; ++kb) {
         mbar_wait(&full[stage], phase);
-        fence_after_sync();
         const uint64_t adesc = smem_desc_sw128(smem_u32(smem_a + stage * Cfg::kABytes));
-        const uint64_t bdesc = smem_desc_sw128(smem_u32(smem_b + stage * Cfg::kBBytes));
-        if (elect_one()) {
-#pragma unroll
-          for (int k = 0; k < Cfg::kBlockK / 16; ++k) {
-            // advance 16 elements (32 bytes) along K inside the 128B swizzle span: +2 in 16-byte units
-            umma_f16(d_tmem, adesc + 2 * k, bdesc + 2 * k, idesc, (kb | k) != 0);
-          }
-          umma_commit(&empty[stage]);           // frees the smem slot once these MMAs have read it
-          if (kb == num_kb - 1) umma_commit(&tfull[as]);
-        }
+        const uint64_t bdesc = smem_desc_sw128(smem_u32(smem_b + stage * Cfg::kBBytes + half * (BLOCK_N / 2) * 128));
+        mma_block<BLOCK_N / 2, FMT>(acc, adesc, bdesc, 512, 2, Cfg::kBlockK / 16, kb != 0);
+        // keep this block's MMAs in flight while the next stage is awaited: wait for the PREVIOUS block only and
+        // free its slot (this warp's MMAs have read it)
+        wgmma_wait<1>();
         __syncwarp();
+        if (lane == 0 && kb > 0) mbar_arrive(&empty[prev]);
+        prev = stage;
         if (++stage == Cfg::kStages) { stage = 0; phase ^= 1u; }
       }
-    }
-  } else {
-    // ---------------------------------------------------------------- epilogue warps 2..9
-    // Two warps per TMEM lane quarter, each owning half of the tile's columns; TMEM loads are software
-    // pipelined (chunk c+1 is in flight while chunk c is converted and stored) -- ncu r1a showed the
-    // 4-warp, load-wait-store epilogue, not the tensor pipe or L2, bounding the K=64 GEMMs.
-    const int quarter = warp % 4;     // TMEM lane quarter this warp may access
-    const int half = (warp - 2) / 4;  // which half of the BLOCK_N columns
-    constexpr int kChunks = BLOCK_N / 64;          // 32-column chunks per half
-    int it = 0;
-    uint32_t piece = 0;   // TMA-store pieces issued by this warp (selects the staging buffer)
-    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x, ++it) {
-      const int mb = t / n_blocks, nb = t % n_blocks;
-      const int as = it & 1;
-      mbar_wait(&tfull[as], (it >> 1) & 1);
-      fence_after_sync();
-      const int row = mb * Cfg::kBlockM + quarter * 32 + lane;
+      wgmma_wait<0>();
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty[prev]);
+      const int row = mb * Cfg::kBlockM + acc_row(quarter, lane);
       const bool row_ok = row < a.M;
       uint16_t* crow = reinterpret_cast<uint16_t*>(a.C) + static_cast<int64_t>(row) * a.ldc;
       const int64_t grow = a.c_row0 + row;
-      const uint32_t tbase = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + as * BLOCK_N +
-                             half * (BLOCK_N / 2);
-      uint32_t v[2][32];
-      tmem_ld32(tbase, v[0]);
-      tmem_ld_wait();
+      uint32_t v[32];
       const float accs = (EPI == EPI_SPLIT && a.acc_scale != nullptr) ? __ldg(a.acc_scale) : 1.f;
       const bool use_tma = Cfg::kStoreBytes > 0 && a.tma_store != 0;
       // this warp's staging: 2 buffers of 32 rows x 64 B; 16-byte unit u of row r sits at (u ^ ((r >> 1) & 3))
       // (SWIZZLE_64B of tmC) -- conflict-free for the 8-lane phases of a v4 shared store
-      const uint32_t stage0 = smem_u32(smem_c) + (warp - 2) * 4096;
+      const uint32_t stage0 = smem_u32(smem_c) + warp * 4096;
       const uint32_t sw = static_cast<uint32_t>((lane >> 1) & 3);
 #pragma unroll
       for (int cc = 0; cc < kChunks; ++cc) {
-        if (cc + 1 < kChunks) tmem_ld32(tbase + (cc + 1) * 32, v[(cc + 1) & 1]);
+        acc_rows<BLOCK_N / 2, 32>(acc, cc * 32, wb, v);
         const int col0 = nb * BLOCK_N + half * (BLOCK_N / 2) + cc * 32;
         if (col0 < a.N && (row_ok || use_tma)) {
-          const uint32_t* vv = v[cc & 1];
+          const uint32_t* vv = v;
           uint32_t packed[16], packed_lo[EPI == EPI_SPLIT ? 16 : 1];
           float vm[4] = {0.f, 0.f, 0.f, 0.f};       // four independent max chains (one chain of 32 is latency bound)
           uint32_t mkw[16];                         // EPI_MASK: the row's 32 stored activations (64 B, four 16-byte loads)
@@ -312,12 +282,16 @@ k_gemm_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
               fence_proxy_async_smem();
               __syncwarp();
               if (issuer) {
-                const int r0 = mb * Cfg::kBlockM + quarter * 32;
-                if (a.chunk_rows_pad > 0)
-                  tma_store_2d(&tmC, buf, colx & 63,
-                               static_cast<int>((colx >> 6) * a.chunk_rows_pad + a.c_row0 + r0));
-                else
-                  tma_store_2d(&tmC, buf, colx, r0);
+                // lanes 0..15 and 16..31 hold two 16-row runs of the tile (acc_row): two [16 x 32] panels
+#pragma unroll
+                for (int hh = 0; hh < 2; ++hh) {
+                  const int r0 = mb * Cfg::kBlockM + 64 * hh + 16 * quarter;
+                  if (a.chunk_rows_pad > 0)
+                    tma_store_2d(&tmC, buf + hh * 1024, colx & 63,
+                                 static_cast<int>((colx >> 6) * a.chunk_rows_pad + a.c_row0 + r0));
+                  else
+                    tma_store_2d(&tmC, buf + hh * 1024, colx, r0);
+                }
                 bulk_commit();
               }
               ++piece;
@@ -326,8 +300,8 @@ k_gemm_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
                                   ? reinterpret_cast<uint16_t*>(a.C) +
                                         (static_cast<int64_t>(colx >> 6) * a.chunk_rows_pad + grow) * 64 + (colx & 63)
                                   : crow + colx;
-              st_global_v8(dst, pk);            // 2 x 32 B: full sectors (16 B stores were half-used
-              st_global_v8(dst + 16, pk + 8);   // sectors, ncu r1a)
+              st_global_32b(dst, pk);            // 2 x 32 B: full sectors (16 B stores were half-used
+              st_global_32b(dst + 16, pk + 8);   // sectors)
             }
           };
           if (EPI != EPI_F32) {
@@ -335,22 +309,13 @@ k_gemm_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
             if (FMT == 0 && EPI == EPI_SPLIT) store_piece(packed_lo, col0 + a.N);
           }
         }
-        if (cc + 1 < kChunks) tmem_ld_wait();
       }
-      fence_before_sync();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty[as]);
     }
   }
-  if (Cfg::kStoreBytes > 0 && a.tma_store && warp >= 2 && elect_one()) bulk_wait0();
-  fence_before_sync();
+  if (Cfg::kStoreBytes > 0 && a.tma_store && warp < 8 && elect_one()) bulk_wait0();
   if (a.done_cnt != nullptr) signal_done(a.done_cnt, a.done_ok);   // includes __syncthreads
   else __syncthreads();
   if (threadIdx.x == 0) trace_write(a.trace, (100u + (a.K > 64 ? 1u : 0u)) | (a.trace_seq << 12), tr0, tr1, a.trace.rec ? gtime() : 0ull);
-  if (warp == 1) {
-    fence_after_sync();
-    tmem_dealloc(tmem_base, Cfg::kTmemCols);
-  }
 }
 
 int g_num_sms = 0;
@@ -370,7 +335,7 @@ int launch_gemm_cfg(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtens
   const int grid = tiles < max_ctas ? tiles : max_ctas;
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3(grid);
-  cfg.blockDim = dim3(320);
+  cfg.blockDim = dim3(288);
   cfg.dynamicSmemBytes = Cfg::kSmemBytes;
   cfg.stream = st;
   cudaLaunchAttribute attr[1];
@@ -390,8 +355,8 @@ int tc_init() {
   NNC_CHECK_CUDA(cudaGetDevice(&dev));
   cudaDeviceProp prop;
   NNC_CHECK_CUDA(cudaGetDeviceProperties(&prop, dev));
-  NNC_REQUIRE(prop.major == 10, NNCONV_ERR_UNSUPPORTED,
-              "libnnconv_b200 needs an sm_100-class GPU (found sm_%d%d)", prop.major, prop.minor);
+  NNC_REQUIRE(prop.major == 9 && prop.minor == 0, NNCONV_ERR_UNSUPPORTED,
+              "libnnconv_b200 needs an sm_90 GPU (found sm_%d%d)", prop.major, prop.minor);
   int s = tmap_init();
   if (s != NNCONV_OK) return s;
   g_num_sms = prop.multiProcessorCount;
@@ -451,7 +416,7 @@ int launch_gemm_tc(int prec, const void* A_base, int64_t a_rows_total, int64_t a
     a.trace = TraceBuf{th.rec, th.count, th.cap};
     a.trace_seq = launch_seq++;
   }
-  // TMA-store epilogue: [32 x 32] pieces; rows past M are clipped by the tensor bounds (row-major) or land in
+  // TMA-store epilogue: [16 x 32] panels; rows past M are clipped by the tensor bounds (row-major) or land in
   // the row padding of each chunk panel (chunk-major, chunk_rows_pad >= round_up(c_row0 + M, 32))
   const bool no_tma_store = options().gemm_direct_store != 0;
   a.tma_store = 0;

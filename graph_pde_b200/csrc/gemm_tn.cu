@@ -1,4 +1,4 @@
-// tcgen05 "TN" GEMM: a reduction over ROWS (edges / sources), the shape every parameter gradient of the
+// wgmma "TN" GEMM: a reduction over ROWS (edges / sources), the shape every parameter gradient of the
 // NNConv path has (SURVEY Appendix A: dW_l = sum_e dz_l[e] (x) h_{l-1}[e]; dW_L = sum_c x_c (x) dY_c):
 //
 //     C[M, N] (fp32)  (+)=  alpha * sum_{r < R} A[r, m] * B[r, n]        A: [R, lda], B: [R, ldb] 16-bit row-major
@@ -7,10 +7,11 @@
 // a TMA box of [64 rows x 64 columns] with SWIZZLE_128B lands in shared memory exactly in the canonical
 // MN-major SW128 layout (8 rows of 128 B per swizzle atom; atoms 1024 B apart along K = SBO; the next 64
 // columns of M / N are the next box = LBO), so the rows are used as they lie in HBM -- no transposed copy
-// of the 2 KB/edge activations is ever written.  Instruction descriptor bits 15 / 16 select MN-major A / B.
+// of the 2 KB/edge activations is ever written.  The wgmma transpose flags select MN-major A / B.
 //
-// Work split: tiles of 128 x BLOCK_N of C times `ksplit` row ranges; each CTA accumulates its range in TMEM and
-// adds the tile to C with red.global.add.v4.f32 (C is a zero-initialised fp32 accumulator owned by the caller).
+// Work split: tiles of 128 x BLOCK_N of C times `ksplit` row ranges; each CTA accumulates its range in the registers
+// of two warpgroups (BLOCK_N / 2 columns each) and adds the tile to C with red.global.add.v4.f32 (C is a
+// zero-initialised fp32 accumulator owned by the caller).
 // Rows past R are zero-filled by TMA, so R needs no padding.
 #include "kernels.h"
 #include "tc05.cuh"
@@ -41,35 +42,22 @@ struct TnCfg {
   static constexpr int kABytes = 2 * kBoxBytes;           // M = 128: two boxes
   static constexpr int kBBytes = (BLOCK_N / 64) * kBoxBytes;
   static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr int kStages = (200 * 1024 / kStageBytes) > 6 ? 6 : (200 * 1024 / kStageBytes);
-  static constexpr int kSmemBytes = kStages * kStageBytes + 1024 + 256;
-  static constexpr int kTmemCols = BLOCK_N < 32 ? 32 : BLOCK_N;
+  static constexpr int kScratchBytes = 8 * acc_scratch_bytes<32>();
+  static constexpr int kStages = (180 * 1024 / kStageBytes) > 6 ? 6 : (180 * 1024 / kStageBytes);
+  static constexpr int kSmemBytes = kStages * kStageBytes + kScratchBytes + 1024 + 256;
 };
 
-// MN-major SW128 operand: start address, LBO = bytes between consecutive 64-element blocks along M / N,
-// SBO = 1024 B between consecutive 8-row groups along K.
-__device__ __forceinline__ uint64_t smem_desc_mn_sw128(uint32_t smem_addr, uint32_t lbo_bytes) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);
-  d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;
-  d |= static_cast<uint64_t>(1024 >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;             // version = 1 (sm_100)
-  d |= static_cast<uint64_t>(2) << 61;             // SWIZZLE_128B
-  return d;
-}
-
 template <int BLOCK_N, int FMT>
-__global__ void __launch_bounds__(192, 1)
+__global__ void __launch_bounds__(288, 1)
 k_gemm_tn(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, GemmTnArgs a) {
   using Cfg = TnCfg<BLOCK_N>;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
   uint8_t* smem = smem_raw + (((raw + 1023u) & ~1023u) - raw);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::kStages * Cfg::kStageBytes);
+  float* scratch = reinterpret_cast<float*>(smem + Cfg::kStages * Cfg::kStageBytes);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::kStages * Cfg::kStageBytes + Cfg::kScratchBytes);
   uint64_t* full = bars;
   uint64_t* empty = bars + Cfg::kStages;
-  uint64_t* tfull = bars + 2 * Cfg::kStages;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tfull + 1);
 
   const int warp = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x / 32), 0), lane = threadIdx.x % 32;
   const int n_blocks = ceil_div(a.N, BLOCK_N);
@@ -79,28 +67,20 @@ k_gemm_tn(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
   const int kb0 = split * a.kb_per_split;
   const int kb1 = min(total_kb, kb0 + a.kb_per_split);
   const int num_kb = kb1 - kb0;
-  if (num_kb <= 0) return;     // uniform per CTA, before any barrier / TMEM allocation
+  if (num_kb <= 0) return;     // uniform per CTA, before any barrier
 
-  if (warp == 0 && lane == 0) {
+  if (warp == 8 && lane == 0) {
     prefetch_tmap(&tmA);
     prefetch_tmap(&tmB);
     for (int s = 0; s < Cfg::kStages; ++s) {
       mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 1);
+      mbar_init(&empty[s], 8);   // one arrive per consumer warp
     }
-    mbar_init(tfull, 1);
     fence_barrier_init();
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, Cfg::kTmemCols);
-    tmem_relinquish();
-  }
-  fence_before_sync();
   __syncthreads();
-  fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp == 8) {
     // ---------------------------------------------------------------- TMA producer
     int stage = 0;
     uint32_t phase = 0;
@@ -121,63 +101,55 @@ k_gemm_tn(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
       __syncwarp();
       if (++stage == Cfg::kStages) { stage = 0; phase ^= 1u; }
     }
-  } else if (warp == 1) {
-    // ---------------------------------------------------------------- MMA issuer
-    constexpr uint32_t idesc = idesc_f16(FMT, 128, BLOCK_N) | (1u << 15) | (1u << 16);   // A and B MN-major
+  } else {
+    // ---------------------------------------------------------------- consumer warpgroups: columns [half * BLOCK_N / 2, ...)
+    constexpr int NH = BLOCK_N / 2;                 // whole 64-column boxes of B
+    const int quarter = warp % 4, half = warp / 4;
+    const int n_base = nb * BLOCK_N + half * NH;
+    const bool live = n_base < a.N;                 // N <= BLOCK_N / 2: the second warpgroup only drains the ring
+    float* wb = scratch + warp * (acc_scratch_bytes<32>() / 4);
+    Acc<NH> acc;
     int stage = 0;
     uint32_t phase = 0;
     for (int kb = 0; kb < num_kb; ++kb) {
       mbar_wait(&full[stage], phase);
-      fence_after_sync();
-      const uint32_t sa = smem_u32(smem + stage * Cfg::kStageBytes);
-      const uint64_t adesc = smem_desc_mn_sw128(sa, Cfg::kBoxBytes);
-      const uint64_t bdesc = smem_desc_mn_sw128(sa + Cfg::kABytes, Cfg::kBoxBytes);
-      if (elect_one()) {
-#pragma unroll
-        for (int k = 0; k < Cfg::kRowsK / 16; ++k) {
-          // 16 reduction rows = two 8-row groups of 1024 B: advance the start address by 2048 B (>> 4 = 128)
-          umma_f16(tmem_base, adesc + 128 * k, bdesc + 128 * k, idesc, (kb | k) != 0);
-        }
-        umma_commit(&empty[stage]);
-        if (kb == num_kb - 1) umma_commit(tfull);
+      if (live) {
+        const uint32_t sa = smem_u32(smem + stage * Cfg::kStageBytes);
+        const uint64_t adesc = smem_desc_mn_sw128(sa, Cfg::kBoxBytes);
+        const uint64_t bdesc = smem_desc_mn_sw128(sa + Cfg::kABytes + half * (NH / 64) * Cfg::kBoxBytes, Cfg::kBoxBytes);
+        // the second m64 half of A is the next [64 x 64] box; 16 reduction rows = two 8-row groups of 1024 B
+        mma_block<NH, FMT, 1, 1>(acc, adesc, bdesc, Cfg::kBoxBytes >> 4, 128, Cfg::kRowsK / 16, kb != 0);
+        wgmma_wait<0>();
       }
       __syncwarp();
+      if (lane == 0) mbar_arrive(&empty[stage]);
       if (++stage == Cfg::kStages) { stage = 0; phase ^= 1u; }
     }
-  } else {
-    // ---------------------------------------------------------------- epilogue warps 2..5: C += alpha * D
-    const int quarter = warp % 4;
-    mbar_wait(tfull, 0);
-    fence_after_sync();
-    float alpha = a.alpha;
-    if (a.alpha_dev != nullptr) alpha *= __ldg(a.alpha_dev);
-    const int m = mb * 128 + quarter * 32 + lane;
-    float* crow = a.C + static_cast<int64_t>(m) * a.ldc + nb * BLOCK_N;
-#pragma unroll 1
-    for (int cc = 0; cc < BLOCK_N; cc += 32) {
-      uint32_t v[32];
-      tmem_ld32(tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + cc, v);
-      tmem_ld_wait();
-      if (m < a.M) {
+    if (live) {
+      // ---- epilogue: C += alpha * D
+      float alpha = a.alpha;
+      if (a.alpha_dev != nullptr) alpha *= __ldg(a.alpha_dev);
+      const int m = mb * 128 + acc_row(quarter, lane);
+      float* crow = a.C + static_cast<int64_t>(m) * a.ldc + n_base;
 #pragma unroll
-        for (int q = 0; q < 8; ++q) {
-          const int n = nb * BLOCK_N + cc + 4 * q;
-          if (n + 3 < a.N) {
-            red_add_v4(crow + cc + 4 * q, alpha * __uint_as_float(v[4 * q]), alpha * __uint_as_float(v[4 * q + 1]),
-                       alpha * __uint_as_float(v[4 * q + 2]), alpha * __uint_as_float(v[4 * q + 3]));
-          } else {
-            for (int j = 0; j < 4; ++j)
-              if (n + j < a.N) atomicAdd(crow + cc + 4 * q + j, alpha * __uint_as_float(v[4 * q + j]));
+      for (int cc = 0; cc < NH; cc += 32) {
+        uint32_t v[32];
+        acc_rows<NH, 32>(acc, cc, wb, v);
+        if (m < a.M) {
+#pragma unroll
+          for (int q = 0; q < 8; ++q) {
+            const int n = n_base + cc + 4 * q;
+            if (n + 3 < a.N) {
+              red_add_v4(crow + cc + 4 * q, alpha * __uint_as_float(v[4 * q]), alpha * __uint_as_float(v[4 * q + 1]),
+                         alpha * __uint_as_float(v[4 * q + 2]), alpha * __uint_as_float(v[4 * q + 3]));
+            } else {
+              for (int j = 0; j < 4; ++j)
+                if (n + j < a.N) atomicAdd(crow + cc + 4 * q + j, alpha * __uint_as_float(v[4 * q + j]));
+            }
           }
         }
       }
     }
-  }
-  fence_before_sync();
-  __syncthreads();
-  if (warp == 1) {
-    fence_after_sync();
-    tmem_dealloc(tmem_base, Cfg::kTmemCols);
   }
 }
 
@@ -190,7 +162,7 @@ int launch_tn_cfg(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmTnAr
                                         Cfg::kSmemBytes));
     attr_set = true;
   }
-  k_gemm_tn<BLOCK_N, FMT><<<grid, 192, Cfg::kSmemBytes, st>>>(tmA, tmB, a);
+  k_gemm_tn<BLOCK_N, FMT><<<grid, 288, Cfg::kSmemBytes, st>>>(tmA, tmB, a);
   NNC_CHECK_LAUNCH();
   return NNCONV_OK;
 }
@@ -208,7 +180,7 @@ int launch_gemm_tn(int prec, const void* A, int64_t lda, int a_col0, const void*
   NNC_REQUIRE(ldc % 4 == 0 && (reinterpret_cast<uintptr_t>(C) & 15) == 0, NNCONV_ERR_ARG,
               "gemm_tn: C must be 16-byte aligned with ldc a multiple of 4");
   const int bf = prec == PREC_BF16;
-  const int BN = N > 128 ? 256 : N > 64 ? 128 : 64;
+  const int BN = N > 128 ? 256 : 128;
   CUtensorMap tmA, tmB;
   s = make_tmap_2d_16b(&tmA, bf, A, static_cast<uint64_t>(R), static_cast<uint64_t>(lda), 64);
   if (s != NNCONV_OK) return s;
@@ -229,8 +201,7 @@ int launch_gemm_tn(int prec, const void* A, int64_t lda, int a_col0, const void*
   ksplit = ceil_div(total_kb, a.kb_per_split);
   dim3 grid(tiles, ksplit);
   if (BN == 256) return bf ? launch_tn_cfg<256, 1>(tmA, tmB, a, grid, st) : launch_tn_cfg<256, 0>(tmA, tmB, a, grid, st);
-  if (BN == 128) return bf ? launch_tn_cfg<128, 1>(tmA, tmB, a, grid, st) : launch_tn_cfg<128, 0>(tmA, tmB, a, grid, st);
-  return bf ? launch_tn_cfg<64, 1>(tmA, tmB, a, grid, st) : launch_tn_cfg<64, 0>(tmA, tmB, a, grid, st);
+  return bf ? launch_tn_cfg<128, 1>(tmA, tmB, a, grid, st) : launch_tn_cfg<128, 0>(tmA, tmB, a, grid, st);
 }
 
 }  // namespace nnc

@@ -50,7 +50,7 @@ int trace_dump(unsigned long long* host_rec, unsigned int max_rec, unsigned int*
 // Cross-kernel pipelining of one conv application (PDL + completion flags, see tc05.cuh).
 struct PipeFlags {
   bool pdl;             // launch with programmatic stream serialization
-  bool small_footprint; // GEMM only: 97 KB / 256 TMEM column configuration that can share an SM
+  bool small_footprint; // GEMM only: ~101 KB configuration that can share an SM
   const int* wait_ok;   // flag that must be raised before this kernel touches its dependent buffer (or nullptr)
   int* done_cnt;        // per-kernel CTA counter (or nullptr)
   int* done_ok;         // raised by the last CTA
@@ -58,7 +58,7 @@ struct PipeFlags {
   int join_n;
 };
 
-// ---- gemm_tc.cu (tcgen05): C[M, N] (16-bit) = act(A[M, K] * B[N, K]^T + bias); A rows start at a_row0 of the
+// ---- gemm_tc.cu (wgmma): C[M, N] (16-bit) = act(A[M, K] * B[N, K]^T + bias); A rows start at a_row0 of the
 // tensor A_base[a_rows_total, K]; K, N multiples of 64.  bias == nullptr -> no bias, relu flag separate.
 // split_flags (PREC_F16X2): GEMM_A_SPLIT -> A is [hi | lo] with 2K/3 columns and B is [hi | lo | hi] with K columns;
 // GEMM_C_SPLIT -> C receives [hi | lo] pairs (2N columns / 2N/64 chunks).  overflow: device counter of output
@@ -75,12 +75,12 @@ int launch_gemm_tc(int prec, const void* A_base, int64_t a_rows_total, int64_t a
 int launch_apply_edge(int prec, const Plan* P, const Weights* W, const void* Kmat, const float* x, int aggr_mean, float* out,
                       cudaStream_t st, unsigned node_flags = 0);
 
-// ---- gemm_tn.cu (tcgen05, MN-major operands): C[M, N] fp32 += alpha * sum_{r<R} A[r, a_col0 + m] * B[r, b_col0 + n]
+// ---- gemm_tn.cu (wgmma, MN-major operands): C[M, N] fp32 += alpha * sum_{r<R} A[r, a_col0 + m] * B[r, b_col0 + n]
 // (A: [R, lda], B: [R, ldb] 16-bit row-major; C accumulates with fp32 atomics, the caller zero-initialises it)
 int launch_gemm_tn(int prec, const void* A, int64_t lda, int a_col0, const void* B, int64_t ldb, int b_col0, int64_t R,
                    int M, int N, float* C, int64_t ldc, float alpha, const float* alpha_dev, cudaStream_t st);
 
-// ---- conv_tc.cu (tcgen05): per-source contraction + scatter for tiles [tile_begin, tile_end)
+// ---- conv_tc.cu (wgmma): per-source contraction + scatter for tiles [tile_begin, tile_end)
 int launch_conv_tc(int prec, const Plan* P, const void* h, int Kp, const void* Y, int64_t y_nodes, int cout,
                    int tile_begin, int tile_end, int c0, const float* cvec, const float* xs, int aggr_mean, float* out,
                    cudaStream_t st, const PipeFlags* pf = nullptr);

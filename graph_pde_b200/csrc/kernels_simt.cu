@@ -178,10 +178,10 @@ k_edge_layer1(const float* __restrict__ edge_attr, const int* __restrict__ perm,
 
 // ---- first edge-MLP layer on the tensor cores with fp32-grade inputs -------------------------------
 // v = hi + lo with hi = T(v), lo = T(v - hi): two 16-bit values carry ~22 mantissa bits.  With
-//   A1[p, :] = [hi(ea) | lo(ea) | hi(ea) | 1 | 1 | 0...]            (64 columns, one UMMA K block)
+//   A1[p, :] = [hi(ea) | lo(ea) | hi(ea) | 1 | 1 | 0...]            (64 columns, one wgmma K block)
 //   B1[j, :] = [hi(W1_j) | hi(W1_j) | lo(W1_j) | hi(b1_j) | lo(b1_j) | 0...]
 // A1 . B1^T = ea . W1_j + b1_j up to the dropped lo*lo terms (2^-22 relative): the first Linear keeps
-// fp32-grade accuracy although it runs as a 16-bit tcgen05 GEMM (utilities.py:223-227, first layer).
+// fp32-grade accuracy although it runs as a 16-bit wgmma GEMM (utilities.py:223-227, first layer).
 template <typename T>
 __device__ __forceinline__ float as_float(T v);
 template <>
@@ -341,7 +341,7 @@ __global__ void k_src_prep(const float* __restrict__ x, const int* __restrict__ 
 // One launch for everything a fused application needs before its persistent kernel: blocks [0, g_out) initialise the
 // output rows, blocks [g_out, g_out + g_src) prepare the source rows, and the first threads of the grid clear the batch
 // flags of the application (cntY / cntC / okY / okC [n_batches] at stride flags_stride, and the unit counter) -- in the
-// launch-bound MGKN regime (52 dependent applications per forward) each removed graph node is ~5 us of the chain.
+// launch-bound MGKN regime (52 dependent applications per forward) every launch removed from the chain counts.
 template <typename T, int SPLIT = 0>
 __global__ void k_node_prep(const float* __restrict__ x, const float* __restrict__ root, const float* __restrict__ bias,
                             int64_t N, float* __restrict__ out, int g_out, const int* __restrict__ src_nodes, int S, int cin,
@@ -475,7 +475,7 @@ k_apply_edge(const T2* __restrict__ Kmat, const float* __restrict__ x, const int
              const int* __restrict__ group_ptr, const int* __restrict__ dst_sorted, const float* __restrict__ inv_deg,
              int S, int64_t E, int cin, int cout, float* __restrict__ out, unsigned node_flags) {
   // one warp per EDGE (sorted position p): parallelism = E warps whatever the degree distribution is (one warp per
-  // source serialised the 18-55 edges of MGKN's coarse levels and ran 3x slower than formulation C, run r2i)
+  // source serialises the 18-55 edges of MGKN's coarse levels)
   extern __shared__ float sxe[];
   const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
   const int64_t p = static_cast<int64_t>(blockIdx.x) * (blockDim.x / 32) + warp;
@@ -513,7 +513,7 @@ k_apply_edge(const T2* __restrict__ Kmat, const float* __restrict__ x, const int
 }
 
 // variant for very low out-degree (E <= 8 S, the 1-D multipole stencils): one warp per SOURCE loads x_src once and walks
-// its 2-4 edges -- no per-edge source search, measured 1.27 vs 1.62 ms per config-5 forward (runs r2e / r2j)
+// its 2-4 edges -- no per-edge source search
 template <typename T2>
 __global__ void __launch_bounds__(128)
 k_apply_edge_src(const T2* __restrict__ Kmat, const float* __restrict__ x, const int* __restrict__ src_nodes,
@@ -556,8 +556,7 @@ k_apply_edge_src(const T2* __restrict__ Kmat, const float* __restrict__ x, const
 // A K_e row of COUT 16-bit values is LPR = COUT/8 lanes wide, so ONE warp-wide load instruction covers RPI = 256/COUT
 // input channels and an edge needs only CIN/RPI (= 16 at 64 x 64) independent loads per lane, all issued back to back
 // BEFORE the source search / x staging they do not depend on.  The scalar kernels issue 64 dependent-looking 4-byte
-// loads per lane and were latency bound: 23 us per launch for <= 8192 edges, 96 us for the warp-per-source kernel on a
-// 100-source level of the MGKN V-cycle (profiles/r2u_mgkn_forward_launches.md).
+// loads per lane and are latency bound.
 __device__ __forceinline__ void red_add_v4f(float* addr, float a, float b, float c, float d) {
   asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
 }

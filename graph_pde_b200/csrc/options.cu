@@ -19,7 +19,6 @@ const Entry kEntries[] = {
     {"no_pipe", "NNCONV_NO_PIPE", &Options::no_pipe, 0},
     {"ring", "NNCONV_RING", &Options::ring, 3},
     {"ring_deep", "NNCONV_RING_DEEP", &Options::ring_deep, 0},
-    {"y_block_n", "NNCONV_Y_BLOCKN", &Options::y_block_n, 64},
     {"apply_stages", "NNCONV_APPLY_STAGES", &Options::apply_stages, 0},
     {"apply_passes", "NNCONV_APPLY_PASSES", &Options::apply_passes, 0},
     {"apply_a_policy", "NNCONV_APPLY_A_POLICY", &Options::apply_a_policy, 0},
@@ -43,7 +42,6 @@ std::once_flag g_once;
 
 void sanitize(Options& o) {
   if (o.ring < 2 || o.ring > 8) o.ring = 3;
-  if (o.y_block_n != 128) o.y_block_n = 64;
 }
 }  // namespace
 

@@ -10,17 +10,16 @@ struct Options {
   int ring;               // NNCONV_RING: Y ring depth of the fused kernel (2..8, default 3)
   int ring_deep;          // NNCONV_RING_DEEP (default 0): when the Y budget holds more than ring x 128 sources (narrow edge
                           // networks: 32 KB of Y per source at ker_width 256), keep batches of 128 sources and deepen the
-                          // ring (<= 16) instead of growing the batches.  Measured SLOWER on the MGKN V-cycle (1.86 vs
-                          // 1.61 ms per replayed forward, run r2v): more batches = more flag round trips per launch
-  int y_block_n;          // NNCONV_Y_BLOCKN: N tile of the Y pipeline (64 default | 128)
+                          // ring (<= 16) instead of growing the batches; off by default: more batches = more flag round
+                          // trips per launch
   int apply_stages;       // NNCONV_APPLY_STAGES: cap on the A stages of the fused kernel (0 = no cap)
   int apply_passes;       // NNCONV_APPLY_PASSES: force the number of passes over the B-slot ring (0 = automatic): more
                           // passes = fewer resident B slots = more A stages (bytes of the h stream in flight)
   int apply_a_policy;     // NNCONV_APPLY_A_POLICY: L2 hint of the h stream in the fused kernel: 0 evict-first (default), 1 normal
   int tmap_promo;         // NNCONV_TMAP_PROMO: L2 promotion of operand tensor maps: 2 = 256 B (default), 1 = 128 B, 0 = none
   int scatter_mode;       // NNCONV_SCATTER_MODE: 1 (default) = each edge row staged in shared memory and added to out[dst] with
-                          // ONE cp.reduce.async.bulk (256 B per request, TMA engine); 0 = red.global.add.v4.f32 per lane
-                          // (16 B per request).  Measured 126.3-126.8 vs 129.6-130.3 ms per step (run r2o)
+                          // ONE cp.reduce.async.bulk (256 B per request, TMA engine); 0 = red.global.add.v2.f32 straight
+                          // from the accumulator fragments (8 B per request)
   int debug_scatter;      // NNCONV_DEBUG_SCATTER: timing experiments only (wrong results)
   int y_store_policy;     // NNCONV_Y_STORE_POLICY: 0 normal, 1 evict-last, 2 evict-first
   int l2_persist;         // NNCONV_L2_PERSIST: access-policy window over the Y ring; value = persisting-L2 set-aside in MB

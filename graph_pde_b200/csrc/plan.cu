@@ -5,7 +5,7 @@
 // contraction kernel wants exactly that grouping (all edges of one source share the per-source matrix
 // Y_src), so the plan (a) verifies / establishes the source grouping (stable radix sort only when the
 // caller's list is not already grouped), (b) compacts the sources that have out-edges, (c) cuts every
-// source group into tiles of <= 128 edges (= one UMMA M tile), (d) stores dst as int32 in sorted order
+// source group into tiles of <= 128 edges (= one 128-row wgmma tile), (d) stores dst as int32 in sorted order
 // and 1/max(in_degree,1) for the mean aggregation (PyG scatter_('mean'), empty set -> 0).
 #include <cub/cub.cuh>
 

@@ -38,7 +38,7 @@ struct TmapKey {
   uint64_t rows, cols;
   uint32_t box_rows;
   int bf;
-  int kind;   // 0: [box_rows x 64] SWIZZLE_128B operand tiles, 1: [32 x 32] SWIZZLE_64B store panels
+  int kind;   // 0: [box_rows x 64] SWIZZLE_128B operand tiles, 1: [16 x 32] SWIZZLE_64B store panels
   bool operator==(const TmapKey& o) const {
     return base == o.base && rows == o.rows && cols == o.cols && box_rows == o.box_rows && bf == o.bf &&
            kind == o.kind;
@@ -95,7 +95,7 @@ int make_tmap_2d_16b(CUtensorMap* out, int is_bf16, const void* base, uint64_t r
 }
 
 int make_tmap_store_16b(CUtensorMap* out, int is_bf16, const void* base, uint64_t rows, uint64_t cols) {
-  return make_tmap_kind(out, is_bf16, base, rows, cols, 32, 1);
+  return make_tmap_kind(out, is_bf16, base, rows, cols, 16, 1);
 }
 
 // ---- tracing buffer (debug) ------------------------------------------------------------------------

@@ -9,7 +9,7 @@ namespace nnc {
 
 int tmap_init();
 // 2-D row-major tensor of 16-bit elements [rows, cols] (cols contiguous), box = [box_rows, 64 cols],
-// 128-byte swizzle (the layout tcgen05 K-major SW128 descriptors expect).
+// 128-byte swizzle (the layout wgmma K-major SW128 descriptors expect).
 int make_tmap_2d_16b(CUtensorMap* out, int is_bf16, const void* base, uint64_t rows, uint64_t cols,
                      uint32_t box_rows);
 // same tensor, described for the GEMM epilogue's TMA stores: box = [32 rows, 32 cols], 64-byte swizzle

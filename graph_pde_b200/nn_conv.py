@@ -1,4 +1,4 @@
-"""B200-native drop-in for the reference's edge-conditioned convolution.
+"""H100-native drop-in for the reference's edge-conditioned convolution.
 
 Mirrors the operator interface of the reference (paths relative to neuraloperator/graph-pde):
 
@@ -10,7 +10,7 @@ Mirrors the operator interface of the reference (paths relative to neuraloperato
 
 Same attribute names (``in_channels, out_channels, nn, aggr, root, bias``), same state-dict keys
 (``nn.layers.{0,2,4}.{weight,bias}``, ``root``, ``bias``), same init distributions.  The arithmetic
-runs in libnnconv_b200.so (hand-written sm_100a CUDA, C ABI in include/nnconv_b200.h); PyTorch only
+runs in libnnconv_b200.so (hand-written sm_90a CUDA, C ABI in include/nnconv_b200.h); PyTorch only
 owns the device memory and the stream.  There is no CPU / eager fallback: a CPU tensor, a missing
 library or an unsupported edge network raises.
 
@@ -40,16 +40,18 @@ _PLAN_CACHE_MAX = int(os.environ.get('NNCONV_B200_PLAN_CACHE', '64'))           
 _PLAN_CACHE_MAX_BYTES = int(os.environ.get('NNCONV_B200_PLAN_CACHE_BYTES', str(2 << 30)))   # plan buffers + pinned edge_index
 _OVERFLOW_CHECK = os.environ.get('NNCONV_B200_OVERFLOW_CHECK', '1') != '0'
 _Y_BYTES = int(os.environ.get('NNCONV_B200_Y_BYTES', str(48 << 20)))       # Y ring: 3 x 128 sources at out=64, Kp=1024
-_EF_WS_BYTES = int(os.environ.get('NNCONV_B200_EF_WS_BYTES', str(4 << 30)))  # hidden-layer ping-pong chunk (4 GiB: 25 instead of 97 chunks at 241^2, -1 ms/step, run39)
+_EF_WS_BYTES = int(os.environ.get('NNCONV_B200_EF_WS_BYTES', str(2 << 30)))  # hidden-layer ping-pong chunk (fewer, larger chunks)
 _BWD_WS_BYTES = int(os.environ.get('NNCONV_B200_BWD_WS_BYTES', str(2 << 30)))  # fp32 backward: activations per batch
-# tensor-core backward: per-application workspace (dY of a source batch: 7.6 GB covers 241^2 in one batch) and the
-# per-batch buffers of the deferred pass through the hidden layers
-_BWD_APPLY_WS_BYTES = int(os.environ.get('NNCONV_B200_BWD_APPLY_WS_BYTES', str(9 << 30)))
-_BWD_MLP_WS_BYTES = int(os.environ.get('NNCONV_B200_BWD_MLP_WS_BYTES', str(12 << 30)))   # 1 GiB: +16 ms, 256 MiB: +139 ms per 241^2 step (run r2t)
+# tensor-core backward: per-application workspace (dY of a source batch; larger = fewer batches) and the per-batch
+# buffers of the deferred pass through the hidden layers.  Sized so that a 241^2 training step (47 GiB of edge features)
+# fits an 80 GB H100.
+_BWD_APPLY_WS_BYTES = int(os.environ.get('NNCONV_B200_BWD_APPLY_WS_BYTES', str(4 << 30)))
+_BWD_MLP_WS_BYTES = int(os.environ.get('NNCONV_B200_BWD_MLP_WS_BYTES', str(4 << 30)))
 _BWD_MODE = os.environ.get('NNCONV_B200_BACKWARD', 'auto')       # auto | tc | fp32
 # training: keep the hidden activations h_1..h_{L-2} of the forward for the backward (2 KB per edge and layer at width
-# 1024: 50 GB at 241^2) instead of recomputing them, when they fit this budget
-_KEEP_ACTS_MAX_BYTES = int(os.environ.get('NNCONV_B200_KEEP_ACTS_BYTES', str(64 << 30)))
+# 1024: 47 GiB at 241^2, which does not fit an 80 GB H100 beside the edge features) instead of recomputing them, when
+# they fit this budget
+_KEEP_ACTS_MAX_BYTES = int(os.environ.get('NNCONV_B200_KEEP_ACTS_BYTES', str(8 << 30)))
 # per-edge kernel matrices (formulation B) for graphs with few out-edges per source: auto | on | off
 _EDGE_KERNELS = os.environ.get('NNCONV_B200_EDGE_KERNELS', 'auto')
 _EDGE_KERNELS_MAX_DEG = 8                       # auto: average out-degree of the sources with out-edges ...

@@ -1,6 +1,6 @@
 """Multi-GPU decomposition of the NNConv path (SURVEY 8(e)); the reference itself is single-GPU.
 
-Two ways the path shards, both one process per GPU over torch.distributed (NCCL on the B200 box, gloo in
+Two ways the path shards, both one process per GPU over torch.distributed (NCCL on GPUs, gloo in
 the CPU tests):
 
 1. **Batch sharding** (BASELINE config 3): graphs of a training / inference batch are independent connected

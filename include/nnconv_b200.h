@@ -1,5 +1,5 @@
 /* nnconv_b200.h -- C ABI of libnnconv_b200.so: the NNConv (edge-conditioned convolution) hot path of
- * neuraloperator/graph-pde, hand-written for NVIDIA B200 (sm_100a).
+ * neuraloperator/graph-pde, hand-written for NVIDIA H100 (sm_90a).
  *
  * What it replaces (paths relative to the reference repo):
  *   graph-neural-operator/nn_conv.py:267-282   NNConv_old.forward / message / update
@@ -51,8 +51,8 @@ extern "C" {
 /* precision of the tensor-core operands (accumulation is always fp32; x@root+bias and the first
  * MLP layer are always fp32 CUDA-core math) */
 #define NNCONV_PREC_FP32 0 /* CUDA-core fp32 everywhere, any shape */
-#define NNCONV_PREC_F16 1  /* tcgen05 kind::f16, fp16 operands (10-bit mantissa, TF32-grade) */
-#define NNCONV_PREC_BF16 2 /* tcgen05 kind::f16, bf16 operands */
+#define NNCONV_PREC_F16 1  /* wgmma f16, fp16 operands (10-bit mantissa, TF32-grade) */
+#define NNCONV_PREC_BF16 2 /* wgmma bf16 operands */
 /* fp32-grade results on the fp16 tensor pipe: every operand is an fp16 pair (hi, lo = fp16(v - hi)), every
  * product hi*hi + hi*lo + lo*hi in the fp32 accumulator (3x the MMA work, 2x the activation bytes) */
 #define NNCONV_PREC_F16X2 3
@@ -68,7 +68,7 @@ typedef struct nnconv_weights nnconv_weights_t; /* per parameter version: padded
 
 const char* nnconv_last_error(void);
 int nnconv_abi_version(void);
-/* checks the device (sm_100 class), resolves the TMA descriptor encoder and reads the NNCONV_* tuning
+/* checks the device (sm_90), resolves the TMA descriptor encoder and reads the NNCONV_* tuning
  * variables from the environment (once); idempotent */
 int nnconv_init(void);
 /* tuning / debugging knobs (csrc/options.h lists them: "no_fuse", "ring", "no_coop", ...).  The environment is
@@ -241,7 +241,7 @@ int nnconv_loss_epilogue(const float* out, const float* y, const float* mean, co
 int nnconv_profile_begin(void);
 int nnconv_profile_end(double* ms_by_kind, int64_t* launches_by_kind, int n_kinds);
 
-/* ---- debugging aid: with NNCONV_TRACE=1 in the environment every tcgen05 CTA records
+/* ---- debugging aid: with NNCONV_TRACE=1 in the environment every tensor-core CTA records
  * {tag, blockIdx, smid, t_start, t_ready, t_end} (globaltimer ns); this copies the records to the host and
  * clears the buffer.  tag: 100 = K=64 GEMM, 101 = hidden GEMM, 200 = contraction. */
 int nnconv_debug_trace_dump(unsigned long long* host_rec, unsigned int max_rec, unsigned int* n_out);
@@ -250,7 +250,7 @@ int nnconv_debug_trace_dump(unsigned long long* host_rec, unsigned int max_rec, 
  * `stream` -- used to check that the persistent application kernel tolerates concurrently resident kernels. */
 int nnconv_debug_occupy(int n_ctas, int smem_bytes, long long ns, void* stream);
 
-/* ---- unit-test hook for the tcgen05 GEMM used by the hidden layers and the per-source matrices:
+/* ---- unit-test hook for the wgmma GEMM used by the hidden layers and the per-source matrices:
  * C[M,N] (16-bit) = act(A[M,K] * B[N,K]^T + bias); K, N multiples of 64; bias nullable. ------------- */
 int nnconv_gemm_16b(int precision, const void* A, int64_t M, int K, const void* B, int N, const float* bias,
                     int relu, void* C, void* stream);

@@ -18,6 +18,9 @@ import warnings
 import numpy as np
 import torch
 
+sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), '..'))
+from oracle import golden  # noqa: E402
+
 warnings.filterwarnings('ignore')
 HERE = os.path.dirname(os.path.abspath(__file__))
 REF = '/root/reference'
@@ -90,7 +93,7 @@ def main():
     rec['oned/x'] = x1.numpy()
     rec['oned/edge_attr'] = ea1.numpy()
     rec['oned/out'] = conv(x1, ei, ea1).detach().numpy()
-    np.savez_compressed(os.path.join(OUT, 'g1_tiny_multigraph.npz'), **rec)
+    golden.save(os.path.join(OUT, 'g1_tiny_multigraph.npz'), **rec)
 
     # ---------------- G2: BASELINE config 1 (16x16, r=.25, w=32, kw=1024, T=4), seeded weights ----
     torch.manual_seed(0)
@@ -120,7 +123,7 @@ def main():
         rec['abs/%s' % k] = np.float64(np.abs(v.astype(np.float64)).sum())
         if v.size <= 8192:
             rec['w/%s' % k] = v
-    np.savez_compressed(os.path.join(OUT, 'g2_cfg1_ball16.npz'), **rec)
+    golden.save(os.path.join(OUT, 'g2_cfg1_ball16.npz'), **rec)
 
     # ---------------- G3: shipped checkpoint weights (the reference's only fixture) ---------------
     import __main__
@@ -149,7 +152,7 @@ def main():
                x0=xs[0].numpy(), x_after=np.stack([t.numpy() for t in xs[1:]]))
     for k, v in st.items():
         rec['w/%s' % k] = v.numpy()
-    np.savez_compressed(os.path.join(OUT, 'g3_checkpoint_grain_new.npz'), **rec)
+    golden.save(os.path.join(OUT, 'g3_checkpoint_grain_new.npz'), **rec)
 
     # ---------------- G4: MGKN V-cycle (both script variants) on a small multi-level graph ---------
     torch.manual_seed(0)
@@ -190,7 +193,7 @@ def main():
         rec['general/out'] = model(data).numpy()
     for k, v in _np_state(model).items():
         rec['general/w/%s' % k] = v
-    np.savez_compressed(os.path.join(OUT, 'g4_mgkn_vcycle.npz'), **rec)
+    golden.save(os.path.join(OUT, 'g4_mgkn_vcycle.npz'), **rec)
 
     # ---------------- G5: orthogonal MGKN, Burgers 1-D multipole graph -----------------------------
     torch.Tensor.cuda = lambda self, *a, **k: self      # reference calls .cuda() (MGNO/utilities.py:1743)
@@ -221,7 +224,7 @@ def main():
         rec['edge_attr/%d' % i] = ea_list[i].numpy()
     for k, v in _np_state(model).items():
         rec['w/%s' % k] = v
-    np.savez_compressed(os.path.join(OUT, 'g5_mgkn_burgers1d.npz'), **rec)
+    golden.save(os.path.join(OUT, 'g5_mgkn_burgers1d.npz'), **rec)
 
     # ---------------- G6: graph-generator restatement pins (edge lists from sklearn path) ----------
     rec = {}
@@ -231,7 +234,7 @@ def main():
         th = np.arange(s * s, dtype=np.float64) * 0.01
         rec['ei/%d_%g' % (s, r)] = ei.numpy().astype(np.int32)
         rec['ea/%d_%g' % (s, r)] = mg.attributes(theta=th).numpy()
-    np.savez_compressed(os.path.join(OUT, 'g6_ball_graphs.npz'), **rec)
+    golden.save(os.path.join(OUT, 'g6_ball_graphs.npz'), **rec)
     # ---------------- G7: multi-level (MGKN) graph generator pins, RandomMultiMeshGenerator, seeded ----------
     s, m, ri, rx = 31, [200, 80, 30], [0.155, 0.31, 0.62], [0.21, 0.41]    # radii without lattice ties
     torch.manual_seed(0)

@@ -1,16 +1,16 @@
-"""Put an UNMODIFIED copy of the reference's hot-path files under baseline/_ref/ (git-ignored, travels to the
-GPU box with the gpurun snapshot) so that `bench.py --impl reference` times the reference's OWN code.
+"""Optional, run by hand: put an UNMODIFIED copy of the reference's hot-path files under the git-ignored
+baseline/_ref/ so that `bench.py --impl reference` times the reference's OWN code instead of the oracle port.
+The build never runs it, so by default the reference arm times the oracle port.
 
 TEST / MEASUREMENT INFRASTRUCTURE, never imported by the product path.
 
-The reference is a directory of scripts without setup.py / pyproject.toml, so
-`pip install --target baseline/_ref /root/reference` has nothing to install; this recipe is the equivalent:
-it copies, byte for byte,
+The reference is a directory of scripts without setup.py / pyproject.toml, so there is nothing to install;
+this recipe copies, byte for byte,
     graph-neural-operator/nn_conv.py          (NNConv_old: the operator)
     graph-neural-operator/utilities.py        (DenseNet: the edge MLP)
     multipole-graph-neural-operator/utilities.py
 and records their sha256 in baseline/_ref/MANIFEST.json.  Third-party torch_geometric / torch_scatter are
-not installable here (no wheels, no network): the copied files run over oracle/pyg_stub, the restated
+not needed: the copied files run over oracle/pyg_stub, the restated
 MessagePassing boundary (see its docstring).  Nothing is copied into tracked paths.
 """
 import hashlib

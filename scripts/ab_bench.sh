@@ -2,8 +2,9 @@
 # Same-box A/B of library knobs (csrc/options.h) on the bench workload, forward only:
 #   scripts/ab_bench.sh TAG "base" "NNCONV_SCATTER_MODE=0" "NNCONV_L2_PERSIST=48 NNCONV_GEMM_B_POLICY=0" ...
 # Every variant is one `bench.py --steps 5 --warmup 3` run (no parity / train / CPU legs); one line per variant in
-# gpurun_out/TAG_ab.log.  This is how the tables of profiles/r2f_ab_experiments.md were produced.
-O=gpurun_out
+# $AB_OUT/TAG_ab.log (default: a new temporary directory).  Compare variants only inside one run on one GPU.
+O=${AB_OUT:-$(mktemp -d)}
+mkdir -p "$O"
 TAG=$1; shift
 Q="--no-cpu-baseline --no-parity --no-train --no-other-configs"
 rm -f $O/${TAG}_ab.log

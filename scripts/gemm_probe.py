@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Time the tcgen05 GEMM alone (CUDA events) at the edge-MLP chunk shape for several K, next to a pure
+"""Time the wgmma GEMM alone (CUDA events) at the edge-MLP chunk shape for several K, next to a pure
 write (memset) and a copy of the same output size: separates 'epilogue/store bound' from 'DRAM write bound'."""
 import ctypes
 import os

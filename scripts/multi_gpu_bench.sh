@@ -1,7 +1,7 @@
 #!/bin/bash
-# N-GPU bench under torch.distributed.run exactly as the driver launches it (use with `gpurun --gpus N`):
+# N-GPU bench under torch.distributed.run on one node with N GPUs:
 #   scripts/multi_gpu_bench.sh N TAG [extra bench flags]
-# prints value / train / strip of the JSON line (profiles/r2_measurements.md, "Two / Four / Eight GPUs").
+# prints value / train / strip of the JSON line.
 N=$1; TAG=$2; shift; shift
 O=gpurun_out
 export NCCL_DEBUG=WARN

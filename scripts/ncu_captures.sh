@@ -1,5 +1,5 @@
 #!/bin/bash
-# ncu evidence of one round (B200_PROFILING.md recipe), summaries via scripts/summarize_ncu.py into profiles/:
+# ncu captures of the bench command (summaries via scripts/summarize_ncu.py):
 #   launch list of the bench command, launch list of one training step, --set full of the dominant kernels.
 O=gpurun_out
 TAG=${1:-rX}

@@ -1,5 +1,5 @@
-"""Per-kernel SASS opcode table of libnnconv_b200.so (evidence that the hot kernels are tcgen05 / TMA code):
-    python scripts/sass_table.py > profiles/r2_sass_opcodes.md
+"""Per-kernel SASS opcode table of libnnconv_b200.so (evidence that the hot kernels are wgmma / TMA code):
+    python scripts/sass_table.py > sass_opcodes.md
 Runs on the build container (cuobjdump only needs the .so)."""
 import collections
 import os
@@ -9,7 +9,7 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SO = os.path.join(ROOT, 'graph_pde_b200', 'libnnconv_b200.so')
-OPS = ['UTCHMMA', 'UTMALDG', 'UTMASTG', 'LDTM', 'UTCBAR', 'SYNCS', 'REDG', 'ATOMG', 'STG', 'LDG', 'ELECT', 'HMMA', 'FFMA']
+OPS = ['HGMMA', 'WARPGROUP', 'UTMALDG', 'UTMASTG', 'UBLKRED', 'SYNCS', 'REDG', 'ATOMG', 'STG', 'LDG', 'ELECT', 'HMMA', 'FFMA']
 
 
 def main():
@@ -33,9 +33,9 @@ def main():
         d = d.replace('(anonymous namespace)::', '').replace('nnc::', '').replace('void ', '')
         d = re.sub(r'\(.*', '', d)
         dem[n] = d
-    print('# SASS opcode counts per kernel of libnnconv_b200.so (cuobjdump -sass, sm_100a)\n')
-    print('UTCHMMA = tcgen05.mma, UTMALDG / UTMASTG = TMA tensor load / store, LDTM = tcgen05.ld (TMEM -> registers), '
-          'UTCBAR = tcgen05.commit, SYNCS = mbarrier ops, REDG = red.global (fp32 scatter atomics).  '
+    print('# SASS opcode counts per kernel of libnnconv_b200.so (cuobjdump -sass, sm_90a)\n')
+    print('HGMMA = wgmma.mma_async, WARPGROUP = wgmma fence / arrive / wait, UTMALDG / UTMASTG = TMA tensor load / '
+          'store, UBLKRED = cp.reduce.async.bulk, SYNCS = mbarrier ops, REDG = red.global (fp32 scatter atomics).  '
           'HMMA (mma.sync) must be absent.\n')
     print('| kernel | instr | ' + ' | '.join(OPS) + ' |')
     print('|---|---|' + '---|' * len(OPS))

@@ -26,7 +26,7 @@ def _relerr(got, ref):
 @pytest.mark.parametrize('prec,dt', [('f16', torch.float16), ('bf16', torch.bfloat16)])
 @pytest.mark.parametrize('R,M,N', [(5000, 1024, 1024), (777, 128, 64), (64, 64, 64), (100000, 256, 64), (3001, 192, 320)])
 def test_gemm_tn_matches_torch(prec, dt, R, M, N):
-    """C += alpha * A^T B with both operands taken row-major (MN-major UMMA descriptors), split over the rows."""
+    """C += alpha * A^T B with both operands taken row-major (MN-major wgmma descriptors), split over the rows."""
     from graph_pde_b200 import _lib
     L = _lib.lib()
     _lib.check(L.nnconv_init())

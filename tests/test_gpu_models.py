@@ -8,6 +8,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from oracle import golden
 from tests.helpers import GOLDEN, TOL, cfg1_weights, ei64, rel_err, t
 
 pytestmark = [pytest.mark.gpu, pytest.mark.usefixtures('edge_kernel_mode')]
@@ -55,7 +56,7 @@ def test_mgkn_vcycle(variant, precision, steps, monkeypatch):
     if steps == 'plain' and variant != 'neurips1':
         pytest.skip('only KernelInduced has the fused step chain')
     monkeypatch.setattr(models, '_FUSED_STEPS', steps == 'fused')
-    g = np.load(os.path.join(GOLDEN, 'g4_mgkn_vcycle.npz'))
+    g = golden.load(os.path.join(GOLDEN, 'g4_mgkn_vcycle.npz'))
     pts = [int(p) for p in g['points']]
     cls = KernelInduced if variant == 'neurips1' else MKGN
     model = cls(width=32, ker_width=64, depth=2, ker_in=6, points=pts, level=len(pts), in_width=6,
@@ -113,7 +114,7 @@ def test_cuda_graph_replay_of_kernelnn_and_vcycle():
     assert rel_err(gf.replay(), eager2) < 1e-4
     assert rel_err(eager2, eager) > 1e-2
 
-    g4 = np.load(os.path.join(GOLDEN, 'g4_mgkn_vcycle.npz'))
+    g4 = golden.load(os.path.join(GOLDEN, 'g4_mgkn_vcycle.npz'))
     pts = [int(p) for p in g4['points']]
     vm = KernelInduced(width=32, ker_width=64, depth=2, ker_in=6, points=pts, level=len(pts), in_width=6)
     vm = _load(vm, {k[len('neurips1/w/'):]: g4[k] for k in g4.files if k.startswith('neurips1/w/')})

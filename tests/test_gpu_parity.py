@@ -1,11 +1,12 @@
 """GPU parity: the CUDA path (through the C ABI of libnnconv_b200.so) vs golden vectors produced by the
-reference's own files and vs the CPU oracle on seeded inputs.  Run on the B200 box: pytest -m gpu."""
+reference's own files and vs the CPU oracle on seeded inputs.  Needs a GPU: pytest -m gpu."""
 import os
 
 import numpy as np
 import pytest
 import torch
 
+from oracle import golden
 from oracle import nnconv_oracle as O
 from tests.helpers import GOLDEN, TOL, DenseNetLike, cfg1_weights, ei64, make_conv, rel_err, t
 
@@ -70,7 +71,7 @@ def test_g2_cfg1_conv_stack(dev, precision):
 @pytest.mark.parametrize('precision', ['f16', 'bf16', 'f16x2', 'fp32'])
 def test_g3_checkpoint_weights(dev, precision):
     """Trained weights shipped by the reference (graph-neural-operator/model/grain_new_r64_s64testm100)."""
-    g = np.load(os.path.join(GOLDEN, 'g3_checkpoint_grain_new.npz'))
+    g = golden.load(os.path.join(GOLDEN, 'g3_checkpoint_grain_new.npz'))
     st = {k[2:]: g[k] for k in g.files if k.startswith('w/')}
     ws = [st['conv1.nn.layers.%d.weight' % i] for i in (0, 2, 4)]
     bs = [st['conv1.nn.layers.%d.bias' % i] for i in (0, 2, 4)]
@@ -198,7 +199,7 @@ def test_alternative_schedules_give_the_same_answer(dev, knob, monkeypatch, lib_
             lib_options(k, int(v))
         else:
             lib_options(kv, 1)
-    g = np.load(os.path.join(GOLDEN, 'g3_checkpoint_grain_new.npz'))
+    g = golden.load(os.path.join(GOLDEN, 'g3_checkpoint_grain_new.npz'))
     st = {k[2:]: g[k] for k in g.files if k.startswith('w/')}
     ws = [st['conv1.nn.layers.%d.weight' % i] for i in (0, 2, 4)]
     bs = [st['conv1.nn.layers.%d.bias' % i] for i in (0, 2, 4)]
@@ -273,7 +274,7 @@ def test_node_features_beyond_fp16_range(dev, precision, knob, lib_options):
 @pytest.mark.parametrize('precision', ['f16', 'bf16'])
 def test_low_out_degree_graph_uses_per_edge_kernel_matrices(dev, precision, edge_kernel_mode):
     """The 1-D multipole stencils of MGKN_orthogonal_burgers1d.py give every node 2-4 out-edges: the conv switches
-    to formulation B (K_e built once by the tcgen05 GEMM, one streaming pass per application) and must agree with
+    to formulation B (K_e built once by the wgmma GEMM, one streaming pass per application) and must agree with
     the oracle and with formulation C on the same inputs."""
     from graph_pde_b200 import graphs, nn_conv
     if edge_kernel_mode == 'off':

@@ -10,6 +10,7 @@ import torch
 from graph_pde_b200 import graphs
 from graph_pde_b200.models import DenseNet, KernelInduced, KernelNN, MGKN, MKGN
 from graph_pde_b200.nn_conv import NNConv, NNConv_old, _linear_chain
+from oracle import golden
 from oracle import nnconv_oracle as O
 from tests.helpers import GOLDEN
 
@@ -52,7 +53,7 @@ def test_whole_module_pickle_roundtrip(tmp_path):
 
 
 def test_checkpoint_state_dict_loads_into_our_kernelnn():
-    g = np.load(os.path.join(GOLDEN, 'g3_checkpoint_grain_new.npz'))
+    g = golden.load(os.path.join(GOLDEN, 'g3_checkpoint_grain_new.npz'))
     st = {k[2:]: torch.from_numpy(g[k]) for k in g.files if k.startswith('w/')}
     mlp = DenseNet([6, 64, 128, 4096], torch.nn.ReLU)
     conv = NNConv_old(64, 64, mlp, aggr='mean')
@@ -78,7 +79,7 @@ def test_unsupported_edge_network_is_rejected():
 
 
 def test_model_constructors_match_reference_layouts():
-    g = np.load(os.path.join(GOLDEN, 'g4_mgkn_vcycle.npz'))
+    g = golden.load(os.path.join(GOLDEN, 'g4_mgkn_vcycle.npz'))
     pts = [int(p) for p in g['points']]
     ki = KernelInduced(width=32, ker_width=64, depth=2, ker_in=6, points=pts, level=len(pts), in_width=6)
     ref_keys = sorted(k[len('neurips1/w/'):] for k in g.files if k.startswith('neurips1/w/'))
@@ -217,7 +218,7 @@ def test_vcycle_step_chain_on_preactivations_equals_the_reference_op_sequence(mo
 
     monkeypatch.setattr(nn_conv.NNConv_old, 'forward', conv_forward)
     monkeypatch.setattr(nn_conv.NNConv_old, 'residual_step', residual_step)
-    g = np.load(os.path.join(GOLDEN, 'g4_mgkn_vcycle.npz'))
+    g = golden.load(os.path.join(GOLDEN, 'g4_mgkn_vcycle.npz'))
     pts = [int(p) for p in g['points']]
     model = models.KernelInduced(width=32, ker_width=64, depth=2, ker_in=6, points=pts, level=len(pts), in_width=6)
     pre = 'neurips1/w/'

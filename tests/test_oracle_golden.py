@@ -5,6 +5,7 @@ import os
 import numpy as np
 import torch
 
+from oracle import golden
 from oracle import nnconv_oracle as O
 
 TOL = dict(rtol=2e-5, atol=2e-5)     # fp32 vs fp32, summation order differs only by chunking
@@ -70,7 +71,7 @@ def test_g2_cfg1_seeded_weights_and_stack(golden_dir):
 
 
 def test_g3_checkpoint_weights_stack(golden_dir):
-    g = np.load(os.path.join(golden_dir, 'g3_checkpoint_grain_new.npz'))
+    g = golden.load(os.path.join(golden_dir, 'g3_checkpoint_grain_new.npz'))
     st = {k[2:]: _t(g[k]) for k in g.files if k.startswith('w/')}
     ws, bs = O.mlp_params_from_state(st, 'conv1.nn.')
     assert [tuple(w.shape) for w in ws] == [(64, 6), (128, 64), (4096, 128)]
@@ -83,7 +84,7 @@ def test_g3_checkpoint_weights_stack(golden_dir):
 
 
 def test_g4_mgkn_vcycle_both_variants(golden_dir):
-    g = np.load(os.path.join(golden_dir, 'g4_mgkn_vcycle.npz'))
+    g = golden.load(os.path.join(golden_dir, 'g4_mgkn_vcycle.npz'))
     data = dict(edge_index_mid=_ei(g['edge_index_mid']), edge_index_down=_ei(g['edge_index_down']),
                 edge_index_up=_ei(g['edge_index_up']), edge_attr_mid=_t(g['edge_attr_mid']),
                 edge_attr_down=_t(g['edge_attr_down']), edge_attr_up=_t(g['edge_attr_up']),
