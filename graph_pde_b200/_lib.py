@@ -34,6 +34,7 @@ SYMBOLS = [
     'nnconv_ball_count', 'nnconv_ball_fill',
     'nnconv_edge_kernels_sizes', 'nnconv_edge_kernels', 'nnconv_apply_edge',
     'nnconv_edge_acts_sizes', 'nnconv_edge_features_keep', 'nnconv_apply_ex', 'nnconv_apply_edge_ex',
+    'nnconv_backward_ex', 'nnconv_backward_mlp_ex',
 ]
 
 
@@ -102,6 +103,8 @@ def lib():
     L.nnconv_backward_mlp_sizes.argtypes = [c_vp, c_vp, c_int, c_sz, P(c_sz)]
     L.nnconv_backward_mlp.argtypes = [c_vp, c_vp, c_vp, c_vp, c_int, P(c_vp), P(c_vp), c_int, P(c_vp), P(c_vp), c_vp,
                                       c_sz, c_vp, c_vp]
+    L.nnconv_backward_ex.argtypes = list(L.nnconv_backward.argtypes) + [c_vp]          # + grad_edge_attr
+    L.nnconv_backward_mlp_ex.argtypes = list(L.nnconv_backward_mlp.argtypes) + [c_vp]  # + grad_edge_attr
     L.nnconv_edge_acts_sizes.argtypes = [c_vp, c_vp, P(c_sz)]
     L.nnconv_edge_features_keep.argtypes = [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_sz, c_vp, P(c_i64)]
     L.nnconv_halo_push.argtypes = [c_vp, c_int, c_i64, c_int, c_i64, c_i64, c_vp, c_vp, c_i64, c_i64, c_i64, c_vp, c_i64,

@@ -793,11 +793,21 @@ int nnconv_backward(const nnconv_plan_t* plan, const nnconv_weights_t* w, const 
                     const float* root, int aggr, const float* grad_out, float* grad_x, float* const* grad_W,
                     float* const* grad_b, float* grad_root, float* grad_bias, void* ws, size_t ws_bytes,
                     void* stream) {
+  return nnconv_backward_ex(plan, w, edge_attr, x, root, aggr, grad_out, grad_x, grad_W, grad_b, grad_root, grad_bias, ws,
+                            ws_bytes, stream, nullptr);
+}
+
+int nnconv_backward_ex(const nnconv_plan_t* plan, const nnconv_weights_t* w, const float* edge_attr, const float* x,
+                       const float* root, int aggr, const float* grad_out, float* grad_x, float* const* grad_W,
+                       float* const* grad_b, float* grad_root, float* grad_bias, void* ws, size_t ws_bytes,
+                       void* stream, float* grad_edge_attr) {
   NNC_REQUIRE(plan && w && x && grad_out && grad_x && grad_W && grad_b, NNCONV_ERR_ARG, "null pointer");
   NNC_REQUIRE(aggr == NNCONV_AGGR_ADD || aggr == NNCONV_AGGR_MEAN, NNCONV_ERR_UNSUPPORTED, "aggr must be add or mean");
   NNC_REQUIRE((root == nullptr) == (grad_root == nullptr), NNCONV_ERR_ARG, "root / grad_root must both be given or both be NULL");
+  NNC_REQUIRE(grad_edge_attr == nullptr || edge_attr != nullptr || plan->p.E == 0, NNCONV_ERR_ARG,
+              "grad_edge_attr needs edge_attr");
   return backward_fp32(&plan->p, &w->w, edge_attr, x, root, aggr == NNCONV_AGGR_MEAN, grad_out, grad_x, grad_W,
-                       grad_b, grad_root, grad_bias, ws, ws_bytes, static_cast<cudaStream_t>(stream));
+                       grad_b, grad_root, grad_bias, ws, ws_bytes, static_cast<cudaStream_t>(stream), grad_edge_attr);
 }
 
 int nnconv_backward_tc_supported(const nnconv_weights_t* w) { return w && backward_tc_supported(&w->w) ? 1 : 0; }
@@ -832,11 +842,19 @@ int nnconv_backward_mlp_sizes(const nnconv_plan_t* plan, const nnconv_weights_t*
 int nnconv_backward_mlp(const nnconv_plan_t* plan, const nnconv_weights_t* w, const float* edge_attr, const void* h,
                         int n_apps, const float* const* grad_out, const float* const* x, int aggr, float* const* grad_W,
                         float* const* grad_b, void* ws, size_t ws_bytes, void* stream, const void* acts) {
+  return nnconv_backward_mlp_ex(plan, w, edge_attr, h, n_apps, grad_out, x, aggr, grad_W, grad_b, ws, ws_bytes, stream, acts,
+                                nullptr);
+}
+
+int nnconv_backward_mlp_ex(const nnconv_plan_t* plan, const nnconv_weights_t* w, const float* edge_attr, const void* h,
+                           int n_apps, const float* const* grad_out, const float* const* x, int aggr, float* const* grad_W,
+                           float* const* grad_b, void* ws, size_t ws_bytes, void* stream, const void* acts,
+                           float* grad_edge_attr) {
   NNC_REQUIRE(plan && w && grad_out && x && grad_W && grad_b && ((edge_attr && h) || plan->p.E == 0), NNCONV_ERR_ARG,
               "null pointer");
   NNC_REQUIRE(aggr == NNCONV_AGGR_ADD || aggr == NNCONV_AGGR_MEAN, NNCONV_ERR_UNSUPPORTED, "aggr must be add or mean");
   return backward_mlp_tc(&plan->p, &w->w, edge_attr, h, n_apps, grad_out, x, aggr == NNCONV_AGGR_MEAN, grad_W, grad_b, ws,
-                         ws_bytes, static_cast<cudaStream_t>(stream), acts);
+                         ws_bytes, static_cast<cudaStream_t>(stream), acts, grad_edge_attr);
 }
 
 int nnconv_gemm_tn_16b(int precision, const void* A, int64_t lda, const void* B, int64_t ldb, int64_t R, int M, int N,

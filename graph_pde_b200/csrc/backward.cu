@@ -9,7 +9,8 @@
 //   dY_c[o,k] = sum_{e in c} G_e[o] h_e[k]                   Gs_c = sum_{e in c} G_e
 //   dW_L[i*out+o, k] = sum_c x_c[i] dY_c[o,k]                db_L.view(in,out) = sum_c x_c (x) Gs_c
 //   dx_c += dY_c : W_L  +  B_L Gs_c
-//   dh_e[k] = sum_o G_e[o] Y_c[o,k]        then the usual MLP backward through ReLU for layers L-1 .. 1.
+//   dh_e[k] = sum_o G_e[o] Y_c[o,k]        then the usual MLP backward through ReLU for layers L-1 .. 1,
+//   d ea_e  = dz_1[e, :] . W_1             (on request; dh_e[:k_in] for a single-Linear edge network).
 // Sources are processed in batches (contiguous sorted edges) so that activations are recomputed and freed
 // batch by batch; parameter gradients accumulate across batches.
 #include "kernels.h"
@@ -166,6 +167,21 @@ __global__ void k_gather_ea(const float* __restrict__ edge_attr, const int* __re
   out[i] = edge_attr[src * k_in + c];
 }
 
+// grad_edge_attr[perm[e0 + p], i] = sum_{j < kw} dz[p, j] W1[j, i]      (W1 == nullptr: identity features, dz[p, i])
+__global__ void k_ea_grad_fp32(const float* __restrict__ dz, int ne, int ld, const float* __restrict__ W1, int kw,
+                               int k_in, const int* __restrict__ perm, int e0, float* __restrict__ out) {
+  int64_t idx = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
+  if (idx >= static_cast<int64_t>(ne) * k_in) return;
+  const int p = static_cast<int>(idx / k_in), i = static_cast<int>(idx % k_in);
+  const float* row = dz + static_cast<int64_t>(p) * ld;
+  float acc = 0.f;
+  if (W1 == nullptr) acc = row[i];
+  else
+    for (int j = 0; j < kw; ++j) acc = fmaf(row[j], W1[static_cast<int64_t>(j) * k_in + i], acc);
+  const int64_t e = static_cast<int64_t>(e0) + p;
+  out[(perm ? perm[e] : e) * k_in + i] = acc;
+}
+
 // dx[src_nodes[c0 + c], i] += dXc[c, i]
 __global__ void k_scatter_dx(const float* __restrict__ dXc, const int* __restrict__ src_nodes, int c0, int nb, int cin,
                              int cin_p, float* __restrict__ dx) {
@@ -257,7 +273,7 @@ size_t backward_ws_bytes(const Plan* P, const Weights* W, size_t want_bytes) {
 
 int backward_fp32(const Plan* P, const Weights* W, const float* edge_attr, const float* x, const float* root,
                   int aggr_mean, const float* gout, float* dx, float* const* dWs, float* const* dbs, float* droot,
-                  float* dbias, void* ws, size_t ws_bytes, cudaStream_t st) {
+                  float* dbias, void* ws, size_t ws_bytes, cudaStream_t st, float* grad_ea) {
   NNC_REQUIRE(W->prec == PREC_FP32, NNCONV_ERR_ARG, "backward needs weights prepared with precision fp32");
   const int nl = W->n_layers;
   const int cin = W->cin, cout = W->cout, Kp = W->Kp, cin_p = W->cin_p;
@@ -370,8 +386,9 @@ int backward_fp32(const Plan* P, const Weights* W, const float* edge_attr, const
       k_scatter_dx<<<(unsigned)ceil_div64(static_cast<int64_t>(nb) * cin, TB), TB, 0, st>>>(dXc, P->src_nodes, c0, nb, cin,
                                                                                           cin_p, dx);
       NNC_CHECK_LAUNCH();
-      if (nl >= 2) {
-        // ---- dh = G_c Y_c (grouped, rows = edges of the group)
+      if (nl >= 2 || grad_ea != nullptr) {
+        // ---- dh = G_c Y_c (grouped, rows = edges of the group); with a single Linear (identity features) the
+        // gradient w.r.t. edge_attr is its first k_in columns
         {
           AnyGemm g{};
           g.A = G; g.sa_m = cout; g.sa_k = 1; g.B = Y; g.sb_k = Kp; g.sb_n = 1; g.C = dhA; g.ldc = Kp;
@@ -382,9 +399,11 @@ int backward_fp32(const Plan* P, const Weights* W, const float* edge_attr, const
           NNC_CHECK_LAUNCH();
         }
         // ---- MLP backward through the hidden layers
-        k_gather_ea<<<(unsigned)ceil_div64(static_cast<int64_t>(ne) * W->kp[0], TB), TB, 0, st>>>(
-            edge_attr, P->perm, e0, ne, W->kp[0], ea);
-        NNC_CHECK_LAUNCH();
+        if (nl >= 2) {
+          k_gather_ea<<<(unsigned)ceil_div64(static_cast<int64_t>(ne) * W->kp[0], TB), TB, 0, st>>>(
+              edge_attr, P->perm, e0, ne, W->kp[0], ea);
+          NNC_CHECK_LAUNCH();
+        }
         float* cur = dhA;
         float* nxt = dhB;
         for (int l = nl - 1; l >= 1; --l) {
@@ -403,6 +422,13 @@ int backward_fp32(const Plan* P, const Weights* W, const float* edge_attr, const
             if (s) return s;
             float* t = cur; cur = nxt; nxt = t;
           }
+        }
+        // ---- cur = dz_1 (masked, [ne, kp1]) or, for a single Linear, dh ([ne, Kp]): edge_attr rows of the batch
+        if (grad_ea != nullptr) {
+          k_ea_grad_fp32<<<(unsigned)ceil_div64(static_cast<int64_t>(ne) * W->dims[0], TB), TB, 0, st>>>(
+              cur, ne, nl >= 2 ? W->kp[1] : Kp, nl >= 2 ? W->W1 : nullptr, nl >= 2 ? W->dims[1] : 0, W->dims[0], P->perm,
+              e0, grad_ea);
+          NNC_CHECK_LAUNCH();
         }
       }
       c0 = c1;

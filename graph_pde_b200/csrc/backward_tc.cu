@@ -16,12 +16,15 @@
 //   followed by ONE backward pass through the hidden layers (k_gemm_tc with the ReLU-mask epilogue for
 //   dz_{l-1} = (dz_l W_l) * [h_{l-1} > 0]; k_gemm_tn for dW_l = dz_l^T h_{l-1} and, against the split-precision
 //   first-layer image A1, for db_l and dW_1).  The reference pays that pass T times.
+//   On request the same pass also yields the gradient w.r.t. edge_attr, d ea_e = dz_1[e, :] . W_1 (k_ea_grad, one
+//   read of dz_1 per batch, rows scattered back to the caller's edge order).
 //
 // 16-bit range: gradients are normalised by powers of two computed on the device (no host sync): G by the
 // largest |G| of the application(s), x by its largest magnitude; the fp32 epilogues multiply the scales back.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
+#include <algorithm>
 #include <type_traits>
 
 #include "kernels.h"
@@ -586,6 +589,95 @@ k_dh(const __grid_constant__ Maps8 tmA, const __grid_constant__ CUtensorMap tmB,
   }
 }
 
+// =====================================================================================================
+// k_ea_grad: grad_edge_attr[perm[e_base + r], i] = s * sum_j dz_1[r, j] W_1[j, i]   for the rows r < n of a batch
+//   (edge_attr enters the op only through the first Linear).  dz_1 is 16-bit [n, kp1] row-major, scaled by 1 / s like
+//   every gradient of the pass, and read once; W_1 (fp32 [kp1, k_in], zero rows past k_1) sits transposed in shared
+//   memory.  Eight lanes share a row (64 consecutive columns per step, 16-byte loads), each lane carries kEaRows rows,
+//   so a warp covers 4 * kEaRows rows and a row's sum needs three shuffles.  Padding rows [n, n_pad) are never read.
+// =====================================================================================================
+constexpr int kEaRows = 2;
+constexpr int kEaRowsPerBlock = 8 * 4 * kEaRows;   // 256 threads
+
+template <int FMT>
+__device__ __forceinline__ void unpack8(const uint4 u, float* v) {
+  const uint32_t w[4] = {u.x, u.y, u.z, u.w};
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    float2 f;
+    if (FMT == 0) f = __half22float2(*reinterpret_cast<const __half2*>(&w[k]));
+    else f = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&w[k]));
+    v[2 * k] = f.x;
+    v[2 * k + 1] = f.y;
+  }
+}
+
+template <int FMT, int KMAX>
+__global__ void __launch_bounds__(256) k_ea_grad(const uint16_t* __restrict__ dz, int n, int kp1,
+                                                 const float* __restrict__ W1, int k_in, const int* __restrict__ perm,
+                                                 int e_base, const float* __restrict__ scal, int scal_idx,
+                                                 float* __restrict__ out) {
+  extern __shared__ __align__(16) float sw[];     // [k_in][kp1]: sw[i * kp1 + j] = W1[j, i]
+  for (int t = threadIdx.x; t < k_in * kp1; t += blockDim.x) sw[(t % k_in) * kp1 + t / k_in] = W1[t];
+  __syncthreads();
+  const float s = scal[scal_idx];
+  const int lane = threadIdx.x & 31, grp = lane >> 3, q = lane & 7;
+  const int64_t warp = (static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
+  const int64_t n_warps = (static_cast<int64_t>(gridDim.x) * blockDim.x) >> 5;
+  for (int64_t r0 = warp * 4 * kEaRows; r0 < n; r0 += n_warps * 4 * kEaRows) {
+    int64_t row[kEaRows];
+    float acc[kEaRows][KMAX];
+#pragma unroll
+    for (int rr = 0; rr < kEaRows; ++rr) {
+      row[rr] = r0 + grp * kEaRows + rr;
+#pragma unroll
+      for (int i = 0; i < KMAX; ++i) acc[rr][i] = 0.f;
+    }
+    for (int j0 = q * 8; j0 < kp1; j0 += 64) {
+      float v[kEaRows][8];
+#pragma unroll
+      for (int rr = 0; rr < kEaRows; ++rr) {
+        uint4 u = make_uint4(0u, 0u, 0u, 0u);
+        if (row[rr] < n) u = __ldcs(reinterpret_cast<const uint4*>(dz + row[rr] * kp1 + j0));
+        unpack8<FMT>(u, v[rr]);
+      }
+#pragma unroll
+      for (int i = 0; i < KMAX; ++i) {
+        if (i >= k_in) break;
+        const float4 w0 = *reinterpret_cast<const float4*>(sw + i * kp1 + j0);
+        const float4 w1 = *reinterpret_cast<const float4*>(sw + i * kp1 + j0 + 4);
+#pragma unroll
+        for (int rr = 0; rr < kEaRows; ++rr) {
+          float a = acc[rr][i];
+          a = fmaf(v[rr][0], w0.x, a); a = fmaf(v[rr][1], w0.y, a); a = fmaf(v[rr][2], w0.z, a);
+          a = fmaf(v[rr][3], w0.w, a); a = fmaf(v[rr][4], w1.x, a); a = fmaf(v[rr][5], w1.y, a);
+          a = fmaf(v[rr][6], w1.z, a); a = fmaf(v[rr][7], w1.w, a);
+          acc[rr][i] = a;
+        }
+      }
+    }
+#pragma unroll
+    for (int rr = 0; rr < kEaRows; ++rr) {
+#pragma unroll
+      for (int i = 0; i < KMAX; ++i) {
+        if (i >= k_in) break;
+        float a = acc[rr][i];
+        a += __shfl_xor_sync(0xffffffffu, a, 4);
+        a += __shfl_xor_sync(0xffffffffu, a, 2);
+        a += __shfl_xor_sync(0xffffffffu, a, 1);
+        acc[rr][i] = a;
+      }
+      if (row[rr] < n) {
+        const int64_t e = e_base + row[rr];
+        const int64_t dst = perm ? perm[e] : e;
+#pragma unroll
+        for (int i = 0; i < KMAX; ++i)
+          if (i < k_in && (i & 7) == q) out[dst * k_in + i] = acc[rr][i] * s;
+      }
+    }
+  }
+}
+
 }  // namespace
 
 // =====================================================================================================
@@ -798,7 +890,7 @@ size_t backward_mlp_ws_bytes(const Plan* P, const Weights* W, int T, size_t want
 
 int backward_mlp_tc(const Plan* P, const Weights* W, const float* edge_attr, const void* h, int T,
                     const float* const* gouts, const float* const* xs_in, int aggr_mean, float* const* dWs,
-                    float* const* dbs, void* ws, size_t ws_bytes, cudaStream_t st, const void* acts) {
+                    float* const* dbs, void* ws, size_t ws_bytes, cudaStream_t st, const void* acts, float* grad_ea) {
   NNC_REQUIRE(backward_tc_supported(W), NNCONV_ERR_UNSUPPORTED, "tensor-core backward: unsupported shape / precision");
   if (acts != nullptr && edge_acts_bytes(P, W) == 0) acts = nullptr;
   NNC_REQUIRE(T >= 1 && T <= kMaxApps, NNCONV_ERR_ARG, "backward_mlp: 1..%d applications per pass", kMaxApps);
@@ -807,6 +899,10 @@ int backward_mlp_tc(const Plan* P, const Weights* W, const float* edge_attr, con
   const int bf = W->prec == PREC_BF16;
   int s = tc_init();
   if (s) return s;
+  // gradient w.r.t. edge_attr: W_1 transposed in shared memory (k_in <= 20 on this path)
+  const int ea_smem = static_cast<int>(sizeof(float)) * k_in * W->kp[1];
+  NNC_REQUIRE(grad_ea == nullptr || (k_in <= 20 && ea_smem <= 227 * 1024), NNCONV_ERR_UNSUPPORTED,
+              "backward_mlp: edge_attr gradient needs k_in * k_1 <= 58112 (first Linear in shared memory)");
   // zero gradients for an empty graph
   if (P->E == 0 || P->n_src == 0) {
     for (int l = 1; l <= nl - 1; ++l) {
@@ -855,6 +951,10 @@ int backward_mlp_tc(const Plan* P, const Weights* W, const float* edge_attr, con
     NNC_CHECK_CUDA(cudaFuncSetAttribute(k_dh<1, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     NNC_CHECK_CUDA(cudaFuncSetAttribute(k_dh<0, 128>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     NNC_CHECK_CUDA(cudaFuncSetAttribute(k_dh<1, 128>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    NNC_CHECK_CUDA(cudaFuncSetAttribute(k_ea_grad<0, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    NNC_CHECK_CUDA(cudaFuncSetAttribute(k_ea_grad<1, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    NNC_CHECK_CUDA(cudaFuncSetAttribute(k_ea_grad<0, 20>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    NNC_CHECK_CUDA(cudaFuncSetAttribute(k_ea_grad<1, 20>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     attr_set = true;
   }
   int dh_smem = T * kDhAChunk + kDhBStages * BN * 128 + 1024 + kDhScratch;
@@ -969,6 +1069,17 @@ int backward_mlp_tc(const Plan* P, const Weights* W, const float* edge_attr, con
         if (s) return s;
         uint16_t* tmp = cur; cur = nxt; nxt = tmp;
       }
+    }
+    // ---- cur = dz_1 of the batch (summed over the applications): grad_edge_attr rows of its edges
+    if (grad_ea != nullptr) {
+      auto kern = k_in <= 8 ? (bf ? k_ea_grad<1, 8> : k_ea_grad<0, 8>) : (bf ? k_ea_grad<1, 20> : k_ea_grad<0, 20>);
+      // as many resident CTAs as fit (a bandwidth-bound stream: every resident warp keeps loads in flight)
+      int per_sm = 0;
+      NNC_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, 256, ea_smem));
+      const int64_t resident = static_cast<int64_t>(per_sm > 0 ? per_sm : 1) * tc_num_sms();
+      const unsigned grid = static_cast<unsigned>(std::min<int64_t>(ceil_div64(n, kEaRowsPerBlock), resident));
+      kern<<<grid, 256, ea_smem, st>>>(cur, n, W->kp[1], W->W1, k_in, P->perm, e_base, scal, 16, grad_ea);
+      NNC_CHECK_LAUNCH();
     }
     c0 = c1;
   }

@@ -93,7 +93,8 @@ int apply(const Plan* P, const Weights* W, const void* h, const float* x, const 
           unsigned node_flags = 0);
 
 // tensor-core backward (backward_tc.cu): per application (dx, dW_L, db_L, droot, dbias) and, once per
-// (edge_attr, parameters) for all T applications of a shared conv, the pass through the hidden layers
+// (edge_attr, parameters) for all T applications of a shared conv, the pass through the hidden layers.
+// grad_ea (nullable): [E, k_in] fp32 in the caller's edge order, WRITTEN -- the gradient w.r.t. edge_attr.
 bool backward_tc_supported(const Weights* W);
 size_t backward_apply_ws_bytes(const Plan* P, const Weights* W, size_t want_bytes);
 int backward_apply_tc(const Plan* P, const Weights* W, const void* h, const float* x, const float* root,
@@ -102,7 +103,8 @@ int backward_apply_tc(const Plan* P, const Weights* W, const void* h, const floa
 size_t backward_mlp_ws_bytes(const Plan* P, const Weights* W, int T, size_t want_bytes);
 int backward_mlp_tc(const Plan* P, const Weights* W, const float* edge_attr, const void* h, int T,
                     const float* const* gouts, const float* const* xs_in, int aggr_mean, float* const* dWs,
-                    float* const* dbs, void* ws, size_t ws_bytes, cudaStream_t st, const void* acts = nullptr);
+                    float* const* dbs, void* ws, size_t ws_bytes, cudaStream_t st, const void* acts = nullptr,
+                    float* grad_ea = nullptr);
 
 // per-edge kernel matrices for low out-degree graphs (formulation B): Kmat [E, cin*cout] 16-bit in sorted edge order
 size_t edge_kernels_bytes(const Plan* P, const Weights* W);
@@ -111,10 +113,10 @@ int edge_kernels(const Plan* P, const Weights* W, const void* h, void* Kmat, cud
 int apply_edge(const Plan* P, const Weights* W, const void* Kmat, const float* x, const float* root, const float* bias,
                int aggr_mean, float* out, cudaStream_t st, unsigned node_flags = 0);
 
-// backward of one application (fp32 CUDA-core path), backward.cu
+// backward of one application (fp32 CUDA-core path), backward.cu; grad_ea as for backward_mlp_tc
 size_t backward_ws_bytes(const Plan* P, const Weights* W, size_t want_bytes);
 int backward_fp32(const Plan* P, const Weights* W, const float* edge_attr, const float* x, const float* root,
                   int aggr_mean, const float* gout, float* dx, float* const* dWs, float* const* dbs, float* droot,
-                  float* dbias, void* ws, size_t ws_bytes, cudaStream_t st);
+                  float* dbias, void* ws, size_t ws_bytes, cudaStream_t st, float* grad_ea = nullptr);
 
 }  // namespace nnc

@@ -120,7 +120,8 @@ class KernelInduced(_VCycleBase):
         ei_m, ea_m = data.edge_index_mid, data.edge_attr_mid
         ei_u, ea_u = data.edge_index_up, data.edge_attr_up
         x = self.fc_in(data.x)
-        needs_grad = torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for p in self.parameters()))
+        needs_grad = torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for p in self.parameters()) or
+                                                   any(t.requires_grad for t in (ea_d, ea_m, ea_u)))
         if _FUSED_STEPS and not needs_grad:
             # inference: the 13 * depth dependent steps  x <- relu(x + conv(x))  chained on pre-activations, ReLU and
             # residual inside each application's node-prep launch (NNConv_old.residual_step) -- 2 launches per step

@@ -196,9 +196,8 @@ class _Prepared(object):
 
 class _NNConvFunction(torch.autograd.Function):
     """Differentiable wrapper, CUDA-core variant: forward = the configured precision path, backward =
-    nnconv_backward (fp32 CUDA-core kernels, csrc/backward.cu; any shape, activations recomputed).  Gradients flow
-    to x, the edge-MLP Linear weights/biases, root and bias; edge_index / edge_attr are leaf inputs in every
-    reference script and get none."""
+    nnconv_backward_ex (fp32 CUDA-core kernels, csrc/backward.cu; any shape, activations recomputed).  Gradients flow
+    to x, edge_attr, the edge-MLP Linear weights/biases, root and bias; edge_index gets none."""
 
     @staticmethod
     def forward(ctx, module, x, edge_index, edge_attr, *params):
@@ -211,10 +210,10 @@ class _NNConvFunction(torch.autograd.Function):
     def backward(ctx, grad_out):
         module = ctx.module
         x, edge_attr = ctx.saved_tensors
-        grads = module._backward_impl(x, ctx.edge_index, edge_attr, grad_out)
+        grads = module._backward_impl(x, ctx.edge_index, edge_attr, grad_out, want_ea=ctx.needs_input_grad[3])
         # order of *params in forward(): list(module.parameters())
         by_id = {id(p): g for p, g in grads['params']}
-        return (None, grads['x'] if ctx.needs_input_grad[1] else None, None, None) + tuple(
+        return (None, grads['x'] if ctx.needs_input_grad[1] else None, None, grads.get('edge_attr')) + tuple(
             by_id.get(id(p)) for p in module.parameters())
 
 
@@ -235,21 +234,23 @@ class _EdgeFeaturesFn(torch.autograd.Function):
     """Autograd node of the x-independent part h = MLP_without_last_Linear(edge_attr).  Its output is a 1-element
     token (h itself lives in the module's cache: 2 KB per edge): every application's backward returns a dummy
     gradient for the token, so autograd runs THIS backward exactly once, after all of them -- with every
-    (grad_out, x) pair collected in the state, the hidden layers are differentiated once for all T applications."""
+    (grad_out, x) pair collected in the state, the hidden layers are differentiated once for all T applications.
+    edge_attr is an input so that its gradient (summed over the applications) comes out of the same pass."""
 
     @staticmethod
-    def forward(ctx, module, state, *hidden_params):
+    def forward(ctx, module, state, edge_attr, *hidden_params):
         ctx.module, ctx.state = module, state
+        ctx.ea_dtype = edge_attr.dtype
         return torch.zeros(1, device=state.h.device)
 
     @staticmethod
     def backward(ctx, _):
         state = ctx.state
-        grads = ctx.module._backward_mlp_impl(state)
+        grads, gea = ctx.module._backward_mlp_impl(state, want_ea=ctx.needs_input_grad[2])
         state.consumed = True
         state.apps = []
         state.h = state.ea32 = state.acts = None     # the per-edge buffers are no longer pinned by this (finished) graph
-        return (None, None) + tuple(grads)
+        return (None, None, gea.to(ctx.ea_dtype) if gea is not None else None) + tuple(grads)
 
 
 class _ApplyFn(torch.autograd.Function):
@@ -339,7 +340,7 @@ class NNConv_old(torch.nn.Module):
         x = x.unsqueeze(-1) if x.dim() == 1 else x
         pseudo = edge_attr.unsqueeze(-1) if edge_attr.dim() == 1 else edge_attr
         needs_grad = torch.is_grad_enabled() and (
-            x.requires_grad or any(p.requires_grad for p in self.parameters()))
+            x.requires_grad or pseudo.requires_grad or any(p.requires_grad for p in self.parameters()))
         if needs_grad:
             if self.aggr == 'max':
                 raise NotImplementedError("aggr='max' is used by no call site of the reference and is not built")
@@ -522,7 +523,8 @@ class NNConv_old(torch.nn.Module):
         has no elementwise kernels between its applications."""
         if self.in_channels != self.out_channels:
             raise ValueError('residual_step needs in_channels == out_channels')
-        if torch.is_grad_enabled() and (z.requires_grad or any(p.requires_grad for p in self.parameters())):
+        if torch.is_grad_enabled() and (z.requires_grad or edge_attr.requires_grad or
+                                        any(p.requires_grad for p in self.parameters())):
             raise RuntimeError('residual_step is a forward-only path: call it under torch.no_grad()')
         if self.aggr == 'max':
             raise NotImplementedError("aggr='max' is used by no call site of the reference and is not built")
@@ -535,7 +537,7 @@ class NNConv_old(torch.nn.Module):
         """State shared by the applications of this conv on (edge_attr, parameters), or None when the tensor-core
         backward does not cover the configuration (the fp32 CUDA-core backward is used then)."""
         mode = _BWD_MODE
-        if mode == 'fp32' or pseudo.requires_grad:
+        if mode == 'fp32':
             return None
         self._check_inputs(x, edge_index, pseudo)
         with torch.cuda.device(x.device):
@@ -544,7 +546,9 @@ class NNConv_old(torch.nn.Module):
                 if mode == 'tc':
                     raise NotImplementedError('NNCONV_B200_BACKWARD=tc: shape / precision not covered by the tensor-core backward')
                 return None
-            key = (plan.key, ea32.data_ptr(), tuple(ea32.shape), ea32._version, id(prepared))
+            # requires_grad is part of the key: a state whose token is not connected to edge_attr cannot serve an
+            # application that must deliver its gradient
+            key = (plan.key, ea32.data_ptr(), tuple(ea32.shape), ea32._version, id(prepared), pseudo.requires_grad)
             st = getattr(self, '_tstate', None)
             if st is None or st.key != key or st.consumed or st.h is not h:
                 st = _TrainState(key, plan, prepared, h, ea32)
@@ -552,7 +556,7 @@ class NNConv_old(torch.nn.Module):
                 hidden = []
                 for l in _linear_chain(self.nn)[:-1]:
                     hidden += [l.weight, l.bias]
-                st.token = _EdgeFeaturesFn.apply(self, st, *hidden)
+                st.token = _EdgeFeaturesFn.apply(self, st, pseudo, *hidden)
                 self._tstate = st
             return st
 
@@ -577,14 +581,16 @@ class NNConv_old(torch.nn.Module):
             stats['backwards'] = stats.get('backwards', 0) + 1
         return dx, dwl, dbl, droot, dbias
 
-    def _backward_mlp_impl(self, state):
+    def _backward_mlp_impl(self, state, want_ea=False):
         """Gradients of the hidden Linear layers, one pass for all applications recorded in the state (in groups
-        of <= 6 when a conv is applied more often)."""
+        of <= 6 when a conv is applied more often), and with ``want_ea`` the fp32 gradient w.r.t. edge_attr
+        ([E, k_in], summed over the groups; else None)."""
         L = _lib.lib()
         plan, prep = state.plan, state.prepared
         hidden = _linear_chain(self.nn)[:-1]
         dev = state.h.device
         total = None
+        gea_total = None
         with torch.cuda.device(dev):
             for i0 in range(0, len(state.apps), 6):
                 apps = state.apps[i0:i0 + 6]
@@ -594,23 +600,28 @@ class NNConv_old(torch.nn.Module):
                 ws = torch.empty(ws_b.value, dtype=torch.uint8, device=dev)
                 dws = [torch.empty_like(l.weight, dtype=torch.float32) for l in hidden]
                 dbs = [torch.empty_like(l.bias, dtype=torch.float32) for l in hidden]
+                gea = torch.empty(state.ea32.shape, dtype=torch.float32, device=dev) if want_ea else None
                 gp = (ctypes.c_void_p * n)(*[g.data_ptr() for g, _ in apps])
                 xp = (ctypes.c_void_p * n)(*[x.data_ptr() for _, x in apps])
                 wp = (ctypes.c_void_p * len(hidden))(*[t.data_ptr() for t in dws])
                 bp = (ctypes.c_void_p * len(hidden))(*[t.data_ptr() for t in dbs])
-                _lib.check(L.nnconv_backward_mlp(plan.handle, prep.handle, _ptr(state.ea32), _ptr(state.h), n, gp, xp,
-                                                 _lib.AGGR[self.aggr], wp, bp, _ptr(ws), ws_b.value, _stream_ptr(dev),
-                                                 _ptr(getattr(state, 'acts', None))))
+                _lib.check(L.nnconv_backward_mlp_ex(plan.handle, prep.handle, _ptr(state.ea32), _ptr(state.h), n, gp, xp,
+                                                    _lib.AGGR[self.aggr], wp, bp, _ptr(ws), ws_b.value, _stream_ptr(dev),
+                                                    _ptr(getattr(state, 'acts', None)), _ptr(gea)))
                 flat = [t for pair in zip(dws, dbs) for t in pair]
                 total = flat if total is None else [a + b for a, b in zip(total, flat)]
+                if gea is not None:
+                    gea_total = gea if gea_total is None else gea_total + gea
             stats['mlp_backwards'] = stats.get('mlp_backwards', 0) + 1
         if total is None:     # no application contributed (cannot happen through autograd, kept for safety)
             total = [torch.zeros_like(p, dtype=torch.float32) for l in hidden for p in (l.weight, l.bias)]
-        return total
+            if want_ea:
+                gea_total = torch.zeros(state.ea32.shape, dtype=torch.float32, device=dev)
+        return total, gea_total
 
-    def _backward_impl(self, x, edge_index, pseudo, grad_out):
-        if pseudo.requires_grad:
-            raise NotImplementedError('gradients w.r.t. edge_attr are not built (leaf input in the reference)')
+    def _backward_impl(self, x, edge_index, pseudo, grad_out, want_ea=False):
+        """fp32 CUDA-core backward of one application; with ``want_ea`` also the gradient w.r.t. edge_attr
+        (returned under 'edge_attr' in pseudo's dtype)."""
         L = _lib.lib()
         with torch.cuda.device(x.device):
             x32 = x.detach().contiguous().float()
@@ -637,16 +648,20 @@ class NNConv_old(torch.nn.Module):
             wp = (ctypes.c_void_p * nl)(*[t.data_ptr() for t in dws])
             bp = (ctypes.c_void_p * nl)(*[t.data_ptr() for t in dbs])
             root = self.root.detach().contiguous().float() if self.root is not None else None
-            _lib.check(L.nnconv_backward(plan.handle, prep.handle, _ptr(ea32), _ptr(x32), _ptr(root),
-                                         _lib.AGGR[self.aggr], _ptr(g32), _ptr(dx), wp, bp, _ptr(droot), _ptr(dbias),
-                                         _ptr(ws), ws_b.value, _stream_ptr(x.device)))
+            gea = torch.empty_like(ea32) if want_ea else None
+            _lib.check(L.nnconv_backward_ex(plan.handle, prep.handle, _ptr(ea32), _ptr(x32), _ptr(root),
+                                            _lib.AGGR[self.aggr], _ptr(g32), _ptr(dx), wp, bp, _ptr(droot), _ptr(dbias),
+                                            _ptr(ws), ws_b.value, _stream_ptr(x.device), _ptr(gea)))
             stats['backwards'] = stats.get('backwards', 0) + 1
         params = [(l.weight, dw) for l, dw in zip(linears, dws)] + [(l.bias, db) for l, db in zip(linears, dbs)]
         if self.root is not None:
             params.append((self.root, droot))
         if self.bias is not None:
             params.append((self.bias, dbias))
-        return {'x': dx.to(x.dtype), 'params': params}
+        grads = {'x': dx.to(x.dtype), 'params': params}
+        if gea is not None:
+            grads['edge_attr'] = gea.to(pseudo.dtype)
+        return grads
 
 
 class NNConv(NNConv_old):

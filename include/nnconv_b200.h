@@ -157,13 +157,21 @@ int nnconv_apply_ex(const nnconv_plan_t* plan, const nnconv_weights_t* w, const 
 /* ---- backward of one application (what autograd generates for nn_conv.py:267-282 + utilities.py:223-227):
  * grad_x [N,in], grad_W[l] / grad_b[l] in the torch.nn.Linear layouts of the edge MLP, grad_root [in,out],
  * grad_bias [out] (NULL when the module has no root / bias).  fp32 CUDA-core path for arbitrary shapes: `w`
- * must have been created with NNCONV_PREC_FP32.  Gradients are WRITTEN (not accumulated). edge_attr and
- * edge_index receive no gradient (they are leaf inputs in every reference script). ------------------------- */
+ * must have been created with NNCONV_PREC_FP32.  Gradients are WRITTEN (not accumulated).  edge_index receives no
+ * gradient; edge_attr receives one through nnconv_backward_ex. ------------------------------------------------- */
 int nnconv_backward_sizes(const nnconv_plan_t* plan, const nnconv_weights_t* w, size_t want_bytes, size_t* ws_bytes);
 int nnconv_backward(const nnconv_plan_t* plan, const nnconv_weights_t* w, const float* edge_attr, const float* x,
                     const float* root, int aggr, const float* grad_out, float* grad_x, float* const* grad_W,
                     float* const* grad_b, float* grad_root, float* grad_bias, void* ws, size_t ws_bytes,
                     void* stream);
+/* nnconv_backward plus the gradient w.r.t. edge_attr: grad_edge_attr [E, k_in] fp32 in the caller's edge order,
+ * WRITTEN (d edge_attr_e = dz_1[e] . W_1, dz_1 = gradient at the first hidden pre-activation; for a single-Linear
+ * edge network the gradient w.r.t. the identity features).  NULL = exactly nnconv_backward: no extra launch, and the
+ * workspace of nnconv_backward_sizes serves both. */
+int nnconv_backward_ex(const nnconv_plan_t* plan, const nnconv_weights_t* w, const float* edge_attr, const float* x,
+                       const float* root, int aggr, const float* grad_out, float* grad_x, float* const* grad_W,
+                       float* const* grad_b, float* grad_root, float* grad_bias, void* ws, size_t ws_bytes,
+                       void* stream, float* grad_edge_attr /* nullable */);
 
 /* ---- tensor-core backward (16-bit precisions, out_channels = 64, in_channels <= 64, edge MLP with >= 2 Linear
  * layers; nnconv_backward_tc_supported tells).  Split in two because the edge features h do not depend on x:
@@ -188,6 +196,15 @@ int nnconv_backward_mlp(const nnconv_plan_t* plan, const nnconv_weights_t* w, co
                         int n_apps, const float* const* grad_out, const float* const* x, int aggr, float* const* grad_W,
                         float* const* grad_b, void* ws, size_t ws_bytes, void* stream,
                         const void* acts /* from nnconv_edge_features_keep, or NULL = recompute */);
+/* nnconv_backward_mlp plus the gradient w.r.t. edge_attr, summed over the n_apps applications: grad_edge_attr
+ * [E, k_in] fp32 in the caller's edge order, WRITTEN (one extra pass per source batch that reads the 16-bit dz_1 once;
+ * no host sync).  A conv applied more often than one call takes gets one call per group of applications, and the
+ * caller sums the groups, as for grad_W / grad_b.  NULL = exactly nnconv_backward_mlp: no extra launch, and the
+ * workspace of nnconv_backward_mlp_sizes serves both. */
+int nnconv_backward_mlp_ex(const nnconv_plan_t* plan, const nnconv_weights_t* w, const float* edge_attr, const void* h,
+                           int n_apps, const float* const* grad_out, const float* const* x, int aggr,
+                           float* const* grad_W, float* const* grad_b, void* ws, size_t ws_bytes, void* stream,
+                           const void* acts, float* grad_edge_attr /* nullable */);
 
 /* ---- halo exchange of the node-range (strip) partition by peer stores over NVLink (no NCCL call, no host round
  * trip between applications).  `out` [n_local, channels] is the result of one application on this rank (owned rows

@@ -4,8 +4,16 @@ cudaProfilerStart/Stop so that `ncu --profile-from-start off` sees exactly one s
 
     ncu --metrics gpu__time_duration.sum --clock-control none --profile-from-start off --csv \
         --log-file gpurun_out/train_launches.csv python scripts/train_probe.py [darcy241|darcy85]
-Without ncu it prints the CUDA-event time of the step."""
+Without ncu it prints the CUDA-event time of the step.
+
+    python scripts/train_probe.py [darcy241|darcy85] --edge-attr-grad [--rounds N]
+times the same step with edge_attr built from a coefficient field theta by graphs.ball_edge_attr, once with theta a
+plain tensor and once with theta a leaf that requires grad (so that the step also delivers d loss / d edge_attr and
+d loss / d theta), alternating the two in one run, and prints both median step times, the device and its power limit."""
+import argparse
 import os
+import statistics
+import subprocess
 import sys
 
 import torch
@@ -17,8 +25,35 @@ from graph_pde_b200 import graphs  # noqa: E402
 from graph_pde_b200.models import KernelNN  # noqa: E402
 
 
+class _Data(object):
+    pass
+
+
+def _power_limit():
+    try:
+        res = subprocess.run(['nvidia-smi', '--query-gpu=power.limit', '--format=csv,noheader'], stdout=subprocess.PIPE,
+                             stderr=subprocess.STDOUT, text=True, timeout=30)
+        return res.stdout.strip().splitlines()[0] if res.returncode == 0 else 'unknown (nvidia-smi failed)'
+    except (OSError, subprocess.SubprocessError, IndexError):
+        return 'unknown (nvidia-smi not available)'
+
+
+def _timed(fn):
+    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    a.record()
+    fn()
+    b.record()
+    torch.cuda.synchronize()
+    return a.elapsed_time(b)
+
+
 def main():
-    cfg = WORKLOADS[sys.argv[1] if len(sys.argv) > 1 else 'darcy241']
+    ap = argparse.ArgumentParser()
+    ap.add_argument('workload', nargs='?', default='darcy241', choices=sorted(WORKLOADS))
+    ap.add_argument('--edge-attr-grad', action='store_true')
+    ap.add_argument('--rounds', type=int, default=5)
+    args = ap.parse_args()
+    cfg = WORKLOADS[args.workload]
     dev = torch.device('cuda:0')
     s, r, w, kw, T = cfg['s'], cfg['r'], cfg['width'], cfg['ker_width'], cfg['depth']
     torch.manual_seed(0)
@@ -26,10 +61,7 @@ def main():
     opt = torch.optim.Adam(model.parameters(), lr=1e-4)
     x6, ei, ea = graphs.darcy_sample(s, r, dev, seed=0)
     y = torch.randn(s * s, 1, device=dev)
-
-    class D(object):
-        pass
-    d = D()
+    d = _Data()
     d.x, d.edge_index, d.edge_attr = x6, ei, ea
 
     def step():
@@ -38,16 +70,41 @@ def main():
         loss.backward()
         opt.step()
         return loss
-    step()
+
+    if not args.edge_attr_grad:
+        step()
+        torch.cuda.synchronize()
+        torch.cuda.profiler.start()
+        ms = _timed(step)
+        torch.cuda.profiler.stop()
+        print('one training step: %.2f ms (E=%d, T=%d)' % (ms, ei.size(1), T))
+        return
+
+    # theta = the coefficient column of the node features (darcy_sample: x = [grid, a, ...], edge_attr uses a)
+    grid = graphs.square_grid(s, dev)
+    theta0 = x6[:, 2].clone()
+
+    def step_theta(need):
+        theta = theta0.clone().requires_grad_(need)
+        d.edge_attr = graphs.ball_edge_attr(grid, ei, theta)
+        step()
+        if need:
+            assert theta.grad is not None and bool(torch.isfinite(theta.grad).all())
+
+    times = {False: [], True: []}
+    for need in (False, True):             # warm-up: both variants, every shape
+        step_theta(need)
     torch.cuda.synchronize()
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    torch.cuda.profiler.start()
-    a.record()
-    step()
-    b.record()
-    torch.cuda.synchronize()
-    torch.cuda.profiler.stop()
-    print('one training step: %.2f ms (E=%d, T=%d)' % (a.elapsed_time(b), ei.size(1), T))
+    for _ in range(args.rounds):
+        for need in (False, True):
+            times[need].append(_timed(lambda: step_theta(need)))
+    base, with_ea = statistics.median(times[False]), statistics.median(times[True])
+    print('device: %s, power limit: %s' % (torch.cuda.get_device_name(dev), _power_limit()))
+    print('%s: E=%d, T=%d, width=%d, ker_width=%d, %d alternating rounds' % (args.workload, ei.size(1), T, w, kw,
+                                                                              args.rounds))
+    print('training step, edge_attr without grad: median %.2f ms  (all: %s)' % (base, ', '.join('%.2f' % v for v in times[False])))
+    print('training step, edge_attr with grad:    median %.2f ms  (all: %s)' % (with_ea, ', '.join('%.2f' % v for v in times[True])))
+    print('overhead: %.2f ms (%.1f %%)' % (with_ea - base, 100.0 * (with_ea - base) / base))
 
 
 if __name__ == '__main__':
