@@ -96,13 +96,17 @@ static WeightsLayout layout_weights(const Weights* W) {
   L.off_wscale = c.off; c.take<float>(2 * (kMaxLayers + 2));
   L.off_W3p = c.off; c.take<char>(static_cast<size_t>(W->cout) * W->Kp * W->cin_p * W->esize * (W->split ? 3 : 1));
   L.off_B3 = c.off; c.take<float>(static_cast<size_t>(W->cin) * W->cout);
-  // images for the tensor-core backward (same conditions as backward_tc_supported)
-  L.bwd = (W->prec == PREC_F16 || W->prec == PREC_BF16) && W->cout == 64 && W->cin <= 64 && nl >= 2 &&
-          3 * W->dims[0] + 2 <= 64;
+  // images for the tensor-core backward (same conditions as backward_tc_supported); PREC_F16X2: split [hi | lo | hi]
+  // along the reduction dimension and pre-scaled by the power of two of the forward image (wscale)
+  L.bwd = (W->prec == PREC_F16 || W->prec == PREC_BF16 || W->prec == PREC_F16X2) && W->cout == 64 && W->cin <= 64 &&
+          nl >= 2 && 3 * W->dims[0] + 2 <= 64;
   if (L.bwd) {
-    L.off_W3q = c.off; c.take<char>(static_cast<size_t>(W->cout) * W->Kp * W->cin_p * 2);
-    L.off_W3t = c.off; c.take<char>(static_cast<size_t>(W->cout) * W->Kp * W->cin_p * 2);
-    for (int l = 2; l <= nl - 1; ++l) { L.off_WhT[l] = c.off; c.take<char>(static_cast<size_t>(W->kp[l]) * W->kp[l - 1] * 2); }
+    const size_t kmul = W->split ? 3 : 1;
+    L.off_W3q = c.off; c.take<char>(static_cast<size_t>(W->cout) * W->Kp * W->cin_p * 2 * kmul);
+    L.off_W3t = c.off; c.take<char>(static_cast<size_t>(W->cout) * W->Kp * W->cin_p * 2 * kmul);
+    for (int l = 2; l <= nl - 1; ++l) {
+      L.off_WhT[l] = c.off; c.take<char>(static_cast<size_t>(W->kp[l]) * W->kp[l - 1] * 2 * kmul);
+    }
   }
   if (W->prec == PREC_F16 || W->prec == PREC_BF16) {
     L.off_W3n = c.off; c.take<char>(static_cast<size_t>(W->cin) * W->cout * W->Kp * 2);
@@ -178,14 +182,16 @@ int weights_prepare(Weights* W, int n_layers, const int* dims, int cin, int cout
     W->W3n = base + L.off_W3n;
   }
   if (L.bwd) {
-    s = launch_w3q(prec, Wsrc[nl - 1], cin, cout, W->K, W->Kp, W->cin_p, 0, base + L.off_W3q, st);
+    const float* sL = W->split ? wscale + 2 * nl : nullptr;
+    s = launch_w3q(prec, Wsrc[nl - 1], cin, cout, W->K, W->Kp, W->cin_p, 0, base + L.off_W3q, st, sL);
     if (s) return s;
-    s = launch_w3q(prec, Wsrc[nl - 1], cin, cout, W->K, W->Kp, W->cin_p, 1, base + L.off_W3t, st);
+    s = launch_w3q(prec, Wsrc[nl - 1], cin, cout, W->K, W->Kp, W->cin_p, 1, base + L.off_W3t, st, sL);
     if (s) return s;
     W->W3q = base + L.off_W3q;
     W->W3t = base + L.off_W3t;
     for (int l = 2; l <= nl - 1; ++l) {
-      s = launch_transpose_pad(prec, Wsrc[l - 1], dims[l], dims[l - 1], base + L.off_WhT[l], W->kp[l], W->kp[l - 1], st);
+      s = launch_transpose_pad(prec, Wsrc[l - 1], dims[l], dims[l - 1], base + L.off_WhT[l], W->kp[l], W->kp[l - 1], st,
+                               W->split ? wscale + 2 * l : nullptr);
       if (s) return s;
       W->WhT[l] = base + L.off_WhT[l];
     }

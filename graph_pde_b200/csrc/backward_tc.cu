@@ -1,6 +1,7 @@
 // Tensor-core backward of the NNConv path (SURVEY 8(a) row a11; what autograd generates for
 // graph-neural-operator/nn_conv.py:267-282 + utilities.py:223-227), for the shapes of the GKN / MGKN
-// training configurations (out_channels = 64, in_channels <= 64, 16-bit operand precisions).
+// training configurations (out_channels = 64, in_channels <= 64, operand precisions f16, bf16 and f16x2; the split
+// variant of each kernel is described next to it).
 //
 // Notation (DESIGN.md section 2): h_e = edge features (cached by the forward), Y_c = x_c (x) W_L per source,
 // G_e = g[dst_e] / max(deg_in(dst_e),1) (mean) or g[dst_e] (add), g = dL/dout.
@@ -50,6 +51,15 @@ __device__ __forceinline__ uint32_t pack2(float a, float b) {
     __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
     return *reinterpret_cast<uint32_t*>(&h);
   }
+}
+
+// PREC_F16X2: (a, b) as fp16 pairs, hi = fp16(v), lo = fp16(v - hi)
+__device__ __forceinline__ void pack2_split(float a, float b, uint32_t& hi, uint32_t& lo) {
+  const __half2 h = __floats2half2_rn(a, b);
+  const float2 hf = __half22float2(h);
+  const __half2 l = __floats2half2_rn(a - hf.x, b - hf.y);
+  hi = *reinterpret_cast<const uint32_t*>(&h);
+  lo = *reinterpret_cast<const uint32_t*>(&l);
 }
 
 struct Maps8 {
@@ -167,7 +177,8 @@ __global__ void k_colsum(const float* __restrict__ g, int64_t N, int C, float* _
 
 // G16[t*128 + r, o] = (g[dst, o] * inv_deg[dst]) / gs  for r < cnt_t, zero rows up to 128 (cout == 64)
 // and, in the same pass, Gs[c, o] += sum of the tile's UNSCALED G rows (Gs zero-initialised by the caller)
-template <typename T16>
+// SPLIT (PREC_F16X2, T16 = __half): G16 holds the hi halves, the lo halves follow at row n_tiles*128 (one block per tile)
+template <typename T16, int SPLIT = 0>
 __global__ void __launch_bounds__(256) k_gather_g16(const float* __restrict__ g, const int* __restrict__ dst_sorted,
                                                     const float* __restrict__ inv_deg, const int* __restrict__ tile_c,
                                                     const int* __restrict__ tile_e0,
@@ -181,7 +192,7 @@ __global__ void __launch_bounds__(256) k_gather_g16(const float* __restrict__ g,
   // thread -> (row r = threadIdx / 8 + 32 * pass, 8 columns)
   for (int pass = 0; pass < 4; ++pass) {
     const int r = pass * 32 + threadIdx.x / 8, c0 = (threadIdx.x % 8) * 8;
-    uint32_t w[4] = {0u, 0u, 0u, 0u};
+    uint32_t w[4] = {0u, 0u, 0u, 0u}, wl[4] = {0u, 0u, 0u, 0u};
     if (r < cnt) {
       const int d = dst_sorted[e0 + r];
       const float dsc = inv_deg ? inv_deg[d] : 1.f;
@@ -190,7 +201,10 @@ __global__ void __launch_bounds__(256) k_gather_g16(const float* __restrict__ g,
       const float4 b = *reinterpret_cast<const float4*>(g + static_cast<int64_t>(d) * 64 + c0 + 4);
       colsum[0] += a.x * dsc; colsum[1] += a.y * dsc; colsum[2] += a.z * dsc; colsum[3] += a.w * dsc;
       colsum[4] += b.x * dsc; colsum[5] += b.y * dsc; colsum[6] += b.z * dsc; colsum[7] += b.w * dsc;
-      if (std::is_same<T16, __half>::value) {
+      if (SPLIT) {
+        pack2_split(a.x * sc, a.y * sc, w[0], wl[0]); pack2_split(a.z * sc, a.w * sc, w[1], wl[1]);
+        pack2_split(b.x * sc, b.y * sc, w[2], wl[2]); pack2_split(b.z * sc, b.w * sc, w[3], wl[3]);
+      } else if (std::is_same<T16, __half>::value) {
         w[0] = pack2<0>(a.x * sc, a.y * sc); w[1] = pack2<0>(a.z * sc, a.w * sc);
         w[2] = pack2<0>(b.x * sc, b.y * sc); w[3] = pack2<0>(b.z * sc, b.w * sc);
       } else {
@@ -199,6 +213,9 @@ __global__ void __launch_bounds__(256) k_gather_g16(const float* __restrict__ g,
       }
     }
     *reinterpret_cast<uint4*>(G16 + (static_cast<int64_t>(t) * 128 + r) * 64 + c0) = make_uint4(w[0], w[1], w[2], w[3]);
+    if (SPLIT)
+      *reinterpret_cast<uint4*>(G16 + (static_cast<int64_t>(gridDim.x + t) * 128 + r) * 64 + c0) =
+          make_uint4(wl[0], wl[1], wl[2], wl[3]);
   }
   // thread (rr = threadIdx / 8, cg = threadIdx % 8) holds the sums of rows rr, rr+32, rr+64, rr+96 for 8 columns
   {
@@ -216,21 +233,29 @@ __global__ void __launch_bounds__(256) k_gather_g16(const float* __restrict__ g,
 }
 
 // Xg16[c, i] = x[src_c, i] / xs   (global power-of-two scale, zero padded to cin_p)
-template <typename T16>
+// SPLIT (PREC_F16X2, T16 = __half): rows of 2 * cin_p, [hi | lo]
+template <typename T16, int SPLIT = 0>
 __global__ void k_prep_xg(const float* __restrict__ x, const int* __restrict__ src_nodes, int S, int cin, int cin_p,
                           const float* __restrict__ scal, T16* __restrict__ Xg) {
   const int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
   if (i >= static_cast<int64_t>(S) * cin_p) return;
   const int c = static_cast<int>(i / cin_p), ii = static_cast<int>(i % cin_p);
   const float v = ii < cin ? x[static_cast<int64_t>(src_nodes[c]) * cin + ii] * scal[5] : 0.f;
-  if (std::is_same<T16, __half>::value) reinterpret_cast<__half*>(Xg)[i] = __float2half_rn(v);
+  if (SPLIT) {
+    const __half hi = __float2half_rn(v);
+    __half* row = reinterpret_cast<__half*>(Xg) + static_cast<int64_t>(c) * 2 * cin_p;
+    row[ii] = hi;
+    row[cin_p + ii] = __float2half_rn(v - __half2float(hi));
+  } else if (std::is_same<T16, __half>::value) reinterpret_cast<__half*>(Xg)[i] = __float2half_rn(v);
   else reinterpret_cast<__nv_bfloat16*>(Xg)[i] = __float2bfloat16_rn(v);
 }
 
-// dx[src_{c0+c}, i] += gs * dxp[c, i] + sum_o B3[i, o] * Gs[c0+c, o]
+// dx[src_{c0+c}, i] += gs * winv * dxp[c, i] + sum_o B3[i, o] * Gs[c0+c, o]
+// (winv: the inverse power of two of a pre-scaled split W3t image, nullptr = 1)
 __global__ void k_scatter_dx_tc(const float* __restrict__ dxp, int ld, const float* __restrict__ Gs,
                                 const float* __restrict__ B3, const int* __restrict__ src_nodes, int c0, int nb,
-                                int cin, int cout, const float* __restrict__ scal, float* __restrict__ dx) {
+                                int cin, int cout, const float* __restrict__ scal, const float* __restrict__ winv,
+                                float* __restrict__ dx) {
   extern __shared__ float sb3[];     // [cin][cout + 1]
   const int ldb = cout + 1;
   for (int t = threadIdx.x; t < cin * cout; t += blockDim.x) sb3[(t / cout) * ldb + t % cout] = B3[t];
@@ -238,7 +263,7 @@ __global__ void k_scatter_dx_tc(const float* __restrict__ dxp, int ld, const flo
   const int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
   if (i >= static_cast<int64_t>(nb) * cin) return;
   const int c = static_cast<int>(i / cin), ii = static_cast<int>(i % cin);
-  float acc = dxp[static_cast<int64_t>(c) * ld + ii] * scal[1];
+  float acc = dxp[static_cast<int64_t>(c) * ld + ii] * (winv ? scal[1] * winv[0] : scal[1]);
   const float* gs = Gs + static_cast<int64_t>(c0 + c) * cout;
   for (int o = 0; o < cout; ++o) acc = fmaf(sb3[ii * ldb + o], __ldg(gs + o), acc);
   dx[static_cast<int64_t>(src_nodes[c0 + c]) * cin + ii] += acc;
@@ -282,7 +307,8 @@ struct GatherGArgs {
   const float* xs[kMaxApps];    // [S] per-source power-of-two scale of the forward's Y operand
   int T;
 };
-template <typename T16>
+// SPLIT (PREC_F16X2, T16 = __half): rows of 2 * T * 64, the hi halves in columns [0, T*64), the lo halves after them
+template <typename T16, int SPLIT = 0>
 __global__ void __launch_bounds__(256) k_gather_ghat(GatherGArgs ga, const int* __restrict__ dst_sorted,
                                                      const float* __restrict__ inv_deg, const int* __restrict__ tile_c,
                                                      const int* __restrict__ tile_e0, const int* __restrict__ tile_cnt,
@@ -291,7 +317,7 @@ __global__ void __launch_bounds__(256) k_gather_ghat(GatherGArgs ga, const int* 
   const int t = tile0 + blockIdx.x;
   const int e0 = tile_e0[t], cnt = tile_cnt[t], c = tile_c[t];
   const float inv_s = scal[17];
-  const int ld = ga.T * 64;
+  const int ld = (SPLIT ? 2 : 1) * ga.T * 64;
   for (int a = 0; a < ga.T; ++a) {
     const float xsc = ga.xs[a][c] * inv_s;
     const float* g = ga.g[a];
@@ -302,16 +328,20 @@ __global__ void __launch_bounds__(256) k_gather_ghat(GatherGArgs ga, const int* 
       const float sc = (inv_deg ? inv_deg[d] : 1.f) * xsc;
       const float4 p = *reinterpret_cast<const float4*>(g + static_cast<int64_t>(d) * 64 + c0);
       const float4 q = *reinterpret_cast<const float4*>(g + static_cast<int64_t>(d) * 64 + c0 + 4);
-      uint32_t w[4];
-      if (std::is_same<T16, __half>::value) {
+      uint32_t w[4], wl[4];
+      if (SPLIT) {
+        pack2_split(p.x * sc, p.y * sc, w[0], wl[0]); pack2_split(p.z * sc, p.w * sc, w[1], wl[1]);
+        pack2_split(q.x * sc, q.y * sc, w[2], wl[2]); pack2_split(q.z * sc, q.w * sc, w[3], wl[3]);
+      } else if (std::is_same<T16, __half>::value) {
         w[0] = pack2<0>(p.x * sc, p.y * sc); w[1] = pack2<0>(p.z * sc, p.w * sc);
         w[2] = pack2<0>(q.x * sc, q.y * sc); w[3] = pack2<0>(q.z * sc, q.w * sc);
       } else {
         w[0] = pack2<1>(p.x * sc, p.y * sc); w[1] = pack2<1>(p.z * sc, p.w * sc);
         w[2] = pack2<1>(q.x * sc, q.y * sc); w[3] = pack2<1>(q.z * sc, q.w * sc);
       }
-      *reinterpret_cast<uint4*>(Gh + static_cast<int64_t>(e0 - e_base + r) * ld + a * 64 + c0) =
-          make_uint4(w[0], w[1], w[2], w[3]);
+      T16* row = Gh + static_cast<int64_t>(e0 - e_base + r) * ld + a * 64 + c0;
+      *reinterpret_cast<uint4*>(row) = make_uint4(w[0], w[1], w[2], w[3]);
+      if (SPLIT) *reinterpret_cast<uint4*>(row + ga.T * 64) = make_uint4(wl[0], wl[1], wl[2], wl[3]);
     }
   }
 }
@@ -329,6 +359,9 @@ __global__ void k_max_f(const float* __restrict__ v, int n, float* __restrict__ 
 //   One (source, 128-k block) at a time per CTA, its [128 x 64] accumulator in the registers of the warpgroup; a
 //   stage holds the k block's two h boxes and the G box of one tile of the source.
 //   roles: warps 0..3 consumer warpgroup (wgmma, then 16-bit -> dY[c, k*64 + o]) | warp 4 TMA producer
+// SPLIT (PREC_F16X2): h and G are fp16 pairs (the lo panels of h start at panel nk, the lo rows of G at g_lo_row);
+//   every tile is three stages of the same shape, (h_hi, G_hi), (h_hi, G_lo), (h_lo, G_hi), accumulated into one
+//   fp32 tile, i.e. the reduction over edges runs three times as long; dY rows are [hi | lo] pairs (2 * Kp * 64).
 // =====================================================================================================
 constexpr int kDyStage = 48 * 1024;    // two [<=128 rows x 128 B] h boxes + one G box
 constexpr int kDyStages = 4;
@@ -342,12 +375,14 @@ struct DyArgs {
   int e_pad, nk;            // nk = Kp / 64 chunk panels
   int num_mt;               // ceil(nk / 2)
   int Kp;
-  uint16_t* dY;             // [c1 - c0, Kp * 64]
+  int g_lo_row;             // SPLIT: first row of the lo halves of G (n_tiles * 128)
+  uint16_t* dY;             // [c1 - c0, Kp * 64]   (SPLIT: [c1 - c0, 2 * Kp * 64])
 };
 
-template <int FMT>
+template <int FMT, int SPLIT = 0>
 __global__ void __launch_bounds__(160, 1)
 k_dy(const __grid_constant__ Maps8 tmH, const __grid_constant__ Maps8 tmG, DyArgs a) {
+  constexpr int kTerms = SPLIT ? 3 : 1;
   extern __shared__ __align__(1024) uint8_t smem[];
   if ((smem_u32(smem) & 1023u) != 0) __trap();
   float* scratch = reinterpret_cast<float*>(smem + kDyStages * kDyStage);
@@ -374,16 +409,22 @@ k_dy(const __grid_constant__ Maps8 tmH, const __grid_constant__ Maps8 tmG, DyArg
           const int e0 = __ldg(a.tile_e0 + t);
           const int box = (__ldg(a.tile_cnt + t) + 15) >> 4;       // 16-row units, 1..8
           const uint32_t box_bytes = static_cast<uint32_t>(box) * 16u * 128u;
-          mbar_wait(&empty[stage], phase ^ 1u);
-          if (elect_one()) {
-            uint8_t* st = smem + stage * kDyStage;
-            mbar_arrive_expect_tx(&full[stage], (two ? 3u : 2u) * box_bytes);
-            tma_load_2d(st, &tmH.m[box - 1], &full[stage], 0, (2 * m) * a.e_pad + e0, kEvictFirst);
-            if (two) tma_load_2d(st + 16384, &tmH.m[box - 1], &full[stage], 0, (2 * m + 1) * a.e_pad + e0, kEvictFirst);
-            tma_load_2d(st + 32768, &tmG.m[box - 1], &full[stage], 0, t * 128, kEvictFirst);
+          for (int term = 0; term < kTerms; ++term) {
+            const int hp = 2 * m + (term == 2 ? a.nk : 0);           // h panel (hi, or lo for the lo*hi term)
+            const int gr = t * 128 + (term == 1 ? a.g_lo_row : 0);   // G rows (hi, or lo for the hi*lo term)
+            // the h_hi boxes of the second term were loaded by the first: keep them for it (evict-first otherwise)
+            const uint64_t hpol = (SPLIT && term == 0) ? kEvictNormal : kEvictFirst;
+            mbar_wait(&empty[stage], phase ^ 1u);
+            if (elect_one()) {
+              uint8_t* st = smem + stage * kDyStage;
+              mbar_arrive_expect_tx(&full[stage], (two ? 3u : 2u) * box_bytes);
+              tma_load_2d(st, &tmH.m[box - 1], &full[stage], 0, hp * a.e_pad + e0, hpol);
+              if (two) tma_load_2d(st + 16384, &tmH.m[box - 1], &full[stage], 0, (hp + 1) * a.e_pad + e0, hpol);
+              tma_load_2d(st + 32768, &tmG.m[box - 1], &full[stage], 0, gr, kEvictFirst);
+            }
+            __syncwarp();
+            if (++stage == kDyStages) { stage = 0; phase ^= 1u; }
           }
-          __syncwarp();
-          if (++stage == kDyStages) { stage = 0; phase ^= 1u; }
         }
       }
     }
@@ -395,19 +436,21 @@ k_dy(const __grid_constant__ Maps8 tmH, const __grid_constant__ Maps8 tmG, DyArg
     uint32_t phase = 0;
     for (int c = a.c0 + blockIdx.x; c < a.c1; c += gridDim.x) {
       const int t0 = __ldg(a.tile_ptr + c), t1 = __ldg(a.tile_ptr + c + 1);
-      uint16_t* yrow = a.dY + static_cast<int64_t>(c - a.c0) * a.Kp * 64;
+      uint16_t* yrow = a.dY + static_cast<int64_t>(c - a.c0) * (SPLIT ? 2 : 1) * a.Kp * 64;
       for (int m = 0; m < a.num_mt; ++m) {
         for (int t = t0; t < t1; ++t) {
           const int ksteps = (__ldg(a.tile_cnt + t) + 15) >> 4;
-          mbar_wait(&full[stage], phase);
-          const uint32_t st = smem_u32(smem + stage * kDyStage);
-          // second m64 half = the second h box (+16 KB); 16 edges = two 8-row groups of 1024 B (+128 units)
-          mma_block<64, FMT, 1, 1>(acc, smem_desc_mn_sw128(st, 16384), smem_desc_mn_sw128(st + 32768, 16384), 16384 >> 4,
-                                   128, ksteps, t != t0);
-          wgmma_wait<0>();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&empty[stage]);
-          if (++stage == kDyStages) { stage = 0; phase ^= 1u; }
+          for (int term = 0; term < kTerms; ++term) {
+            mbar_wait(&full[stage], phase);
+            const uint32_t st = smem_u32(smem + stage * kDyStage);
+            // second m64 half = the second h box (+16 KB); 16 edges = two 8-row groups of 1024 B (+128 units)
+            mma_block<64, FMT, 1, 1>(acc, smem_desc_mn_sw128(st, 16384), smem_desc_mn_sw128(st + 32768, 16384),
+                                     16384 >> 4, 128, ksteps, t != t0 || term != 0);
+            wgmma_wait<0>();
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&empty[stage]);
+            if (++stage == kDyStages) { stage = 0; phase ^= 1u; }
+          }
         }
         const int k = m * 128 + acc_row(quarter, lane);
 #pragma unroll
@@ -415,12 +458,19 @@ k_dy(const __grid_constant__ Maps8 tmH, const __grid_constant__ Maps8 tmG, DyArg
           uint32_t v[32];
           acc_rows<64, 32>(acc, cc, wb, v);
           if (k < a.Kp) {
-            uint32_t pk[16];
+            uint32_t pk[16], pl[16];
 #pragma unroll
-            for (int j = 0; j < 16; ++j) pk[j] = pack2<FMT>(__uint_as_float(v[2 * j]), __uint_as_float(v[2 * j + 1]));
+            for (int j = 0; j < 16; ++j) {
+              if (SPLIT) pack2_split(__uint_as_float(v[2 * j]), __uint_as_float(v[2 * j + 1]), pk[j], pl[j]);
+              else pk[j] = pack2<FMT>(__uint_as_float(v[2 * j]), __uint_as_float(v[2 * j + 1]));
+            }
             uint16_t* dst = yrow + static_cast<int64_t>(k) * 64 + cc;
             st_global_32b(dst, pk);
             st_global_32b(dst + 16, pk + 8);
+            if (SPLIT) {
+              st_global_32b(dst + static_cast<int64_t>(a.Kp) * 64, pl);
+              st_global_32b(dst + static_cast<int64_t>(a.Kp) * 64 + 16, pl + 8);
+            }
           }
         }
       }
@@ -434,6 +484,11 @@ k_dy(const __grid_constant__ Maps8 tmH, const __grid_constant__ Maps8 tmG, DyArg
 //         N = BN k's  (B = rows (t, c, k) of the per-application Y^T matrices, K-major [BN x 64] boxes),
 //         K = T * 64; the accumulator lives in the registers of the consumer warpgroup (warps 0..3, warp 4 = TMA
 //   producer), which runs the epilogue: ReLU mask from the chunk-major h -> 16-bit -> dz[e - e_base, k].
+// SPLIT (PREC_F16X2): Ghat and Y^T are fp16 pairs.  Resident pairs would need 32 KB per application (256 KB at
+//   kMaxApps), more than shared memory holds beside the B ring, so A is streamed with B instead: a stage holds the
+//   (hi, lo) Ghat chunks of application j and the (hi, lo) Y^T boxes of (j, k block) -- 2 x 16 KB + 2 x BN x 128 B --
+//   and runs the three MMA blocks hi*hi, hi*lo, lo*hi.  The Ghat chunks are re-read once per k block (L2 hits: a tile's
+//   2 x T x 16 KB stay hot while its k blocks run).  dz rows are [hi | lo] pairs (2 * Kp); the mask is h's hi half.
 // =====================================================================================================
 constexpr int kDhAChunk = 16 * 1024;
 constexpr int kDhBStages = 3;
@@ -448,7 +503,7 @@ struct DhArgs {
   int e_pad;
   int T, Kp, n_nb;          // n_nb = Kp / BN
   const uint16_t* h;        // chunk-major edge features (the ReLU mask)
-  uint16_t* dz;             // [batch edges, Kp] row-major
+  uint16_t* dz;             // [batch edges, Kp] row-major (SPLIT: [batch edges, 2 * Kp], [hi | lo])
   // optional fused bias gradient: colsum[k * colsum_stride] += sum over the batch's edges of dz[e, k] (fp32, unscaled by
   // the caller's power-of-two factor like dz itself).  Column sums are formed per warp piece through a [32][33] shared
   // transpose and accumulated in a per-warp shared array; needs 4 * (4224 + 4 * Kp) extra bytes of shared memory.
@@ -458,15 +513,21 @@ struct DhArgs {
 
 constexpr int kDhScratch = 4 * acc_scratch_bytes<32>();
 
-template <int FMT, int BN>
+// bytes of the operand stages of k_dh (everything before its barriers)
+__host__ __device__ constexpr int dh_pipe_bytes(int split, int BN, int T) {
+  return split ? kDhBStages * (2 * kDhAChunk + 2 * BN * 128) : T * kDhAChunk + kDhBStages * BN * 128;
+}
+
+template <int FMT, int BN, int SPLIT = 0>
 __global__ void __launch_bounds__(160, 1)
 k_dh(const __grid_constant__ Maps8 tmA, const __grid_constant__ CUtensorMap tmB, DhArgs a) {
   extern __shared__ __align__(1024) uint8_t smem[];
   if ((smem_u32(smem) & 1023u) != 0) __trap();
   const int b_stage_bytes = BN * 128;
+  constexpr int kSplitStage = 2 * kDhAChunk + 2 * BN * 128;  // SPLIT: [A hi | A lo | B hi | B lo]
   uint8_t* smem_a = smem;                                   // [kMaxApps? T] chunks of 16 KB
-  uint8_t* smem_b = smem + a.T * kDhAChunk;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem_b + kDhBStages * b_stage_bytes);
+  uint8_t* smem_b = SPLIT ? smem : smem + a.T * kDhAChunk;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + dh_pipe_bytes(SPLIT, BN, a.T));
   uint64_t* a_full = bars;                   // [kMaxApps]
   uint64_t* a_empty = a_full + kMaxApps;
   uint64_t* b_full = a_empty + kMaxApps;
@@ -485,7 +546,32 @@ k_dh(const __grid_constant__ Maps8 tmA, const __grid_constant__ CUtensorMap tmB,
   }
   __syncthreads();
 
-  if (warp == 4) {
+  if (warp == 4 && SPLIT) {
+    int bs = 0;
+    uint32_t bph = 0;
+    for (int t = a.tile0 + blockIdx.x; t < a.tile1; t += gridDim.x) {
+      const int e0 = __ldg(a.tile_e0 + t);
+      const int box = (__ldg(a.tile_cnt + t) + 15) >> 4;
+      const int cl = __ldg(a.tile_c + t) - a.c0;
+      const uint32_t a_bytes = static_cast<uint32_t>(box) * 16u * 128u;
+      for (int nb = 0; nb < a.n_nb; ++nb) {
+        for (int j = 0; j < a.T; ++j) {
+          mbar_wait(&b_empty[bs], bph ^ 1u);
+          if (elect_one()) {
+            uint8_t* sp = smem + bs * kSplitStage;
+            const int yrow = (j * a.Sb + cl) * 2 * a.Kp + nb * BN;      // Y^T rows of (j, c): [hi Kp | lo Kp]
+            mbar_arrive_expect_tx(&b_full[bs], 2u * a_bytes + 2u * static_cast<uint32_t>(b_stage_bytes));
+            tma_load_2d(sp, &tmA.m[box - 1], &b_full[bs], j * 64, e0 - a.e_base, kEvictNormal);
+            tma_load_2d(sp + kDhAChunk, &tmA.m[box - 1], &b_full[bs], (a.T + j) * 64, e0 - a.e_base, kEvictNormal);
+            tma_load_2d(sp + 2 * kDhAChunk, &tmB, &b_full[bs], 0, yrow, kEvictLast);
+            tma_load_2d(sp + 2 * kDhAChunk + b_stage_bytes, &tmB, &b_full[bs], 0, yrow + a.Kp, kEvictLast);
+          }
+          __syncwarp();
+          if (++bs == kDhBStages) { bs = 0; bph ^= 1u; }
+        }
+      }
+    }
+  } else if (warp == 4) {
     int bs = 0;
     uint32_t bph = 0, aph = 0;
     for (int t = a.tile0 + blockIdx.x; t < a.tile1; t += gridDim.x, aph ^= 1u) {
@@ -529,15 +615,28 @@ k_dh(const __grid_constant__ Maps8 tmA, const __grid_constant__ CUtensorMap tmB,
       const bool ok = r < cnt;
       for (int nb = 0; nb < a.n_nb; ++nb) {
         for (int j = 0; j < a.T; ++j) {
-          if (nb == 0) mbar_wait(&a_full[j], aph);
-          mbar_wait(&b_full[bs], bph);
-          mma_block<BN, FMT>(acc, smem_desc_sw128(smem_u32(smem_a + j * kDhAChunk)),
-                             smem_desc_sw128(smem_u32(smem_b + bs * b_stage_bytes)), 512, 2, 4, j != 0);
-          wgmma_wait<0>();
-          __syncwarp();
-          if (lane == 0) {
-            mbar_arrive(&b_empty[bs]);
-            if (nb == a.n_nb - 1) mbar_arrive(&a_empty[j]);
+          if (SPLIT) {
+            mbar_wait(&b_full[bs], bph);
+            const uint32_t sp = smem_u32(smem + bs * kSplitStage);
+            const uint64_t ah = smem_desc_sw128(sp), al = smem_desc_sw128(sp + kDhAChunk);
+            const uint64_t bh = smem_desc_sw128(sp + 2 * kDhAChunk), bl = smem_desc_sw128(sp + 2 * kDhAChunk + b_stage_bytes);
+            mma_block<BN, FMT>(acc, ah, bh, 512, 2, 4, j != 0);
+            mma_block<BN, FMT>(acc, ah, bl, 512, 2, 4, true);
+            mma_block<BN, FMT>(acc, al, bh, 512, 2, 4, true);
+            wgmma_wait<0>();
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&b_empty[bs]);
+          } else {
+            if (nb == 0) mbar_wait(&a_full[j], aph);
+            mbar_wait(&b_full[bs], bph);
+            mma_block<BN, FMT>(acc, smem_desc_sw128(smem_u32(smem_a + j * kDhAChunk)),
+                               smem_desc_sw128(smem_u32(smem_b + bs * b_stage_bytes)), 512, 2, 4, j != 0);
+            wgmma_wait<0>();
+            __syncwarp();
+            if (lane == 0) {
+              mbar_arrive(&b_empty[bs]);
+              if (nb == a.n_nb - 1) mbar_arrive(&a_empty[j]);
+            }
           }
           if (++bs == kDhBStages) { bs = 0; bph ^= 1u; }
         }
@@ -547,8 +646,9 @@ k_dh(const __grid_constant__ Maps8 tmA, const __grid_constant__ CUtensorMap tmB,
           acc_rows<BN, 32>(acc, cc, wb, v);
           const int k0 = nb * BN + cc;
           if (ok) {
+            // (SPLIT: the hi panels of h come first, so this is the hi half)
             const uint16_t* hp = a.h + (static_cast<int64_t>(k0 >> 6) * a.e_pad + e0 + r) * 64 + (k0 & 63);
-            uint32_t pk[16];
+            uint32_t pk[16], pl[16];
 #pragma unroll
             for (int q = 0; q < 4; ++q) {
               const uint4 mk = __ldg(reinterpret_cast<const uint4*>(hp) + q);
@@ -557,14 +657,19 @@ k_dh(const __grid_constant__ Maps8 tmA, const __grid_constant__ CUtensorMap tmB,
               for (int j = 0; j < 4; ++j) {
                 const float f0 = (mw[j] & 0x7FFFu) ? __uint_as_float(v[8 * q + 2 * j]) : 0.f;
                 const float f1 = (mw[j] & 0x7FFF0000u) ? __uint_as_float(v[8 * q + 2 * j + 1]) : 0.f;
-                pk[4 * q + j] = pack2<FMT>(f0, f1);
+                if (SPLIT) pack2_split(f0, f1, pk[4 * q + j], pl[4 * q + j]);
+                else pk[4 * q + j] = pack2<FMT>(f0, f1);
                 v[8 * q + 2 * j] = __float_as_uint(f0);
                 v[8 * q + 2 * j + 1] = __float_as_uint(f1);
               }
             }
-            uint16_t* dst = a.dz + static_cast<int64_t>(e0 - a.e_base + r) * a.Kp + k0;
+            uint16_t* dst = a.dz + static_cast<int64_t>(e0 - a.e_base + r) * (SPLIT ? 2 : 1) * a.Kp + k0;
             st_global_32b(dst, pk);
             st_global_32b(dst + 16, pk + 8);
+            if (SPLIT) {
+              st_global_32b(dst + a.Kp, pl);
+              st_global_32b(dst + a.Kp + 16, pl + 8);
+            }
           }
           if (a.colsum != nullptr) {          // column sums of this warp's [32 rows x 32 columns] piece
 #pragma unroll
@@ -595,6 +700,7 @@ k_dh(const __grid_constant__ Maps8 tmA, const __grid_constant__ CUtensorMap tmB,
 //   every gradient of the pass, and read once; W_1 (fp32 [kp1, k_in], zero rows past k_1) sits transposed in shared
 //   memory.  Eight lanes share a row (64 consecutive columns per step, 16-byte loads), each lane carries kEaRows rows,
 //   so a warp covers 4 * kEaRows rows and a row's sum needs three shuffles.  Padding rows [n, n_pad) are never read.
+//   SPLIT (PREC_F16X2): dz_1 rows are [hi | lo] pairs (2 * kp1), summed in fp32 as they are read.
 // =====================================================================================================
 constexpr int kEaRows = 2;
 constexpr int kEaRowsPerBlock = 8 * 4 * kEaRows;   // 256 threads
@@ -612,7 +718,7 @@ __device__ __forceinline__ void unpack8(const uint4 u, float* v) {
   }
 }
 
-template <int FMT, int KMAX>
+template <int FMT, int KMAX, int SPLIT = 0>
 __global__ void __launch_bounds__(256) k_ea_grad(const uint16_t* __restrict__ dz, int n, int kp1,
                                                  const float* __restrict__ W1, int k_in, const int* __restrict__ perm,
                                                  int e_base, const float* __restrict__ scal, int scal_idx,
@@ -637,9 +743,19 @@ __global__ void __launch_bounds__(256) k_ea_grad(const uint16_t* __restrict__ dz
       float v[kEaRows][8];
 #pragma unroll
       for (int rr = 0; rr < kEaRows; ++rr) {
-        uint4 u = make_uint4(0u, 0u, 0u, 0u);
-        if (row[rr] < n) u = __ldcs(reinterpret_cast<const uint4*>(dz + row[rr] * kp1 + j0));
+        uint4 u = make_uint4(0u, 0u, 0u, 0u), ul = make_uint4(0u, 0u, 0u, 0u);
+        const uint16_t* zr = dz + row[rr] * (SPLIT ? 2 : 1) * kp1 + j0;
+        if (row[rr] < n) {
+          u = __ldcs(reinterpret_cast<const uint4*>(zr));
+          if (SPLIT) ul = __ldcs(reinterpret_cast<const uint4*>(zr + kp1));
+        }
         unpack8<FMT>(u, v[rr]);
+        if (SPLIT) {
+          float vl[8];
+          unpack8<FMT>(ul, vl);
+#pragma unroll
+          for (int k = 0; k < 8; ++k) v[rr][k] += vl[k];
+        }
       }
 #pragma unroll
       for (int i = 0; i < KMAX; ++i) {
@@ -684,7 +800,7 @@ __global__ void __launch_bounds__(256) k_ea_grad(const uint16_t* __restrict__ dz
 // host side
 // =====================================================================================================
 bool backward_tc_supported(const Weights* W) {
-  if (W->prec != PREC_F16 && W->prec != PREC_BF16) return false;
+  if (W->prec != PREC_F16 && W->prec != PREC_BF16 && W->prec != PREC_F16X2) return false;
   if (W->cout != 64 || W->cin > 64 || W->n_layers < 2 || W->W1aug == nullptr) return false;
   if (W->W3q == nullptr || W->W3t == nullptr) return false;
   for (int l = 2; l <= W->n_layers - 1; ++l)
@@ -702,18 +818,30 @@ ApplyBwdLayout apply_bwd_layout(const Plan* P, const Weights* W) {
   Carver c(nullptr, ~size_t(0));
   ApplyBwdLayout L{};
   const size_t S = P->n_src > 0 ? P->n_src : 1;
+  const size_t pm = W->split ? 2 : 1;      // PREC_F16X2: x, G and dY as [hi | lo] pairs
   L.off_scal = c.off; c.take<float>(64);
-  L.off_Xg = c.off; c.take<char>((S + 128) * W->cin_p * 2);
+  L.off_Xg = c.off; c.take<char>((S + 128) * W->cin_p * 2 * pm);
   L.off_Gs = c.off; c.take<float>(S * W->cout);
-  L.off_G16 = c.off; c.take<char>(static_cast<size_t>(P->n_tiles > 0 ? P->n_tiles : 1) * 128 * 64 * 2);
+  L.off_G16 = c.off; c.take<char>(static_cast<size_t>(P->n_tiles > 0 ? P->n_tiles : 1) * 128 * 64 * 2 * pm);
   L.off_dW3 = c.off; c.take<float>(static_cast<size_t>(W->Kp) * W->cout * W->cin_p);
   L.fixed = c.off;
-  L.per_src = static_cast<size_t>(W->Kp) * W->cout * 2 + static_cast<size_t>(W->cin_p) * 4;   // dY row + dxp row
+  L.per_src = static_cast<size_t>(W->Kp) * W->cout * 2 * pm + static_cast<size_t>(W->cin_p) * 4;   // dY row + dxp row
   return L;
 }
 
-template <typename F>
-int for_fmt(int prec, F f) { return prec == PREC_BF16 ? f(std::integral_constant<int, 1>()) : f(std::integral_constant<int, 0>()); }
+// C[M, N] += sum_{r < R} A[r, m] B[r, n] (see launch_gemm_tn).  PREC_F16X2: A and B are [hi | lo] pairs whose lo halves
+// start at columns a_lo / b_lo (b_lo < 0: B is a single operand, e.g. the split first-layer image A1), and the product
+// is hi*hi + hi*lo + lo*hi as accumulating fp16 calls (hi*hi + lo*hi when B is single)
+int gemm_tn_pairs(const Weights* W, const void* A, int64_t lda, int a_lo, const void* B, int64_t ldb, int b_lo, int64_t R,
+                  int M, int N, float* C, int64_t ldc, cudaStream_t st) {
+  if (!W->split) return launch_gemm_tn(W->prec, A, lda, 0, B, ldb, 0, R, M, N, C, ldc, 1.f, nullptr, st);
+  const int cols[3][2] = {{0, 0}, {a_lo, 0}, {0, b_lo}};
+  for (int i = 0; i < (b_lo < 0 ? 2 : 3); ++i) {
+    const int s = launch_gemm_tn(PREC_F16, A, lda, cols[i][0], B, ldb, cols[i][1], R, M, N, C, ldc, 1.f, nullptr, st);
+    if (s) return s;
+  }
+  return NNCONV_OK;
+}
 
 }  // namespace
 
@@ -733,6 +861,7 @@ int backward_apply_tc(const Plan* P, const Weights* W, const void* h, const floa
   const int cin = W->cin, cout = W->cout, Kp = W->Kp, cin_p = W->cin_p;
   const int64_t N = P->N;
   const int bf = W->prec == PREC_BF16;
+  const int sp = W->split;
   int s = tc_init();
   if (s) return s;
   // ---- node-level terms
@@ -783,12 +912,16 @@ int backward_apply_tc(const Plan* P, const Weights* W, const void* h, const floa
   k_apply_scales<<<1, 1, 0, st>>>(scal);
   NNC_CHECK_LAUNCH();
   NNC_CHECK_CUDA(cudaMemsetAsync(Gs, 0, sizeof(float) * static_cast<size_t>(S) * cout, st));
-  if (bf) k_gather_g16<__nv_bfloat16><<<P->n_tiles, 256, 0, st>>>(gout, P->dst_sorted, inv_deg, P->tile_c, P->tile_e0,
-                                                                  P->tile_cnt, scal, static_cast<__nv_bfloat16*>(G16), Gs);
+  if (sp) k_gather_g16<__half, 1><<<P->n_tiles, 256, 0, st>>>(gout, P->dst_sorted, inv_deg, P->tile_c, P->tile_e0,
+                                                              P->tile_cnt, scal, static_cast<__half*>(G16), Gs);
+  else if (bf) k_gather_g16<__nv_bfloat16><<<P->n_tiles, 256, 0, st>>>(gout, P->dst_sorted, inv_deg, P->tile_c, P->tile_e0,
+                                                                       P->tile_cnt, scal, static_cast<__nv_bfloat16*>(G16), Gs);
   else k_gather_g16<__half><<<P->n_tiles, 256, 0, st>>>(gout, P->dst_sorted, inv_deg, P->tile_c, P->tile_e0, P->tile_cnt, scal,
                                                         static_cast<__half*>(G16), Gs);
   NNC_CHECK_LAUNCH();
-  if (bf) k_prep_xg<__nv_bfloat16><<<(unsigned)ceil_div64(static_cast<int64_t>(S) * cin_p, 256), 256, 0, st>>>(
+  if (sp) k_prep_xg<__half, 1><<<(unsigned)ceil_div64(static_cast<int64_t>(S) * cin_p, 256), 256, 0, st>>>(
+      x, P->src_nodes, S, cin, cin_p, scal, static_cast<__half*>(Xg));
+  else if (bf) k_prep_xg<__nv_bfloat16><<<(unsigned)ceil_div64(static_cast<int64_t>(S) * cin_p, 256), 256, 0, st>>>(
       x, P->src_nodes, S, cin, cin_p, scal, static_cast<__nv_bfloat16*>(Xg));
   else k_prep_xg<__half><<<(unsigned)ceil_div64(static_cast<int64_t>(S) * cin_p, 256), 256, 0, st>>>(
       x, P->src_nodes, S, cin, cin_p, scal, static_cast<__half*>(Xg));
@@ -801,15 +934,16 @@ int backward_apply_tc(const Plan* P, const Weights* W, const void* h, const floa
   const int64_t e_pad = round_up64(P->E, 128);
   Maps8 tmH, tmG;
   for (int i = 0; i < 8; ++i) {
-    s = make_tmap_2d_16b(&tmH.m[i], bf, h, static_cast<uint64_t>(Kp / 64) * e_pad, 64, 16 * (i + 1));
+    s = make_tmap_2d_16b(&tmH.m[i], bf, h, static_cast<uint64_t>((sp ? 2 : 1) * Kp / 64) * e_pad, 64, 16 * (i + 1));
     if (s) return s;
-    s = make_tmap_2d_16b(&tmG.m[i], bf, G16, static_cast<uint64_t>(P->n_tiles) * 128, 64, 16 * (i + 1));
+    s = make_tmap_2d_16b(&tmG.m[i], bf, G16, static_cast<uint64_t>((sp ? 2 : 1) * P->n_tiles) * 128, 64, 16 * (i + 1));
     if (s) return s;
   }
   static bool attr_set = false;
   if (!attr_set) {
     NNC_CHECK_CUDA(cudaFuncSetAttribute(k_dy<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, kDySmem));
     NNC_CHECK_CUDA(cudaFuncSetAttribute(k_dy<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, kDySmem));
+    NNC_CHECK_CUDA(cudaFuncSetAttribute(k_dy<0, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, kDySmem));
     attr_set = true;
   }
   const int NY = Kp * cout;
@@ -819,21 +953,23 @@ int backward_apply_tc(const Plan* P, const Weights* W, const void* h, const floa
     a.tile_ptr = P->tile_ptr; a.tile_e0 = P->tile_e0; a.tile_cnt = P->tile_cnt;
     a.c0 = static_cast<int>(c0); a.c1 = static_cast<int>(c0) + nb;
     a.e_pad = static_cast<int>(e_pad); a.nk = Kp / 64; a.num_mt = (a.nk + 1) / 2;
-    a.Kp = Kp; a.dY = dY;
+    a.Kp = Kp; a.g_lo_row = P->n_tiles * 128; a.dY = dY;
     const int grid = nb < tc_num_sms() ? nb : tc_num_sms();
-    if (bf) k_dy<1><<<grid, 160, kDySmem, st>>>(tmH, tmG, a);
+    if (sp) k_dy<0, 1><<<grid, 160, kDySmem, st>>>(tmH, tmG, a);
+    else if (bf) k_dy<1><<<grid, 160, kDySmem, st>>>(tmH, tmG, a);
     else k_dy<0><<<grid, 160, kDySmem, st>>>(tmH, tmG, a);
     NNC_CHECK_LAUNCH();
-    // dxp[c, i] = sum_n dY[c, n] W3t[i, n]      (fp32 out)
-    s = launch_gemm_tc(W->prec, dY, nb, 0, nb, NY, W->W3t, cin_p, nullptr, 0, dxp, cin_p, st, nullptr, 0, 0, 0, nullptr,
-                       nullptr, 0, 1);
+    // dxp[c, i] = sum_n dY[c, n] W3t[i, n]      (fp32 out; PREC_F16X2: split A against the pre-scaled split W3t)
+    s = launch_gemm_tc(W->prec, dY, nb, 0, nb, (sp ? 3 : 1) * NY, W->W3t, cin_p, nullptr, 0, dxp, cin_p, st, nullptr, 0, 0,
+                       sp ? GEMM_A_SPLIT : 0, nullptr, nullptr, 0, 1);
     if (s) return s;
     k_scatter_dx_tc<<<(unsigned)ceil_div64(static_cast<int64_t>(nb) * cin, 256), 256, sizeof(float) * cin * (cout + 1), st>>>(
-        dxp, cin_p, Gs, W->B3, P->src_nodes, static_cast<int>(c0), nb, cin, cout, scal, dx);
+        dxp, cin_p, Gs, W->B3, P->src_nodes, static_cast<int>(c0), nb, cin, cout, scal,
+        sp ? W->wscale + 2 * W->n_layers + 1 : nullptr, dx);
     NNC_CHECK_LAUNCH();
     // dW3[(k,o), i] += sum_c dY[c, (k,o)] Xg[c0 + c, i]
-    s = launch_gemm_tn(W->prec, dY, NY, 0, static_cast<const char*>(Xg) + static_cast<size_t>(c0) * cin_p * 2, cin_p, 0, nb,
-                       NY, cin_p, dW3, cin_p, 1.f, nullptr, st);
+    s = gemm_tn_pairs(W, dY, (sp ? 2 : 1) * NY, NY, static_cast<const char*>(Xg) + static_cast<size_t>(c0) * cin_p * 2 * (sp ? 2 : 1),
+                      (sp ? 2 : 1) * cin_p, cin_p, nb, NY, cin_p, dW3, cin_p, st);
     if (s) return s;
   }
   k_unpermute_w3q<<<(unsigned)ceil_div64(nWL, 256), 256, 0, st>>>(dW3, cin, cout, W->K, cin_p, scal, 6, dWL);
@@ -855,9 +991,10 @@ MlpBwdLayout mlp_bwd_layout(const Plan* P, const Weights* W, int T) {
   MlpBwdLayout L{};
   const size_t S = P->n_src > 0 ? P->n_src : 1;
   const int nl = W->n_layers;
+  const size_t pm = W->split ? 2 : 1;      // PREC_F16X2: [hi | lo] pairs (Xc: [hi | hi | lo], see launch_src_prep)
   L.off_scal = c.off; c.take<float>(64);
   for (int t = 0; t < T; ++t) {
-    L.off_Xc[t] = c.off; c.take<char>((S + 128) * W->cin_p * 2);
+    L.off_Xc[t] = c.off; c.take<char>((S + 128) * W->cin_p * 2 * (W->split ? 3 : 1));
     L.off_xs[t] = c.off; c.take<float>(S);
   }
   L.off_cvec = c.off; c.take<float>(S * W->cout);
@@ -872,8 +1009,8 @@ MlpBwdLayout mlp_bwd_layout(const Plan* P, const Weights* W, int T) {
     maxkp = static_cast<size_t>(W->kp[l]) > maxkp ? W->kp[l] : maxkp;
   }
   // Ghat row + dz ping/pong + stored hidden activations h_1..h_{L-2} + A1 row
-  L.per_edge = static_cast<size_t>(T) * 128 + 2 * maxkp * 2 + acts * 2 + 128;
-  L.per_src = static_cast<size_t>(T) * W->Kp * 64 * 2;      // Y^T rows of the T applications
+  L.per_edge = (static_cast<size_t>(T) * 128 + 2 * maxkp * 2 + acts * 2) * pm + 128;
+  L.per_src = static_cast<size_t>(T) * W->Kp * 64 * 2 * pm;      // Y^T rows of the T applications
   return L;
 }
 }  // namespace
@@ -897,6 +1034,9 @@ int backward_mlp_tc(const Plan* P, const Weights* W, const float* edge_attr, con
   const int nl = W->n_layers;
   const int cin = W->cin, cout = W->cout, Kp = W->Kp, cin_p = W->cin_p, k_in = W->dims[0];
   const int bf = W->prec == PREC_BF16;
+  // PREC_F16X2: every 16-bit buffer of the pass holds [hi | lo] pairs (pm = 2), the GEMMs read split operands
+  // (K tripled, kmul = 3) against the pre-scaled split weight images, whose power of two the epilogues undo
+  const int sp = W->split, pm = sp ? 2 : 1, kmul = sp ? 3 : 1;
   int s = tc_init();
   if (s) return s;
   // gradient w.r.t. edge_attr: W_1 transposed in shared memory (k_in <= 20 on this path)
@@ -955,9 +1095,13 @@ int backward_mlp_tc(const Plan* P, const Weights* W, const float* edge_attr, con
     NNC_CHECK_CUDA(cudaFuncSetAttribute(k_ea_grad<1, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     NNC_CHECK_CUDA(cudaFuncSetAttribute(k_ea_grad<0, 20>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     NNC_CHECK_CUDA(cudaFuncSetAttribute(k_ea_grad<1, 20>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    NNC_CHECK_CUDA(cudaFuncSetAttribute(k_dh<0, 64, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    NNC_CHECK_CUDA(cudaFuncSetAttribute(k_dh<0, 128, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    NNC_CHECK_CUDA(cudaFuncSetAttribute(k_ea_grad<0, 8, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    NNC_CHECK_CUDA(cudaFuncSetAttribute(k_ea_grad<0, 20, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     attr_set = true;
   }
-  int dh_smem = T * kDhAChunk + kDhBStages * BN * 128 + 1024 + kDhScratch;
+  int dh_smem = dh_pipe_bytes(sp, BN, T) + 1024 + kDhScratch;
   NNC_REQUIRE(dh_smem <= 227 * 1024, NNCONV_ERR_UNSUPPORTED, "backward_mlp: T=%d applications do not fit shared memory", T);
   // bias gradient of the top hidden layer fused into k_dh (one pass over dz_{L-1} saved) when the transpose + column
   // accumulators fit next to the operand stages; layer 1 (nl == 2) needs the full dz^T A1 product anyway
@@ -979,10 +1123,10 @@ int backward_mlp_tc(const Plan* P, const Weights* W, const float* edge_attr, con
     const int nb = c1 - c0, e_base = hgp[c0], n = hgp[c1] - hgp[c0];
     const int64_t n_pad = round_up64(n, 128) + 128;
     Carver cv(base + L.fixed, avail + (1 << 16));
-    uint16_t* Yt = cv.take<uint16_t>(static_cast<size_t>(T) * nb * Kp * 64);
-    uint16_t* Gh = cv.take<uint16_t>(static_cast<size_t>(n_pad) * T * 64);
-    uint16_t* dzA = cv.take<uint16_t>(static_cast<size_t>(n_pad) * maxkp);
-    uint16_t* dzB = cv.take<uint16_t>(static_cast<size_t>(n_pad) * maxkp);
+    uint16_t* Yt = cv.take<uint16_t>(static_cast<size_t>(T) * nb * Kp * 64 * pm);
+    uint16_t* Gh = cv.take<uint16_t>(static_cast<size_t>(n_pad) * T * 64 * pm);
+    uint16_t* dzA = cv.take<uint16_t>(static_cast<size_t>(n_pad) * maxkp * pm);
+    uint16_t* dzB = cv.take<uint16_t>(static_cast<size_t>(n_pad) * maxkp * pm);
     uint16_t* A1 = cv.take<uint16_t>(static_cast<size_t>(n_pad) * 64);
     uint16_t* act[kMaxLayers + 1] = {nullptr};
     for (int l = 1; l <= nl - 2; ++l) {
@@ -990,20 +1134,25 @@ int backward_mlp_tc(const Plan* P, const Weights* W, const float* edge_attr, con
         act[l] = const_cast<uint16_t*>(reinterpret_cast<const uint16_t*>(static_cast<const char*>(acts) + edge_acts_offset(P, W, l))) +
                  static_cast<size_t>(e_base) * W->kp[l];
       else
-        act[l] = cv.take<uint16_t>(static_cast<size_t>(n_pad) * W->kp[l]);
+        act[l] = cv.take<uint16_t>(static_cast<size_t>(n_pad) * W->kp[l] * pm);
     }
     NNC_REQUIRE(cv.ok(), NNCONV_ERR_WORKSPACE, "backward_mlp: workspace carve overflow");
     // ---- Y^T of the batch for every application: Yt[t][(c, k), o] = sum_i Xc_t[c, i] W_L[i*out + o, k]
+    //      (PREC_F16X2: row c of application t is [hi | lo], 2 * Kp * 64)
     for (int t = 0; t < T; ++t) {
-      s = launch_gemm_tc(W->prec, base + L.off_Xc[t], S, c0, nb, cin_p, W->W3q, Kp * 64, nullptr, 0,
-                         Yt + static_cast<size_t>(t) * nb * Kp * 64, static_cast<int64_t>(Kp) * 64, st);
+      s = launch_gemm_tc(W->prec, base + L.off_Xc[t], S, c0, nb, kmul * cin_p, W->W3q, Kp * 64, nullptr, 0,
+                         Yt + static_cast<size_t>(t) * nb * Kp * 64 * pm, static_cast<int64_t>(pm) * Kp * 64, st, nullptr, 0,
+                         0, sp ? GEMM_C_SPLIT : 0, nullptr, nullptr, 0, 0, 0, sp ? W->wscale + 2 * nl + 1 : nullptr);
       if (s) return s;
     }
     // ---- Ghat rows of the batch
     {
       const int nt = htp[c1] - htp[c0];
-      if (bf) k_gather_ghat<__nv_bfloat16><<<nt, 256, 0, st>>>(ga, P->dst_sorted, inv_deg, P->tile_c, P->tile_e0, P->tile_cnt,
-                                                                htp[c0], e_base, scal, reinterpret_cast<__nv_bfloat16*>(Gh));
+      if (sp) k_gather_ghat<__half, 1><<<nt, 256, 0, st>>>(ga, P->dst_sorted, inv_deg, P->tile_c, P->tile_e0, P->tile_cnt,
+                                                           htp[c0], e_base, scal, reinterpret_cast<__half*>(Gh));
+      else if (bf) k_gather_ghat<__nv_bfloat16><<<nt, 256, 0, st>>>(ga, P->dst_sorted, inv_deg, P->tile_c, P->tile_e0,
+                                                                     P->tile_cnt, htp[c0], e_base, scal,
+                                                                     reinterpret_cast<__nv_bfloat16*>(Gh));
       else k_gather_ghat<__half><<<nt, 256, 0, st>>>(ga, P->dst_sorted, inv_deg, P->tile_c, P->tile_e0, P->tile_cnt, htp[c0],
                                                      e_base, scal, reinterpret_cast<__half*>(Gh));
       NNC_CHECK_LAUNCH();
@@ -1013,10 +1162,10 @@ int backward_mlp_tc(const Plan* P, const Weights* W, const float* edge_attr, con
       Maps8 tmA;
       CUtensorMap tmB;
       for (int i = 0; i < 8; ++i) {
-        s = make_tmap_2d_16b(&tmA.m[i], bf, Gh, static_cast<uint64_t>(n_pad), static_cast<uint64_t>(T) * 64, 16 * (i + 1));
+        s = make_tmap_2d_16b(&tmA.m[i], bf, Gh, static_cast<uint64_t>(n_pad), static_cast<uint64_t>(pm) * T * 64, 16 * (i + 1));
         if (s) return s;
       }
-      s = make_tmap_2d_16b(&tmB, bf, Yt, static_cast<uint64_t>(T) * nb * Kp, 64, BN);
+      s = make_tmap_2d_16b(&tmB, bf, Yt, static_cast<uint64_t>(pm) * T * nb * Kp, 64, BN);
       if (s) return s;
       DhArgs a;
       a.tile_c = P->tile_c; a.tile_e0 = P->tile_e0; a.tile_cnt = P->tile_cnt;
@@ -1027,7 +1176,10 @@ int backward_mlp_tc(const Plan* P, const Weights* W, const float* edge_attr, con
       a.colsum_stride = 64;
       const int tiles = a.tile1 - a.tile0;
       const int grid = tiles < tc_num_sms() ? tiles : tc_num_sms();
-      if (BN == 128) {
+      if (sp) {
+        if (BN == 128) k_dh<0, 128, 1><<<grid, 160, dh_smem, st>>>(tmA, tmB, a);
+        else k_dh<0, 64, 1><<<grid, 160, dh_smem, st>>>(tmA, tmB, a);
+      } else if (BN == 128) {
         if (bf) k_dh<1, 128><<<grid, 160, dh_smem, st>>>(tmA, tmB, a);
         else k_dh<0, 128><<<grid, 160, dh_smem, st>>>(tmA, tmB, a);
       } else {
@@ -1040,10 +1192,13 @@ int backward_mlp_tc(const Plan* P, const Weights* W, const float* edge_attr, con
     s = launch_build_a1(W->prec, edge_attr, P->perm, e_base, n, k_in, A1, st);
     if (s) return s;
     if (nl >= 3 && acts == nullptr) {
-      s = launch_gemm_tc(W->prec, A1, n, 0, n, 64, W->W1aug, W->kp[1], nullptr, 1, act[1], W->kp[1], st);
+      s = launch_gemm_tc(W->prec, A1, n, 0, n, 64, W->W1aug, W->kp[1], nullptr, 1, act[1], pm * W->kp[1], st, nullptr, 0, 0,
+                         sp ? GEMM_C_SPLIT : 0);
       if (s) return s;
       for (int l = 2; l <= nl - 2; ++l) {
-        s = launch_gemm_tc(W->prec, act[l - 1], n, 0, n, W->kp[l - 1], W->Wh[l], W->kp[l], W->bh[l], 1, act[l], W->kp[l], st);
+        s = launch_gemm_tc(W->prec, act[l - 1], n, 0, n, kmul * W->kp[l - 1], W->Wh[l], W->kp[l], W->bh[l], 1, act[l],
+                           pm * W->kp[l], st, nullptr, 0, 0, sp ? (GEMM_A_SPLIT | GEMM_C_SPLIT) : 0, nullptr, nullptr, 0, 0, 0,
+                           sp ? W->wscale + 2 * l + 1 : nullptr);
         if (s) return s;
       }
     }
@@ -1055,24 +1210,26 @@ int backward_mlp_tc(const Plan* P, const Weights* W, const float* edge_attr, con
       // D_l[j, :] += dz_l^T A1   (column 3*k_in = the bias gradient; for l = 1 also dW_1 in split form); the top
       // layer's column comes out of k_dh when fused
       if (!(fuse_colsum && l == nl - 1)) {
-        s = launch_gemm_tn(W->prec, cur, W->kp[l], 0, A1, 64, 0, n, W->kp[l], 64, Dl, 64, 1.f, nullptr, st);
+        s = gemm_tn_pairs(W, cur, pm * W->kp[l], W->kp[l], A1, 64, -1, n, W->kp[l], 64, Dl, 64, st);
         if (s) return s;
       }
       if (l >= 2) {
         float* dWl = reinterpret_cast<float*>(base + L.off_dW[l]);
-        s = launch_gemm_tn(W->prec, cur, W->kp[l], 0, act[l - 1], W->kp[l - 1], 0, n, W->kp[l], W->kp[l - 1], dWl,
-                           W->kp[l - 1], 1.f, nullptr, st);
+        s = gemm_tn_pairs(W, cur, pm * W->kp[l], W->kp[l], act[l - 1], pm * W->kp[l - 1], W->kp[l - 1], n, W->kp[l],
+                          W->kp[l - 1], dWl, W->kp[l - 1], st);
         if (s) return s;
-        // dz_{l-1} = (dz_l W_l) * [h_{l-1} > 0]
-        s = launch_gemm_tc(W->prec, cur, n, 0, n, W->kp[l], W->WhT[l], W->kp[l - 1], nullptr, 0, nxt, W->kp[l - 1], st,
-                           nullptr, 0, 0, 0, nullptr, act[l - 1], W->kp[l - 1], 0);
+        // dz_{l-1} = (dz_l W_l) * [h_{l-1} > 0]   (PREC_F16X2: the mask is the hi half of the activation pair)
+        s = launch_gemm_tc(W->prec, cur, n, 0, n, kmul * W->kp[l], W->WhT[l], W->kp[l - 1], nullptr, 0, nxt,
+                           pm * W->kp[l - 1], st, nullptr, 0, 0, sp ? (GEMM_A_SPLIT | GEMM_C_SPLIT) : 0, nullptr, act[l - 1],
+                           pm * W->kp[l - 1], 0, 0, sp ? W->wscale + 2 * l + 1 : nullptr);
         if (s) return s;
         uint16_t* tmp = cur; cur = nxt; nxt = tmp;
       }
     }
     // ---- cur = dz_1 of the batch (summed over the applications): grad_edge_attr rows of its edges
     if (grad_ea != nullptr) {
-      auto kern = k_in <= 8 ? (bf ? k_ea_grad<1, 8> : k_ea_grad<0, 8>) : (bf ? k_ea_grad<1, 20> : k_ea_grad<0, 20>);
+      auto kern = sp ? (k_in <= 8 ? k_ea_grad<0, 8, 1> : k_ea_grad<0, 20, 1>)
+                     : k_in <= 8 ? (bf ? k_ea_grad<1, 8> : k_ea_grad<0, 8>) : (bf ? k_ea_grad<1, 20> : k_ea_grad<0, 20>);
       // as many resident CTAs as fit (a bandwidth-bound stream: every resident warp keeps loads in flight)
       int per_sm = 0;
       NNC_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, 256, ea_smem));

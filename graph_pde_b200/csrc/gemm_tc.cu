@@ -84,13 +84,16 @@ struct GemmCfg {
 //   EPI_PLAIN bias / ReLU / 16-bit store     EPI_SPLIT the same, written as (hi, lo) fp16 pairs (PREC_F16X2)
 //   EPI_MASK  ReLU-derivative mask from a stored activation (backward)     EPI_F32 fp32 output, plain stores
 //   EPI_NOCHECK = EPI_PLAIN without the fp16 range tracking (bf16 outputs, option overflow_check = 0, test hooks)
-enum { EPI_PLAIN = 0, EPI_SPLIT = 1, EPI_MASK = 2, EPI_F32 = 3, EPI_NOCHECK = 4 };
+//   EPI_MASK_SPLIT = EPI_MASK with acc_scale, written as (hi, lo) pairs (PREC_F16X2 backward; the mask is the hi half)
+enum { EPI_PLAIN = 0, EPI_SPLIT = 1, EPI_MASK = 2, EPI_F32 = 3, EPI_NOCHECK = 4, EPI_MASK_SPLIT = 5 };
 
 template <int BLOCK_N, int FMT, int SMALL, int EPI>
 __global__ void __launch_bounds__(288, SMALL ? 2 : 1)
 k_gemm_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
           const __grid_constant__ CUtensorMap tmC, GemmTcArgs a) {
   using Cfg = GemmCfg<BLOCK_N, SMALL>;
+  constexpr bool kSplitOut = EPI == EPI_SPLIT || EPI == EPI_MASK_SPLIT;
+  constexpr bool kMask = EPI == EPI_MASK || EPI == EPI_MASK_SPLIT;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
   uint8_t* smem = smem_raw + (((raw + 1023u) & ~1023u) - raw);
@@ -185,7 +188,7 @@ k_gemm_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
       uint16_t* crow = reinterpret_cast<uint16_t*>(a.C) + static_cast<int64_t>(row) * a.ldc;
       const int64_t grow = a.c_row0 + row;
       uint32_t v[32];
-      const float accs = (EPI == EPI_SPLIT && a.acc_scale != nullptr) ? __ldg(a.acc_scale) : 1.f;
+      const float accs = (kSplitOut && a.acc_scale != nullptr) ? __ldg(a.acc_scale) : 1.f;
       const bool use_tma = Cfg::kStoreBytes > 0 && a.tma_store != 0;
       // this warp's staging: 2 buffers of 32 rows x 64 B; 16-byte unit u of row r sits at (u ^ ((r >> 1) & 3))
       // (SWIZZLE_64B of tmC) -- conflict-free for the 8-lane phases of a v4 shared store
@@ -197,10 +200,10 @@ k_gemm_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
         const int col0 = nb * BLOCK_N + half * (BLOCK_N / 2) + cc * 32;
         if (col0 < a.N && (row_ok || use_tma)) {
           const uint32_t* vv = v;
-          uint32_t packed[16], packed_lo[EPI == EPI_SPLIT ? 16 : 1];
+          uint32_t packed[16], packed_lo[kSplitOut ? 16 : 1];
           float vm[4] = {0.f, 0.f, 0.f, 0.f};       // four independent max chains (one chain of 32 is latency bound)
           uint32_t mkw[16];                         // EPI_MASK: the row's 32 stored activations (64 B, four 16-byte loads)
-          if (EPI == EPI_MASK && row_ok) {
+          if (kMask && row_ok) {
             const uint4* mp = reinterpret_cast<const uint4*>(a.mask + static_cast<int64_t>(row) * a.mask_ld + col0);
 #pragma unroll
             for (int q = 0; q < 4; ++q) {
@@ -212,7 +215,7 @@ k_gemm_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
           for (int j4 = 0; j4 < 8; ++j4) {
             float f[4] = {__uint_as_float(vv[4 * j4]), __uint_as_float(vv[4 * j4 + 1]),
                           __uint_as_float(vv[4 * j4 + 2]), __uint_as_float(vv[4 * j4 + 3])};
-            if (EPI == EPI_SPLIT) {
+            if (kSplitOut) {
 #pragma unroll
               for (int q = 0; q < 4; ++q) f[q] *= accs;
             }
@@ -229,7 +232,7 @@ k_gemm_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
 #pragma unroll
               for (int q = 0; q < 4; ++q) f[q] = fmaxf(f[q], 0.f);
             }
-            if (EPI == EPI_MASK) {
+            if (kMask) {
               if (row_ok) {
                 const uint32_t mx = mkw[2 * j4], my = mkw[2 * j4 + 1];
                 if ((mx & 0x7FFFu) == 0u) f[0] = 0.f;
@@ -252,7 +255,7 @@ k_gemm_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
                 if (FMT == 0) {
                   __half2 h = __floats2half2_rn(f[2 * q], f[2 * q + 1]);
                   packed[2 * j4 + q] = *reinterpret_cast<uint32_t*>(&h);
-                  if (EPI == EPI_SPLIT) {
+                  if (kSplitOut) {
                     const float2 hf = __half22float2(h);
                     __half2 l = __floats2half2_rn(f[2 * q] - hf.x, f[2 * q + 1] - hf.y);
                     packed_lo[2 * j4 + q] = *reinterpret_cast<uint32_t*>(&l);
@@ -306,7 +309,7 @@ k_gemm_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
           };
           if (EPI != EPI_F32) {
             store_piece(packed, col0);
-            if (FMT == 0 && EPI == EPI_SPLIT) store_piece(packed_lo, col0 + a.N);
+            if (FMT == 0 && kSplitOut) store_piece(packed_lo, col0 + a.N);
           }
         }
       }
@@ -382,7 +385,11 @@ int launch_gemm_tc(int prec, const void* A_base, int64_t a_rows_total, int64_t a
               "gemm_tc: C must be 32-byte aligned with ldc a multiple of 16 elements");
   const int bf = prec == PREC_BF16;
   const bool small = pf && pf->small_footprint && N >= 128;
-  const int BN = small ? 128 : (N % 256 == 0 || N > 256) ? 256 : (N % 128 == 0 || N > 128) ? 128 : 64;
+  // the split mask epilogue (two output pieces plus the mask words per 32 columns) spills at BLOCK_N = 256
+  const bool mask_split = mask != nullptr && c_split;
+  const int BN = small ? 128
+                 : mask_split ? ((N % 128 == 0 || N > 128) ? 128 : 64)
+                 : (N % 256 == 0 || N > 256) ? 256 : (N % 128 == 0 || N > 128) ? 128 : 64;
   CUtensorMap tmA, tmB;
   if (a_chunk_rows_pad > 0) {
     NNC_REQUIRE(!a_split && static_cast<int64_t>(K / 64) * a_chunk_rows_pad < (int64_t(1) << 31), NNCONV_ERR_ARG,
@@ -447,7 +454,12 @@ int launch_gemm_tc(int prec, const void* A_base, int64_t a_rows_total, int64_t a
     return bf ? launch_gemm_cfg<64, 1, 0, E>(tmA, tmB, tmC, a, st, pdl) : launch_gemm_cfg<64, 0, 0, E>(tmA, tmB, tmC, a, st, pdl); \
   } while (0)
   if (out_f32) { NNC_REQUIRE(!small && !c_split && mask == nullptr, NNCONV_ERR_ARG, "gemm_tc: fp32 output excludes split / mask"); NNC_GEMM_EPI(EPI_F32); }
-  if (mask != nullptr) { NNC_REQUIRE(!small && !c_split, NNCONV_ERR_ARG, "gemm_tc: mask excludes split"); NNC_GEMM_EPI(EPI_MASK); }
+  if (mask_split) {
+    NNC_REQUIRE(!small && !bf, NNCONV_ERR_ARG, "gemm_tc: split mask epilogue is fp16 only");
+    if (BN == 128) return launch_gemm_cfg<128, 0, 0, EPI_MASK_SPLIT>(tmA, tmB, tmC, a, st, pdl);
+    return launch_gemm_cfg<64, 0, 0, EPI_MASK_SPLIT>(tmA, tmB, tmC, a, st, pdl);
+  }
+  if (mask != nullptr) { NNC_REQUIRE(!small, NNCONV_ERR_ARG, "gemm_tc: mask excludes the small-footprint configuration"); NNC_GEMM_EPI(EPI_MASK); }
   if (c_split) {
     NNC_REQUIRE(!small, NNCONV_ERR_ARG, "gemm_tc: split output excludes the small-footprint configuration");
     if (BN == 256) return launch_gemm_cfg<256, 0, 0, EPI_SPLIT>(tmA, tmB, tmC, a, st, pdl);

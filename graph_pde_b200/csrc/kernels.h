@@ -13,10 +13,12 @@ int launch_w3p(int prec, const float* WL, int cin, int cout, int K, int Kp, int 
 int launch_pow2_scale(const float* src, int64_t n, float* scale2, cudaStream_t st);
 int launch_pad_convert_split3(const float* src, int R, int C, void* dst, int Rp, int Cp, const float* scale, cudaStream_t st);
 // backward images of the last Linear: transposed == 0 -> W3q [Kp*cout, cin_p], 1 -> W3t [cin_p, Kp*cout]
+// (PREC_F16X2: the reduction dimension is tripled, [hi | lo | hi], and the values are multiplied by *scale first)
 int launch_w3q(int prec, const float* WL, int cin, int cout, int K, int Kp, int cin_p, int transposed, void* dst,
-               cudaStream_t st);
-// dst[Cp x Rp] (16-bit) = src[R x C]^T, zero padded
-int launch_transpose_pad(int prec, const float* src, int R, int C, void* dst, int Rp, int Cp, cudaStream_t st);
+               cudaStream_t st, const float* scale = nullptr);
+// dst[Cp x Rp] (16-bit) = src[R x C]^T, zero padded (PREC_F16X2: [Cp x 3*Rp], [hi | lo | hi] of *scale times the value)
+int launch_transpose_pad(int prec, const float* src, int R, int C, void* dst, int Rp, int Cp, cudaStream_t st,
+                         const float* scale = nullptr);
 int launch_edge_layer1(int prec, const float* edge_attr, const int* perm, int64_t e_begin, int64_t e_count, int k_in,
                        const float* W1, const float* b1, int kp1, int identity, void* out, cudaStream_t st,
                        int64_t chunk_rows_pad = 0, int64_t out_row0 = 0);

@@ -124,6 +124,40 @@ __global__ void k_w3p_split3(const float* __restrict__ WL, int cin, int cout, in
   const float v = (i < cin && k < K) ? WL[(static_cast<int64_t>(i) * cout + o) * K + k] * (scale ? scale[0] : 1.f) : 0.f;
   dst[idx] = split_part(v, part);
 }
+// backward images of the split last Linear (see k_w3q), pre-scaled like W3p:
+//   transposed == 0: W3q [Kp*cout, 3*cin_p], column part*cin_p + i;  1: W3t [cin_p, 3*Kp*cout], column part*NY + (k*cout + o)
+__global__ void k_w3q_split3(const float* __restrict__ WL, int cin, int cout, int K, int Kp, int cin_p, int transposed,
+                             __half* __restrict__ dst, const float* __restrict__ scale) {
+  const int64_t idx = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
+  const int64_t NY = static_cast<int64_t>(Kp) * cout;
+  if (idx >= 3 * NY * cin_p) return;
+  int i, part;
+  int64_t ko;
+  if (transposed) {
+    i = static_cast<int>(idx / (3 * NY));
+    const int64_t cc = idx % (3 * NY);
+    part = static_cast<int>(cc / NY);
+    ko = cc % NY;
+  } else {
+    const int ii = static_cast<int>(idx % (3 * cin_p));
+    part = ii / cin_p;
+    i = ii % cin_p;
+    ko = idx / (3 * cin_p);
+  }
+  const int o = static_cast<int>(ko % cout), k = static_cast<int>(ko / cout);
+  const float v = (i < cin && k < K) ? WL[(static_cast<int64_t>(i) * cout + o) * K + k] * scale[0] : 0.f;
+  dst[idx] = split_part(v, part);
+}
+// dst[c, part*Rp + r] ([Cp, 3*Rp]) = split part of scale * src[r, c] (src [R, C]), zero padded
+__global__ void k_transpose_pad_split3(const float* __restrict__ src, int R, int C, __half* __restrict__ dst, int Rp,
+                                       int Cp, const float* __restrict__ scale) {
+  const int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
+  if (i >= static_cast<int64_t>(Cp) * 3 * Rp) return;
+  const int c = static_cast<int>(i / (3 * Rp)), rr = static_cast<int>(i % (3 * Rp));
+  const int part = rr / Rp, r = rr % Rp;
+  const float v = (r < R && c < C) ? src[static_cast<int64_t>(r) * C + c] * scale[0] : 0.f;
+  dst[i] = split_part(v, part);
+}
 
 // First layer: h1[p, j] = relu(b1[j] + sum_c W1[j, c] * edge_attr[perm[p], c]),  j < kp1 (pad rows of W1/b1 are 0)
 // identity (single-Linear MLP): h[p, j] = edge_attr[perm[p], j] (zero padded), no ReLU.
@@ -733,18 +767,33 @@ int launch_w3p(int prec, const float* WL, int cin, int cout, int K, int Kp, int 
 }
 
 int launch_w3q(int prec, const float* WL, int cin, int cout, int K, int Kp, int cin_p, int transposed, void* dst,
-               cudaStream_t st) {
+               cudaStream_t st, const float* scale) {
   const int64_t total = static_cast<int64_t>(cout) * Kp * cin_p;
   const unsigned g = (unsigned)ceil_div64(total, 256);
+  if (prec == PREC_F16X2) {
+    NNC_REQUIRE(scale != nullptr, NNCONV_ERR_ARG, "w3q: split images need their power-of-two scale");
+    k_w3q_split3<<<(unsigned)ceil_div64(3 * total, 256), 256, 0, st>>>(WL, cin, cout, K, Kp, cin_p, transposed,
+                                                                       static_cast<__half*>(dst), scale);
+    NNC_CHECK_LAUNCH();
+    return NNCONV_OK;
+  }
   if (prec == PREC_F16) k_w3q<__half><<<g, 256, 0, st>>>(WL, cin, cout, K, Kp, cin_p, transposed, static_cast<__half*>(dst));
   else k_w3q<__nv_bfloat16><<<g, 256, 0, st>>>(WL, cin, cout, K, Kp, cin_p, transposed, static_cast<__nv_bfloat16*>(dst));
   NNC_CHECK_LAUNCH();
   return NNCONV_OK;
 }
 
-int launch_transpose_pad(int prec, const float* src, int R, int C, void* dst, int Rp, int Cp, cudaStream_t st) {
+int launch_transpose_pad(int prec, const float* src, int R, int C, void* dst, int Rp, int Cp, cudaStream_t st,
+                         const float* scale) {
   const int64_t total = static_cast<int64_t>(Rp) * Cp;
   const unsigned g = (unsigned)ceil_div64(total, 256);
+  if (prec == PREC_F16X2) {
+    NNC_REQUIRE(scale != nullptr, NNCONV_ERR_ARG, "transpose_pad: split images need their power-of-two scale");
+    k_transpose_pad_split3<<<(unsigned)ceil_div64(3 * total, 256), 256, 0, st>>>(src, R, C, static_cast<__half*>(dst), Rp,
+                                                                                 Cp, scale);
+    NNC_CHECK_LAUNCH();
+    return NNCONV_OK;
+  }
   if (prec == PREC_F16) k_transpose_pad<__half><<<g, 256, 0, st>>>(src, R, C, static_cast<__half*>(dst), Rp, Cp);
   else k_transpose_pad<__nv_bfloat16><<<g, 256, 0, st>>>(src, R, C, static_cast<__nv_bfloat16*>(dst), Rp, Cp);
   NNC_CHECK_LAUNCH();

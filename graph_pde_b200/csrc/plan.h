@@ -60,16 +60,17 @@ struct Weights {
   const float* bh[kMaxLayers];  // [kp[l]] fp32
   const void* W3p;              // [cout*Kp, cin_p] in `prec`:  W3p[(o*Kp + k), i] = W_L[i*cout + o, k] (split: 3*cin_p columns)
   const float* B3;              // [cin, cout] fp32 = b_L viewed (in, out)
-  // extra images for the tensor-core backward (16-bit, non-split precisions only; nullptr otherwise)
+  // extra images for the tensor-core backward (16-bit precisions; PREC_F16X2: split [hi | lo | hi] along the reduction
+  // dimension and pre-scaled by wscale like W3p / Wh; nullptr when the backward does not cover the shape)
   // PREC_F16X2: every split weight matrix is stored multiplied by a power of two that brings its largest entry
   // into [0.5, 1) -- the lo halves of U(+-1/32)-sized weights would otherwise be fp16 subnormals (8 instead of 11
   // bits) -- and the epilogue multiplies the fp32 accumulator by the inverse.  wscale[2*l] = scale of layer l's
   // matrix (l = n_layers: the last Linear), wscale[2*l + 1] = its inverse; device floats, nullptr when not split.
   const float* wscale;
   const void* W3n;              // [cin*cout, Kp]: the last Linear in its own layout, padded (per-edge kernel matrices)
-  const void* W3q;              // [Kp*cout, cin_p]:  W3q[(k*cout + o), i] = W_L[i*cout + o, k]   (Y^T rows per source)
-  const void* W3t;              // [cin_p, Kp*cout]:  W3t[i, (k*cout + o)] = W_L[i*cout + o, k]   (dx = dY : W_L)
-  const void* WhT[kMaxLayers];  // hidden layers l = 2 .. L-1 transposed: [kp[l-1], kp[l]]       (dz_{l-1} = dz_l W_l)
+  const void* W3q;              // [Kp*cout, cin_p]:  W3q[(k*cout + o), i] = W_L[i*cout + o, k]   (Y^T rows per source; split: 3*cin_p)
+  const void* W3t;              // [cin_p, Kp*cout]:  W3t[i, (k*cout + o)] = W_L[i*cout + o, k]   (dx = dY : W_L; split: 3*Kp*cout)
+  const void* WhT[kMaxLayers];  // hidden layers l = 2 .. L-1 transposed: [kp[l-1], kp[l]]  (dz_{l-1} = dz_l W_l; split: 3*kp[l])
 };
 
 size_t weights_bytes(int n_layers, const int* dims, int cin, int cout, int prec);

@@ -173,7 +173,7 @@ int nnconv_backward_ex(const nnconv_plan_t* plan, const nnconv_weights_t* w, con
                        float* const* grad_b, float* grad_root, float* grad_bias, void* ws, size_t ws_bytes,
                        void* stream, float* grad_edge_attr /* nullable */);
 
-/* ---- tensor-core backward (16-bit precisions, out_channels = 64, in_channels <= 64, edge MLP with >= 2 Linear
+/* ---- tensor-core backward (f16, bf16, f16x2; out_channels = 64, in_channels <= 64, edge MLP with >= 2 Linear
  * layers; nnconv_backward_tc_supported tells).  Split in two because the edge features h do not depend on x:
  *
  *   nnconv_backward_apply   one call per application, given that application's grad_out: writes grad_x,

@@ -4,7 +4,12 @@ cudaProfilerStart/Stop so that `ncu --profile-from-start off` sees exactly one s
 
     ncu --metrics gpu__time_duration.sum --clock-control none --profile-from-start off --csv \
         --log-file gpurun_out/train_launches.csv python scripts/train_probe.py [darcy241|darcy85]
-Without ncu it prints the CUDA-event time of the step.
+Without ncu it prints the CUDA-event time of the step (the median of --rounds steps), the device and its power limit.
+
+    python scripts/train_probe.py darcy85 --precision f16x2 [--backward fp32] [--rounds N] [--kernels]
+selects the operand precision of the step and pins the backward to the fp32 CUDA-core path (--backward fp32; the
+default 'auto' takes the tensor-core backward where it covers the shapes); --kernels adds a torch.profiler table of
+the per-kernel CUDA times of one step.
 
     python scripts/train_probe.py [darcy241|darcy85] --edge-attr-grad [--rounds N]
 times the same step with edge_attr built from a coefficient field theta by graphs.ball_edge_attr, once with theta a
@@ -52,12 +57,17 @@ def main():
     ap.add_argument('workload', nargs='?', default='darcy241', choices=sorted(WORKLOADS))
     ap.add_argument('--edge-attr-grad', action='store_true')
     ap.add_argument('--rounds', type=int, default=5)
+    ap.add_argument('--precision', default='f16', choices=['f16', 'bf16', 'f16x2'])
+    ap.add_argument('--backward', default='auto', choices=['auto', 'fp32'])
+    ap.add_argument('--kernels', action='store_true')
     args = ap.parse_args()
+    from graph_pde_b200 import nn_conv
+    nn_conv._BWD_MODE = args.backward
     cfg = WORKLOADS[args.workload]
     dev = torch.device('cuda:0')
     s, r, w, kw, T = cfg['s'], cfg['r'], cfg['width'], cfg['ker_width'], cfg['depth']
     torch.manual_seed(0)
-    model = KernelNN(w, kw, T, 6, in_width=6, precision='f16').to(dev)
+    model = KernelNN(w, kw, T, 6, in_width=6, precision=args.precision).to(dev)
     opt = torch.optim.Adam(model.parameters(), lr=1e-4)
     x6, ei, ea = graphs.darcy_sample(s, r, dev, seed=0)
     y = torch.randn(s * s, 1, device=dev)
@@ -75,9 +85,20 @@ def main():
         step()
         torch.cuda.synchronize()
         torch.cuda.profiler.start()
-        ms = _timed(step)
+        times = [_timed(step)]
         torch.cuda.profiler.stop()
-        print('one training step: %.2f ms (E=%d, T=%d)' % (ms, ei.size(1), T))
+        for _ in range(args.rounds - 1):
+            times.append(_timed(step))
+        n_mlp = nn_conv.stats.get('mlp_backwards', 0)
+        print('device: %s, power limit: %s' % (torch.cuda.get_device_name(dev), _power_limit()))
+        print('%s: E=%d, T=%d, width=%d, ker_width=%d, precision=%s, backward=%s (tensor-core MLP passes so far: %d)' % (
+            args.workload, ei.size(1), T, w, kw, args.precision, args.backward, n_mlp))
+        print('training step: median %.2f ms  (all: %s)' % (statistics.median(times), ', '.join('%.2f' % v for v in times)))
+        if args.kernels:
+            with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
+                step()
+                torch.cuda.synchronize()
+            print(prof.key_averages().table(sort_by='cuda_time_total', row_limit=25, max_name_column_width=90))
         return
 
     # theta = the coefficient column of the node features (darcy_sample: x = [grid, a, ...], edge_attr uses a)
