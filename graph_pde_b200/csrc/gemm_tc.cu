@@ -4,11 +4,14 @@
 // Linear + ReLU) over a chunk of edges and (b) the per-source matrices
 // Y[c, (o,k)] = sum_i x[c, i] * W_L[i*out + o, k]  (the last Linear reassociated, nn_conv.py:274-275).
 //
-// Structure: persistent CTAs (grid = #SMs), 9 warps: warps 0..7 = two consumer warpgroups, each owning half of
+// Structure: persistent CTAs (grid = #SMs), 12 warps: warps 0..7 = two consumer warpgroups, each owning half of
 // the BLOCK_N columns of the tile (wgmma into registers, then the epilogue: bias/ReLU -> 16-bit -> per-warp
-// swizzled smem piece -> TMA store; direct 32-byte stores for pipelined / small launches), warp 8 = TMA producer.
-// Operands are K-major 128B-swizzled tiles [128 x 64] / [BLOCK_N x 64] staged by TMA in a ring of kStages, so the
-// producer runs ahead into the next tile while the warpgroups run the epilogue of this one.
+// swizzled smem piece -> TMA store; direct 32-byte stores for pipelined / small launches), warps 8..11 = the TMA
+// producer warpgroup (warp 8 loops, one elected lane issues).  The producer gives its registers to the consumers
+// (setmaxnreg), so a [128 x 128] fp32 accumulator per warpgroup and the epilogue fit without spilling.  The SMALL
+// configuration keeps a single producer warp (9 warps) so that two CTAs share an SM.  Operands are K-major
+// 128B-swizzled tiles [128 x 64] / [BLOCK_N x 64] staged by TMA in a ring of kStages, so the producer runs ahead
+// into the next tile while the warpgroups run the epilogue of this one.
 #include "kernels.h"
 #include "options.h"
 #include "tc05.cuh"
@@ -61,11 +64,16 @@ struct GemmTcArgs {
   unsigned int trace_seq;
 };
 
-// SMALL = 1: a 2-stage, BLOCK_N = 128 footprint (~101 KB smem) that can share an SM with a
+// SMALL = 1: a 2-stage, BLOCK_N = 128, 288-thread footprint (~101 KB smem) that can share an SM with a
 // contraction CTA or a second GEMM CTA -- used for the per-source Y GEMM, which is store bound and runs
 // concurrently with the contraction of the previous batch.
 template <int BLOCK_N, int SMALL = 0>
 struct GemmCfg {
+  static constexpr int kThreads = SMALL ? 288 : 384;
+  // setmaxnreg budgets of the 384-thread CTA: (40 + 2 * 232) * 128 = 64512 <= 65536 registers, the launch-time
+  // allocation of 168 per thread (65536 / 384 rounded down to a multiple of 8)
+  static constexpr uint32_t kProducerRegs = 40;
+  static constexpr uint32_t kConsumerRegs = 232;
   static constexpr int kBlockM = 128;
   static constexpr int kBlockK = 64;
   static constexpr int kABytes = kBlockM * kBlockK * 2;
@@ -88,7 +96,7 @@ struct GemmCfg {
 enum { EPI_PLAIN = 0, EPI_SPLIT = 1, EPI_MASK = 2, EPI_F32 = 3, EPI_NOCHECK = 4, EPI_MASK_SPLIT = 5 };
 
 template <int BLOCK_N, int FMT, int SMALL, int EPI>
-__global__ void __launch_bounds__(288, SMALL ? 2 : 1)
+__global__ void __launch_bounds__(GemmCfg<BLOCK_N, SMALL>::kThreads, SMALL ? 2 : 1)
 k_gemm_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
           const __grid_constant__ CUtensorMap tmC, GemmTcArgs a) {
   using Cfg = GemmCfg<BLOCK_N, SMALL>;
@@ -122,40 +130,47 @@ k_gemm_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
     }
     fence_barrier_init();
   }
-  const unsigned long long tr0 = a.trace.rec ? gtime() : 0ull;
+  // trace times of thread 0 (which writes the record), kept in shared memory rather than in registers that would
+  // stay live through the mainloop and the epilogue
+  __shared__ unsigned long long trace_t[2];
+  if (threadIdx.x == 0 && a.trace.rec) trace_t[0] = gtime();
   pdl_launch_dependents();
   if (a.wait_ok != nullptr && threadIdx.x == 0) flag_wait(a.wait_ok);
-  const unsigned long long tr1 = a.trace.rec ? gtime() : 0ull;
+  if (threadIdx.x == 0 && a.trace.rec) trace_t[1] = gtime();
   __syncthreads();
 
-  if (warp == 8) {
-    // -------------------------------------------------------------- TMA producer (whole warp, elected lane issues)
-    int stage = 0;
-    uint32_t phase = 0;
-    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-      const int mb = t / n_blocks, nb = t % n_blocks;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(&empty[stage], phase ^ 1u);
-        if (elect_one()) {
-          mbar_arrive_expect_tx(&full[stage], Cfg::kStageBytes);
-          const int ka = (a.a_split_nk > 0 && kb >= a.a_split_nk) ? kb - a.a_split_nk : kb;
-          if (a.a_chunk_rows_pad > 0)
-            tma_load_2d(smem_a + stage * Cfg::kABytes, &tmA, &full[stage], 0,
-                        static_cast<int>(ka * a.a_chunk_rows_pad) + a.a_row0 + mb * Cfg::kBlockM, kEvictNormal);
-          else
-            tma_load_2d(smem_a + stage * Cfg::kABytes, &tmA, &full[stage], ka * Cfg::kBlockK,
-                        a.a_row0 + mb * Cfg::kBlockM, kEvictNormal);
-          tma_load_2d(smem_b + stage * Cfg::kBBytes, &tmB, &full[stage], kb * Cfg::kBlockK, nb * BLOCK_N,
-                      a.b_policy);
+  if (warp >= 8) {
+    // -------------------------------------------------------------- TMA producer (warp 8 loops, elected lane issues)
+    if (!SMALL) warpgroup_reg_dealloc<Cfg::kProducerRegs>();
+    if (warp == 8) {
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
+        const int mb = t / n_blocks, nb = t % n_blocks;
+        for (int kb = 0; kb < num_kb; ++kb) {
+          mbar_wait(&empty[stage], phase ^ 1u);
+          if (elect_one()) {
+            mbar_arrive_expect_tx(&full[stage], Cfg::kStageBytes);
+            const int ka = (a.a_split_nk > 0 && kb >= a.a_split_nk) ? kb - a.a_split_nk : kb;
+            if (a.a_chunk_rows_pad > 0)
+              tma_load_2d(smem_a + stage * Cfg::kABytes, &tmA, &full[stage], 0,
+                          static_cast<int>(ka * a.a_chunk_rows_pad) + a.a_row0 + mb * Cfg::kBlockM, kEvictNormal);
+            else
+              tma_load_2d(smem_a + stage * Cfg::kABytes, &tmA, &full[stage], ka * Cfg::kBlockK,
+                          a.a_row0 + mb * Cfg::kBlockM, kEvictNormal);
+            tma_load_2d(smem_b + stage * Cfg::kBBytes, &tmB, &full[stage], kb * Cfg::kBlockK, nb * BLOCK_N,
+                        a.b_policy);
+          }
+          __syncwarp();
+          if (++stage == Cfg::kStages) { stage = 0; phase ^= 1u; }
         }
-        __syncwarp();
-        if (++stage == Cfg::kStages) { stage = 0; phase ^= 1u; }
       }
     }
   } else {
     // ---------------------------------------------------------------- consumer warpgroups (warps 0..7)
     // warpgroup `half` computes columns [half * BLOCK_N / 2, (half + 1) * BLOCK_N / 2) of the tile, then stores them;
     // warp `quarter` of it owns tile rows acc_row(quarter, lane) in the epilogue
+    if (!SMALL) warpgroup_reg_alloc<Cfg::kConsumerRegs>();
     const int quarter = warp % 4;
     const int half = warp / 4;
     constexpr int kChunks = BLOCK_N / 64;          // 32-column chunks per half
@@ -202,15 +217,9 @@ k_gemm_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
           const uint32_t* vv = v;
           uint32_t packed[16], packed_lo[kSplitOut ? 16 : 1];
           float vm[4] = {0.f, 0.f, 0.f, 0.f};       // four independent max chains (one chain of 32 is latency bound)
-          uint32_t mkw[16];                         // EPI_MASK: the row's 32 stored activations (64 B, four 16-byte loads)
-          if (kMask && row_ok) {
-            const uint4* mp = reinterpret_cast<const uint4*>(a.mask + static_cast<int64_t>(row) * a.mask_ld + col0);
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {
-              const uint4 m = __ldg(mp + q);
-              mkw[4 * q] = m.x; mkw[4 * q + 1] = m.y; mkw[4 * q + 2] = m.z; mkw[4 * q + 3] = m.w;
-            }
-          }
+          // EPI_MASK: the row's 32 stored activations (64 B), one 16-byte load per 8 columns
+          const uint4* mp = reinterpret_cast<const uint4*>(a.mask + static_cast<int64_t>(row) * a.mask_ld + col0);
+          uint4 mkw = make_uint4(0u, 0u, 0u, 0u);
 #pragma unroll
           for (int j4 = 0; j4 < 8; ++j4) {
             float f[4] = {__uint_as_float(vv[4 * j4]), __uint_as_float(vv[4 * j4 + 1]),
@@ -234,7 +243,8 @@ k_gemm_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
             }
             if (kMask) {
               if (row_ok) {
-                const uint32_t mx = mkw[2 * j4], my = mkw[2 * j4 + 1];
+                if (j4 % 2 == 0) mkw = __ldg(mp + j4 / 2);
+                const uint32_t mx = j4 % 2 ? mkw.z : mkw.x, my = j4 % 2 ? mkw.w : mkw.y;
                 if ((mx & 0x7FFFu) == 0u) f[0] = 0.f;
                 if ((mx & 0x7FFF0000u) == 0u) f[1] = 0.f;
                 if ((my & 0x7FFFu) == 0u) f[2] = 0.f;
@@ -318,7 +328,7 @@ k_gemm_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
   if (Cfg::kStoreBytes > 0 && a.tma_store && warp < 8 && elect_one()) bulk_wait0();
   if (a.done_cnt != nullptr) signal_done(a.done_cnt, a.done_ok);   // includes __syncthreads
   else __syncthreads();
-  if (threadIdx.x == 0) trace_write(a.trace, (100u + (a.K > 64 ? 1u : 0u)) | (a.trace_seq << 12), tr0, tr1, a.trace.rec ? gtime() : 0ull);
+  if (threadIdx.x == 0) trace_write(a.trace, (100u + (a.K > 64 ? 1u : 0u)) | (a.trace_seq << 12), trace_t[0], trace_t[1], a.trace.rec ? gtime() : 0ull);
 }
 
 int g_num_sms = 0;
@@ -338,7 +348,7 @@ int launch_gemm_cfg(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtens
   const int grid = tiles < max_ctas ? tiles : max_ctas;
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3(grid);
-  cfg.blockDim = dim3(288);
+  cfg.blockDim = dim3(Cfg::kThreads);
   cfg.dynamicSmemBytes = Cfg::kSmemBytes;
   cfg.stream = st;
   cudaLaunchAttribute attr[1];
@@ -385,7 +395,7 @@ int launch_gemm_tc(int prec, const void* A_base, int64_t a_rows_total, int64_t a
               "gemm_tc: C must be 32-byte aligned with ldc a multiple of 16 elements");
   const int bf = prec == PREC_BF16;
   const bool small = pf && pf->small_footprint && N >= 128;
-  // the split mask epilogue (two output pieces plus the mask words per 32 columns) spills at BLOCK_N = 256
+  // the split mask epilogue (two output pieces plus the mask words per 32 columns) runs at half width
   const bool mask_split = mask != nullptr && c_split;
   const int BN = small ? 128
                  : mask_split ? ((N % 128 == 0 || N > 128) ? 128 : 64)

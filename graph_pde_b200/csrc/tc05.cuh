@@ -86,6 +86,18 @@ __device__ __forceinline__ void bulk_wait0() { asm volatile("cp.async.bulk.wait_
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
+
+// Register reallocation between warpgroups (setmaxnreg): every warp of the warpgroup executes it; R is a multiple
+// of 8 in [24, 256].  A producer warpgroup hands registers back so the consumer warpgroups can hold their
+// accumulators and run the epilogue without spilling.
+template <uint32_t R>
+__device__ __forceinline__ void warpgroup_reg_dealloc() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R));
+}
+template <uint32_t R>
+__device__ __forceinline__ void warpgroup_reg_alloc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R));
+}
 __device__ __forceinline__ void st_shared_v4(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
   asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
 }

@@ -1,6 +1,9 @@
 #!/usr/bin/env python
 """Time the wgmma GEMM alone (CUDA events) at the edge-MLP chunk shape for several K, next to a pure
-write (memset) and a copy of the same output size: separates 'epilogue/store bound' from 'DRAM write bound'."""
+write (memset), a copy of the same output size and the same product through torch.mm (cuBLAS, fp16) as the
+yardstick: separates 'epilogue/store bound' from 'DRAM write bound'.  The last lines run the product's real
+configuration, the edge-feature pass of a ker_width-1024 conv (overflow check on, bias and ReLU, chunk-major
+output at the edge-feature chunk shape), and report its per-chunk kernel times."""
 import ctypes
 import os
 import sys
@@ -50,6 +53,43 @@ def main():
             t = timed(run)
             print('gemm K=%4d bias=%d %8.1f us  %6.0f GB/s written  %7.1f TFLOP/s' %
                   (K, b is not None, t, out_mb / t * 1e3, 2.0 * M * N * K / t / 1e6))
+        t = timed(lambda: torch.mm(A, B.t(), out=C))
+        print('cublas K=%4d      %8.1f us  %6.0f GB/s written  %7.1f TFLOP/s' %
+              (K, t, out_mb / t * 1e3, 2.0 * M * N * K / t / 1e6))
+        del A, B
+    del C, C2
+    edge_feature_pass(L, dev)
+
+
+def edge_feature_pass(L, dev, chunks=4, width=64, ker_width=1024):
+    """nnconv_edge_features over `chunks` edge-feature chunks of the default workspace (the rows one chunk of the
+    241x241 Darcy graph has), timed per kernel kind with the library's profiler."""
+    from graph_pde_b200 import nn_conv
+    torch.manual_seed(0)
+    n_nodes, rows = 58081, 508288
+    E = chunks * rows
+    ei = torch.randint(0, n_nodes, (2, E), device=dev)
+    ea = torch.rand(E, 6, device=dev)
+    mlp = torch.nn.Sequential(torch.nn.Linear(6, ker_width), torch.nn.ReLU(), torch.nn.Linear(ker_width, ker_width),
+                              torch.nn.ReLU(), torch.nn.Linear(ker_width, width * width))
+    conv = nn_conv.NNConv_old(width, width, mlp, aggr='mean').to(dev)
+    plan = nn_conv.get_plan(ei, n_nodes)
+    prepared = conv._get_prepared('f16')
+    for _ in range(2):
+        conv._h_cache.clear()
+        conv.edge_features(plan, prepared, ea)
+    torch.cuda.synchronize()
+    reps = 3
+    _lib.check(L.nnconv_profile_begin())
+    for _ in range(reps):
+        conv._h_cache.clear()
+        conv.edge_features(plan, prepared, ea)
+    ms_k = (ctypes.c_double * 8)()
+    n_k = (ctypes.c_int64 * 8)()
+    _lib.check(L.nnconv_profile_end(ms_k, n_k, 8))
+    for k, name in ((0, 'edge_layer1'), (1, 'hidden_gemm')):
+        per = ms_k[k] * 1e3 / max(1, n_k[k])
+        print('%-11s E=%d: %d launches, %8.1f us per launch' % (name, E, n_k[k], per))
 
 
 if __name__ == '__main__':
