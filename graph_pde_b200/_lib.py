@@ -35,6 +35,7 @@ SYMBOLS = [
     'nnconv_edge_kernels_sizes', 'nnconv_edge_kernels', 'nnconv_apply_edge',
     'nnconv_edge_acts_sizes', 'nnconv_edge_features_keep', 'nnconv_apply_ex', 'nnconv_apply_edge_ex',
     'nnconv_backward_ex', 'nnconv_backward_mlp_ex',
+    'nnconv_stream_split', 'nnconv_edge_features_prefix', 'nnconv_apply_streamed',
 ]
 
 
@@ -129,6 +130,10 @@ def lib():
                                      c_vp]
     L.nnconv_gemm_16b_ex.argtypes = [c_int, c_vp, c_i64, c_int, c_vp, c_int, c_vp, c_int, c_vp, c_i64, c_vp, c_i64, c_int,
                                      c_vp]
+    L.nnconv_stream_split.argtypes = [c_vp, c_vp, c_sz, c_sz, P(c_i64), P(c_sz), P(c_sz), P(c_i64)]
+    L.nnconv_edge_features_prefix.argtypes = [c_vp, c_vp, c_vp, c_i64, c_vp, c_vp, c_sz, c_vp, P(c_i64)]
+    L.nnconv_apply_streamed.argtypes = [c_vp, c_vp, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_int, ctypes.c_uint, c_vp, c_vp,
+                                        c_sz, c_vp, P(c_i64)]
     for name in SYMBOLS:
         getattr(L, name)
     if L.nnconv_abi_version() != ABI_VERSION:

@@ -242,18 +242,10 @@ size_t edge_acts_bytes(const Plan* P, const Weights* W) {
   return edge_acts_offset(P, W, W->n_layers - 1) + 1024;
 }
 
-int edge_features(const Plan* P, const Weights* W, const float* edge_attr, void* h, void* ws, size_t ws_bytes,
-                  cudaStream_t st, int64_t* launches, void* acts) {
-  if (acts != nullptr && edge_acts_bytes(P, W) == 0) acts = nullptr;
-  const int64_t E = P->E;
-  NNC_REQUIRE(ws != nullptr && ws_bytes >= kEfHeader, NNCONV_ERR_WORKSPACE, "edge_features: workspace too small");
-  int* overflow = static_cast<int*>(ws);
-  NNC_CHECK_CUDA(cudaMemsetAsync(overflow, 0, sizeof(int), st));
-  if (options().l2_reset) cudaCtxResetPersistingL2Cache();   // experiment knob: drop the Y ring's persisting lines
-  if (E == 0) return NNCONV_OK;
-  if (!options().overflow_check) overflow = nullptr;
-  ws = static_cast<char*>(ws) + kEfHeader;
-  ws_bytes -= kEfHeader;
+// h for the sorted edges [e_begin, e_begin + E): h row p holds edge e_begin + p (16-bit: chunk-major panels of
+// round_up(E, 128) rows).  ws / ws_bytes: the workspace past its header; overflow (nullable) accumulates.
+static int edge_features_rows(const Plan* P, const Weights* W, const float* edge_attr, int64_t e_begin, int64_t E, void* h,
+                              void* ws, size_t ws_bytes, int* overflow, cudaStream_t st, int64_t* launches, void* acts) {
   const int nl = W->n_layers;
   const bool tc = tc_shapes_supported(W);
   NNC_REQUIRE(tc || W->prec == PREC_FP32, NNCONV_ERR_UNSUPPORTED,
@@ -271,14 +263,14 @@ int edge_features(const Plan* P, const Weights* W, const float* edge_attr, void*
   }
   if (nl == 1) {   // single Linear: h_last = edge_attr (padded)
     ProfScope ps(PK_LAYER1, st);
-    s = launch_edge_layer1(W->prec, edge_attr, P->perm, 0, E, W->dims[0], nullptr, nullptr, W->Kp, 1, h, st, hpad, 0);
+    s = launch_edge_layer1(W->prec, edge_attr, P->perm, e_begin, E, W->dims[0], nullptr, nullptr, W->Kp, 1, h, st, hpad, 0);
     if (launches) ++*launches;
     return s;
   }
   const size_t rowb = ef_row_bytes(W);
   if (rowb == 0) {   // CUDA-core first layer straight into h (fp32 path, 2-layer MLP)
     ProfScope ps(PK_LAYER1, st);
-    s = launch_edge_layer1(W->prec, edge_attr, P->perm, 0, E, W->dims[0], W->W1, W->b1, W->kp[1], 0, h, st, hpad, 0);
+    s = launch_edge_layer1(W->prec, edge_attr, P->perm, e_begin, E, W->dims[0], W->W1, W->b1, W->kp[1], 0, h, st, hpad, 0);
     if (launches) ++*launches;
     return s;
   }
@@ -299,15 +291,15 @@ int edge_features(const Plan* P, const Weights* W, const float* edge_attr, void*
     {
       ProfScope ps(PK_LAYER1, st);
       if (W->W1aug) {
-        s = launch_build_a1(W->prec, edge_attr, P->perm, e0, n, W->dims[0], a1, st);
+        s = launch_build_a1(W->prec, edge_attr, P->perm, e_begin + e0, n, W->dims[0], a1, st);
         if (s) return s;
         s = launch_gemm_tc(W->prec, a1, n, 0, static_cast<int>(n), 64, W->W1aug, W->kp[1], nullptr, 1, dst1,
                            static_cast<int64_t>(amul) * W->kp[1], st, nullptr, h_pad_l1, e0,
                            W->split ? GEMM_C_SPLIT : 0, overflow);
         if (launches) ++*launches;
       } else {
-        s = launch_edge_layer1(W->prec, edge_attr, P->perm, e0, n, W->dims[0], W->W1, W->b1, W->kp[1], 0, dst1, st,
-                               h_pad_l1, e0);
+        s = launch_edge_layer1(W->prec, edge_attr, P->perm, e_begin + e0, n, W->dims[0], W->W1, W->b1, W->kp[1], 0, dst1,
+                               st, h_pad_l1, e0);
       }
     }
     if (s) return s;
@@ -335,6 +327,20 @@ int edge_features(const Plan* P, const Weights* W, const float* edge_attr, void*
     }
   }
   return NNCONV_OK;
+}
+
+int edge_features(const Plan* P, const Weights* W, const float* edge_attr, void* h, void* ws, size_t ws_bytes,
+                  cudaStream_t st, int64_t* launches, void* acts, int64_t n_edges) {
+  if (acts != nullptr && edge_acts_bytes(P, W) == 0) acts = nullptr;
+  const int64_t E = n_edges < 0 ? P->E : n_edges;
+  NNC_REQUIRE(ws != nullptr && ws_bytes >= kEfHeader, NNCONV_ERR_WORKSPACE, "edge_features: workspace too small");
+  int* overflow = static_cast<int*>(ws);
+  NNC_CHECK_CUDA(cudaMemsetAsync(overflow, 0, sizeof(int), st));
+  if (options().l2_reset) cudaCtxResetPersistingL2Cache();   // experiment knob: drop the Y ring's persisting lines
+  if (E == 0) return NNCONV_OK;
+  if (!options().overflow_check) overflow = nullptr;
+  return edge_features_rows(P, W, edge_attr, 0, E, h, static_cast<char*>(ws) + kEfHeader, ws_bytes - kEfHeader, overflow,
+                            st, launches, acts);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -402,6 +408,23 @@ size_t apply_ws_bytes(const Plan* P, const Weights* W, size_t want_y_bytes) {
   return L.fixed_bytes + nodes * L.per_node + 1024;
 }
 
+// Batch geometry of the fused persistent kernel for a Y region of nodes_cap source matrices: ring slots and sources
+// per batch.  false: the per-batch kernels run instead.
+static bool fused_geometry(const Weights* W, int64_t n_src, int64_t nodes_cap, int* ring_out, int64_t* nb_out) {
+  const Options& opt = options();
+  const bool no_fuse_env = opt.no_fuse != 0 && !W->split;      // measurement / debugging knob
+  if (W->prec == PREC_FP32 || no_fuse_env || !apply_fused_supported(W)) return false;
+  int ring = opt.ring;   // with dynamic unit scheduling 3 x 128 sources (48 MB at out=64, Kp=1024) is best
+  if (opt.ring_deep && nodes_cap / 128 > ring) ring = nodes_cap / 128 < 16 ? static_cast<int>(nodes_cap / 128) : 16;
+  if (nodes_cap < ring) ring = nodes_cap >= 2 ? static_cast<int>(nodes_cap) : 1;
+  int64_t nb = nodes_cap / ring;
+  if (nb >= 128) nb = nb / 128 * 128;
+  if (nb > n_src) nb = n_src;
+  *ring_out = ring;
+  *nb_out = nb;
+  return ring >= 2;
+}
+
 int apply(const Plan* P, const Weights* W, const void* h, const float* x, const float* root, const float* bias,
           int aggr_mean, float* out, void* ws, size_t ws_bytes, cudaStream_t st, int64_t* launches, unsigned node_flags) {
   int s;
@@ -427,18 +450,9 @@ int apply(const Plan* P, const Weights* W, const void* h, const float* x, const 
   int64_t nodes_cap = static_cast<int64_t>((ws_bytes - L.fixed_bytes) / L.per_node);
   const Options& opt = options();
   // fused persistent kernel (below): its batch geometry is needed here because the node-prep launch also clears its flags
-  const bool no_fuse_env = opt.no_fuse != 0 && !W->split;      // measurement / debugging knob
-  bool fused = W->prec != PREC_FP32 && !no_fuse_env && apply_fused_supported(W);
-  int ring = opt.ring;   // with dynamic unit scheduling 3 x 128 sources (48 MB at out=64, Kp=1024) is best
+  int ring = 0;
   int64_t nb = 0;
-  if (fused) {
-    if (opt.ring_deep && nodes_cap / 128 > ring) ring = nodes_cap / 128 < 16 ? static_cast<int>(nodes_cap / 128) : 16;
-    if (nodes_cap < ring) ring = nodes_cap >= 2 ? static_cast<int>(nodes_cap) : 1;
-    nb = nodes_cap / ring;
-    if (nb >= 128) nb = nb / 128 * 128;
-    if (nb > P->n_src) nb = P->n_src;
-    fused = ceil_div64(P->n_src, nb) <= kMaxPipeBatches && ring >= 2;
-  }
+  const bool fused = fused_geometry(W, P->n_src, nodes_cap, &ring, &nb) && ceil_div64(P->n_src, nb) <= kMaxPipeBatches;
   int* flags = reinterpret_cast<int*>(base + L.off_flags);
   if (fused) {
     ProfScope ps(PK_NODE_PREP, st);
@@ -572,6 +586,242 @@ int apply(const Plan* P, const Weights* W, const void* h, const float* x, const 
   return NNCONV_OK;
 }
 
+// ------------------------------------------------------------------------------------------------
+// partially resident edge features: the cached h covers the sorted edges [0, E_res), the rest is recomputed chunk by
+// chunk inside every application.  Chunks end at unit boundaries (a unit is <= 2 tiles of one source), so every unit
+// of the contraction reads one h buffer; a source whose units straddle a chunk end gets its Y built in both launches.
+// ------------------------------------------------------------------------------------------------
+constexpr int64_t kUnitEdges = 2 * kTileEdges;
+constexpr size_t kStreamYBytes = size_t(48) << 20;   // Y ring of the streamed application (as nn_conv.py's default)
+
+static size_t h_row_bytes(const Weights* W) { return static_cast<size_t>(W->Kp) * 2 * (W->split ? 2 : 1); }
+
+// compact source whose edges contain sorted edge e (0 <= e < E)
+static int src_of_edge(const Plan* P, int64_t e) {
+  const int* g = P->h_group_ptr;
+  int lo = 0, hi = P->n_src;   // g[lo] <= e < g[hi]
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) / 2;
+    if (g[mid] <= e) lo = mid; else hi = mid;
+  }
+  return lo;
+}
+
+// largest unit boundary <= lim
+static int64_t unit_floor(const Plan* P, int64_t lim) {
+  if (lim >= P->E) return P->E;
+  if (lim <= 0) return 0;
+  const int c = src_of_edge(P, lim);
+  const int64_t g = P->h_group_ptr[c];
+  return g + (lim - g) / kUnitEdges * kUnitEdges;
+}
+
+bool is_unit_boundary(const Plan* P, int64_t e) { return e >= 0 && e <= P->E && unit_floor(P, e) == e; }
+
+// contraction work of the sorted edges [e_lo, e_hi) (unit boundaries, e_lo < e_hi) with h holding exactly those rows
+static UnitRange edge_range(const Plan* P, int64_t e_lo, int64_t e_hi) {
+  UnitRange r;
+  const int c_lo = src_of_edge(P, e_lo);
+  r.u_begin = P->h_unit_ptr[c_lo] + static_cast<int>((e_lo - P->h_group_ptr[c_lo]) / kUnitEdges);
+  if (e_hi >= P->E) {
+    r.u_end = P->n_units;
+  } else {
+    const int c_hi = src_of_edge(P, e_hi);
+    r.u_end = P->h_unit_ptr[c_hi] + static_cast<int>((e_hi - P->h_group_ptr[c_hi]) / kUnitEdges);
+  }
+  r.c_begin = c_lo;
+  r.c_end = src_of_edge(P, e_hi - 1) + 1;
+  r.e_base = e_lo;
+  r.h_rows = round_up64(e_hi - e_lo, 128);
+  return r;
+}
+
+// first tile of the unit boundary e
+static int tile_at(const Plan* P, int64_t e) {
+  if (e >= P->E) return P->n_tiles;
+  const int c = src_of_edge(P, e);
+  return P->h_tile_ptr[c] + static_cast<int>((e - P->h_group_ptr[c]) / kTileEdges);
+}
+
+// workspace of apply_streamed: [edge-feature header (overflow counter) | application workspace | chunk h | chunk
+// edge-feature rows]; the chunk rows follow from ws_bytes
+struct StreamLayout {
+  size_t off_apply, apply_bytes, off_h, off_ef, ef_bytes;
+  int64_t rows;
+};
+
+static StreamLayout layout_stream(const Plan* P, const Weights* W, size_t ws_bytes) {
+  StreamLayout L{};
+  L.off_apply = kEfHeader;
+  L.apply_bytes = round_up64(static_cast<int64_t>(apply_ws_bytes(P, W, kStreamYBytes)), 1024);
+  L.off_h = L.off_apply + L.apply_bytes;
+  const size_t fixed = L.off_h + 4096;
+  const size_t row = h_row_bytes(W) + ef_row_bytes(W);
+  L.rows = ws_bytes > fixed ? static_cast<int64_t>((ws_bytes - fixed) / row / 128 * 128) : 0;
+  L.off_ef = L.off_h + static_cast<size_t>(L.rows) * h_row_bytes(W);
+  L.ef_bytes = static_cast<size_t>(L.rows) * ef_row_bytes(W) + 4096;
+  return L;
+}
+
+static int64_t count_chunks(const Plan* P, int64_t E_res, int64_t rows) {
+  int64_t n = 0;
+  for (int64_t e = E_res; e < P->E; e = unit_floor(P, e + rows)) ++n;
+  return n;
+}
+
+int stream_split(const Plan* P, const Weights* W, size_t resident_bytes, size_t chunk_ws_bytes, int64_t* E_res,
+                 size_t* h_res_bytes, size_t* ws_bytes, int64_t* n_chunks) {
+  NNC_REQUIRE(W->prec == PREC_F16 || W->prec == PREC_BF16 || W->prec == PREC_F16X2, NNCONV_ERR_UNSUPPORTED,
+              "streamed edge features need precision f16, bf16 or f16x2");
+  const size_t hrow = h_row_bytes(W);
+  const size_t full = static_cast<size_t>(round_up64(P->E, 128)) * hrow;
+  *E_res = resident_bytes >= full ? P->E : unit_floor(P, static_cast<int64_t>(resident_bytes / hrow) / 128 * 128);
+  *h_res_bytes = static_cast<size_t>(round_up64(*E_res, 128)) * hrow;
+  // chunk rows: a multiple of 128, at least one unit, at most the streamed edges
+  const size_t row = hrow + ef_row_bytes(W);
+  int64_t rows = static_cast<int64_t>(chunk_ws_bytes / row) / 128 * 128;
+  const int64_t rest = round_up64(P->E - *E_res, 128);
+  if (rows > rest) rows = rest;
+  if (rows < kUnitEdges) rows = kUnitEdges;
+  StreamLayout L = layout_stream(P, W, 0);
+  *ws_bytes = L.off_h + 4096 + static_cast<size_t>(rows) * row;
+  *n_chunks = count_chunks(P, *E_res, rows);
+  return NNCONV_OK;
+}
+
+// contraction of one unit range: the persistent kernel (flags at batch offset *boff), else per-batch kernels in
+// plain stream order
+static int contract_range(const Plan* P, const Weights* W, const UnitRange& R, int64_t e_hi, const void* h, bool fused, int ring,
+                          int64_t nb, int64_t nodes_cap, void* Xc, void* Y, const float* cvec, const float* xs,
+                          int aggr_mean, float* out, int* flags, int* boff, cudaStream_t st, int64_t* launches) {
+  if (fused) {
+    int s;
+    {
+      ProfScope ps(PK_APPLY_FUSED, st);
+      s = launch_apply_tc(W->prec, P, W, h, Xc, Y, static_cast<int>(nb), ring, cvec, xs, aggr_mean, out, flags + *boff,
+                          kMaxPipeBatches, st, &R);
+    }
+    *boff += static_cast<int>(ceil_div64(R.c_end - R.c_begin, nb));
+    if (s == NNCONV_OK) {
+      if (launches) ++*launches;
+      return NNCONV_OK;
+    }
+    if (s != kApplyCannotCoSchedule) return s;
+  }
+  NNC_REQUIRE(!W->split, NNCONV_ERR_UNSUPPORTED,
+              "precision f16x2 runs in the fused persistent kernel only (shape or workspace not supported)");
+  const int NY = W->cout * W->Kp;
+  const int t_lo = tile_at(P, R.e_base), t_hi = tile_at(P, e_hi);
+  for (int64_t c0 = R.c_begin; c0 < R.c_end; c0 += nodes_cap) {
+    const int nbat = static_cast<int>((R.c_end - c0) < nodes_cap ? (R.c_end - c0) : nodes_cap);
+    const int tb = P->h_tile_ptr[c0] > t_lo ? P->h_tile_ptr[c0] : t_lo;
+    const int te = P->h_tile_ptr[c0 + nbat] < t_hi ? P->h_tile_ptr[c0 + nbat] : t_hi;
+    PipeFlags pf{};
+    pf.small_footprint = true;
+    {
+      ProfScope ps(PK_Y_GEMM, st);
+      int s = launch_gemm_tc(W->prec, Xc, P->n_src, c0, nbat, W->cin_p, W->W3p, NY, nullptr, 0, Y, NY, st, &pf);
+      if (s) return s;
+    }
+    {
+      ProfScope ps(PK_CONV, st);
+      int s = launch_conv_tc(W->prec, P, h, W->Kp, Y, nbat, W->cout, tb, te, static_cast<int>(c0), cvec, xs, aggr_mean,
+                             out, st, nullptr, R.e_base, R.h_rows);
+      if (s) return s;
+    }
+    if (launches) *launches += 2;
+  }
+  return NNCONV_OK;
+}
+
+int apply_streamed(const Plan* P, const Weights* W, const float* edge_attr, const void* h_res, int64_t E_res,
+                   const float* x, const float* root, const float* bias, int aggr_mean, float* out, void* ws,
+                   size_t ws_bytes, cudaStream_t st, int64_t* launches, unsigned node_flags) {
+  int s;
+  NNC_REQUIRE(!(node_flags & NNCONV_APPLY_RESIDUAL) || W->cin == W->cout, NNCONV_ERR_ARG,
+              "NNCONV_APPLY_RESIDUAL needs in_channels == out_channels");
+  NNC_REQUIRE(W->prec == PREC_F16 || W->prec == PREC_BF16 || W->prec == PREC_F16X2, NNCONV_ERR_UNSUPPORTED,
+              "streamed edge features need precision f16, bf16 or f16x2");
+  NNC_REQUIRE(tc_shapes_supported(W), NNCONV_ERR_UNSUPPORTED,
+              "shape not supported by the tensor-core path (out=%d, K=%d)", W->cout, W->K);
+  NNC_REQUIRE(is_unit_boundary(P, E_res), NNCONV_ERR_ARG,
+              "apply_streamed: E_res = %lld is not a unit boundary of the plan (use nnconv_stream_split)", (long long)E_res);
+  NNC_REQUIRE(ws != nullptr && ws_bytes >= kEfHeader, NNCONV_ERR_WORKSPACE, "apply_streamed: workspace too small");
+  char* base = static_cast<char*>(ws);
+  int* overflow = reinterpret_cast<int*>(base);
+  NNC_CHECK_CUDA(cudaMemsetAsync(overflow, 0, sizeof(int), st));
+  if (!options().overflow_check) overflow = nullptr;
+  if (P->E == 0 || P->n_src == 0) {
+    ProfScope ps(PK_NODE_PREP, st);
+    s = launch_out_init(x, root, bias, P->N, W->cin, W->cout, out, st, node_flags);
+    if (s == NNCONV_OK && launches) ++*launches;
+    return s;
+  }
+  const StreamLayout SL = layout_stream(P, W, ws_bytes);
+  NNC_REQUIRE(E_res == P->E || SL.rows >= kUnitEdges, NNCONV_ERR_WORKSPACE,
+              "apply_streamed: workspace too small (use the size nnconv_stream_split returns)");
+  NNC_REQUIRE(E_res == 0 || h_res != nullptr, NNCONV_ERR_ARG, "apply_streamed: null resident edge features");
+  const ApplyLayout L = layout_apply(P, W);
+  char* abase = base + SL.off_apply;
+  void* Xc = abase + L.off_Xc;
+  float* cvec = reinterpret_cast<float*>(abase + L.off_cvec);
+  float* xs = reinterpret_cast<float*>(abase + L.off_xs);
+  int* flags = reinterpret_cast<int*>(abase + L.off_flags);
+  void* Y = abase + L.off_Y;
+  const int64_t nodes_cap = static_cast<int64_t>((SL.apply_bytes - L.fixed_bytes) / L.per_node);
+  int ring = 0;
+  int64_t nb = 0;
+  const bool fused = fused_geometry(W, P->n_src, nodes_cap, &ring, &nb);
+  if (fused) {
+    // every persistent launch gets its own slice of the flag arrays: batches of all launches must fit the table
+    int64_t total = E_res > 0 ? ceil_div64(edge_range(P, 0, E_res).c_end, nb) : 0;
+    for (int64_t e = E_res; e < P->E;) {
+      const int64_t e2 = unit_floor(P, e + SL.rows);
+      const UnitRange r = edge_range(P, e, e2);
+      total += ceil_div64(r.c_end - r.c_begin, nb);
+      e = e2;
+    }
+    NNC_REQUIRE(total <= kMaxPipeBatches, NNCONV_ERR_WORKSPACE,
+                "apply_streamed: %lld source batches over all chunks exceed %d: use larger chunks", (long long)total,
+                kMaxPipeBatches);
+    NNC_CHECK_CUDA(cudaMemsetAsync(flags, 0, sizeof(int) * 5 * kMaxPipeBatches, st));
+    ProfScope ps(PK_NODE_PREP, st);
+    s = launch_node_prep(W->prec, x, root, bias, P->N, out, P->src_nodes, P->n_src, W->cin, W->cin_p, W->cout, W->B3, Xc,
+                         cvec, xs, flags, kMaxPipeBatches, 0, st, node_flags);
+    if (s) return s;
+    if (launches) ++*launches;
+  } else {
+    {
+      ProfScope ps(PK_NODE_PREP, st);
+      s = launch_out_init(x, root, bias, P->N, W->cin, W->cout, out, st, node_flags);
+    }
+    if (s) return s;
+    {
+      ProfScope ps(PK_NODE_PREP, st);
+      s = launch_src_prep(W->prec, x, P->src_nodes, P->n_src, W->cin, W->cin_p, W->cout, W->B3, Xc, cvec, xs, st, node_flags);
+    }
+    if (s) return s;
+    if (launches) *launches += 2;
+  }
+  int boff = 0;
+  if (E_res > 0) {
+    s = contract_range(P, W, edge_range(P, 0, E_res), E_res, h_res, fused, ring, nb, nodes_cap, Xc, Y, cvec, xs, aggr_mean, out,
+                       flags, &boff, st, launches);
+    if (s) return s;
+  }
+  void* hc = base + SL.off_h;
+  for (int64_t e = E_res; e < P->E;) {
+    const int64_t e2 = unit_floor(P, e + SL.rows);
+    s = edge_features_rows(P, W, edge_attr, e, e2 - e, hc, base + SL.off_ef, SL.ef_bytes, overflow, st, launches, nullptr);
+    if (s) return s;
+    s = contract_range(P, W, edge_range(P, e, e2), e2, hc, fused, ring, nb, nodes_cap, Xc, Y, cvec, xs, aggr_mean, out, flags,
+                       &boff, st, launches);
+    if (s) return s;
+    e = e2;
+  }
+  return NNCONV_OK;
+}
+
 }  // namespace nnc
 
 // ==================================================================================================
@@ -581,7 +831,7 @@ using namespace nnc;
 
 struct nnconv_plan {
   Plan p;
-  int* h_tile_ptr_storage;     // [2*(S+1)]: tile_ptr mirror, then group_ptr mirror
+  int* h_tile_ptr_storage;     // [3*(S+1)]: tile_ptr mirror, group_ptr mirror, unit_ptr
 };
 struct nnconv_weights {
   Weights w;
@@ -628,7 +878,7 @@ int nnconv_plan_create(const int64_t* row0, const int64_t* row1, int64_t E, int6
   if (s != NNCONV_OK) { delete h; return s; }
   // host mirror of tile_ptr (S+1 ints) so that batch tile ranges need no device read later
   const int S = h->p.n_src;
-  h->h_tile_ptr_storage = new (std::nothrow) int[2 * (static_cast<size_t>(S) + 1)];
+  h->h_tile_ptr_storage = new (std::nothrow) int[3 * (static_cast<size_t>(S) + 1)];
   if (!h->h_tile_ptr_storage) { delete h; set_error("out of host memory"); return NNCONV_ERR_ARG; }
   cudaError_t e = cudaMemcpyAsync(h->h_tile_ptr_storage, h->p.tile_ptr, (static_cast<size_t>(S) + 1) * sizeof(int),
                                   cudaMemcpyDeviceToHost, st);
@@ -644,6 +894,11 @@ int nnconv_plan_create(const int64_t* row0, const int64_t* row1, int64_t E, int6
   }
   h->p.h_tile_ptr = h->h_tile_ptr_storage;
   h->p.h_group_ptr = h->h_tile_ptr_storage + S + 1;
+  // unit_ptr follows from tile_ptr (a source's units are pairs of its tiles, plan.cu)
+  int* hu = h->h_tile_ptr_storage + 2 * (static_cast<size_t>(S) + 1);
+  hu[0] = 0;
+  for (int c = 0; c < S; ++c) hu[c + 1] = hu[c] + (h->p.h_tile_ptr[c + 1] - h->p.h_tile_ptr[c] + 1) / 2;
+  h->p.h_unit_ptr = hu;
   *out = h;
   return NNCONV_OK;
 }
@@ -707,6 +962,33 @@ int nnconv_edge_features(const nnconv_plan_t* plan, const nnconv_weights_t* w, c
                          void* ws, size_t ws_bytes, void* stream, int64_t* launches) {
   NNC_REQUIRE(plan && w && (edge_attr || plan->p.E == 0) && h, NNCONV_ERR_ARG, "null pointer");
   return edge_features(&plan->p, &w->w, edge_attr, h, ws, ws_bytes, static_cast<cudaStream_t>(stream), launches);
+}
+
+int nnconv_stream_split(const nnconv_plan_t* plan, const nnconv_weights_t* w, size_t resident_bytes, size_t chunk_ws_bytes,
+                        int64_t* E_res, size_t* h_res_bytes, size_t* ws_bytes, int64_t* n_chunks) {
+  NNC_REQUIRE(plan && w && E_res && h_res_bytes && ws_bytes && n_chunks, NNCONV_ERR_ARG, "null pointer");
+  return stream_split(&plan->p, &w->w, resident_bytes, chunk_ws_bytes, E_res, h_res_bytes, ws_bytes, n_chunks);
+}
+
+int nnconv_edge_features_prefix(const nnconv_plan_t* plan, const nnconv_weights_t* w, const float* edge_attr, int64_t E_res,
+                                void* h, void* ws, size_t ws_bytes, void* stream, int64_t* launches) {
+  NNC_REQUIRE(plan && w && (edge_attr || E_res == 0) && (h || E_res == 0), NNCONV_ERR_ARG, "null pointer");
+  NNC_REQUIRE(is_unit_boundary(&plan->p, E_res), NNCONV_ERR_ARG,
+              "edge_features_prefix: E_res = %lld is not a unit boundary of the plan", (long long)E_res);
+  return edge_features(&plan->p, &w->w, edge_attr, h, ws, ws_bytes, static_cast<cudaStream_t>(stream), launches, nullptr,
+                       E_res);
+}
+
+int nnconv_apply_streamed(const nnconv_plan_t* plan, const nnconv_weights_t* w, const float* edge_attr, const void* h_res,
+                          int64_t E_res, const float* x, const float* root, const float* bias, int aggr, unsigned flags,
+                          float* out, void* ws, size_t ws_bytes, void* stream, int64_t* launches) {
+  NNC_REQUIRE(plan && w && x && out && (edge_attr || plan->p.E == 0), NNCONV_ERR_ARG, "null pointer");
+  NNC_REQUIRE(aggr == NNCONV_AGGR_ADD || aggr == NNCONV_AGGR_MEAN, NNCONV_ERR_UNSUPPORTED,
+              "aggr must be add (0) or mean (1); 'max' is used by no call site of the reference and is not built");
+  NNC_REQUIRE((flags & ~(NNCONV_APPLY_RELU_IN | NNCONV_APPLY_RESIDUAL)) == 0, NNCONV_ERR_ARG, "unknown apply flag");
+  NNC_REQUIRE(x != out, NNCONV_ERR_ARG, "out must not alias x");
+  return apply_streamed(&plan->p, &w->w, edge_attr, h_res, E_res, x, root, bias, aggr == NNCONV_AGGR_MEAN, out, ws,
+                        ws_bytes, static_cast<cudaStream_t>(stream), launches, flags);
 }
 
 int nnconv_edge_acts_sizes(const nnconv_plan_t* plan, const nnconv_weights_t* w, size_t* bytes) {

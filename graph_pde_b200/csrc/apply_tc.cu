@@ -55,7 +55,10 @@ struct ApplyArgs {
   const float* cvec;      // [S, cout]
   const float* xs;        // [S] power-of-two row scale of the Y operand (see k_src_prep)
   float* out;             // [N, cout]
-  int n_src, nb, n_batches, ring;
+  // the launch contracts units [u_begin, u_end) of sources [c_begin, c_end); its Y batches are numbered from c_begin
+  // (batch b = sources c_begin + b*nb ..), and h holds the rows of sorted edges [e_base, e_base + e_pad) only
+  int u_begin, u_end, c_begin, c_end, e_base;
+  int nb, n_batches, ring;
   int nb_slots, passes, a_stages, e_pad;
   // PREC_F16X2 (plan.h): split_nk = Kp/64 > 0 -> h holds 2*split_nk chunk panels [hi | lo], a Y ring row is
   // [cout][hi(Kp) | lo(Kp)], and contraction step j = 3q + r pairs (A, B) = (hi_q, Yhi_q), (hi_q, Ylo_q), (lo_q, Yhi_q)
@@ -176,10 +179,10 @@ k_apply_tc(const __grid_constant__ HMaps tmH, const __grid_constant__ CUtensorMa
     // current one streams (no exposed atomic round trip at batch boundaries).
     auto grab = [&]() {
       int v = 0;
-      if (lane == 0) v = atomicAdd(a.cntU, 1);
+      if (lane == 0) v = a.u_begin + atomicAdd(a.cntU, 1);
       return __shfl_sync(0xffffffffu, v, 0);
     };
-    const int n_units = __ldg(a.unit_ptr + a.n_src);
+    const int n_units = a.u_end;
     int nxt = grab();
     int cur_b = -1;
     while (nxt < n_units) {
@@ -188,7 +191,7 @@ k_apply_tc(const __grid_constant__ HMaps tmH, const __grid_constant__ CUtensorMa
       const int ut = __shfl_sync(0xffffffffu, __ldg(a.unit_t + ui), 0);
       const int uu = __shfl_sync(0xffffffffu, __ldg(a.unit_u + ui), 0);
       const int uc = __shfl_sync(0xffffffffu, __ldg(a.tile_c + ut), 0);
-      const int b = uc / a.nb;
+      const int b = (uc - a.c_begin) / a.nb;
       if (b != cur_b) {
         const unsigned long long tw0 = a.trace.rec ? gtime() : 0ull;
         if (lane == 0) flag_wait(a.okY + b);              // Y of this batch is complete (and visible to TMA)
@@ -198,7 +201,7 @@ k_apply_tc(const __grid_constant__ HMaps tmH, const __grid_constant__ CUtensorMa
           trace_write(a.trace, 301u | (static_cast<unsigned>(b) << 12), tw0, gtime(), 0ull);
         cur_b = b;
       }
-      const int ring_row0 = (b % a.ring) * a.nb - b * a.nb;
+      const int ring_row0 = (b % a.ring) * a.nb - b * a.nb - a.c_begin;
       publish(ut, uu, uc, b);
       int te0[kTU], tbox[kTU];
 #pragma unroll
@@ -232,7 +235,8 @@ k_apply_tc(const __grid_constant__ HMaps tmH, const __grid_constant__ CUtensorMa
             mbar_wait(&a_empty[stage], ring[ti].phase ^ 1u);
             if (elect_one()) {
               mbar_arrive_expect_tx(&a_full[stage], a_bytes);
-              tma_load_2d(smem_a + stage * kATileBytes, mh, &a_full[stage], 0, ja * a.e_pad + te0[ti], a.a_policy);
+              tma_load_2d(smem_a + stage * kATileBytes, mh, &a_full[stage], 0, ja * a.e_pad + te0[ti] - a.e_base,
+                          a.a_policy);
             }
             __syncwarp();
             ring[ti].next();
@@ -284,8 +288,8 @@ k_apply_tc(const __grid_constant__ HMaps tmH, const __grid_constant__ CUtensorMa
       // ring slot for the Y pipeline
       named_bar_sync(1, 256);
       if (warp == 0 && lane == 0) {
-        const int c0 = en.w * a.nb;
-        const int target = __ldg(a.unit_ptr + min(c0 + a.nb, a.n_src)) - __ldg(a.unit_ptr + c0);
+        const int c0 = a.c_begin + en.w * a.nb;
+        const int target = min(__ldg(a.unit_ptr + min(c0 + a.nb, a.c_end)), a.u_end) - max(__ldg(a.unit_ptr + c0), a.u_begin);
         raise_when_all(a.cntC + en.w, a.okC + en.w, target);
       }
       if (g >= en.y) continue;
@@ -359,8 +363,8 @@ k_apply_tc(const __grid_constant__ HMaps tmH, const __grid_constant__ CUtensorMa
     int stage = 0;
     uint32_t phase = 0;
     for (int b = 0; b < a.n_batches; ++b) {
-      const int c0 = b * a.nb;
-      const int rows = min(a.nb, a.n_src - c0);
+      const int c0 = a.c_begin + b * a.nb;
+      const int rows = min(a.nb, a.c_end - c0);
       const int tiles = ((rows + 127) / 128) * n_blocks;
       for (int i = static_cast<int>((blockIdx.x + 7u * b) % gridDim.x); i < tiles; i += gridDim.x) {
         const int mb = i / n_blocks, nbk = i % n_blocks;
@@ -386,8 +390,8 @@ k_apply_tc(const __grid_constant__ HMaps tmH, const __grid_constant__ CUtensorMa
     int stage = 0;
     uint32_t phase = 0;
     for (int b = 0; b < a.n_batches; ++b) {
-      const int c0 = b * a.nb;
-      const int rows = min(a.nb, a.n_src - c0);
+      const int c0 = a.c_begin + b * a.nb;
+      const int rows = min(a.nb, a.c_end - c0);
       const int tiles = ((rows + 127) / 128) * n_blocks;
       const unsigned long long ty0 = a.trace.rec ? gtime() : 0ull;
       if (b >= a.ring) {                         // the ring slot must have been consumed by every CTA
@@ -549,7 +553,7 @@ int launch_variant(int grid, int smem_bytes, bool coop, cudaStream_t st, const H
 
 int launch_apply_tc(int prec, const Plan* P, const Weights* W, const void* h, const void* Xc, void* Yring, int nb,
                     int ring, const float* cvec, const float* xs, int aggr_mean, float* out, int* flags,
-                    int flags_stride, cudaStream_t st) {
+                    int flags_stride, cudaStream_t st, const UnitRange* range) {
   int s = tc_init();
   if (s != NNCONV_OK) return s;
   const Options& opt = options();
@@ -559,11 +563,13 @@ int launch_apply_tc(int prec, const Plan* P, const Weights* W, const void* h, co
   ApplyShape as;
   NNC_REQUIRE(apply_shape(W->cout, eff_kp(W), ybn, &as), NNCONV_ERR_UNSUPPORTED, "apply_tc: unsupported shape");
   if (opt.apply_stages >= 2 && opt.apply_stages < as.a_stages) as.a_stages = opt.apply_stages;
-  const int64_t e_pad = round_up64(P->E, 128);
+  const UnitRange whole{0, P->n_units, 0, P->n_src, 0, round_up64(P->E, 128)};
+  const UnitRange& R = range ? *range : whole;
+  const int64_t e_pad = R.h_rows;
   const int NY = W->cout * W->Kp;
   const int kmul = split ? 2 : 1;      // [hi | lo] activations / Y rows
   const int xmul = split ? 3 : 1;      // [hi | hi | lo] x [hi | lo | hi] operands of the Y GEMM
-  const int n_batches = ceil_div(P->n_src, nb);
+  const int n_batches = ceil_div(R.c_end - R.c_begin, nb);
   NNC_REQUIRE(n_batches <= flags_stride, NNCONV_ERR_WORKSPACE, "apply_tc: too many source batches (%d)", n_batches);
   NNC_REQUIRE(static_cast<uint64_t>(kmul * W->Kp / 64) * e_pad < (1ull << 31), NNCONV_ERR_UNSUPPORTED,
               "apply_tc: edge-feature tensor exceeds 2^31 rows of 64 columns");
@@ -584,7 +590,9 @@ int launch_apply_tc(int prec, const Plan* P, const Weights* W, const void* h, co
   a.tile_c = P->tile_c; a.tile_e0 = P->tile_e0; a.tile_cnt = P->tile_cnt; a.tile_ptr = P->tile_ptr;
   a.unit_ptr = P->unit_ptr; a.unit_t = P->unit_t; a.unit_u = P->unit_u;
   a.dst_sorted = P->dst_sorted; a.inv_deg = aggr_mean ? P->inv_deg : nullptr; a.cvec = cvec; a.xs = xs; a.out = out;
-  a.n_src = P->n_src; a.nb = nb; a.n_batches = n_batches; a.ring = ring;
+  a.u_begin = R.u_begin; a.u_end = R.u_end; a.c_begin = R.c_begin; a.c_end = R.c_end;
+  a.e_base = static_cast<int>(R.e_base);
+  a.nb = nb; a.n_batches = n_batches; a.ring = ring;
   a.nb_slots = as.nb_slots; a.passes = as.passes; a.a_stages = as.a_stages;
   a.e_pad = static_cast<int>(e_pad);
   a.split_nk = split ? W->Kp / 64 : 0;

@@ -66,6 +66,7 @@ struct ConvTcArgs {
   int passes;             // nb_slots * passes == Kp / 64
   int a_stages;
   int e_pad;              // rows per 64-column panel of the chunk-major h
+  int e_base;             // sorted edge of h row 0 (0 unless h is a chunk of the edges)
   int debug;              // NNCONV_DEBUG bit0: skip the scatter (measurement experiments only)
   // cross-kernel pipelining (tc05.cuh): Y of this batch must be complete; raise done when all reds are out;
   // the last kernel of an application also joins every earlier kernel of the chain before it exits
@@ -166,7 +167,7 @@ k_conv_tc(const __grid_constant__ HMaps tmH, const __grid_constant__ CUtensorMap
               const int stage = ring[ti].stage;
               mbar_wait(&a_empty[stage], ring[ti].phase ^ 1u);
               mbar_arrive_expect_tx(&a_full[stage], a_bytes);
-              tma_load_2d(smem_a + stage * kATileBytes, mh, &a_full[stage], 0, j * a.e_pad + e0, kEvictFirst);
+              tma_load_2d(smem_a + stage * kATileBytes, mh, &a_full[stage], 0, j * a.e_pad + e0 - a.e_base, kEvictFirst);
               ring[ti].next();
             }
           }
@@ -305,12 +306,12 @@ bool tc_shapes_supported(const Weights* W) {
 
 int launch_conv_tc(int prec, const Plan* P, const void* h, int Kp, const void* Y, int64_t y_nodes, int cout,
                    int tile_begin, int tile_end, int c0, const float* cvec, const float* xs, int aggr_mean, float* out,
-                   cudaStream_t st, const PipeFlags* pf) {
+                   cudaStream_t st, const PipeFlags* pf, int64_t e_base, int64_t h_rows) {
   if (tile_end <= tile_begin) return NNCONV_OK;
   int s = tc_init();
   if (s != NNCONV_OK) return s;
   const int bf = prec == PREC_BF16;
-  const int64_t e_pad = round_up64(P->E, 128);
+  const int64_t e_pad = h_rows > 0 ? h_rows : round_up64(P->E, 128);
   ConvShape cs;
   NNC_REQUIRE(conv_shape(cout, Kp, &cs), NNCONV_ERR_UNSUPPORTED,
               "conv_tc: shape not supported by the tensor-core contraction (cout=%d Kp=%d)", cout, Kp);
@@ -325,6 +326,7 @@ int launch_conv_tc(int prec, const Plan* P, const void* h, int Kp, const void* Y
   if (s != NNCONV_OK) return s;
   ConvTcArgs a{};
   a.e_pad = static_cast<int>(e_pad);
+  a.e_base = static_cast<int>(e_base);
   a.tile_c = P->tile_c; a.tile_e0 = P->tile_e0; a.tile_cnt = P->tile_cnt; a.dst_sorted = P->dst_sorted;
   a.inv_deg = aggr_mean ? P->inv_deg : nullptr; a.cvec = cvec; a.xs = xs; a.out = out;
   a.tile_begin = tile_begin; a.tile_end = tile_end; a.c0 = c0;

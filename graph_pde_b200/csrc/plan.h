@@ -37,6 +37,7 @@ struct Plan {
   const float* inv_deg;   // [N] 1/max(in_degree,1)
   const int* h_tile_ptr;  // HOST mirror of tile_ptr ([S+1]) owned by the C handle
   const int* h_group_ptr; // HOST mirror of group_ptr ([S+1]) owned by the C handle
+  const int* h_unit_ptr;  // HOST copy of unit_ptr ([S+1]) owned by the C handle
 };
 
 void plan_sizes(int64_t E, int64_t N, size_t* ws_bytes, size_t* tmp_bytes);
@@ -84,14 +85,26 @@ size_t edge_features_ws_bytes(const Plan* P, const Weights* W, size_t want_bytes
 // edge_acts_offset(l)) instead of recycling them chunk by chunk, so that the backward need not recompute them
 size_t edge_acts_bytes(const Plan* P, const Weights* W);
 size_t edge_acts_offset(const Plan* P, const Weights* W, int l);
+// n_edges >= 0: only the sorted edges [0, n_edges) (a unit boundary), into panels of round_up(n_edges, 128) rows
 int edge_features(const Plan* P, const Weights* W, const float* edge_attr, void* h, void* ws, size_t ws_bytes,
-                  cudaStream_t st, int64_t* launches, void* acts = nullptr);
+                  cudaStream_t st, int64_t* launches, void* acts = nullptr, int64_t n_edges = -1);
 
 // one conv application given h_last
 size_t apply_ws_bytes(const Plan* P, const Weights* W, size_t want_bytes);
 int apply(const Plan* P, const Weights* W, const void* h, const float* x, const float* root, const float* bias,
           int aggr_mean, float* out, void* ws, size_t ws_bytes, cudaStream_t st, int64_t* launches,
           unsigned node_flags = 0);
+
+// partially resident edge features (16-bit precisions): the edge features of the sorted edges [0, E_res) are cached by
+// the caller (edge_features with n_edges = E_res), those of [E_res, E) are recomputed chunk by chunk inside every
+// application.  stream_split picks the largest unit-aligned E_res whose h fits resident_bytes and sizes the workspace
+// of apply_streamed for chunks of chunk_ws_bytes (h rows + edge-feature workspace).
+int stream_split(const Plan* P, const Weights* W, size_t resident_bytes, size_t chunk_ws_bytes, int64_t* E_res,
+                 size_t* h_res_bytes, size_t* ws_bytes, int64_t* n_chunks);
+bool is_unit_boundary(const Plan* P, int64_t e);
+int apply_streamed(const Plan* P, const Weights* W, const float* edge_attr, const void* h_res, int64_t E_res,
+                   const float* x, const float* root, const float* bias, int aggr_mean, float* out, void* ws,
+                   size_t ws_bytes, cudaStream_t st, int64_t* launches, unsigned node_flags);
 
 // tensor-core backward (backward_tc.cu): per application (dx, dW_L, db_L, droot, dbias) and, once per
 // (edge_attr, parameters) for all T applications of a shared conv, the pass through the hidden layers.

@@ -33,7 +33,8 @@ from . import _lib
 
 __all__ = ['NNConv_old', 'NNConv', 'ECConv', 'stats', 'clear_caches', 'default_precision']
 
-stats = {'launches': 0, 'plans_built': 0, 'edge_feature_passes': 0, 'applies': 0, 'weight_preps': 0}
+stats = {'launches': 0, 'plans_built': 0, 'edge_feature_passes': 0, 'applies': 0, 'weight_preps': 0,
+         'streamed_chunk_passes': 0}
 
 _PLAN_CACHE = collections.OrderedDict()
 _PLAN_CACHE_MAX = int(os.environ.get('NNCONV_B200_PLAN_CACHE', '64'))                 # entries
@@ -59,6 +60,10 @@ _EDGE_KERNELS_MAX_DEG = 8                       # auto: average out-degree of th
 _EDGE_KERNELS_MAX_EDGES = int(os.environ.get('NNCONV_B200_EDGE_KERNELS_MAX_EDGES', '8192'))
                                                 # than the fixed cost of the persistent kernel (MGKN's coarse levels)
 _EDGE_KERNELS_MAX_BYTES = 2 << 30
+# budget (bytes) of the cached edge features h; a graph whose h is larger keeps a prefix of h resident and recomputes
+# the rest chunk by chunk inside every application (see NNConv_old).  Unset: the whole h, streaming only on an OOM.
+_EDGE_FEATURE_BYTES = os.environ.get('NNCONV_B200_EDGE_FEATURE_BYTES')
+_STREAM_MARGIN_BYTES = 1 << 30     # left free beside the resident prefix when the budget comes from mem_get_info
 
 
 def default_precision():
@@ -113,6 +118,14 @@ class _Plan(object):
         self.E, self.N, self.n_src, self.n_tiles, self.max_out_deg, self.src_sorted = [int(v) for v in info[:6]]
         stats['plans_built'] += 1
         self._finalizer = weakref.finalize(self, L.nnconv_plan_destroy, h)
+
+
+class _Streamed(object):
+    """Partially resident edge features: h of the sorted edges [0, E_res) (``h_res``, nnconv_edge_features_prefix);
+    every application recomputes the other edges' h in ``n_chunks`` chunks from ``ea32`` (nnconv_apply_streamed)."""
+
+    def __init__(self, h_res, E_res, ws_bytes, n_chunks, ea32):
+        self.h_res, self.E_res, self.ws_bytes, self.n_chunks, self.ea32 = h_res, E_res, ws_bytes, n_chunks, ea32
 
 
 def _plan_key(edge_index, n_nodes, flow):
@@ -204,7 +217,7 @@ class _NNConvFunction(torch.autograd.Function):
         ctx.module = module
         ctx.edge_index = edge_index
         ctx.save_for_backward(x, edge_attr)
-        return module._forward_impl(x, edge_index, edge_attr)
+        return module._forward_impl(x, edge_index, edge_attr, for_grad=True)
 
     @staticmethod
     def backward(ctx, grad_out):
@@ -284,6 +297,13 @@ class NNConv_old(torch.nn.Module):
     operand as an fp16 (hi, lo) pair -- fp32-grade results (tolerance 2e-5) on the tensor cores at ~2.4x the
     time of 'f16'; 'fp32' = CUDA-core path for arbitrary shapes.  ``flow`` is PyG's MessagePassing kwarg.
 
+    ``edge_feature_bytes`` (default: environment NNCONV_B200_EDGE_FEATURE_BYTES, else unlimited) bounds the cached edge
+    features (``Kp * 2`` bytes per edge, twice that at 'f16x2').  A graph whose features exceed it keeps a unit-aligned
+    prefix resident and recomputes the rest chunk by chunk inside every application (same bits, more time); without a
+    budget that happens only when allocating the whole h runs out of device memory.  Inference only: training needs the
+    whole h resident.  Precision 'fp32' and the per-edge kernel matrices (graphs with few out-edges per source) never
+    stream.
+
     Caches: the down-converted weights and the x-independent edge features are cached per (parameter versions,
     edge_attr version).  Optimizer steps, ``load_state_dict`` and ``train()/eval()`` invalidate them; writes that
     bypass autograd's version counter (``p.data.copy_()``, ``p.data.clamp_()``) do NOT -- call ``invalidate()``
@@ -294,6 +314,7 @@ class NNConv_old(torch.nn.Module):
         super(NNConv_old, self).__init__()
         self.precision = kwargs.pop('precision', None)
         self.flow = kwargs.pop('flow', 'source_to_target')
+        self.edge_feature_bytes = kwargs.pop('edge_feature_bytes', None)
         if kwargs:
             raise TypeError('unexpected keyword arguments %s' % sorted(kwargs))
         if aggr not in ('add', 'mean', 'max'):
@@ -385,9 +406,21 @@ class NNConv_old(torch.nn.Module):
             self._k_cache = None
         return self._prepared
 
-    def edge_features(self, plan, prepared, edge_attr, keep_acts=False):
+    def _budget(self):
+        b = self.edge_feature_bytes
+        if b is None and _EDGE_FEATURE_BYTES is not None:
+            b = int(_EDGE_FEATURE_BYTES)
+        return b
+
+    def _streams(self, plan, prepared):
+        """Whether these features may be streamed: 16-bit formulation C (the per-edge kernel matrices and fp32 need
+        the whole h)."""
+        return prepared.precision in ('f16', 'fp16', 'bf16', 'f16x2') and not self._wants_edge_kernels(plan, prepared)
+
+    def edge_features(self, plan, prepared, edge_attr, keep_acts=False, for_grad=False):
         """x-independent part of message(): cached across the T applications of a shared conv.  keep_acts (training):
-        also keep the hidden activations for the backward (returned by ``kept_acts``)."""
+        also keep the hidden activations for the backward (returned by ``kept_acts``).  Returns h, or a _Streamed
+        when only a prefix of h fits (see the class docstring)."""
         key = (plan.key, edge_attr.data_ptr(), tuple(edge_attr.shape), edge_attr._version, id(prepared))
         hit = self._h_cache.get(key)
         L = _lib.lib()
@@ -396,6 +429,8 @@ class NNConv_old(torch.nn.Module):
             _lib.check(L.nnconv_edge_acts_sizes(plan.handle, prepared.handle, ctypes.byref(acts_b)))
             if acts_b.value > _KEEP_ACTS_MAX_BYTES:
                 acts_b = ctypes.c_size_t(0)
+        if hit is not None and isinstance(hit[0], _Streamed) and for_grad:
+            self._streaming_grad_error(hit[0].h_res.numel())
         if hit is not None and (acts_b.value == 0 or hit[2] is not None):
             return hit[0]
         h_b, ws_b = ctypes.c_size_t(), ctypes.c_size_t()
@@ -404,8 +439,25 @@ class NNConv_old(torch.nn.Module):
         dev = edge_attr.device
         self._h_cache.clear()                       # free the previous sample's features first
         self._k_cache = None
-        h = torch.empty(h_b.value, dtype=torch.uint8, device=dev)
-        ws = torch.empty(ws_b.value, dtype=torch.uint8, device=dev)
+        budget = self._budget()
+        streams = self._streams(plan, prepared)
+        if budget is not None and h_b.value > budget and streams:
+            if for_grad:
+                self._streaming_grad_error(budget)
+            return self._streamed_features(key, plan, prepared, edge_attr, budget)
+        try:
+            h = torch.empty(h_b.value, dtype=torch.uint8, device=dev)
+            ws = torch.empty(ws_b.value, dtype=torch.uint8, device=dev)
+        except torch.cuda.OutOfMemoryError:
+            if not streams:
+                raise
+            h = ws = None
+            if for_grad:
+                self._streaming_grad_error(h_b.value)
+            self._h_cache.clear()
+            self._k_cache = None
+            self._tstate = None
+            return self._streamed_features(key, plan, prepared, edge_attr, None)
         acts = torch.empty(acts_b.value, dtype=torch.uint8, device=dev) if acts_b.value else None
         n_l = ctypes.c_int64(0)
         if acts is not None:
@@ -416,17 +468,72 @@ class NNConv_old(torch.nn.Module):
                                               ws_b.value, _stream_ptr(dev), ctypes.byref(n_l)))
         stats['launches'] += n_l.value
         stats['edge_feature_passes'] += 1
+        self._check_overflow(prepared, ws, dev)
+        self._h_cache[key] = (h, edge_attr, acts)    # hold edge_attr so its address cannot be recycled
+        return h
+
+    @staticmethod
+    def _streaming_grad_error(nbytes):
+        raise RuntimeError(
+            'graph_pde_b200.NNConv: the edge features of this graph do not fit on the device or in the cache budget '
+            '(%d bytes), and training needs the whole h resident: streamed edge features are inference only (call '
+            'under torch.no_grad(), or raise edge_feature_bytes / NNCONV_B200_EDGE_FEATURE_BYTES)' % nbytes)
+
+    def _streamed_features(self, key, plan, prepared, edge_attr, budget):
+        """Cache the unit-aligned prefix of h that fits ``budget`` bytes (None: what the device has free beside the
+        streaming workspace) and return the _Streamed the applications run from."""
+        L = _lib.lib()
+        dev = edge_attr.device
+
+        def split(b):
+            e_res, h_b, ws_b, n_ch = ctypes.c_int64(), ctypes.c_size_t(), ctypes.c_size_t(), ctypes.c_int64()
+            _lib.check(L.nnconv_stream_split(plan.handle, prepared.handle, max(int(b), 0), _EF_WS_BYTES,
+                                             ctypes.byref(e_res), ctypes.byref(h_b), ctypes.byref(ws_b),
+                                             ctypes.byref(n_ch)))
+            return e_res.value, h_b.value, ws_b.value, n_ch.value
+
+        e_res, h_b, ws_b, n_ch = split(budget if budget is not None else 0)
+        if budget is None:
+            free = torch.cuda.mem_get_info(dev)[0] + torch.cuda.memory_reserved(dev) - torch.cuda.memory_allocated(dev)
+            e_res, h_b, ws_b, n_ch = split(free - ws_b - _STREAM_MARGIN_BYTES)
+        h_res = None
+        if e_res > 0:
+            try:
+                h_res = torch.empty(h_b, dtype=torch.uint8, device=dev)
+            except torch.cuda.OutOfMemoryError:
+                if budget is not None:
+                    raise
+                e_res, h_b, ws_b, n_ch = split(0)
+        if h_res is None:
+            h_res = torch.empty(0, dtype=torch.uint8, device=dev)
+        if e_res > 0:
+            ef_h, ef_ws = ctypes.c_size_t(), ctypes.c_size_t()
+            _lib.check(L.nnconv_edge_features_sizes(plan.handle, prepared.handle, _EF_WS_BYTES, ctypes.byref(ef_h),
+                                                    ctypes.byref(ef_ws)))
+            ws = torch.empty(ef_ws.value, dtype=torch.uint8, device=dev)
+            n_l = ctypes.c_int64(0)
+            _lib.check(L.nnconv_edge_features_prefix(plan.handle, prepared.handle, _ptr(edge_attr), e_res, _ptr(h_res),
+                                                     _ptr(ws), ef_ws.value, _stream_ptr(dev), ctypes.byref(n_l)))
+            stats['launches'] += n_l.value
+            stats['edge_feature_passes'] += 1
+            self._check_overflow(prepared, ws, dev)
+            del ws
+        st = _Streamed(h_res, e_res, ws_b, n_ch, edge_attr)
+        self._h_cache[key] = (st, edge_attr, None)
+        return st
+
+    @staticmethod
+    def _check_overflow(prepared, ws, dev):
+        """One host sync: raise when edge-MLP activations written with ``ws`` left the fp16 range."""
         if _OVERFLOW_CHECK and prepared.precision in ('f16', 'fp16', 'f16x2') and \
                 not torch.cuda.is_current_stream_capturing():
             cnt = ctypes.c_int64(0)
-            _lib.check(L.nnconv_edge_features_overflow(_ptr(ws), _stream_ptr(dev), ctypes.byref(cnt)))
+            _lib.check(_lib.lib().nnconv_edge_features_overflow(_ptr(ws), _stream_ptr(dev), ctypes.byref(cnt)))
             if cnt.value:
                 raise FloatingPointError(
                     'graph_pde_b200.NNConv: %d blocks of edge-MLP activations left the fp16 range (|h| > 65504 or '
                     "NaN); use precision='bf16' or 'fp32' for this parameter scale (NNCONV_B200_OVERFLOW_CHECK=0 "
                     'disables this check and its one host sync per edge-feature pass)' % cnt.value)
-        self._h_cache[key] = (h, edge_attr, acts)    # hold edge_attr so its address cannot be recycled
-        return h
 
     def kept_acts(self, h):
         for ent in self._h_cache.values():
@@ -447,7 +554,7 @@ class NNConv_old(torch.nn.Module):
         if pseudo.size(0) != edge_index.size(1):
             raise ValueError('edge_attr has %d rows for %d edges' % (pseudo.size(0), edge_index.size(1)))
 
-    def _prepare(self, x, edge_index, pseudo, keep_acts=False):
+    def _prepare(self, x, edge_index, pseudo, keep_acts=False, for_grad=False):
         """plan, prepared weights, fp32 edge_attr and the (cached) edge features for this call."""
         precision = self.precision or default_precision()
         ea32 = pseudo.detach()
@@ -455,17 +562,21 @@ class NNConv_old(torch.nn.Module):
             ea32 = ea32.contiguous().float()
         plan = get_plan(edge_index, x.size(0), self.flow)
         prepared = self._get_prepared(precision)
-        h = self.edge_features(plan, prepared, ea32, keep_acts and prepared.bwd_tc)
+        h = self.edge_features(plan, prepared, ea32, keep_acts and prepared.bwd_tc, for_grad)
         return plan, prepared, ea32, h
+
+    def _wants_edge_kernels(self, plan, prepared):
+        """The graph-shape policy of formulation B (see _edge_kernels)."""
+        if _EDGE_KERNELS == 'off' or prepared.precision not in ('f16', 'fp16', 'bf16') or plan.E == 0:
+            return False
+        return _EDGE_KERNELS == 'on' or ((plan.E <= _EDGE_KERNELS_MAX_DEG * max(plan.n_src, 1) or
+                                          plan.E <= _EDGE_KERNELS_MAX_EDGES) and
+                                         plan.E * self.in_channels * self.out_channels * 2 <= _EDGE_KERNELS_MAX_BYTES)
 
     def _edge_kernels(self, plan, prepared, h):
         """K_e = W_L h_e + b_L for every edge (formulation B) when the graph has few out-edges per source, else None.
         Cached with h: as x-independent as the edge features."""
-        if _EDGE_KERNELS == 'off' or prepared.precision not in ('f16', 'fp16', 'bf16') or plan.E == 0:
-            return None
-        if _EDGE_KERNELS != 'on' and not ((plan.E <= _EDGE_KERNELS_MAX_DEG * max(plan.n_src, 1) or
-                                           plan.E <= _EDGE_KERNELS_MAX_EDGES) and
-                                          plan.E * self.in_channels * self.out_channels * 2 <= _EDGE_KERNELS_MAX_BYTES):
+        if isinstance(h, _Streamed) or not self._wants_edge_kernels(plan, prepared):
             return None
         hit = getattr(self, '_k_cache', None)
         if hit is not None and hit[0] is h:
@@ -484,6 +595,8 @@ class NNConv_old(torch.nn.Module):
     def _apply_impl(self, plan, prepared, h, x32, flags=0):
         L = _lib.lib()
         dev = x32.device
+        if isinstance(h, _Streamed):
+            return self._apply_streamed(plan, prepared, h, x32, flags)
         kmat = self._edge_kernels(plan, prepared, h)
         if kmat is not None:
             out = torch.empty(x32.size(0), self.out_channels, dtype=torch.float32, device=dev)
@@ -508,11 +621,31 @@ class NNConv_old(torch.nn.Module):
         stats['applies'] += 1
         return out
 
-    def _forward_impl(self, x, edge_index, pseudo, flags=0):
+    def _apply_streamed(self, plan, prepared, st, x32, flags):
+        """One application with partially resident edge features (nnconv_apply_streamed): no allocation inside the
+        library and, besides the optional overflow check, no host sync -- capturable by capture.GraphedForward."""
+        L = _lib.lib()
+        dev = x32.device
+        ws = torch.empty(st.ws_bytes, dtype=torch.uint8, device=dev)
+        out = torch.empty(x32.size(0), self.out_channels, dtype=torch.float32, device=dev)
+        root = self.root.detach().contiguous().float() if self.root is not None else None
+        bias = self.bias.detach().contiguous().float() if self.bias is not None else None
+        n_l = ctypes.c_int64(0)
+        _lib.check(L.nnconv_apply_streamed(plan.handle, prepared.handle, _ptr(st.ea32), _ptr(st.h_res), st.E_res,
+                                           _ptr(x32), _ptr(root), _ptr(bias), _lib.AGGR[self.aggr], flags, _ptr(out),
+                                           _ptr(ws), st.ws_bytes, _stream_ptr(dev), ctypes.byref(n_l)))
+        stats['launches'] += n_l.value
+        stats['applies'] += 1
+        stats['streamed_chunk_passes'] += st.n_chunks
+        if st.n_chunks:
+            self._check_overflow(prepared, ws, dev)
+        return out
+
+    def _forward_impl(self, x, edge_index, pseudo, flags=0, for_grad=False):
         self._check_inputs(x, edge_index, pseudo)
         with torch.cuda.device(x.device):
             x32 = x.detach().contiguous().float()
-            plan, prepared, _, h = self._prepare(x32, edge_index, pseudo)
+            plan, prepared, _, h = self._prepare(x32, edge_index, pseudo, for_grad=for_grad)
             return self._apply_impl(plan, prepared, h, x32, flags)
 
     def residual_step(self, z, edge_index, edge_attr, relu_in=True):
@@ -541,7 +674,7 @@ class NNConv_old(torch.nn.Module):
             return None
         self._check_inputs(x, edge_index, pseudo)
         with torch.cuda.device(x.device):
-            plan, prepared, ea32, h = self._prepare(x, edge_index, pseudo, keep_acts=True)
+            plan, prepared, ea32, h = self._prepare(x, edge_index, pseudo, keep_acts=True, for_grad=True)
             if not prepared.bwd_tc:
                 if mode == 'tc':
                     raise NotImplementedError('NNCONV_B200_BACKWARD=tc: shape / precision not covered by the tensor-core backward')

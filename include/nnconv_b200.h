@@ -121,6 +121,23 @@ int nnconv_edge_features_keep(const nnconv_plan_t* plan, const nnconv_weights_t*
  * Copies one int to the host and synchronises `stream`.  A non-zero count means h holds inf: use bf16 / fp32. */
 int nnconv_edge_features_overflow(const void* ws, void* stream, int64_t* count);
 
+/* ---- partially resident edge features, for graphs whose h does not fit the device (16-bit precisions):
+ * the h of the sorted edges [0, E_res) is cached as above, and every application recomputes the h of [E_res, E)
+ * chunk by chunk (same bits as the cached pass) and contracts each chunk right after computing it.
+ *   nnconv_stream_split: E_res = the largest unit-aligned prefix whose h (h_res_bytes) fits resident_bytes
+ *     (resident_bytes >= the whole h -> E_res = E); ws_bytes = workspace of nnconv_apply_streamed for chunks of
+ *     about chunk_ws_bytes (chunk h + edge-feature workspace); n_chunks = chunks per application.
+ *   nnconv_edge_features_prefix: h of [0, E_res) into h_res_bytes (ws of nnconv_edge_features_sizes).
+ *   nnconv_apply_streamed: nnconv_apply_ex given that prefix.  No allocation, no host synchronisation (capturable);
+ *     the first int of ws counts fp16 overflows of the streamed chunks (nnconv_edge_features_overflow(ws, ...)). */
+int nnconv_stream_split(const nnconv_plan_t* plan, const nnconv_weights_t* w, size_t resident_bytes, size_t chunk_ws_bytes,
+                        int64_t* E_res, size_t* h_res_bytes, size_t* ws_bytes, int64_t* n_chunks);
+int nnconv_edge_features_prefix(const nnconv_plan_t* plan, const nnconv_weights_t* w, const float* edge_attr, int64_t E_res,
+                                void* h, void* ws, size_t ws_bytes, void* stream, int64_t* launches /*nullable*/);
+int nnconv_apply_streamed(const nnconv_plan_t* plan, const nnconv_weights_t* w, const float* edge_attr, const void* h_res,
+                          int64_t E_res, const float* x, const float* root, const float* bias, int aggr, unsigned flags,
+                          float* out, void* ws, size_t ws_bytes, void* stream, int64_t* launches /*nullable*/);
+
 /* ---- per-edge kernel matrices for graphs with few out-edges per source (the 1-D multipole hierarchy of
  * MGKN_orthogonal_burgers1d.py has 2-4): K_e = W_L h_e + b_L ([in, out] 16-bit per edge, sorted edge order) is as
  * x-independent as h, so it is built ONCE per (edge_attr, parameters) from the h of nnconv_edge_features
