@@ -400,8 +400,35 @@ static ApplyLayout layout_apply(const Plan* P, const Weights* W) {
   return L;
 }
 
+// Default Y ring of the persistent kernel (DESIGN 4.3): what the device's L2 holds beside the rows of `out` that the
+// application scatters into (fp32 bulk reductions, also L2 traffic), less L2 / kL2HeadroomDiv for the evict-first h
+// stream and the plan arrays.  Floor: one 128-source m-block of the Y GEMM per ring slot (smaller batches cost more
+// Y tiles and W3p reads than they save in L2 misses), capped at the L2 size.
+constexpr int kL2HeadroomDiv = 8;
+
+static size_t default_y_bytes(const Plan* P, const Weights* W) {
+  static int l2_bytes[64] = {};
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) {
+    cudaGetLastError();
+    dev = 0;
+  }
+  if (l2_bytes[dev] <= 0 && cudaDeviceGetAttribute(&l2_bytes[dev], cudaDevAttrL2CacheSize, dev) != cudaSuccess) {
+    cudaGetLastError();
+    l2_bytes[dev] = 0;
+  }
+  const size_t l2 = static_cast<size_t>(l2_bytes[dev] > 0 ? l2_bytes[dev] : 50 << 20);
+  const size_t per_node = layout_apply(P, W).per_node;
+  const size_t used = static_cast<size_t>(P->N) * W->cout * sizeof(float) + l2 / kL2HeadroomDiv;
+  const size_t fit = l2 > used ? l2 - used : 0;
+  size_t floor_bytes = static_cast<size_t>(options().ring) * 128 * per_node;
+  if (floor_bytes > l2) floor_bytes = l2;
+  return fit > floor_bytes ? fit : floor_bytes;
+}
+
 size_t apply_ws_bytes(const Plan* P, const Weights* W, size_t want_y_bytes) {
   ApplyLayout L = layout_apply(P, W);
+  if (want_y_bytes == 0) want_y_bytes = default_y_bytes(P, W);
   size_t nodes = want_y_bytes / L.per_node;
   if (nodes < 1) nodes = 1;
   if (nodes > static_cast<size_t>(P->n_src > 0 ? P->n_src : 1)) nodes = P->n_src > 0 ? P->n_src : 1;
@@ -414,7 +441,7 @@ static bool fused_geometry(const Weights* W, int64_t n_src, int64_t nodes_cap, i
   const Options& opt = options();
   const bool no_fuse_env = opt.no_fuse != 0 && !W->split;      // measurement / debugging knob
   if (W->prec == PREC_FP32 || no_fuse_env || !apply_fused_supported(W)) return false;
-  int ring = opt.ring;   // with dynamic unit scheduling 3 x 128 sources (48 MB at out=64, Kp=1024) is best
+  int ring = opt.ring;   // slots (default 3); the sources per slot follow from the Y budget (default_y_bytes)
   if (opt.ring_deep && nodes_cap / 128 > ring) ring = nodes_cap / 128 < 16 ? static_cast<int>(nodes_cap / 128) : 16;
   if (nodes_cap < ring) ring = nodes_cap >= 2 ? static_cast<int>(nodes_cap) : 1;
   int64_t nb = nodes_cap / ring;
@@ -592,7 +619,6 @@ int apply(const Plan* P, const Weights* W, const void* h, const float* x, const 
 // of the contraction reads one h buffer; a source whose units straddle a chunk end gets its Y built in both launches.
 // ------------------------------------------------------------------------------------------------
 constexpr int64_t kUnitEdges = 2 * kTileEdges;
-constexpr size_t kStreamYBytes = size_t(48) << 20;   // Y ring of the streamed application (as nn_conv.py's default)
 
 static size_t h_row_bytes(const Weights* W) { return static_cast<size_t>(W->Kp) * 2 * (W->split ? 2 : 1); }
 
@@ -653,7 +679,7 @@ struct StreamLayout {
 static StreamLayout layout_stream(const Plan* P, const Weights* W, size_t ws_bytes) {
   StreamLayout L{};
   L.off_apply = kEfHeader;
-  L.apply_bytes = round_up64(static_cast<int64_t>(apply_ws_bytes(P, W, kStreamYBytes)), 1024);
+  L.apply_bytes = round_up64(static_cast<int64_t>(apply_ws_bytes(P, W, 0)), 1024);   // the default Y ring
   L.off_h = L.off_apply + L.apply_bytes;
   const size_t fixed = L.off_h + 4096;
   const size_t row = h_row_bytes(W) + ef_row_bytes(W);

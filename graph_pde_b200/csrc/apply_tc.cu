@@ -38,8 +38,10 @@ constexpr int kThreads = 14 * 32;
 constexpr int kConvProducer = 12, kYProducer = 13;
 constexpr int kQueue = 8;                  // unit queue between the scheduler and the conv warpgroups
 constexpr int kScatterPitch = 272;         // bytes per staged edge row (64 fp32 + 16 B)
-constexpr int kScatterBytes = 8 * 32 * kScatterPitch;
-constexpr int kYScratchBytes = 4 * acc_scratch_bytes<16>();
+constexpr int kScatterRows = 16;           // staged rows per conv warp: its 32 rows go out as two halves
+constexpr int kScatterBytes = 8 * kScatterRows * kScatterPitch;
+constexpr int kMaxXBytes = 3 * kATileBytes;   // largest Xc tile (num_kx boxes) the Y GEMM keeps resident
+constexpr int kYStagingBytes = 4 * 32 * 128;   // Y epilogue: per Y warp, its 32 rows x 64 16-bit columns
 
 struct ApplyArgs {
   // plan
@@ -60,6 +62,8 @@ struct ApplyArgs {
   int u_begin, u_end, c_begin, c_end, e_base;
   int nb, n_batches, ring;
   int nb_slots, passes, a_stages, e_pad;
+  int x_resident;         // Y GEMM: the Xc tile of a (batch, m-block) stays in shared memory while its n-blocks stream
+  int y_bytes;            // shared memory of the Y GEMM (resident Xc tile and / or its stages)
   // PREC_F16X2 (plan.h): split_nk = Kp/64 > 0 -> h holds 2*split_nk chunk panels [hi | lo], a Y ring row is
   // [cout][hi(Kp) | lo(Kp)], and contraction step j = 3q + r pairs (A, B) = (hi_q, Yhi_q), (hi_q, Ylo_q), (lo_q, Yhi_q)
   int split_nk;
@@ -97,15 +101,18 @@ template <int FMT, int kYBlockN, int NC>
 __global__ void __launch_bounds__(kThreads, 1)
 k_apply_tc(const __grid_constant__ HMaps tmH, const __grid_constant__ CUtensorMap tmY,
            const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmW, ApplyArgs a) {
-  constexpr int kYStageBytes = kATileBytes + kYBlockN * 64 * 2;   // Xc tile + W3p tile
+  constexpr int kWBytes = kYBlockN * 64 * 2;   // one W3p box
   extern __shared__ __align__(1024) uint8_t smem[];
   if ((smem_u32(smem) & 1023u) != 0) __trap();
   const int b_chunk_bytes = NC * 128;
   const int b_stride = (b_chunk_bytes + 1023) & ~1023;
   uint8_t* smem_b = smem;
   uint8_t* smem_a = smem_b + a.nb_slots * b_stride;
-  uint8_t* smem_y = smem_a + a.a_stages * kATileBytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem_y + kYStages * kYStageBytes);
+  // Y GEMM: [Xc tile: num_kx boxes, if resident][kYStages x (W3p box, preceded by its Xc box if not resident)]
+  const int y_stage_bytes = a.x_resident ? kWBytes : kATileBytes + kWBytes;
+  uint8_t* smem_x = smem_a + a.a_stages * kATileBytes;
+  uint8_t* smem_y = smem_x + (a.x_resident ? a.num_kx * kATileBytes : 0);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem_a + a.a_stages * kATileBytes + a.y_bytes);
   uint64_t* a_full = bars;
   uint64_t* a_empty = a_full + kMaxAStages;
   uint64_t* b_full = a_empty + kMaxAStages;
@@ -114,11 +121,13 @@ k_apply_tc(const __grid_constant__ HMaps tmH, const __grid_constant__ CUtensorMa
   uint64_t* y_empty = y_full + kYStages;
   uint64_t* q_full = y_empty + kYStages;   // [kQueue] 1 arrival (scheduler)
   uint64_t* q_empty = q_full + kQueue;   // [kQueue] 8 arrivals (the conv warps)
-  int4* q_ent = reinterpret_cast<int4*>(q_empty + kQueue);
-  // Y transposes (4 warps), then the scatter staging (scatter_mode 1: 8 conv warps x 32 rows x kScatterPitch bytes),
-  // after the 1 KB barrier block
-  float* y_scratch = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(bars) + 1024);
-  uint8_t* smem_sc = reinterpret_cast<uint8_t*>(bars) + 1024 + kYScratchBytes;
+  uint64_t* x_full = q_empty + kQueue;     // resident Xc tile: 1 arrival (+ tx)
+  uint64_t* x_empty = x_full + 1;          // 4 arrivals (the Y warps, when they move on to the next tile)
+  int4* q_ent = reinterpret_cast<int4*>(x_empty + 1);
+  // Y epilogue staging (4 warps), then the scatter staging (scatter_mode 1: 8 conv warps x kScatterRows x
+  // kScatterPitch bytes), after the 1 KB barrier block
+  uint8_t* y_staging = reinterpret_cast<uint8_t*>(bars) + 1024;
+  uint8_t* smem_sc = reinterpret_cast<uint8_t*>(bars) + 1024 + kYStagingBytes;
 
   // shfl: the warp index is warp-uniform for the compiler (see tc05::elect_one)
   const int warp = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x / 32), 0), lane = threadIdx.x % 32;
@@ -145,6 +154,8 @@ k_apply_tc(const __grid_constant__ HMaps tmH, const __grid_constant__ CUtensorMa
       mbar_init(&q_full[s], 1);
       mbar_init(&q_empty[s], 8);
     }
+    mbar_init(x_full, 1);
+    mbar_init(x_empty, 4);
     fence_barrier_init();
   }
   __syncthreads();
@@ -258,7 +269,7 @@ k_apply_tc(const __grid_constant__ HMaps tmH, const __grid_constant__ CUtensorMa
     uint32_t qph = 0;
     // fragment rows of this thread (acc_row numbering: lane L of the warp stands for row acc_row(quarter, L))
     const int fr = lane >> 2, fc = (lane & 3) * 2;
-    const uint32_t my_rows = smem_u32(smem_sc) + static_cast<uint32_t>(warp * 32 * kScatterPitch);
+    const uint32_t my_rows = smem_u32(smem_sc) + static_cast<uint32_t>(warp * kScatterRows * kScatterPitch);
     for (;;) {
       mbar_wait(&q_full[qi], qph);
       int4 en = q_ent[qi];
@@ -268,6 +279,8 @@ k_apply_tc(const __grid_constant__ HMaps tmH, const __grid_constant__ CUtensorMa
       if (++qi == kQueue) { qi = 0; qph ^= 1u; }
       if (en.y < 0) break;
       if (en.y == 0) continue;
+      // a block's A stage and B slot are released as soon as its MMAs retire: keeping one block in flight (as
+      // k_gemm_tc does) holds every stage and B slot one block longer, which measured slower here (DESIGN 4.3)
       for (int j = 0; j < num_kc; ++j) {
         mbar_wait(&b_full[bs], bph);
         const uint64_t bdesc = smem_desc_sw128(smem_u32(smem_b + bs * b_stride));
@@ -317,25 +330,30 @@ k_apply_tc(const __grid_constant__ HMaps tmH, const __grid_constant__ CUtensorMa
         fok[i] = __shfl_sync(0xffffffffu, ok ? 1 : 0, L) != 0;
       }
       if (a.scatter_mode == 1) {
-        // rows staged in shared memory, then one bulk reduction per row (its lane issues it)
-        bulk_wait_read0();                                 // this lane's previous row has left its staging slot
-        __syncwarp();
+        // rows staged in shared memory, then one bulk reduction per row (its lane issues it); the warp's 32 rows go
+        // out as two halves of 16 through the same staging slots: rows 16 h + r (fragment i = 2 h, 2 h + 1) in half h
 #pragma unroll
-        for (int jj = 0; jj < NC / 8; ++jj) {
-          const float2 cq = __ldg(reinterpret_cast<const float2*>(cv + 8 * jj + fc));
+        for (int h = 0; h < 2; ++h) {
+          bulk_wait_read0();                               // this lane's previous row has left its staging slot
+          __syncwarp();
 #pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            const float* dv = acc.d[i >> 1] + 4 * jj + 2 * (i & 1);
-            const uint32_t addr = my_rows + static_cast<uint32_t>((fr + 8 * i) * kScatterPitch + (8 * jj + fc) * 4);
-            asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(fmaf(dv[0], xsc, cq.x) * fsc[i]),
-                         "f"(fmaf(dv[1], xsc, cq.y) * fsc[i])
-                         : "memory");
+          for (int jj = 0; jj < NC / 8; ++jj) {
+            const float2 cq = __ldg(reinterpret_cast<const float2*>(cv + 8 * jj + fc));
+#pragma unroll
+            for (int i = 2 * h; i < 2 * h + 2; ++i) {
+              const float* dv = acc.d[i >> 1] + 4 * jj + 2 * (i & 1);
+              const uint32_t addr = my_rows + static_cast<uint32_t>((fr + 8 * (i & 1)) * kScatterPitch + (8 * jj + fc) * 4);
+              asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(fmaf(dv[0], xsc, cq.x) * fsc[i]),
+                           "f"(fmaf(dv[1], xsc, cq.y) * fsc[i])
+                           : "memory");
+            }
           }
+          fence_proxy_async_smem();                       // generic-proxy writes of the warp -> async proxy
+          __syncwarp();
+          if (ok && (lane >> 4) == h)
+            bulk_reduce_add_f32(orow, my_rows + static_cast<uint32_t>((lane & 15) * kScatterPitch), static_cast<uint32_t>(NC) * 4u);
+          bulk_commit();
         }
-        fence_proxy_async_smem();                         // generic-proxy writes of the warp -> async proxy
-        __syncwarp();
-        if (ok) bulk_reduce_add_f32(orow, my_rows + static_cast<uint32_t>(lane * kScatterPitch), static_cast<uint32_t>(NC) * 4u);
-        bulk_commit();
       } else if (a.debug_scatter != 1) {
 #pragma unroll
         for (int jj = 0; jj < NC / 8; ++jj) {
@@ -362,19 +380,37 @@ k_apply_tc(const __grid_constant__ HMaps tmH, const __grid_constant__ CUtensorMa
     const int n_blocks = a.NY / kYBlockN;
     int stage = 0;
     uint32_t phase = 0;
+    uint32_t xph = 0;
+    int x_b = -1, x_mb = -1;   // (batch, m-block) of the resident Xc tile
     for (int b = 0; b < a.n_batches; ++b) {
       const int c0 = a.c_begin + b * a.nb;
       const int rows = min(a.nb, a.c_end - c0);
       const int tiles = ((rows + 127) / 128) * n_blocks;
-      for (int i = static_cast<int>((blockIdx.x + 7u * b) % gridDim.x); i < tiles; i += gridDim.x) {
+      // a contiguous range of the batch's tiles per CTA (rotated by batch), so that the resident Xc tile changes at
+      // most once per n_blocks tiles
+      const int64_t rot = (blockIdx.x + 7u * b) % gridDim.x;
+      const int t_end = static_cast<int>(tiles * (rot + 1) / gridDim.x);
+      for (int i = static_cast<int>(tiles * rot / gridDim.x); i < t_end; ++i) {
         const int mb = i / n_blocks, nbk = i % n_blocks;
+        if (a.x_resident && (b != x_b || mb != x_mb)) {
+          mbar_wait(x_empty, xph ^ 1u);                    // the Y warps are done with the previous tile
+          if (elect_one()) {
+            mbar_arrive_expect_tx(x_full, a.num_kx * kATileBytes);
+            for (int kx = 0; kx < a.num_kx; ++kx)
+              tma_load_2d(smem_x + kx * kATileBytes, &tmX, x_full, kx * 64, c0 + mb * 128, kEvictLast);
+          }
+          __syncwarp();
+          xph ^= 1u;
+          x_b = b;
+          x_mb = mb;
+        }
         for (int kx = 0; kx < a.num_kx; ++kx) {
           mbar_wait(&y_empty[stage], phase ^ 1u);
           if (elect_one()) {
-            mbar_arrive_expect_tx(&y_full[stage], kYStageBytes);
-            uint8_t* st = smem_y + stage * kYStageBytes;
-            tma_load_2d(st, &tmX, &y_full[stage], kx * 64, c0 + mb * 128, kEvictLast);
-            tma_load_2d(st + kATileBytes, &tmW, &y_full[stage], kx * 64, nbk * kYBlockN, kEvictLast);
+            mbar_arrive_expect_tx(&y_full[stage], y_stage_bytes);
+            uint8_t* st = smem_y + stage * y_stage_bytes;
+            if (!a.x_resident) tma_load_2d(st + kWBytes, &tmX, &y_full[stage], kx * 64, c0 + mb * 128, kEvictLast);
+            tma_load_2d(st, &tmW, &y_full[stage], kx * 64, nbk * kYBlockN, kEvictLast);
           }
           __syncwarp();
           if (++stage == kYStages) { stage = 0; phase ^= 1u; }
@@ -385,10 +421,13 @@ k_apply_tc(const __grid_constant__ HMaps tmH, const __grid_constant__ CUtensorMa
     // ================================================================ Y GEMM: warpgroup of warps 8..11
     const int quarter = warp % 4;
     const int n_blocks = a.NY / kYBlockN;
-    float* wb = y_scratch + quarter * (acc_scratch_bytes<16>() / 4);
+    const uint32_t stg = smem_u32(y_staging) + static_cast<uint32_t>(quarter * 32 * 128);
+    const int fr = lane >> 2, fc = (lane & 3) * 2;
     Acc<kYBlockN> acc;
     int stage = 0;
     uint32_t phase = 0;
+    uint32_t xph = 0;
+    int x_b = -1, x_mb = -1;
     for (int b = 0; b < a.n_batches; ++b) {
       const int c0 = a.c_begin + b * a.nb;
       const int rows = min(a.nb, a.c_end - c0);
@@ -404,50 +443,87 @@ k_apply_tc(const __grid_constant__ HMaps tmH, const __grid_constant__ CUtensorMa
       const int ymul = a.split_nk > 0 ? 2 : 1;
       const float ysc = a.y_scale != nullptr ? __ldg(a.y_scale) : 1.f;
       uint16_t* ybase = reinterpret_cast<uint16_t*>(a.Yring) + static_cast<int64_t>(b % a.ring) * a.nb * a.NY * ymul;
-      for (int i = static_cast<int>((blockIdx.x + 7u * b) % gridDim.x); i < tiles; i += gridDim.x) {
+      // a contiguous range of the batch's tiles per CTA (rotated by batch), so that the resident Xc tile changes at
+      // most once per n_blocks tiles
+      const int64_t rot = (blockIdx.x + 7u * b) % gridDim.x;
+      const int t_end = static_cast<int>(tiles * (rot + 1) / gridDim.x);
+      for (int i = static_cast<int>(tiles * rot / gridDim.x); i < t_end; ++i) {
         const int mb = i / n_blocks, nbk = i % n_blocks;
+        if (a.x_resident && (b != x_b || mb != x_mb)) {
+          if (x_b >= 0) {                                  // every MMA on the previous tile has retired (wait<0> below)
+            __syncwarp();
+            if (lane == 0) mbar_arrive(x_empty);
+          }
+          mbar_wait(x_full, xph);
+          xph ^= 1u;
+          x_b = b;
+          x_mb = mb;
+        }
         for (int kx = 0; kx < a.num_kx; ++kx) {
           mbar_wait(&y_full[stage], phase);
-          uint8_t* st = smem_y + stage * kYStageBytes;
-          mma_block<kYBlockN, FMT>(acc, smem_desc_sw128(smem_u32(st)), smem_desc_sw128(smem_u32(st + kATileBytes)), 512, 2,
-                                   4, kx != 0);
+          uint8_t* st = smem_y + stage * y_stage_bytes;
+          const uint8_t* xt = a.x_resident ? smem_x + kx * kATileBytes : st + kWBytes;
+          mma_block<kYBlockN, FMT>(acc, smem_desc_sw128(smem_u32(xt)), smem_desc_sw128(smem_u32(st)), 512, 2, 4, kx != 0);
           wgmma_wait<0>();
           __syncwarp();
           if (lane == 0) mbar_arrive(&y_empty[stage]);
           if (++stage == kYStages) { stage = 0; phase ^= 1u; }
         }
-        const int row = mb * 128 + acc_row(quarter, lane);
-        const bool row_ok = row < rows;
-        // column n = o * Kp + k of the source's matrix; with split rows of 2*Kp: offset n + o * Kp
+        // epilogue: the warp converts its 32 rows x 64 columns to 16 bits into its staging tile (128-byte rows, 16-byte
+        // chunks XOR-swizzled by row: conflict-free both ways), then stores whole 128-byte row segments, 8 lanes per
+        // row and 4 rows per instruction (storing lane = row splits every 128-byte line into eight 16-byte writes).
+        // Column n = o * Kp + k of the source's matrix; with split rows of 2 * Kp ([hi | lo] per o): n + o * Kp, and
+        // the lo half (part 1) another Kp further.
         const int n0 = nbk * kYBlockN;
-        uint16_t* yrow0 = ybase + static_cast<int64_t>(row) * a.NY * ymul;
+        const int ncol = n0 + (a.split_nk > 0 ? (n0 / a.Kp) * a.Kp : 0);
+        const int n_parts = (FMT == 0 && a.split_nk > 0) ? 2 : 1;
+        if (FMT == 0 && a.split_nk > 0) {
 #pragma unroll
-        for (int cc = 0; cc < kYBlockN / 16; ++cc) {
-          uint32_t vv[16];
-          acc_rows<kYBlockN, 16>(acc, cc * 16, wb, vv);
-          if (row_ok) {
-            uint32_t packed[8], packed_lo[8];
+          for (int h = 0; h < 2; ++h)
 #pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              float f0 = __uint_as_float(vv[2 * j]), f1 = __uint_as_float(vv[2 * j + 1]);
-              if (FMT == 0 && a.split_nk > 0) { f0 *= ysc; f1 *= ysc; }
+            for (int k = 0; k < kYBlockN / 2; ++k) acc.d[h][k] *= ysc;
+        }
+#pragma unroll 1
+        for (int part = 0; part < n_parts; ++part) {
+          __syncwarp();                                    // the previous part's reads of the staging tile are done
+#pragma unroll
+          for (int j = 0; j < kYBlockN / 8; ++j) {
+#pragma unroll
+            for (int q = 0; q < 4; ++q) {                  // m64 half q / 2, rows fr (+ 8 for odd q) of the warp
+              const int R = 16 * (q >> 1) + fr + 8 * (q & 1);
+              float f0 = acc.d[q >> 1][4 * j + 2 * (q & 1)], f1 = acc.d[q >> 1][4 * j + 2 * (q & 1) + 1];
+              uint32_t p;
               if (FMT == 0) {
                 __half2 hh = __floats2half2_rn(f0, f1);
-                packed[j] = *reinterpret_cast<uint32_t*>(&hh);
-                if (a.split_nk > 0) {
+                if (part == 1) {
                   const float2 hf = __half22float2(hh);
-                  __half2 ll = __floats2half2_rn(f0 - hf.x, f1 - hf.y);
-                  packed_lo[j] = *reinterpret_cast<uint32_t*>(&ll);
+                  hh = __floats2half2_rn(f0 - hf.x, f1 - hf.y);
                 }
+                p = *reinterpret_cast<uint32_t*>(&hh);
               } else {
                 __nv_bfloat162 hh = __floats2bfloat162_rn(f0, f1);
-                packed[j] = *reinterpret_cast<uint32_t*>(&hh);
+                p = *reinterpret_cast<uint32_t*>(&hh);
               }
+              const uint32_t addr = stg + static_cast<uint32_t>(R * 128 + ((j ^ (R & 7)) << 4) + fc * 2);
+              asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(p) : "memory");
             }
-            const int n = n0 + cc * 16;
-            uint16_t* yrow = yrow0 + n + (a.split_nk > 0 ? (n / a.Kp) * a.Kp : 0);
-            st_global_32b_hint(yrow, packed, a.y_store_policy);
-            if (FMT == 0 && a.split_nk > 0) st_global_32b_hint(yrow + a.Kp, packed_lo, a.y_store_policy);
+          }
+          __syncwarp();
+          uint16_t* ytile = ybase + ncol + part * a.Kp;
+#pragma unroll
+          for (int it = 0; it < 8; ++it) {
+            const int R = 4 * it + (lane >> 3), ch = lane & 7;
+            const int row = mb * 128 + acc_row(quarter, R);
+            uint32_t v[4];
+            const uint32_t addr = stg + static_cast<uint32_t>(R * 128 + ((ch ^ (R & 7)) << 4));
+            asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]) : "r"(addr)
+                         : "memory");
+            if (row < rows) {
+              uint16_t* dst = ytile + static_cast<int64_t>(row) * a.NY * ymul + ch * 8;
+              asm volatile("st.global.L2::cache_hint.v4.b32 [%0], {%1, %2, %3, %4}, %5;" ::"l"(dst), "r"(v[0]), "r"(v[1]),
+                           "r"(v[2]), "r"(v[3]), "l"(a.y_store_policy)
+                           : "memory");
+            }
           }
         }
       }
@@ -464,33 +540,40 @@ k_apply_tc(const __grid_constant__ HMaps tmH, const __grid_constant__ CUtensorMa
 }
 
 struct ApplyShape {
-  int nb_slots, passes, a_stages, smem_bytes;
+  int nb_slots, passes, a_stages, x_resident, y_bytes, smem_bytes;
 };
 
-bool apply_shape(int cout, int Kp, int ybn, ApplyShape* as) {
-  const int kYStageBytes = kATileBytes + ybn * 64 * 2;
+// num_kx: 64-column boxes of the Y GEMM's K (the Xc tile of a 128-source m-block is num_kx * 16 KiB)
+bool apply_shape(int cout, int Kp, int ybn, int num_kx, ApplyShape* as) {
+  const int w_bytes = ybn * 64 * 2;
   if (cout % 16 != 0 || cout < 16 || cout > 64 || Kp % 64 != 0) return false;
   const int num_kc = Kp / 64;
   const int b_stride = (cout * 128 + 1023) & ~1023;
-  const int bar_bytes = 1024 + kYScratchBytes + (options().scatter_mode == 1 ? kScatterBytes : 0);
-  const int budget = 227 * 1024 - bar_bytes - kYStages * kYStageBytes;
-  // fewest passes that leave >= 7 A stages (the h stream needs the bytes in flight), else >= 5, else >= 3
+  const int bar_bytes = 1024 + kYStagingBytes + (options().scatter_mode == 1 ? kScatterBytes : 0);
+  // fewest passes that leave >= 7 A stages (the h stream needs the bytes in flight), else >= 5, else >= 3; at each
+  // level a resident Xc tile (loaded once per m-block instead of once per n-block) first, where it fits
   const int forced = options().apply_passes;
   for (int min_stages = 7; min_stages >= 3; min_stages -= 2) {
-    for (int passes = 1; passes <= num_kc; ++passes) {
-      if (num_kc % passes) continue;
-      if (forced > 0 && passes != forced && num_kc % forced == 0) continue;
-      const int nb = num_kc / passes;
-      if (nb > kMaxSlots) continue;
-      if (passes > 1 && nb < 4) continue;   // too little time between a slot's release and its next use
-      int stages = (budget - nb * b_stride) / kATileBytes;
-      if (stages > kMaxAStages) stages = kMaxAStages;
-      if (stages >= min_stages) {
-        as->nb_slots = nb;
-        as->passes = passes;
-        as->a_stages = stages;
-        as->smem_bytes = nb * b_stride + stages * kATileBytes + kYStages * kYStageBytes + bar_bytes;
-        return true;
+    for (int xres = num_kx * kATileBytes <= kMaxXBytes ? 1 : 0; xres >= 0; --xres) {
+      const int y_bytes = xres ? num_kx * kATileBytes + kYStages * w_bytes : kYStages * (kATileBytes + w_bytes);
+      const int budget = 227 * 1024 - bar_bytes - y_bytes;
+      for (int passes = 1; passes <= num_kc; ++passes) {
+        if (num_kc % passes) continue;
+        if (forced > 0 && passes != forced && num_kc % forced == 0) continue;
+        const int nb = num_kc / passes;
+        if (nb > kMaxSlots) continue;
+        if (passes > 1 && nb < 4) continue;   // too little time between a slot's release and its next use
+        int stages = (budget - nb * b_stride) / kATileBytes;
+        if (stages > kMaxAStages) stages = kMaxAStages;
+        if (stages >= min_stages) {
+          as->nb_slots = nb;
+          as->passes = passes;
+          as->a_stages = stages;
+          as->x_resident = xres;
+          as->y_bytes = y_bytes;
+          as->smem_bytes = nb * b_stride + stages * kATileBytes + y_bytes + bar_bytes;
+          return true;
+        }
       }
     }
   }
@@ -504,12 +587,13 @@ bool apply_shape(int cout, int Kp, int ybn, ApplyShape* as) {
 constexpr int kYBN = 64;
 
 static int eff_kp(const Weights* W) { return W->split ? 3 * W->Kp : W->Kp; }
+static int y_num_kx(const Weights* W) { return (W->split ? 3 : 1) * W->cin_p / 64; }
 
 bool apply_fused_supported(const Weights* W) {
   if (W->prec != PREC_F16 && W->prec != PREC_BF16 && W->prec != PREC_F16X2) return false;
   if ((W->cout * W->Kp) % 128 != 0) return false;
   ApplyShape as;
-  return apply_shape(W->cout, eff_kp(W), kYBN, &as);
+  return apply_shape(W->cout, eff_kp(W), kYBN, y_num_kx(W), &as);
 }
 
 namespace {
@@ -561,7 +645,8 @@ int launch_apply_tc(int prec, const Plan* P, const Weights* W, const void* h, co
   const int split = W->split ? 1 : 0;
   const int ybn = kYBN;
   ApplyShape as;
-  NNC_REQUIRE(apply_shape(W->cout, eff_kp(W), ybn, &as), NNCONV_ERR_UNSUPPORTED, "apply_tc: unsupported shape");
+  NNC_REQUIRE(apply_shape(W->cout, eff_kp(W), ybn, y_num_kx(W), &as), NNCONV_ERR_UNSUPPORTED,
+              "apply_tc: unsupported shape");
   if (opt.apply_stages >= 2 && opt.apply_stages < as.a_stages) as.a_stages = opt.apply_stages;
   const UnitRange whole{0, P->n_units, 0, P->n_src, 0, round_up64(P->E, 128)};
   const UnitRange& R = range ? *range : whole;
@@ -594,6 +679,7 @@ int launch_apply_tc(int prec, const Plan* P, const Weights* W, const void* h, co
   a.e_base = static_cast<int>(R.e_base);
   a.nb = nb; a.n_batches = n_batches; a.ring = ring;
   a.nb_slots = as.nb_slots; a.passes = as.passes; a.a_stages = as.a_stages;
+  a.x_resident = as.x_resident; a.y_bytes = as.y_bytes;
   a.e_pad = static_cast<int>(e_pad);
   a.split_nk = split ? W->Kp / 64 : 0;
   a.Kp = W->Kp;

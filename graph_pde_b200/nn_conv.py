@@ -40,7 +40,7 @@ _PLAN_CACHE = collections.OrderedDict()
 _PLAN_CACHE_MAX = int(os.environ.get('NNCONV_B200_PLAN_CACHE', '64'))                 # entries
 _PLAN_CACHE_MAX_BYTES = int(os.environ.get('NNCONV_B200_PLAN_CACHE_BYTES', str(2 << 30)))   # plan buffers + pinned edge_index
 _OVERFLOW_CHECK = os.environ.get('NNCONV_B200_OVERFLOW_CHECK', '1') != '0'
-_Y_BYTES = int(os.environ.get('NNCONV_B200_Y_BYTES', str(48 << 20)))       # Y ring: 3 x 128 sources at out=64, Kp=1024
+_Y_BYTES = int(os.environ.get('NNCONV_B200_Y_BYTES', '0'))   # Y ring bytes; 0: the library sizes it from the device's L2
 _EF_WS_BYTES = int(os.environ.get('NNCONV_B200_EF_WS_BYTES', str(2 << 30)))  # hidden-layer ping-pong chunk (fewer, larger chunks)
 _BWD_WS_BYTES = int(os.environ.get('NNCONV_B200_BWD_WS_BYTES', str(2 << 30)))  # fp32 backward: activations per batch
 # tensor-core backward: per-application workspace (dY of a source batch; larger = fewer batches) and the per-batch

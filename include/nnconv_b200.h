@@ -151,7 +151,10 @@ int nnconv_apply_edge(const nnconv_plan_t* plan, const nnconv_weights_t* w, cons
 int nnconv_apply_edge_ex(const nnconv_plan_t* plan, const nnconv_weights_t* w, const void* kmat, const float* x,
                          const float* root, const float* bias, int aggr, unsigned flags, float* out, void* stream);
 
-/* ---- one NNConv application: gather + last Linear + per-edge contraction + scatter + root + bias --- */
+/* ---- one NNConv application: gather + last Linear + per-edge contraction + scatter + root + bias ---
+ * want_y_bytes: bytes of per-source Y matrices the workspace holds; 0 = the library's default, sized from the
+ * current device's L2 (what it holds beside the application's `out` rows, less headroom, but at least 128 sources per
+ * ring slot up to the L2 size). */
 int nnconv_apply_sizes(const nnconv_plan_t* plan, const nnconv_weights_t* w, size_t want_y_bytes, size_t* ws_bytes);
 /* x [N,in] fp32, root [in,out] or NULL, bias [out] or NULL, out [N,out] fp32 (fully overwritten). */
 int nnconv_apply(const nnconv_plan_t* plan, const nnconv_weights_t* w, const void* h, const float* x,
