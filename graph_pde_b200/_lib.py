@@ -36,6 +36,8 @@ SYMBOLS = [
     'nnconv_edge_acts_sizes', 'nnconv_edge_features_keep', 'nnconv_apply_ex', 'nnconv_apply_edge_ex',
     'nnconv_backward_ex', 'nnconv_backward_mlp_ex',
     'nnconv_stream_split', 'nnconv_edge_features_prefix', 'nnconv_apply_streamed',
+    'nnconv_backward_apply_streamed_sizes', 'nnconv_backward_apply_streamed', 'nnconv_backward_mlp_streamed_sizes',
+    'nnconv_backward_mlp_streamed', 'nnconv_backward_streamed_chunks',
 ]
 
 
@@ -134,6 +136,13 @@ def lib():
     L.nnconv_edge_features_prefix.argtypes = [c_vp, c_vp, c_vp, c_i64, c_vp, c_vp, c_sz, c_vp, P(c_i64)]
     L.nnconv_apply_streamed.argtypes = [c_vp, c_vp, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_int, ctypes.c_uint, c_vp, c_vp,
                                         c_sz, c_vp, P(c_i64)]
+    L.nnconv_backward_apply_streamed_sizes.argtypes = [c_vp, c_vp, c_i64, c_sz, c_sz, P(c_sz)]
+    L.nnconv_backward_apply_streamed.argtypes = [c_vp, c_vp, c_vp, c_vp, c_i64, c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp,
+                                                 c_vp, c_vp, c_vp, c_sz, c_vp, P(c_i64)]
+    L.nnconv_backward_mlp_streamed_sizes.argtypes = [c_vp, c_vp, c_i64, c_int, c_sz, P(c_sz)]
+    L.nnconv_backward_mlp_streamed.argtypes = [c_vp, c_vp, c_vp, c_vp, c_i64, c_int, P(c_vp), P(c_vp), c_int, P(c_vp),
+                                               P(c_vp), c_vp, c_sz, c_vp, c_vp]
+    L.nnconv_backward_streamed_chunks.argtypes = [c_vp, c_vp, c_i64, c_int, c_sz, P(c_i64)]
     for name in SYMBOLS:
         getattr(L, name)
     if L.nnconv_abi_version() != ABI_VERSION:

@@ -210,7 +210,7 @@ static int max_hidden_kp(const Weights* W) {
 
 constexpr size_t kEfHeader = 1024;   // start of the edge-feature workspace: [0] = overflow counter (int)
 
-static size_t ef_row_bytes(const Weights* W) {
+size_t ef_row_bytes(const Weights* W) {
   // per edge row of workspace: A1 (64 x 16-bit, tensor-core first layer) + ping/pong hidden activations
   // (PREC_F16X2: [hi | lo] pairs, twice the width)
   size_t row = 0;
@@ -244,8 +244,8 @@ size_t edge_acts_bytes(const Plan* P, const Weights* W) {
 
 // h for the sorted edges [e_begin, e_begin + E): h row p holds edge e_begin + p (16-bit: chunk-major panels of
 // round_up(E, 128) rows).  ws / ws_bytes: the workspace past its header; overflow (nullable) accumulates.
-static int edge_features_rows(const Plan* P, const Weights* W, const float* edge_attr, int64_t e_begin, int64_t E, void* h,
-                              void* ws, size_t ws_bytes, int* overflow, cudaStream_t st, int64_t* launches, void* acts) {
+int edge_features_rows(const Plan* P, const Weights* W, const float* edge_attr, int64_t e_begin, int64_t E, void* h,
+                       void* ws, size_t ws_bytes, int* overflow, cudaStream_t st, int64_t* launches, void* acts) {
   const int nl = W->n_layers;
   const bool tc = tc_shapes_supported(W);
   NNC_REQUIRE(tc || W->prec == PREC_FP32, NNCONV_ERR_UNSUPPORTED,
@@ -620,7 +620,7 @@ int apply(const Plan* P, const Weights* W, const void* h, const float* x, const 
 // ------------------------------------------------------------------------------------------------
 constexpr int64_t kUnitEdges = 2 * kTileEdges;
 
-static size_t h_row_bytes(const Weights* W) { return static_cast<size_t>(W->Kp) * 2 * (W->split ? 2 : 1); }
+size_t h_row_bytes(const Weights* W) { return static_cast<size_t>(W->Kp) * 2 * (W->split ? 2 : 1); }
 
 // compact source whose edges contain sorted edge e (0 <= e < E)
 static int src_of_edge(const Plan* P, int64_t e) {
@@ -1141,8 +1141,69 @@ int nnconv_backward_apply(const nnconv_plan_t* plan, const nnconv_weights_t* w, 
               "null pointer");
   NNC_REQUIRE(aggr == NNCONV_AGGR_ADD || aggr == NNCONV_AGGR_MEAN, NNCONV_ERR_UNSUPPORTED, "aggr must be add or mean");
   NNC_REQUIRE((root == nullptr) == (grad_root == nullptr), NNCONV_ERR_ARG, "root / grad_root must both be given or both be NULL");
-  return backward_apply_tc(&plan->p, &w->w, h, x, root, aggr == NNCONV_AGGR_MEAN, grad_out, grad_x, grad_W_last,
-                           grad_b_last, grad_root, grad_bias, ws, ws_bytes, static_cast<cudaStream_t>(stream));
+  return backward_apply_tc(&plan->p, &w->w, nullptr, h, plan->p.E, x, root, aggr == NNCONV_AGGR_MEAN, grad_out, grad_x,
+                           grad_W_last, grad_b_last, grad_root, grad_bias, ws, ws_bytes, static_cast<cudaStream_t>(stream));
+}
+
+int nnconv_backward_apply_streamed_sizes(const nnconv_plan_t* plan, const nnconv_weights_t* w, int64_t E_res,
+                                         size_t want_bytes, size_t chunk_ws_bytes, size_t* ws_bytes) {
+  NNC_REQUIRE(plan && w && ws_bytes, NNCONV_ERR_ARG, "null pointer");
+  NNC_REQUIRE(backward_tc_supported(&w->w), NNCONV_ERR_UNSUPPORTED, "tensor-core backward: unsupported shape / precision");
+  NNC_REQUIRE(is_unit_boundary(&plan->p, E_res), NNCONV_ERR_ARG,
+              "backward_apply_streamed: E_res = %lld is not a unit boundary of the plan", (long long)E_res);
+  *ws_bytes = backward_apply_ws_bytes(&plan->p, &w->w, want_bytes, E_res, chunk_ws_bytes);
+  return NNCONV_OK;
+}
+
+int nnconv_backward_apply_streamed(const nnconv_plan_t* plan, const nnconv_weights_t* w, const float* edge_attr,
+                                   const void* h_res, int64_t E_res, const float* x, const float* root, int aggr,
+                                   const float* grad_out, float* grad_x, float* grad_W_last, float* grad_b_last,
+                                   float* grad_root, float* grad_bias, void* ws, size_t ws_bytes, void* stream,
+                                   int64_t* launches) {
+  NNC_REQUIRE(plan && w && x && grad_out && grad_x && grad_W_last && grad_b_last && (edge_attr || plan->p.E == 0) &&
+                  (h_res || E_res == 0),
+              NNCONV_ERR_ARG, "null pointer");
+  NNC_REQUIRE(aggr == NNCONV_AGGR_ADD || aggr == NNCONV_AGGR_MEAN, NNCONV_ERR_UNSUPPORTED, "aggr must be add or mean");
+  NNC_REQUIRE((root == nullptr) == (grad_root == nullptr), NNCONV_ERR_ARG, "root / grad_root must both be given or both be NULL");
+  NNC_REQUIRE(is_unit_boundary(&plan->p, E_res), NNCONV_ERR_ARG,
+              "backward_apply_streamed: E_res = %lld is not a unit boundary of the plan (use nnconv_stream_split)",
+              (long long)E_res);
+  return backward_apply_tc(&plan->p, &w->w, edge_attr, h_res, E_res, x, root, aggr == NNCONV_AGGR_MEAN, grad_out, grad_x,
+                           grad_W_last, grad_b_last, grad_root, grad_bias, ws, ws_bytes, static_cast<cudaStream_t>(stream),
+                           launches);
+}
+
+int nnconv_backward_mlp_streamed_sizes(const nnconv_plan_t* plan, const nnconv_weights_t* w, int64_t E_res, int n_apps,
+                                       size_t want_bytes, size_t* ws_bytes) {
+  NNC_REQUIRE(plan && w && ws_bytes && n_apps >= 1, NNCONV_ERR_ARG, "bad arguments");
+  NNC_REQUIRE(backward_tc_supported(&w->w), NNCONV_ERR_UNSUPPORTED, "tensor-core backward: unsupported shape / precision");
+  NNC_REQUIRE(is_unit_boundary(&plan->p, E_res), NNCONV_ERR_ARG,
+              "backward_mlp_streamed: E_res = %lld is not a unit boundary of the plan", (long long)E_res);
+  *ws_bytes = backward_mlp_ws_bytes(&plan->p, &w->w, n_apps, want_bytes, E_res);
+  return NNCONV_OK;
+}
+
+int nnconv_backward_mlp_streamed(const nnconv_plan_t* plan, const nnconv_weights_t* w, const float* edge_attr,
+                                 const void* h_res, int64_t E_res, int n_apps, const float* const* grad_out,
+                                 const float* const* x, int aggr, float* const* grad_W, float* const* grad_b, void* ws,
+                                 size_t ws_bytes, void* stream, float* grad_edge_attr) {
+  NNC_REQUIRE(plan && w && grad_out && x && grad_W && grad_b && (edge_attr || plan->p.E == 0) && (h_res || E_res == 0),
+              NNCONV_ERR_ARG, "null pointer");
+  NNC_REQUIRE(aggr == NNCONV_AGGR_ADD || aggr == NNCONV_AGGR_MEAN, NNCONV_ERR_UNSUPPORTED, "aggr must be add or mean");
+  NNC_REQUIRE(is_unit_boundary(&plan->p, E_res), NNCONV_ERR_ARG,
+              "backward_mlp_streamed: E_res = %lld is not a unit boundary of the plan (use nnconv_stream_split)",
+              (long long)E_res);
+  return backward_mlp_tc(&plan->p, &w->w, edge_attr, h_res, E_res, n_apps, grad_out, x, aggr == NNCONV_AGGR_MEAN, grad_W,
+                         grad_b, ws, ws_bytes, static_cast<cudaStream_t>(stream), nullptr, grad_edge_attr);
+}
+
+int nnconv_backward_streamed_chunks(const nnconv_plan_t* plan, const nnconv_weights_t* w, int64_t E_res, int n_apps,
+                                    size_t ws_bytes, int64_t* n_chunks) {
+  NNC_REQUIRE(plan && w && n_chunks && n_apps >= 0, NNCONV_ERR_ARG, "bad arguments");
+  NNC_REQUIRE(is_unit_boundary(&plan->p, E_res), NNCONV_ERR_ARG,
+              "backward_streamed_chunks: E_res = %lld is not a unit boundary of the plan", (long long)E_res);
+  *n_chunks = backward_streamed_chunks(&plan->p, &w->w, n_apps, E_res, ws_bytes);
+  return NNCONV_OK;
 }
 
 int nnconv_backward_mlp_sizes(const nnconv_plan_t* plan, const nnconv_weights_t* w, int n_apps, size_t want_bytes,
@@ -1167,8 +1228,8 @@ int nnconv_backward_mlp_ex(const nnconv_plan_t* plan, const nnconv_weights_t* w,
   NNC_REQUIRE(plan && w && grad_out && x && grad_W && grad_b && ((edge_attr && h) || plan->p.E == 0), NNCONV_ERR_ARG,
               "null pointer");
   NNC_REQUIRE(aggr == NNCONV_AGGR_ADD || aggr == NNCONV_AGGR_MEAN, NNCONV_ERR_UNSUPPORTED, "aggr must be add or mean");
-  return backward_mlp_tc(&plan->p, &w->w, edge_attr, h, n_apps, grad_out, x, aggr == NNCONV_AGGR_MEAN, grad_W, grad_b, ws,
-                         ws_bytes, static_cast<cudaStream_t>(stream), acts, grad_edge_attr);
+  return backward_mlp_tc(&plan->p, &w->w, edge_attr, h, plan->p.E, n_apps, grad_out, x, aggr == NNCONV_AGGR_MEAN, grad_W,
+                         grad_b, ws, ws_bytes, static_cast<cudaStream_t>(stream), acts, grad_edge_attr);
 }
 
 int nnconv_gemm_tn_16b(int precision, const void* A, int64_t lda, const void* B, int64_t ldb, int64_t R, int M, int N,

@@ -20,6 +20,9 @@
 //   On request the same pass also yields the gradient w.r.t. edge_attr, d ea_e = dz_1[e, :] . W_1 (k_ea_grad, one
 //   read of dz_1 per batch, rows scattered back to the caller's edge order).
 //
+// Partially resident h (E_res < E, DESIGN.md section 3): k_dy and k_dh read h through a row window (h_e_base, h_rows);
+// source batches past the resident prefix recompute their edges' h (per application) or h_{L-1} (MLP pass) first.
+//
 // 16-bit range: gradients are normalised by powers of two computed on the device (no host sync): G by the
 // largest |G| of the application(s), x by its largest magnitude; the fp32 epilogues multiply the scales back.
 #include <cuda_bf16.h>
@@ -372,7 +375,8 @@ struct DyArgs {
   const int* tile_e0;
   const int* tile_cnt;
   int c0, c1;
-  int e_pad, nk;            // nk = Kp / 64 chunk panels
+  int h_e_base, h_rows;     // h holds the sorted edges [h_e_base, ...) in chunk panels of h_rows rows
+  int nk;                   // nk = Kp / 64 chunk panels
   int num_mt;               // ceil(nk / 2)
   int Kp;
   int g_lo_row;             // SPLIT: first row of the lo halves of G (n_tiles * 128)
@@ -418,8 +422,9 @@ k_dy(const __grid_constant__ Maps8 tmH, const __grid_constant__ Maps8 tmG, DyArg
             if (elect_one()) {
               uint8_t* st = smem + stage * kDyStage;
               mbar_arrive_expect_tx(&full[stage], (two ? 3u : 2u) * box_bytes);
-              tma_load_2d(st, &tmH.m[box - 1], &full[stage], 0, hp * a.e_pad + e0, hpol);
-              if (two) tma_load_2d(st + 16384, &tmH.m[box - 1], &full[stage], 0, (hp + 1) * a.e_pad + e0, hpol);
+              const int hr = e0 - a.h_e_base;
+              tma_load_2d(st, &tmH.m[box - 1], &full[stage], 0, hp * a.h_rows + hr, hpol);
+              if (two) tma_load_2d(st + 16384, &tmH.m[box - 1], &full[stage], 0, (hp + 1) * a.h_rows + hr, hpol);
               tma_load_2d(st + 32768, &tmG.m[box - 1], &full[stage], 0, gr, kEvictFirst);
             }
             __syncwarp();
@@ -500,7 +505,7 @@ struct DhArgs {
   int tile0, tile1;
   int c0, Sb;               // batch of sources [c0, c0 + Sb)
   int e_base;               // first sorted edge of the batch
-  int e_pad;
+  int h_e_base, h_rows;     // h holds the sorted edges [h_e_base, ...) in chunk panels of h_rows rows
   int T, Kp, n_nb;          // n_nb = Kp / BN
   const uint16_t* h;        // chunk-major edge features (the ReLU mask)
   uint16_t* dz;             // [batch edges, Kp] row-major (SPLIT: [batch edges, 2 * Kp], [hi | lo])
@@ -647,7 +652,7 @@ k_dh(const __grid_constant__ Maps8 tmA, const __grid_constant__ CUtensorMap tmB,
           const int k0 = nb * BN + cc;
           if (ok) {
             // (SPLIT: the hi panels of h come first, so this is the hi half)
-            const uint16_t* hp = a.h + (static_cast<int64_t>(k0 >> 6) * a.e_pad + e0 + r) * 64 + (k0 & 63);
+            const uint16_t* hp = a.h + (static_cast<int64_t>(k0 >> 6) * a.h_rows + (e0 - a.h_e_base) + r) * 64 + (k0 & 63);
             uint32_t pk[16], pl[16];
 #pragma unroll
             for (int q = 0; q < 4; ++q) {
@@ -843,25 +848,71 @@ int gemm_tn_pairs(const Weights* W, const void* A, int64_t lda, int a_lo, const 
   return NNCONV_OK;
 }
 
+// ---- streamed edge features (E_res < E): the sources whose edges all lie in the resident prefix [0, E_res) run
+// against it; every later source batch first recomputes the h of its edges into a chunk buffer.  Batches are aligned to
+// sources, not units: k_dy writes dY_c from registers, so all edges of one source go through one launch.
+constexpr int64_t kBwdEfRows = 8192;     // rows of the edge-feature scratch of the chunk recomputation
+
+size_t bwd_ef_bytes(const Plan* P, const Weights* W, int64_t E_res) {
+  if (E_res >= P->E) return 0;
+  const int64_t rows = std::min<int64_t>(kBwdEfRows, round_up64(P->E, 128));
+  return static_cast<size_t>(round_up64(static_cast<int64_t>(rows * ef_row_bytes(W)) + 4096, 1024));
+}
+
+// first compact source with an edge at or past E_res (sources [0, c) lie in the resident prefix)
+int first_streamed_src(const Plan* P, int64_t E_res) {
+  if (E_res >= P->E) return P->n_src;
+  const int* g = P->h_group_ptr;
+  return static_cast<int>(std::upper_bound(g, g + P->n_src + 1, static_cast<int>(E_res)) - g) - 1;
+}
+
+// end of the streamed batch starting at c0: sources while their dxp / dY rows and the chunk-major h of their edges fit
+// the pool (c0 = not even one source fits)
+int apply_stream_batch_end(const Plan* P, const Weights* W, const ApplyBwdLayout& L, int c0, size_t pool) {
+  const int* g = P->h_group_ptr;
+  const size_t hrow = h_row_bytes(W);
+  int c1 = c0;
+  while (c1 < P->n_src) {
+    const size_t need = static_cast<size_t>(c1 + 1 - c0 + 128) * L.per_src +
+                        static_cast<size_t>(round_up64(g[c1 + 1] - g[c0], 128)) * hrow;
+    if (need > pool) break;
+    ++c1;
+  }
+  return c1;
+}
+
 }  // namespace
 
-size_t backward_apply_ws_bytes(const Plan* P, const Weights* W, size_t want_bytes) {
+size_t backward_apply_ws_bytes(const Plan* P, const Weights* W, size_t want_bytes, int64_t E_res, size_t chunk_ws_bytes) {
   ApplyBwdLayout L = apply_bwd_layout(P, W);
   const size_t S = P->n_src > 0 ? P->n_src : 1;
   size_t nb = want_bytes > L.fixed ? (want_bytes - L.fixed) / L.per_src : 0;
   if (nb < 128) nb = 128;
   if (nb > S) nb = S;
-  return L.fixed + (nb + 128) * L.per_src + 4096;
+  const size_t cached = L.fixed + (nb + 128) * L.per_src + 4096;
+  if (E_res < 0 || E_res >= P->E) return cached;
+  // chunk rows: about chunk_ws_bytes of h, and at least every edge of the largest source (one batch holds whole sources)
+  const size_t hrow = h_row_bytes(W);
+  const int64_t all_rows = round_up64(P->E, 128);
+  int64_t rows = static_cast<int64_t>(chunk_ws_bytes / hrow) / 128 * 128;
+  const int64_t deg_rows = round_up64(P->max_out_deg > 0 ? P->max_out_deg : 1, 128);
+  if (rows > all_rows) rows = all_rows;
+  if (rows < deg_rows) rows = deg_rows;
+  return cached + bwd_ef_bytes(P, W, E_res) + static_cast<size_t>(rows) * hrow;
 }
 
-int backward_apply_tc(const Plan* P, const Weights* W, const void* h, const float* x, const float* root,
-                      int aggr_mean, const float* gout, float* dx, float* dWL, float* dbL, float* droot, float* dbias,
-                      void* ws, size_t ws_bytes, cudaStream_t st) {
+int backward_apply_tc(const Plan* P, const Weights* W, const float* edge_attr, const void* h, int64_t E_res,
+                      const float* x, const float* root, int aggr_mean, const float* gout, float* dx, float* dWL,
+                      float* dbL, float* droot, float* dbias, void* ws, size_t ws_bytes, cudaStream_t st,
+                      int64_t* launches) {
   NNC_REQUIRE(backward_tc_supported(W), NNCONV_ERR_UNSUPPORTED, "tensor-core backward: unsupported shape / precision");
   const int cin = W->cin, cout = W->cout, Kp = W->Kp, cin_p = W->cin_p;
   const int64_t N = P->N;
   const int bf = W->prec == PREC_BF16;
   const int sp = W->split;
+  const bool streamed = E_res < P->E;
+  NNC_REQUIRE(!streamed || edge_attr != nullptr, NNCONV_ERR_ARG, "backward_apply: streamed edge features need edge_attr");
+  auto count = [&](int64_t k) { if (launches) *launches += k; };
   int s = tc_init();
   if (s) return s;
   // ---- node-level terms
@@ -869,6 +920,7 @@ int backward_apply_tc(const Plan* P, const Weights* W, const void* h, const floa
     NNC_CHECK_CUDA(cudaMemsetAsync(dbias, 0, sizeof(float) * cout, st));
     k_colsum<<<dim3(ceil_div(cout, 32), 64), dim3(32, 8), 0, st>>>(gout, N, cout, dbias);
     NNC_CHECK_LAUNCH();
+    count(1);
   }
   if (root != nullptr) {
     NNC_CHECK_CUDA(cudaMemsetAsync(droot, 0, sizeof(float) * cin * cout, st));
@@ -876,6 +928,7 @@ int backward_apply_tc(const Plan* P, const Weights* W, const void* h, const floa
     NNC_CHECK_LAUNCH();
     k_g_rootT<<<(unsigned)ceil_div64(N * cin, 256), 256, sizeof(float) * cin * (cout + 1), st>>>(gout, root, N, cin, cout, dx);
     NNC_CHECK_LAUNCH();
+    count(2);
   } else {
     NNC_CHECK_CUDA(cudaMemsetAsync(dx, 0, sizeof(float) * N * cin, st));
   }
@@ -886,7 +939,8 @@ int backward_apply_tc(const Plan* P, const Weights* W, const void* h, const floa
     return NNCONV_OK;
   }
   ApplyBwdLayout L = apply_bwd_layout(P, W);
-  NNC_REQUIRE(ws != nullptr && ws_bytes >= L.fixed + 128 * L.per_src, NNCONV_ERR_WORKSPACE,
+  const size_t ef_bytes = bwd_ef_bytes(P, W, E_res);      // 0 when h is whole
+  NNC_REQUIRE(ws != nullptr && ws_bytes >= L.fixed + ef_bytes + 128 * L.per_src, NNCONV_ERR_WORKSPACE,
               "backward_apply: workspace too small");
   char* base = static_cast<char*>(ws);
   float* scal = reinterpret_cast<float*>(base + L.off_scal);
@@ -895,10 +949,12 @@ int backward_apply_tc(const Plan* P, const Weights* W, const void* h, const floa
   void* G16 = base + L.off_G16;
   float* dW3 = reinterpret_cast<float*>(base + L.off_dW3);
   const int S = P->n_src;
-  int64_t nb_max = static_cast<int64_t>((ws_bytes - L.fixed - 4096) / L.per_src) - 128;
+  const size_t pool = ws_bytes - L.fixed - ef_bytes - 4096;   // dxp, dY (and the chunk h) of one source batch
+  int64_t nb_max = static_cast<int64_t>(pool / L.per_src) - 128;
   if (nb_max > S) nb_max = S;
   NNC_REQUIRE(nb_max >= 1, NNCONV_ERR_WORKSPACE, "backward_apply: workspace too small");
-  char* dyn = base + L.fixed;
+  char* ef_ws = base + L.fixed;
+  char* dyn = base + L.fixed + ef_bytes;
   float* dxp = reinterpret_cast<float*>(dyn);
   uint16_t* dY = reinterpret_cast<uint16_t*>(dyn + round_up64(static_cast<int64_t>(nb_max + 128) * cin_p * 4, 1024));
   const float* inv_deg = aggr_mean ? P->inv_deg : nullptr;
@@ -930,12 +986,10 @@ int backward_apply_tc(const Plan* P, const Weights* W, const void* h, const floa
   // dB_L = x_src^T Gs
   k_xtv<<<(unsigned)ceil_div(S, 32), 256, sizeof(float) * 32 * (cin + cout), st>>>(x, P->src_nodes, Gs, S, cin, cout, dbL);
   NNC_CHECK_LAUNCH();
+  count(6);
 
-  const int64_t e_pad = round_up64(P->E, 128);
-  Maps8 tmH, tmG;
+  Maps8 tmG;
   for (int i = 0; i < 8; ++i) {
-    s = make_tmap_2d_16b(&tmH.m[i], bf, h, static_cast<uint64_t>((sp ? 2 : 1) * Kp / 64) * e_pad, 64, 16 * (i + 1));
-    if (s) return s;
     s = make_tmap_2d_16b(&tmG.m[i], bf, G16, static_cast<uint64_t>((sp ? 2 : 1) * P->n_tiles) * 128, 64, 16 * (i + 1));
     if (s) return s;
   }
@@ -947,33 +1001,68 @@ int backward_apply_tc(const Plan* P, const Weights* W, const void* h, const floa
     attr_set = true;
   }
   const int NY = Kp * cout;
-  for (int64_t c0 = 0; c0 < S; c0 += nb_max) {
-    const int nb = static_cast<int>((S - c0) < nb_max ? (S - c0) : nb_max);
+  const int panels = (sp ? 2 : 1) * Kp / 64;
+  // sources [c0, c0 + nb) against h holding the sorted edges [h_e_base, ...) in panels of h_rows rows
+  auto run_batch = [&](int64_t c0, int nb, const void* hb, int64_t h_e_base, int64_t h_rows, float* dxp_b,
+                       uint16_t* dY_b) -> int {
+    Maps8 tmH;
+    for (int i = 0; i < 8; ++i) {
+      int r = make_tmap_2d_16b(&tmH.m[i], bf, hb, static_cast<uint64_t>(panels) * h_rows, 64, 16 * (i + 1));
+      if (r) return r;
+    }
     DyArgs a;
     a.tile_ptr = P->tile_ptr; a.tile_e0 = P->tile_e0; a.tile_cnt = P->tile_cnt;
     a.c0 = static_cast<int>(c0); a.c1 = static_cast<int>(c0) + nb;
-    a.e_pad = static_cast<int>(e_pad); a.nk = Kp / 64; a.num_mt = (a.nk + 1) / 2;
-    a.Kp = Kp; a.g_lo_row = P->n_tiles * 128; a.dY = dY;
+    a.h_e_base = static_cast<int>(h_e_base); a.h_rows = static_cast<int>(h_rows);
+    a.nk = Kp / 64; a.num_mt = (a.nk + 1) / 2;
+    a.Kp = Kp; a.g_lo_row = P->n_tiles * 128; a.dY = dY_b;
     const int grid = nb < tc_num_sms() ? nb : tc_num_sms();
     if (sp) k_dy<0, 1><<<grid, 160, kDySmem, st>>>(tmH, tmG, a);
     else if (bf) k_dy<1><<<grid, 160, kDySmem, st>>>(tmH, tmG, a);
     else k_dy<0><<<grid, 160, kDySmem, st>>>(tmH, tmG, a);
     NNC_CHECK_LAUNCH();
     // dxp[c, i] = sum_n dY[c, n] W3t[i, n]      (fp32 out; PREC_F16X2: split A against the pre-scaled split W3t)
-    s = launch_gemm_tc(W->prec, dY, nb, 0, nb, (sp ? 3 : 1) * NY, W->W3t, cin_p, nullptr, 0, dxp, cin_p, st, nullptr, 0, 0,
-                       sp ? GEMM_A_SPLIT : 0, nullptr, nullptr, 0, 1);
-    if (s) return s;
+    int r = launch_gemm_tc(W->prec, dY_b, nb, 0, nb, (sp ? 3 : 1) * NY, W->W3t, cin_p, nullptr, 0, dxp_b, cin_p, st, nullptr,
+                           0, 0, sp ? GEMM_A_SPLIT : 0, nullptr, nullptr, 0, 1);
+    if (r) return r;
     k_scatter_dx_tc<<<(unsigned)ceil_div64(static_cast<int64_t>(nb) * cin, 256), 256, sizeof(float) * cin * (cout + 1), st>>>(
-        dxp, cin_p, Gs, W->B3, P->src_nodes, static_cast<int>(c0), nb, cin, cout, scal,
+        dxp_b, cin_p, Gs, W->B3, P->src_nodes, static_cast<int>(c0), nb, cin, cout, scal,
         sp ? W->wscale + 2 * W->n_layers + 1 : nullptr, dx);
     NNC_CHECK_LAUNCH();
     // dW3[(k,o), i] += sum_c dY[c, (k,o)] Xg[c0 + c, i]
-    s = gemm_tn_pairs(W, dY, (sp ? 2 : 1) * NY, NY, static_cast<const char*>(Xg) + static_cast<size_t>(c0) * cin_p * 2 * (sp ? 2 : 1),
-                      (sp ? 2 : 1) * cin_p, cin_p, nb, NY, cin_p, dW3, cin_p, st);
+    r = gemm_tn_pairs(W, dY_b, (sp ? 2 : 1) * NY, NY,
+                      static_cast<const char*>(Xg) + static_cast<size_t>(c0) * cin_p * 2 * (sp ? 2 : 1), (sp ? 2 : 1) * cin_p,
+                      cin_p, nb, NY, cin_p, dW3, cin_p, st);
+    count(sp ? 6 : 4);
+    return r;
+  };
+  // sources inside the resident prefix (all of them when h is whole)
+  const int c_res = first_streamed_src(P, E_res);
+  for (int64_t c0 = 0; c0 < c_res; c0 += nb_max) {
+    const int nb = static_cast<int>((c_res - c0) < nb_max ? (c_res - c0) : nb_max);
+    s = run_batch(c0, nb, h, 0, round_up64(E_res, 128), dxp, dY);
     if (s) return s;
+  }
+  // the other sources: recompute the h of each batch's edges [g[c0], g[c1]) into the chunk buffer after its dY rows.
+  // Its padding rows are zeroed (TMA boxes reach them; the G rows they meet are zero)
+  const int* g = P->h_group_ptr;
+  for (int c0 = c_res; c0 < S;) {
+    const int c1 = apply_stream_batch_end(P, W, L, c0, pool);
+    NNC_REQUIRE(c1 > c0, NNCONV_ERR_WORKSPACE,
+                "backward_apply: workspace too small for one source (use nnconv_backward_apply_streamed_sizes)");
+    const int nb = c1 - c0;
+    const int64_t e_lo = g[c0], n = g[c1] - g[c0];
+    uint16_t* dY_b = reinterpret_cast<uint16_t*>(dyn + round_up64(static_cast<int64_t>(nb + 128) * cin_p * 4, 1024));
+    char* hc = reinterpret_cast<char*>(dY_b) + round_up64(static_cast<int64_t>(nb) * NY * 2 * (sp ? 2 : 1), 1024);
+    s = edge_features_rows(P, W, edge_attr, e_lo, n, hc, ef_ws, ef_bytes, nullptr, st, launches, nullptr);
+    if (s) return s;
+    s = run_batch(c0, nb, hc, e_lo, round_up64(n, 128), dxp, dY_b);
+    if (s) return s;
+    c0 = c1;
   }
   k_unpermute_w3q<<<(unsigned)ceil_div64(nWL, 256), 256, 0, st>>>(dW3, cin, cout, W->K, cin_p, scal, 6, dWL);
   NNC_CHECK_LAUNCH();
+  count(1);
   return NNCONV_OK;
 }
 
@@ -986,7 +1075,7 @@ struct MlpBwdLayout {
   size_t per_edge, per_src;
 };
 
-MlpBwdLayout mlp_bwd_layout(const Plan* P, const Weights* W, int T) {
+MlpBwdLayout mlp_bwd_layout(const Plan* P, const Weights* W, int T, bool streamed) {
   Carver c(nullptr, ~size_t(0));
   MlpBwdLayout L{};
   const size_t S = P->n_src > 0 ? P->n_src : 1;
@@ -1010,13 +1099,55 @@ MlpBwdLayout mlp_bwd_layout(const Plan* P, const Weights* W, int T) {
   }
   // Ghat row + dz ping/pong + stored hidden activations h_1..h_{L-2} + A1 row
   L.per_edge = (static_cast<size_t>(T) * 128 + 2 * maxkp * 2 + acts * 2) * pm + 128;
+  // streamed edge features: + the recomputed h_{L-1} of a batch (its ReLU mask), chunk-major
+  if (streamed) L.per_edge += static_cast<size_t>(W->Kp) * 2 * pm;
   L.per_src = static_cast<size_t>(T) * W->Kp * 64 * 2 * pm;      // Y^T rows of the T applications
   return L;
 }
+
+// end of the source batch starting at c0: sources while their Y^T rows and per-edge buffers fit avail (c0 = not even
+// one source group fits)
+int mlp_batch_end(const Plan* P, const MlpBwdLayout& L, int c0, size_t avail) {
+  const int* hgp = P->h_group_ptr;
+  int c1 = c0;
+  size_t used = 0;
+  while (c1 < P->n_src) {
+    const size_t add = L.per_src + L.per_edge * static_cast<size_t>(hgp[c1 + 1] - hgp[c1]);
+    if (used + add + L.per_edge * 256 > avail) break;
+    used += add;
+    ++c1;
+  }
+  return c1;
+}
 }  // namespace
 
-size_t backward_mlp_ws_bytes(const Plan* P, const Weights* W, int T, size_t want_bytes) {
-  MlpBwdLayout L = mlp_bwd_layout(P, W, T);
+int64_t backward_streamed_chunks(const Plan* P, const Weights* W, int T, int64_t E_res, size_t ws_bytes) {
+  if (E_res >= P->E || P->n_src == 0) return 0;
+  int64_t n = 0;
+  if (T == 0) {
+    const ApplyBwdLayout L = apply_bwd_layout(P, W);
+    const size_t fixed = L.fixed + bwd_ef_bytes(P, W, E_res) + 4096;
+    if (ws_bytes <= fixed) return 0;
+    for (int c0 = first_streamed_src(P, E_res); c0 < P->n_src; ++n) {
+      const int c1 = apply_stream_batch_end(P, W, L, c0, ws_bytes - fixed);
+      if (c1 == c0) return 0;
+      c0 = c1;
+    }
+    return n;
+  }
+  const MlpBwdLayout L = mlp_bwd_layout(P, W, T, true);
+  if (ws_bytes <= L.fixed + (1 << 16)) return 0;
+  for (int c0 = 0; c0 < P->n_src;) {
+    const int c1 = mlp_batch_end(P, L, c0, ws_bytes - L.fixed - (1 << 16));
+    if (c1 == c0) return 0;
+    if (P->h_group_ptr[c1] > E_res) ++n;
+    c0 = c1;
+  }
+  return n;
+}
+
+size_t backward_mlp_ws_bytes(const Plan* P, const Weights* W, int T, size_t want_bytes, int64_t E_res) {
+  MlpBwdLayout L = mlp_bwd_layout(P, W, T, E_res >= 0 && E_res < P->E);
   const size_t deg = P->max_out_deg > 0 ? P->max_out_deg : 1;
   const size_t need_min = L.fixed + L.per_src + L.per_edge * (deg + 256) + (1 << 16);
   const size_t all = L.fixed + L.per_src * (P->n_src > 0 ? P->n_src : 1) + L.per_edge * (static_cast<size_t>(P->E) + 256) +
@@ -1025,11 +1156,12 @@ size_t backward_mlp_ws_bytes(const Plan* P, const Weights* W, int T, size_t want
   return w < all ? w : all;
 }
 
-int backward_mlp_tc(const Plan* P, const Weights* W, const float* edge_attr, const void* h, int T,
+int backward_mlp_tc(const Plan* P, const Weights* W, const float* edge_attr, const void* h, int64_t E_res, int T,
                     const float* const* gouts, const float* const* xs_in, int aggr_mean, float* const* dWs,
                     float* const* dbs, void* ws, size_t ws_bytes, cudaStream_t st, const void* acts, float* grad_ea) {
   NNC_REQUIRE(backward_tc_supported(W), NNCONV_ERR_UNSUPPORTED, "tensor-core backward: unsupported shape / precision");
-  if (acts != nullptr && edge_acts_bytes(P, W) == 0) acts = nullptr;
+  const bool streamed = E_res < P->E;
+  if (streamed || (acts != nullptr && edge_acts_bytes(P, W) == 0)) acts = nullptr;
   NNC_REQUIRE(T >= 1 && T <= kMaxApps, NNCONV_ERR_ARG, "backward_mlp: 1..%d applications per pass", kMaxApps);
   const int nl = W->n_layers;
   const int cin = W->cin, cout = W->cout, Kp = W->Kp, cin_p = W->cin_p, k_in = W->dims[0];
@@ -1051,7 +1183,7 @@ int backward_mlp_tc(const Plan* P, const Weights* W, const float* edge_attr, con
     }
     return NNCONV_OK;
   }
-  MlpBwdLayout L = mlp_bwd_layout(P, W, T);
+  MlpBwdLayout L = mlp_bwd_layout(P, W, T, streamed);
   NNC_REQUIRE(ws != nullptr && ws_bytes >= L.fixed + L.per_src + L.per_edge * 256, NNCONV_ERR_WORKSPACE,
               "backward_mlp: workspace too small");
   char* base = static_cast<char*>(ws);
@@ -1081,7 +1213,7 @@ int backward_mlp_tc(const Plan* P, const Weights* W, const float* edge_attr, con
   const int* hgp = P->h_group_ptr;
   const int* htp = P->h_tile_ptr;
   const size_t avail = ws_bytes - L.fixed - (1 << 16);
-  const int64_t e_pad = round_up64(P->E, 128);
+  const int64_t h_rows_res = round_up64(E_res, 128);     // panel height of h (the whole h: round_up(E, 128))
   const int BN = Kp % 128 == 0 ? 128 : 64;   // k block of k_dh (Kp is a multiple of 64; <= 128 accumulator registers)
   int maxkp = 0;
   for (int l = 1; l <= nl - 1; ++l) maxkp = W->kp[l] > maxkp ? W->kp[l] : maxkp;
@@ -1110,18 +1242,13 @@ int backward_mlp_tc(const Plan* P, const Weights* W, const float* edge_attr, con
   if (fuse_colsum) dh_smem += cs_bytes;
   int c0 = 0;
   while (c0 < S) {
-    int c1 = c0;
-    size_t used = 0;
-    while (c1 < S) {
-      const size_t add = L.per_src + L.per_edge * static_cast<size_t>(hgp[c1 + 1] - hgp[c1]);
-      if (used + add + L.per_edge * 256 > avail && c1 > c0) break;
-      NNC_REQUIRE(used + add + L.per_edge * 256 <= avail, NNCONV_ERR_WORKSPACE,
-                  "backward_mlp: workspace too small for one source group");
-      used += add;
-      ++c1;
-    }
+    const int c1 = mlp_batch_end(P, L, c0, avail);
+    NNC_REQUIRE(c1 > c0, NNCONV_ERR_WORKSPACE, "backward_mlp: workspace too small for one source group");
     const int nb = c1 - c0, e_base = hgp[c0], n = hgp[c1] - hgp[c0];
     const int64_t n_pad = round_up64(n, 128) + 128;
+    // a batch with edges past the resident prefix recomputes its own h_{L-1} (the ReLU mask of k_dh) from the hidden
+    // activations below, with the forward's GEMMs (same bits as the h the forward contracted)
+    const bool stream_h = e_base + n > E_res;
     Carver cv(base + L.fixed, avail + (1 << 16));
     uint16_t* Yt = cv.take<uint16_t>(static_cast<size_t>(T) * nb * Kp * 64 * pm);
     uint16_t* Gh = cv.take<uint16_t>(static_cast<size_t>(n_pad) * T * 64 * pm);
@@ -1136,7 +1263,39 @@ int backward_mlp_tc(const Plan* P, const Weights* W, const float* edge_attr, con
       else
         act[l] = cv.take<uint16_t>(static_cast<size_t>(n_pad) * W->kp[l] * pm);
     }
+    uint16_t* hb = stream_h ? cv.take<uint16_t>(static_cast<size_t>(n_pad) * Kp * pm) : nullptr;
     NNC_REQUIRE(cv.ok(), NNCONV_ERR_WORKSPACE, "backward_mlp: workspace carve overflow");
+    // ---- the hidden activations h_1 .. h_{L-2} of the batch (16-bit, row-major) and A1
+    auto recompute_acts = [&]() -> int {
+      int r = launch_build_a1(W->prec, edge_attr, P->perm, e_base, n, k_in, A1, st);
+      if (r) return r;
+      if (nl >= 3 && acts == nullptr) {
+        r = launch_gemm_tc(W->prec, A1, n, 0, n, 64, W->W1aug, W->kp[1], nullptr, 1, act[1], pm * W->kp[1], st, nullptr, 0, 0,
+                           sp ? GEMM_C_SPLIT : 0);
+        if (r) return r;
+        for (int l = 2; l <= nl - 2; ++l) {
+          r = launch_gemm_tc(W->prec, act[l - 1], n, 0, n, kmul * W->kp[l - 1], W->Wh[l], W->kp[l], W->bh[l], 1, act[l],
+                             pm * W->kp[l], st, nullptr, 0, 0, sp ? (GEMM_A_SPLIT | GEMM_C_SPLIT) : 0, nullptr, nullptr, 0, 0,
+                             0, sp ? W->wscale + 2 * l + 1 : nullptr);
+          if (r) return r;
+        }
+      }
+      return NNCONV_OK;
+    };
+    if (stream_h) {
+      s = recompute_acts();
+      if (s) return s;
+      // h_{L-1} of the batch into chunk-major panels of round_up(n, 128) rows (edge_features_rows' last GEMM)
+      const int64_t hpad = round_up64(n, 128);
+      if (nl == 2)
+        s = launch_gemm_tc(W->prec, A1, n, 0, n, 64, W->W1aug, W->kp[1], nullptr, 1, hb, pm * W->kp[1], st, nullptr, hpad, 0,
+                           sp ? GEMM_C_SPLIT : 0);
+      else
+        s = launch_gemm_tc(W->prec, act[nl - 2], n, 0, n, kmul * W->kp[nl - 2], W->Wh[nl - 1], W->kp[nl - 1], W->bh[nl - 1], 1,
+                           hb, pm * W->kp[nl - 1], st, nullptr, hpad, 0, sp ? (GEMM_A_SPLIT | GEMM_C_SPLIT) : 0, nullptr,
+                           nullptr, 0, 0, 0, sp ? W->wscale + 2 * (nl - 1) + 1 : nullptr);
+      if (s) return s;
+    }
     // ---- Y^T of the batch for every application: Yt[t][(c, k), o] = sum_i Xc_t[c, i] W_L[i*out + o, k]
     //      (PREC_F16X2: row c of application t is [hi | lo], 2 * Kp * 64)
     for (int t = 0; t < T; ++t) {
@@ -1169,9 +1328,11 @@ int backward_mlp_tc(const Plan* P, const Weights* W, const float* edge_attr, con
       if (s) return s;
       DhArgs a;
       a.tile_c = P->tile_c; a.tile_e0 = P->tile_e0; a.tile_cnt = P->tile_cnt;
-      a.tile0 = htp[c0]; a.tile1 = htp[c1]; a.c0 = c0; a.Sb = nb; a.e_base = e_base; a.e_pad = static_cast<int>(e_pad);
+      a.tile0 = htp[c0]; a.tile1 = htp[c1]; a.c0 = c0; a.Sb = nb; a.e_base = e_base;
+      a.h_e_base = stream_h ? e_base : 0;
+      a.h_rows = static_cast<int>(stream_h ? round_up64(n, 128) : h_rows_res);
       a.T = T; a.Kp = Kp; a.n_nb = Kp / BN;
-      a.h = static_cast<const uint16_t*>(h); a.dz = dzA;
+      a.h = stream_h ? hb : static_cast<const uint16_t*>(h); a.dz = dzA;
       a.colsum = fuse_colsum ? reinterpret_cast<float*>(base + L.off_D[nl - 1]) + 3 * k_in : nullptr;
       a.colsum_stride = 64;
       const int tiles = a.tile1 - a.tile0;
@@ -1188,19 +1349,9 @@ int backward_mlp_tc(const Plan* P, const Weights* W, const float* edge_attr, con
       }
       NNC_CHECK_LAUNCH();
     }
-    // ---- recompute the hidden activations h_1 .. h_{L-2} of the batch (16-bit, row-major) and A1
-    s = launch_build_a1(W->prec, edge_attr, P->perm, e_base, n, k_in, A1, st);
-    if (s) return s;
-    if (nl >= 3 && acts == nullptr) {
-      s = launch_gemm_tc(W->prec, A1, n, 0, n, 64, W->W1aug, W->kp[1], nullptr, 1, act[1], pm * W->kp[1], st, nullptr, 0, 0,
-                         sp ? GEMM_C_SPLIT : 0);
+    if (!stream_h) {
+      s = recompute_acts();
       if (s) return s;
-      for (int l = 2; l <= nl - 2; ++l) {
-        s = launch_gemm_tc(W->prec, act[l - 1], n, 0, n, kmul * W->kp[l - 1], W->Wh[l], W->kp[l], W->bh[l], 1, act[l],
-                           pm * W->kp[l], st, nullptr, 0, 0, sp ? (GEMM_A_SPLIT | GEMM_C_SPLIT) : 0, nullptr, nullptr, 0, 0, 0,
-                           sp ? W->wscale + 2 * l + 1 : nullptr);
-        if (s) return s;
-      }
     }
     // ---- down through the layers
     uint16_t* cur = dzA;

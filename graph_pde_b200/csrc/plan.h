@@ -102,6 +102,12 @@ int apply(const Plan* P, const Weights* W, const void* h, const float* x, const 
 int stream_split(const Plan* P, const Weights* W, size_t resident_bytes, size_t chunk_ws_bytes, int64_t* E_res,
                  size_t* h_res_bytes, size_t* ws_bytes, int64_t* n_chunks);
 bool is_unit_boundary(const Plan* P, int64_t e);
+// h of the sorted edges [e_begin, e_begin + E) into the chunk-major panels of round_up(E, 128) rows at h (padding rows
+// zeroed); ws: scratch of ef_row_bytes(W) per row plus 4096 bytes; overflow and launches nullable, acts as above
+int edge_features_rows(const Plan* P, const Weights* W, const float* edge_attr, int64_t e_begin, int64_t E, void* h,
+                       void* ws, size_t ws_bytes, int* overflow, cudaStream_t st, int64_t* launches, void* acts);
+size_t ef_row_bytes(const Weights* W);
+size_t h_row_bytes(const Weights* W);      // bytes of one edge's cached h (16-bit: Kp * 2, twice that at f16x2)
 int apply_streamed(const Plan* P, const Weights* W, const float* edge_attr, const void* h_res, int64_t E_res,
                    const float* x, const float* root, const float* bias, int aggr_mean, float* out, void* ws,
                    size_t ws_bytes, cudaStream_t st, int64_t* launches, unsigned node_flags);
@@ -109,16 +115,23 @@ int apply_streamed(const Plan* P, const Weights* W, const float* edge_attr, cons
 // tensor-core backward (backward_tc.cu): per application (dx, dW_L, db_L, droot, dbias) and, once per
 // (edge_attr, parameters) for all T applications of a shared conv, the pass through the hidden layers.
 // grad_ea (nullable): [E, k_in] fp32 in the caller's edge order, WRITTEN -- the gradient w.r.t. edge_attr.
+// h holds the edge features of the sorted edges [0, E_res) (a unit boundary; E_res = E: the whole cached h).  With
+// E_res < E the h of the other edges is recomputed from edge_attr per source batch into a chunk buffer of the
+// workspace (backward_*_ws_bytes with that E_res), and kept activations (acts) are not used.
 bool backward_tc_supported(const Weights* W);
-size_t backward_apply_ws_bytes(const Plan* P, const Weights* W, size_t want_bytes);
-int backward_apply_tc(const Plan* P, const Weights* W, const void* h, const float* x, const float* root,
-                      int aggr_mean, const float* gout, float* dx, float* dWL, float* dbL, float* droot, float* dbias,
-                      void* ws, size_t ws_bytes, cudaStream_t st);
-size_t backward_mlp_ws_bytes(const Plan* P, const Weights* W, int T, size_t want_bytes);
-int backward_mlp_tc(const Plan* P, const Weights* W, const float* edge_attr, const void* h, int T,
+size_t backward_apply_ws_bytes(const Plan* P, const Weights* W, size_t want_bytes, int64_t E_res = -1,
+                               size_t chunk_ws_bytes = 0);
+int backward_apply_tc(const Plan* P, const Weights* W, const float* edge_attr, const void* h, int64_t E_res,
+                      const float* x, const float* root, int aggr_mean, const float* gout, float* dx, float* dWL,
+                      float* dbL, float* droot, float* dbias, void* ws, size_t ws_bytes, cudaStream_t st,
+                      int64_t* launches = nullptr);
+size_t backward_mlp_ws_bytes(const Plan* P, const Weights* W, int T, size_t want_bytes, int64_t E_res = -1);
+int backward_mlp_tc(const Plan* P, const Weights* W, const float* edge_attr, const void* h, int64_t E_res, int T,
                     const float* const* gouts, const float* const* xs_in, int aggr_mean, float* const* dWs,
                     float* const* dbs, void* ws, size_t ws_bytes, cudaStream_t st, const void* acts = nullptr,
                     float* grad_ea = nullptr);
+// source batches whose edge features the call with this workspace recomputes (T = 0: backward_apply_tc)
+int64_t backward_streamed_chunks(const Plan* P, const Weights* W, int T, int64_t E_res, size_t ws_bytes);
 
 // per-edge kernel matrices for low out-degree graphs (formulation B): Kmat [E, cin*cout] 16-bit in sorted edge order
 size_t edge_kernels_bytes(const Plan* P, const Weights* W);

@@ -34,7 +34,7 @@ from . import _lib
 __all__ = ['NNConv_old', 'NNConv', 'ECConv', 'stats', 'clear_caches', 'default_precision']
 
 stats = {'launches': 0, 'plans_built': 0, 'edge_feature_passes': 0, 'applies': 0, 'weight_preps': 0,
-         'streamed_chunk_passes': 0}
+         'streamed_chunk_passes': 0, 'streamed_backward_chunk_passes': 0}
 
 _PLAN_CACHE = collections.OrderedDict()
 _PLAN_CACHE_MAX = int(os.environ.get('NNCONV_B200_PLAN_CACHE', '64'))                 # entries
@@ -64,6 +64,12 @@ _EDGE_KERNELS_MAX_BYTES = 2 << 30
 # the rest chunk by chunk inside every application (see NNConv_old).  Unset: the whole h, streaming only on an OOM.
 _EDGE_FEATURE_BYTES = os.environ.get('NNCONV_B200_EDGE_FEATURE_BYTES')
 _STREAM_MARGIN_BYTES = 1 << 30     # left free beside the resident prefix when the budget comes from mem_get_info
+# ... and in training, beside the backward's workspace: what else a step allocates (autograd's saved tensors, the
+# backward thread's cuBLAS handle and workspace, optimizer state) and the caching allocator's fragmentation
+_STREAM_TRAIN_MARGIN_BYTES = 4 << 30
+# default of NNConv_old(streamed_training=...): '1' lets training run on streamed edge features (see NNConv_old)
+_STREAMED_TRAINING = os.environ.get('NNCONV_B200_STREAMED_TRAINING', '0') == '1'
+_MLP_GROUP = 6                     # applications per deferred pass through the hidden layers
 
 
 def default_precision():
@@ -126,6 +132,14 @@ class _Streamed(object):
 
     def __init__(self, h_res, E_res, ws_bytes, n_chunks, ea32):
         self.h_res, self.E_res, self.ws_bytes, self.n_chunks, self.ea32 = h_res, E_res, ws_bytes, n_chunks, ea32
+
+
+def _streamed_chunks(plan, prepared, e_res, n_apps, ws_bytes):
+    """Source batches whose edge features a streamed backward call recomputes (n_apps = 0: the per-application call)."""
+    n = ctypes.c_int64(0)
+    _lib.check(_lib.lib().nnconv_backward_streamed_chunks(plan.handle, prepared.handle, e_res, n_apps, ws_bytes,
+                                                          ctypes.byref(n)))
+    return n.value
 
 
 def _plan_key(edge_index, n_nodes, flow):
@@ -254,7 +268,7 @@ class _EdgeFeaturesFn(torch.autograd.Function):
     def forward(ctx, module, state, edge_attr, *hidden_params):
         ctx.module, ctx.state = module, state
         ctx.ea_dtype = edge_attr.dtype
-        return torch.zeros(1, device=state.h.device)
+        return torch.zeros(1, device=state.ea32.device)
 
     @staticmethod
     def backward(ctx, _):
@@ -300,9 +314,15 @@ class NNConv_old(torch.nn.Module):
     ``edge_feature_bytes`` (default: environment NNCONV_B200_EDGE_FEATURE_BYTES, else unlimited) bounds the cached edge
     features (``Kp * 2`` bytes per edge, twice that at 'f16x2').  A graph whose features exceed it keeps a unit-aligned
     prefix resident and recomputes the rest chunk by chunk inside every application (same bits, more time); without a
-    budget that happens only when allocating the whole h runs out of device memory.  Inference only: training needs the
-    whole h resident.  Precision 'fp32' and the per-edge kernel matrices (graphs with few out-edges per source) never
-    stream.
+    budget that happens only when allocating the whole h runs out of device memory.  Precision 'fp32' and the per-edge
+    kernel matrices (graphs with few out-edges per source) never stream.
+
+    ``streamed_training`` (default: environment NNCONV_B200_STREAMED_TRAINING == '1', else False) lets training run on
+    such streamed features: the tensor-core backward recomputes the streamed part of h once per application and once
+    more in the pass through the hidden layers (about 2T+1 edge-feature passes over the streamed edges per step instead
+    of none), and the CUDA-core backward recomputes everything from edge_attr anyway.  Off, autograd through streamed
+    features raises.  When the budget comes from the free device memory, the resident prefix leaves room for the
+    backward's workspace.
 
     Caches: the down-converted weights and the x-independent edge features are cached per (parameter versions,
     edge_attr version).  Optimizer steps, ``load_state_dict`` and ``train()/eval()`` invalidate them; writes that
@@ -315,6 +335,7 @@ class NNConv_old(torch.nn.Module):
         self.precision = kwargs.pop('precision', None)
         self.flow = kwargs.pop('flow', 'source_to_target')
         self.edge_feature_bytes = kwargs.pop('edge_feature_bytes', None)
+        self.streamed_training = bool(kwargs.pop('streamed_training', _STREAMED_TRAINING))
         if kwargs:
             raise TypeError('unexpected keyword arguments %s' % sorted(kwargs))
         if aggr not in ('add', 'mean', 'max'):
@@ -429,9 +450,13 @@ class NNConv_old(torch.nn.Module):
             _lib.check(L.nnconv_edge_acts_sizes(plan.handle, prepared.handle, ctypes.byref(acts_b)))
             if acts_b.value > _KEEP_ACTS_MAX_BYTES:
                 acts_b = ctypes.c_size_t(0)
-        if hit is not None and isinstance(hit[0], _Streamed) and for_grad:
-            self._streaming_grad_error(hit[0].h_res.numel())
-        if hit is not None and (acts_b.value == 0 or hit[2] is not None):
+        streamed_hit = hit is not None and isinstance(hit[0], _Streamed)
+        if streamed_hit and for_grad:
+            if not self.streamed_training:
+                self._streaming_grad_error(hit[0].h_res.numel())
+            if hit[0].auto and not hit[0].for_grad:
+                hit = None               # sized for inference: the prefix leaves no room for the backward's workspace
+        if hit is not None and (acts_b.value == 0 or hit[2] is not None or streamed_hit):
             return hit[0]
         h_b, ws_b = ctypes.c_size_t(), ctypes.c_size_t()
         _lib.check(L.nnconv_edge_features_sizes(plan.handle, prepared.handle, _EF_WS_BYTES, ctypes.byref(h_b),
@@ -442,9 +467,9 @@ class NNConv_old(torch.nn.Module):
         budget = self._budget()
         streams = self._streams(plan, prepared)
         if budget is not None and h_b.value > budget and streams:
-            if for_grad:
+            if for_grad and not self.streamed_training:
                 self._streaming_grad_error(budget)
-            return self._streamed_features(key, plan, prepared, edge_attr, budget)
+            return self._streamed_features(key, plan, prepared, edge_attr, budget, for_grad)
         try:
             h = torch.empty(h_b.value, dtype=torch.uint8, device=dev)
             ws = torch.empty(ws_b.value, dtype=torch.uint8, device=dev)
@@ -452,12 +477,12 @@ class NNConv_old(torch.nn.Module):
             if not streams:
                 raise
             h = ws = None
-            if for_grad:
+            if for_grad and not self.streamed_training:
                 self._streaming_grad_error(h_b.value)
             self._h_cache.clear()
             self._k_cache = None
             self._tstate = None
-            return self._streamed_features(key, plan, prepared, edge_attr, None)
+            return self._streamed_features(key, plan, prepared, edge_attr, None, for_grad)
         acts = torch.empty(acts_b.value, dtype=torch.uint8, device=dev) if acts_b.value else None
         n_l = ctypes.c_int64(0)
         if acts is not None:
@@ -477,11 +502,38 @@ class NNConv_old(torch.nn.Module):
         raise RuntimeError(
             'graph_pde_b200.NNConv: the edge features of this graph do not fit on the device or in the cache budget '
             '(%d bytes), and training needs the whole h resident: streamed edge features are inference only (call '
-            'under torch.no_grad(), or raise edge_feature_bytes / NNCONV_B200_EDGE_FEATURE_BYTES)' % nbytes)
+            'under torch.no_grad(), or raise edge_feature_bytes / NNCONV_B200_EDGE_FEATURE_BYTES). Training on '
+            'streamed edge features recomputes them in every backward application: enable it with '
+            'streamed_training=True or NNCONV_B200_STREAMED_TRAINING=1' % nbytes)
 
-    def _streamed_features(self, key, plan, prepared, edge_attr, budget):
+    def _backward_reserve(self, plan, prepared, e_res, edge_attr):
+        """Device bytes the backward of a training step on streamed features needs beside the resident prefix: its
+        workspace plus the fp32 gradient w.r.t. edge_attr."""
+        if _BWD_MODE != 'fp32' and prepared.bwd_tc:
+            need = self._tc_backward_ws_bytes(plan, prepared, e_res)
+        else:
+            b = ctypes.c_size_t()
+            _lib.check(_lib.lib().nnconv_backward_sizes(plan.handle, self._get_prepared32().handle, _BWD_WS_BYTES,
+                                                        ctypes.byref(b)))
+            need = b.value
+        return need + 2 * edge_attr.numel() * 4
+
+    @staticmethod
+    def _tc_backward_ws_bytes(plan, prepared, e_res):
+        """One workspace for the streamed tensor-core backward: its per-application calls and the MLP pass run one after
+        the other on the stream, so the larger of the two sizes serves both."""
+        L = _lib.lib()
+        a, m = ctypes.c_size_t(), ctypes.c_size_t()
+        _lib.check(L.nnconv_backward_apply_streamed_sizes(plan.handle, prepared.handle, e_res, _BWD_APPLY_WS_BYTES,
+                                                          _EF_WS_BYTES, ctypes.byref(a)))
+        _lib.check(L.nnconv_backward_mlp_streamed_sizes(plan.handle, prepared.handle, e_res, _MLP_GROUP,
+                                                        _BWD_MLP_WS_BYTES, ctypes.byref(m)))
+        return max(a.value, m.value)
+
+    def _streamed_features(self, key, plan, prepared, edge_attr, budget, for_grad=False):
         """Cache the unit-aligned prefix of h that fits ``budget`` bytes (None: what the device has free beside the
-        streaming workspace) and return the _Streamed the applications run from."""
+        streaming workspace and, for training, the backward's workspace) and return the _Streamed the applications run
+        from."""
         L = _lib.lib()
         dev = edge_attr.device
 
@@ -495,7 +547,19 @@ class NNConv_old(torch.nn.Module):
         e_res, h_b, ws_b, n_ch = split(budget if budget is not None else 0)
         if budget is None:
             free = torch.cuda.mem_get_info(dev)[0] + torch.cuda.memory_reserved(dev) - torch.cuda.memory_allocated(dev)
-            e_res, h_b, ws_b, n_ch = split(free - ws_b - _STREAM_MARGIN_BYTES)
+            work = ws_b + _STREAM_MARGIN_BYTES
+            if for_grad:
+                # the streamed backward's workspaces do not depend on where the prefix ends: sized at E_res = 0
+                work += self._backward_reserve(plan, prepared, 0, edge_attr) + _STREAM_TRAIN_MARGIN_BYTES
+            e_res, h_b, ws_b, n_ch = split(free - work)
+        # training on the tensor cores: the backward's workspace (several GiB: 9 GiB at 241^2, f16x2) is allocated here,
+        # beside the prefix, and reused by every backward call of this step.  Allocated per call, it would need one
+        # contiguous block of that size after the forward has fragmented the caching allocator's segments.
+        bwd_ws = None
+        if for_grad and _BWD_MODE != 'fp32' and prepared.bwd_tc:
+            # sized at E_res = 0: the streamed sizes do not depend on where the prefix ends, and they bound the whole-h
+            # sizes should the prefix below end up covering every edge
+            bwd_ws = torch.empty(self._tc_backward_ws_bytes(plan, prepared, 0), dtype=torch.uint8, device=dev)
         h_res = None
         if e_res > 0:
             try:
@@ -519,6 +583,7 @@ class NNConv_old(torch.nn.Module):
             self._check_overflow(prepared, ws, dev)
             del ws
         st = _Streamed(h_res, e_res, ws_b, n_ch, edge_attr)
+        st.auto, st.for_grad, st.bwd_ws = budget is None, for_grad, bwd_ws
         self._h_cache[key] = (st, edge_attr, None)
         return st
 
@@ -699,20 +764,54 @@ class NNConv_old(torch.nn.Module):
         plan, prep = state.plan, state.prepared
         lin = _linear_chain(self.nn)[-1]
         with torch.cuda.device(dev):
-            ws_b = ctypes.c_size_t()
-            _lib.check(L.nnconv_backward_apply_sizes(plan.handle, prep.handle, _BWD_APPLY_WS_BYTES, ctypes.byref(ws_b)))
-            ws = torch.empty(ws_b.value, dtype=torch.uint8, device=dev)
             dx = torch.empty_like(x32)
             dwl = torch.empty_like(lin.weight, dtype=torch.float32)
             dbl = torch.empty_like(lin.bias, dtype=torch.float32)
             droot = torch.empty_like(self.root, dtype=torch.float32) if self.root is not None else None
             dbias = torch.empty_like(self.bias, dtype=torch.float32) if self.bias is not None else None
             root = self.root.detach().contiguous().float() if self.root is not None else None
-            _lib.check(L.nnconv_backward_apply(plan.handle, prep.handle, _ptr(state.h), _ptr(x32), _ptr(root),
-                                               _lib.AGGR[self.aggr], _ptr(g32), _ptr(dx), _ptr(dwl), _ptr(dbl),
-                                               _ptr(droot), _ptr(dbias), _ptr(ws), ws_b.value, _stream_ptr(dev)))
+            if isinstance(state.h, _Streamed):
+                self._backward_apply_streamed(state, x32, g32, dx, dwl, dbl, root, droot, dbias)
+            else:
+                ws_b = ctypes.c_size_t()
+                _lib.check(L.nnconv_backward_apply_sizes(plan.handle, prep.handle, _BWD_APPLY_WS_BYTES,
+                                                         ctypes.byref(ws_b)))
+                ws = torch.empty(ws_b.value, dtype=torch.uint8, device=dev)
+                _lib.check(L.nnconv_backward_apply(plan.handle, prep.handle, _ptr(state.h), _ptr(x32), _ptr(root),
+                                                   _lib.AGGR[self.aggr], _ptr(g32), _ptr(dx), _ptr(dwl), _ptr(dbl),
+                                                   _ptr(droot), _ptr(dbias), _ptr(ws), ws_b.value, _stream_ptr(dev)))
             stats['backwards'] = stats.get('backwards', 0) + 1
         return dx, dwl, dbl, droot, dbias
+
+    def _backward_apply_streamed(self, state, x32, g32, dx, dwl, dbl, root, droot, dbias):
+        """nnconv_backward_apply over the resident prefix of h; the other edges' h is recomputed per source batch."""
+        L = _lib.lib()
+        dev = x32.device
+        plan, prep, st = state.plan, state.prepared, state.h
+        ws = self._streamed_bwd_ws(st, plan, prep, 0)
+        n_l = ctypes.c_int64(0)
+        _lib.check(L.nnconv_backward_apply_streamed(plan.handle, prep.handle, _ptr(st.ea32), _ptr(st.h_res), st.E_res,
+                                                    _ptr(x32), _ptr(root), _lib.AGGR[self.aggr], _ptr(g32), _ptr(dx),
+                                                    _ptr(dwl), _ptr(dbl), _ptr(droot), _ptr(dbias), _ptr(ws), ws.numel(),
+                                                    _stream_ptr(dev), ctypes.byref(n_l)))
+        stats['launches'] += n_l.value
+        stats['streamed_backward_chunk_passes'] += _streamed_chunks(plan, prep, st.E_res, 0, ws.numel())
+
+    @staticmethod
+    def _streamed_bwd_ws(st, plan, prep, n_apps):
+        """The workspace allocated with the prefix (see _streamed_features), else one of the size the call needs
+        (n_apps = 0: a per-application call)."""
+        if st.bwd_ws is not None:
+            return st.bwd_ws
+        L = _lib.lib()
+        b = ctypes.c_size_t()
+        if n_apps == 0:
+            _lib.check(L.nnconv_backward_apply_streamed_sizes(plan.handle, prep.handle, st.E_res, _BWD_APPLY_WS_BYTES,
+                                                              _EF_WS_BYTES, ctypes.byref(b)))
+        else:
+            _lib.check(L.nnconv_backward_mlp_streamed_sizes(plan.handle, prep.handle, st.E_res, n_apps,
+                                                            _BWD_MLP_WS_BYTES, ctypes.byref(b)))
+        return torch.empty(b.value, dtype=torch.uint8, device=st.h_res.device)
 
     def _backward_mlp_impl(self, state, want_ea=False):
         """Gradients of the hidden Linear layers, one pass for all applications recorded in the state (in groups
@@ -721,16 +820,21 @@ class NNConv_old(torch.nn.Module):
         L = _lib.lib()
         plan, prep = state.plan, state.prepared
         hidden = _linear_chain(self.nn)[:-1]
-        dev = state.h.device
+        dev = state.ea32.device
+        streamed = state.h if isinstance(state.h, _Streamed) else None
         total = None
         gea_total = None
         with torch.cuda.device(dev):
-            for i0 in range(0, len(state.apps), 6):
-                apps = state.apps[i0:i0 + 6]
+            for i0 in range(0, len(state.apps), _MLP_GROUP):
+                apps = state.apps[i0:i0 + _MLP_GROUP]
                 n = len(apps)
-                ws_b = ctypes.c_size_t()
-                _lib.check(L.nnconv_backward_mlp_sizes(plan.handle, prep.handle, n, _BWD_MLP_WS_BYTES, ctypes.byref(ws_b)))
-                ws = torch.empty(ws_b.value, dtype=torch.uint8, device=dev)
+                if streamed is not None:
+                    ws = self._streamed_bwd_ws(streamed, plan, prep, n)
+                else:
+                    ws_b = ctypes.c_size_t()
+                    _lib.check(L.nnconv_backward_mlp_sizes(plan.handle, prep.handle, n, _BWD_MLP_WS_BYTES,
+                                                           ctypes.byref(ws_b)))
+                    ws = torch.empty(ws_b.value, dtype=torch.uint8, device=dev)
                 dws = [torch.empty_like(l.weight, dtype=torch.float32) for l in hidden]
                 dbs = [torch.empty_like(l.bias, dtype=torch.float32) for l in hidden]
                 gea = torch.empty(state.ea32.shape, dtype=torch.float32, device=dev) if want_ea else None
@@ -738,9 +842,17 @@ class NNConv_old(torch.nn.Module):
                 xp = (ctypes.c_void_p * n)(*[x.data_ptr() for _, x in apps])
                 wp = (ctypes.c_void_p * len(hidden))(*[t.data_ptr() for t in dws])
                 bp = (ctypes.c_void_p * len(hidden))(*[t.data_ptr() for t in dbs])
-                _lib.check(L.nnconv_backward_mlp_ex(plan.handle, prep.handle, _ptr(state.ea32), _ptr(state.h), n, gp, xp,
-                                                    _lib.AGGR[self.aggr], wp, bp, _ptr(ws), ws_b.value, _stream_ptr(dev),
-                                                    _ptr(getattr(state, 'acts', None)), _ptr(gea)))
+                if streamed is not None:
+                    _lib.check(L.nnconv_backward_mlp_streamed(plan.handle, prep.handle, _ptr(state.ea32),
+                                                              _ptr(streamed.h_res), streamed.E_res, n, gp, xp,
+                                                              _lib.AGGR[self.aggr], wp, bp, _ptr(ws), ws.numel(),
+                                                              _stream_ptr(dev), _ptr(gea)))
+                    stats['streamed_backward_chunk_passes'] += _streamed_chunks(plan, prep, streamed.E_res, n,
+                                                                                ws.numel())
+                else:
+                    _lib.check(L.nnconv_backward_mlp_ex(plan.handle, prep.handle, _ptr(state.ea32), _ptr(state.h), n,
+                                                        gp, xp, _lib.AGGR[self.aggr], wp, bp, _ptr(ws), ws_b.value,
+                                                        _stream_ptr(dev), _ptr(getattr(state, 'acts', None)), _ptr(gea)))
                 flat = [t for pair in zip(dws, dbs) for t in pair]
                 total = flat if total is None else [a + b for a, b in zip(total, flat)]
                 if gea is not None:
@@ -751,6 +863,16 @@ class NNConv_old(torch.nn.Module):
             if want_ea:
                 gea_total = torch.zeros(state.ea32.shape, dtype=torch.float32, device=dev)
         return total, gea_total
+
+    def _get_prepared32(self):
+        """fp32 weight snapshot of the CUDA-core backward (cached per parameter versions)."""
+        linears = _linear_chain(self.nn)
+        key = ('fp32',) + tuple((l.weight.data_ptr(), l.weight._version, l.bias.data_ptr(), l.bias._version)
+                                for l in linears)
+        if getattr(self, '_prepared32_key', None) != key:
+            self._prepared32 = _Prepared(linears, self.in_channels, self.out_channels, 'fp32')
+            self._prepared32_key = key
+        return self._prepared32
 
     def _backward_impl(self, x, edge_index, pseudo, grad_out, want_ea=False):
         """fp32 CUDA-core backward of one application; with ``want_ea`` also the gradient w.r.t. edge_attr
@@ -763,12 +885,7 @@ class NNConv_old(torch.nn.Module):
             n = x32.size(0)
             plan = get_plan(edge_index, n, self.flow)
             linears = _linear_chain(self.nn)
-            key = ('fp32',) + tuple((l.weight.data_ptr(), l.weight._version, l.bias.data_ptr(), l.bias._version)
-                                    for l in linears)
-            if getattr(self, '_prepared32_key', None) != key:
-                self._prepared32 = _Prepared(linears, self.in_channels, self.out_channels, 'fp32')
-                self._prepared32_key = key
-            prep = self._prepared32
+            prep = self._get_prepared32()
             ws_b = ctypes.c_size_t()
             _lib.check(L.nnconv_backward_sizes(plan.handle, prep.handle, _BWD_WS_BYTES, ctypes.byref(ws_b)))
             ws = torch.empty(ws_b.value, dtype=torch.uint8, device=x.device)

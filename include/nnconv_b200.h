@@ -226,6 +226,31 @@ int nnconv_backward_mlp_ex(const nnconv_plan_t* plan, const nnconv_weights_t* w,
                            float* const* grad_W, float* const* grad_b, void* ws, size_t ws_bytes, void* stream,
                            const void* acts, float* grad_edge_attr /* nullable */);
 
+/* Tensor-core backward over partially resident edge features (training on graphs whose h does not fit the device):
+ * h_res / E_res as for nnconv_apply_streamed (E_res a unit boundary; E_res = E is the cached call).  The sources whose
+ * edges all lie in [0, E_res) run against h_res; the others run in source batches that first recompute the h of their
+ * edges from edge_attr into a chunk buffer of the workspace (same bits as the cached pass).  The MLP pass recomputes
+ * h_{L-1} of such batches for its ReLU mask.  Gradients are WRITTEN; no allocation, no host synchronisation.
+ *   nnconv_backward_apply_streamed_sizes: want_bytes as for nnconv_backward_apply_sizes, plus chunk rows for about
+ *     chunk_ws_bytes of h, never fewer than the edges of the largest source (a batch holds whole sources).
+ *   nnconv_backward_streamed_chunks: source batches whose h the call with this workspace recomputes (n_apps = 0:
+ *     nnconv_backward_apply_streamed, else nnconv_backward_mlp_streamed with n_apps applications); host only. */
+int nnconv_backward_apply_streamed_sizes(const nnconv_plan_t* plan, const nnconv_weights_t* w, int64_t E_res,
+                                         size_t want_bytes, size_t chunk_ws_bytes, size_t* ws_bytes);
+int nnconv_backward_apply_streamed(const nnconv_plan_t* plan, const nnconv_weights_t* w, const float* edge_attr,
+                                   const void* h_res, int64_t E_res, const float* x, const float* root, int aggr,
+                                   const float* grad_out, float* grad_x, float* grad_W_last, float* grad_b_last,
+                                   float* grad_root, float* grad_bias, void* ws, size_t ws_bytes, void* stream,
+                                   int64_t* launches /*nullable*/);
+int nnconv_backward_mlp_streamed_sizes(const nnconv_plan_t* plan, const nnconv_weights_t* w, int64_t E_res, int n_apps,
+                                       size_t want_bytes, size_t* ws_bytes);
+int nnconv_backward_mlp_streamed(const nnconv_plan_t* plan, const nnconv_weights_t* w, const float* edge_attr,
+                                 const void* h_res, int64_t E_res, int n_apps, const float* const* grad_out,
+                                 const float* const* x, int aggr, float* const* grad_W, float* const* grad_b, void* ws,
+                                 size_t ws_bytes, void* stream, float* grad_edge_attr /* nullable */);
+int nnconv_backward_streamed_chunks(const nnconv_plan_t* plan, const nnconv_weights_t* w, int64_t E_res, int n_apps,
+                                    size_t ws_bytes, int64_t* n_chunks);
+
 /* ---- halo exchange of the node-range (strip) partition by peer stores over NVLink (no NCCL call, no host round
  * trip between applications).  `out` [n_local, channels] is the result of one application on this rank (owned rows
  * [own_lo, own_hi) valid); the call writes relu?(out) of the owned rows into this rank's next-application buffer
