@@ -5,8 +5,9 @@
 // Y[c, (o,k)] = sum_i x[c, i] * W_L[i*out + o, k]  (the last Linear reassociated, nn_conv.py:274-275).
 //
 // Structure: persistent CTAs (grid = #SMs), 12 warps: warps 0..7 = two consumer warpgroups, each owning half of
-// the BLOCK_N columns of the tile (wgmma into registers, then the epilogue: bias/ReLU -> 16-bit -> per-warp
-// swizzled smem piece -> TMA store; direct 32-byte stores for pipelined / small launches), warps 8..11 = the TMA
+// the BLOCK_N columns of the tile (wgmma into registers, then the epilogue: bias/ReLU -> 16-bit on the accumulator
+// fragments -> stmatrix into a per-warp swizzled smem piece -> TMA store; direct 32-byte stores of the staged rows for
+// pipelined / small launches), warps 8..11 = the TMA
 // producer warpgroup (warp 8 loops, one elected lane issues).  The producer gives its registers to the consumers
 // (setmaxnreg), so a [128 x 128] fp32 accumulator per warpgroup and the epilogue fit without spilling.  The SMALL
 // configuration keeps a single producer warp (9 warps) so that two CTAs share an SM.  Operands are K-major
@@ -43,7 +44,7 @@ struct GemmTcArgs {
   // memory (64-byte swizzle) and one lane writes it with TMA (tmC, two [16 x 32] panels): no global stores on the
   // LSU data pipe, no block-level barrier, and the store of piece i drains while piece i+1 is converted.
   int tma_store;
-  int bias_v4;         // bias is 16-byte aligned: float4 loads
+  int bias_v4;         // bias is 16-byte aligned: vector loads
   // PREC_F16X2 (see plan.h): a_split_nk = K/3/64 > 0 -> A holds [hi | lo] (2K/3 columns) and K block kb reads
   // A chunk (kb < nk ? kb : kb - nk), i.e. [hi | hi | lo] against B = [hi | lo | hi]; c_split -> the fp32 result is
   // written as the pair hi = fp16(v) at column c and lo = fp16(v - hi) at column c + N (row-major, ldc = 2N) or at
@@ -54,7 +55,7 @@ struct GemmTcArgs {
   unsigned long long b_policy;   // L2 eviction hint of the B (weight) tiles
   int64_t a_chunk_rows_pad;   // > 0: A is chunk-major [K/64][a_chunk_rows_pad][64] (the edge-feature layout): K block kb of
                               // row r is the box at (0, kb * a_chunk_rows_pad + r) of the [K/64 * rows_pad, 64] view
-  int* overflow;       // counts 32-column pieces holding a value beyond the fp16 range (fp16 outputs only), or nullptr
+  int* overflow;       // counts [32 x 32] warp pieces holding a value beyond the fp16 range (fp16 outputs only), or nullptr
   // backward epilogues: mask != nullptr -> C[r, c] = mask16[r * mask_ld + c] > 0 ? acc : 0 (ReLU derivative taken
   // from the stored 16-bit activation); out_f32 -> C is fp32 [M, ldc], plain stores, no conversion.
   const uint16_t* mask;
@@ -64,10 +65,22 @@ struct GemmTcArgs {
   unsigned int trace_seq;
 };
 
-// SMALL = 1: a 2-stage, BLOCK_N = 128, 288-thread footprint (~101 KB smem) that can share an SM with a
+// EPI selects the epilogue at COMPILE time (runtime flags inside the 32-column inner loop cut it into dozens of
+// tiny basic blocks, and the K = 64 first-layer GEMM is epilogue bound):
+//   EPI_PLAIN bias / ReLU / 16-bit store     EPI_SPLIT the same, written as (hi, lo) fp16 pairs (PREC_F16X2)
+//   EPI_MASK  ReLU-derivative mask from a stored activation (backward)     EPI_F32 fp32 output, plain stores
+//   EPI_NOCHECK = EPI_PLAIN without the fp16 range tracking (bf16 outputs, option overflow_check = 0, test hooks)
+//   EPI_MASK_SPLIT = EPI_MASK with acc_scale, written as (hi, lo) pairs (PREC_F16X2 backward; the mask is the hi half)
+// The forward epilogues (PLAIN, NOCHECK, SPLIT) work on the accumulator fragments and write the 16-bit staging with
+// stmatrix; the backward ones first transpose the fragments through a per-warp fp32 scratch (acc_rows: lane = row),
+// because their mask is read and their fp32 output written a row at a time.
+enum { EPI_PLAIN = 0, EPI_SPLIT = 1, EPI_MASK = 2, EPI_F32 = 3, EPI_NOCHECK = 4, EPI_MASK_SPLIT = 5 };
+constexpr bool epi_uses_rows(int epi) { return epi == EPI_MASK || epi == EPI_MASK_SPLIT || epi == EPI_F32; }
+
+// SMALL = 1: a 2-stage, BLOCK_N = 128, 288-thread footprint (~100 KB smem) that can share an SM with a
 // contraction CTA or a second GEMM CTA -- used for the per-source Y GEMM, which is store bound and runs
 // concurrently with the contraction of the previous batch.
-template <int BLOCK_N, int SMALL = 0>
+template <int BLOCK_N, int SMALL = 0, int EPI = EPI_PLAIN>
 struct GemmCfg {
   static constexpr int kThreads = SMALL ? 288 : 384;
   // setmaxnreg budgets of the 384-thread CTA: (40 + 2 * 232) * 128 = 64512 <= 65536 registers, the launch-time
@@ -79,29 +92,27 @@ struct GemmCfg {
   static constexpr int kABytes = kBlockM * kBlockK * 2;
   static constexpr int kBBytes = BLOCK_N * kBlockK * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr int kStages = SMALL ? 2 : ((155648 / kStageBytes) > 8 ? 8 : (155648 / kStageBytes));
-  // output staging for the TMA-store epilogue: 8 warps x 2 buffers x [32 x 32] 16-bit pieces
-  static constexpr int kStoreBytes = SMALL ? 0 : 8 * 2 * 2048;
-  static constexpr int kScratchBytes = 8 * acc_scratch_bytes<32>();   // per-warp accumulator transposes
-  static constexpr int kSmemBytes =
-      kStages * kStageBytes + kStoreBytes + kScratchBytes + 1024 /*align slack*/ + 256 /*barriers*/;
+  // output staging of the epilogue: 8 warps x 2 buffers x [32 x 32] 16-bit pieces
+  static constexpr int kStoreBytes = 8 * 2 * 2048;
+  static constexpr int kScratchBytes = epi_uses_rows(EPI) ? 8 * acc_scratch_bytes<32>() : 0;   // per-warp transposes
+  static constexpr int kFixedBytes = kStoreBytes + kScratchBytes + 1024 /*align slack*/ + 256 /*barriers*/;
+  // as many stages as the 227 KB an SM gives one CTA hold (less 256 B for the static trace words), at most 8;
+  // 256-column tiles: 4 x 48 KB for the forward epilogues, 3 for the ones with the fp32 scratch
+  static constexpr int kFitStages = (232448 - 256 - kFixedBytes) / kStageBytes;
+  static constexpr int kStages = SMALL ? 2 : (kFitStages > 8 ? 8 : kFitStages);
+  static constexpr int kSmemBytes = kStages * kStageBytes + kFixedBytes;
+  static_assert(SMALL || kStages >= 3, "gemm_tc: ring too shallow");
 };
 
-// EPI selects the epilogue at COMPILE time (runtime flags inside the 32-column inner loop cut it into dozens of
-// tiny basic blocks, and the K = 64 first-layer GEMM is epilogue bound):
-//   EPI_PLAIN bias / ReLU / 16-bit store     EPI_SPLIT the same, written as (hi, lo) fp16 pairs (PREC_F16X2)
-//   EPI_MASK  ReLU-derivative mask from a stored activation (backward)     EPI_F32 fp32 output, plain stores
-//   EPI_NOCHECK = EPI_PLAIN without the fp16 range tracking (bf16 outputs, option overflow_check = 0, test hooks)
-//   EPI_MASK_SPLIT = EPI_MASK with acc_scale, written as (hi, lo) pairs (PREC_F16X2 backward; the mask is the hi half)
-enum { EPI_PLAIN = 0, EPI_SPLIT = 1, EPI_MASK = 2, EPI_F32 = 3, EPI_NOCHECK = 4, EPI_MASK_SPLIT = 5 };
-
 template <int BLOCK_N, int FMT, int SMALL, int EPI>
-__global__ void __launch_bounds__(GemmCfg<BLOCK_N, SMALL>::kThreads, SMALL ? 2 : 1)
+__global__ void __launch_bounds__(GemmCfg<BLOCK_N, SMALL, EPI>::kThreads, SMALL ? 2 : 1)
 k_gemm_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
           const __grid_constant__ CUtensorMap tmC, GemmTcArgs a) {
-  using Cfg = GemmCfg<BLOCK_N, SMALL>;
+  using Cfg = GemmCfg<BLOCK_N, SMALL, EPI>;
   constexpr bool kSplitOut = EPI == EPI_SPLIT || EPI == EPI_MASK_SPLIT;
   constexpr bool kMask = EPI == EPI_MASK || EPI == EPI_MASK_SPLIT;
+  constexpr bool kRows = epi_uses_rows(EPI);
+  constexpr bool kRangeCheck = FMT == 0 && (EPI == EPI_PLAIN || EPI == EPI_SPLIT);
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
   uint8_t* smem = smem_raw + (((raw + 1023u) & ~1023u) - raw);
@@ -174,11 +185,23 @@ k_gemm_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
     const int quarter = warp % 4;
     const int half = warp / 4;
     constexpr int kChunks = BLOCK_N / 64;          // 32-column chunks per half
-    float* wb = scratch + warp * (acc_scratch_bytes<32>() / 4);
+    float* wb = kRows ? scratch + warp * (acc_scratch_bytes<32>() / 4) : nullptr;
     int stage = 0;
     uint32_t phase = 0;
-    uint32_t piece = 0;   // TMA-store pieces issued by this warp (selects the staging buffer)
+    uint32_t piece = 0;   // pieces staged by this warp (selects the staging buffer)
     Acc<BLOCK_N / 2> acc;
+    const bool use_tma = a.tma_store != 0;
+    // this warp's staging: 2 buffers of 32 rows x 64 B, row i = tile row acc_row(quarter, i); 16-byte unit u of row i
+    // sits at (u ^ ((i >> 1) & 3)) (SWIZZLE_64B of tmC) -- conflict-free for the 8-lane phases of whole-row v4 shared
+    // accesses and for the 8 rows of one stmatrix matrix alike
+    const uint32_t stage0 = smem_u32(smem_c) + warp * 4096;
+    const uint32_t sw = static_cast<uint32_t>((lane >> 1) & 3);
+    // stmatrix x4: lane l gives the address of row (l & 7) of matrix l >> 3; matrix m covers staging rows
+    // 8 (m & 1) .. + 7 (of a 16-row half) and the (m >> 1)-th of a pair of 16-byte units
+    const uint32_t sm_row = 8 * ((lane >> 3) & 1) + (lane & 7);
+    const uint32_t sm_sw = (sm_row >> 1) & 3, sm_u = static_cast<uint32_t>(lane >> 4);
+    // accumulator fragment of the lane: rows (lane >> 2) and + 8 of the warp's 16-row runs, columns fc, fc + 1 of every 8
+    const int fr = lane >> 2, fc = 2 * (lane & 3);
     for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
       const int mb = t / n_blocks, nb = t % n_blocks;
       int prev = stage;
@@ -200,30 +223,122 @@ k_gemm_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
       if (lane == 0) mbar_arrive(&empty[prev]);
       const int row = mb * Cfg::kBlockM + acc_row(quarter, lane);
       const bool row_ok = row < a.M;
-      uint16_t* crow = reinterpret_cast<uint16_t*>(a.C) + static_cast<int64_t>(row) * a.ldc;
-      const int64_t grow = a.c_row0 + row;
-      uint32_t v[32];
       const float accs = (kSplitOut && a.acc_scale != nullptr) ? __ldg(a.acc_scale) : 1.f;
-      const bool use_tma = Cfg::kStoreBytes > 0 && a.tma_store != 0;
-      // this warp's staging: 2 buffers of 32 rows x 64 B; 16-byte unit u of row r sits at (u ^ ((r >> 1) & 3))
-      // (SWIZZLE_64B of tmC) -- conflict-free for the 8-lane phases of a v4 shared store
-      const uint32_t stage0 = smem_u32(smem_c) + warp * 4096;
-      const uint32_t sw = static_cast<uint32_t>((lane >> 1) & 3);
+      const bool issuer = elect_one();    // same lane every time: bulk groups are per thread
+      // a piece's staging buffer, once the TMA store issued two pieces ago has finished reading it
+      auto begin_piece = [&]() {
+        const uint32_t buf = stage0 + (piece & 1) * 2048;
+        if (use_tma && issuer) bulk_wait_read1();
+        __syncwarp();
+        return buf;
+      };
+      // the staged [32 rows x 32 cols] piece at column colx of the (possibly doubled) output: two [16 x 32] TMA panels
+      // (staging rows 0..15 and 16..31 are two 16-row runs of the tile), or every lane writes its row directly
+      auto end_piece = [&](uint32_t buf, int colx) {
+        if (use_tma) {
+          fence_proxy_async_smem();
+          __syncwarp();
+          if (issuer) {
+#pragma unroll
+            for (int hh = 0; hh < 2; ++hh) {
+              const int r0 = mb * Cfg::kBlockM + 64 * hh + 16 * quarter;
+              if (a.chunk_rows_pad > 0)
+                tma_store_2d(&tmC, buf + hh * 1024, colx & 63,
+                             static_cast<int>((colx >> 6) * a.chunk_rows_pad + a.c_row0 + r0));
+              else
+                tma_store_2d(&tmC, buf + hh * 1024, colx, r0);
+            }
+            bulk_commit();
+          }
+        } else {
+          __syncwarp();
+          if (row_ok) {
+            uint32_t pk[16];
+#pragma unroll
+            for (int u = 0; u < 4; ++u) ld_shared_v4(buf + lane * 64 + ((static_cast<uint32_t>(u) ^ sw) << 4), pk + 4 * u);
+            uint16_t* dst = a.chunk_rows_pad > 0
+                                ? reinterpret_cast<uint16_t*>(a.C) +
+                                      (static_cast<int64_t>(colx >> 6) * a.chunk_rows_pad + a.c_row0 + row) * 64 + (colx & 63)
+                                : reinterpret_cast<uint16_t*>(a.C) + static_cast<int64_t>(row) * a.ldc + colx;
+            st_global_32b(dst, pk);            // 2 x 32 B: full sectors (16 B stores were half-used
+            st_global_32b(dst + 16, pk + 8);   // sectors)
+          }
+        }
+        ++piece;
+      };
 #pragma unroll
       for (int cc = 0; cc < kChunks; ++cc) {
-        acc_rows<BLOCK_N / 2, 32>(acc, cc * 32, wb, v);
         const int col0 = nb * BLOCK_N + half * (BLOCK_N / 2) + cc * 32;
-        if (col0 < a.N && (row_ok || use_tma)) {
-          const uint32_t* vv = v;
+        if (col0 >= a.N) continue;
+        if constexpr (!kRows) {
+          // ---- forward epilogues, on the fragments: value (h, g, j) of the lane = tile row 64 h + 16 quarter + 8 g + fr,
+          // columns col0 + 8 j + fc and + 1 (accumulator registers 4 (4 cc + j) + 2 g and + 1 of half h)
+          float2 bj[4];
+          if (a.bias) {
+#pragma unroll
+            for (int j = 0; j < 4; ++j)
+              bj[j] = a.bias_v4 ? __ldg(reinterpret_cast<const float2*>(a.bias + col0 + 8 * j + fc))
+                                : make_float2(__ldg(a.bias + col0 + 8 * j + fc), __ldg(a.bias + col0 + 8 * j + fc + 1));
+          }
+          uint32_t hi[2][2][4], lo[2][2][4];
+          float vmax[2] = {0.f, 0.f};   // two independent max chains
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+#pragma unroll
+            for (int g = 0; g < 2; ++g) {
+              const bool ok = mb * Cfg::kBlockM + 64 * h + 16 * quarter + 8 * g + fr < a.M;
+#pragma unroll
+              for (int j = 0; j < 4; ++j) {
+                float f0 = acc.d[h][4 * (4 * cc + j) + 2 * g], f1 = acc.d[h][4 * (4 * cc + j) + 2 * g + 1];
+                if (kSplitOut) { f0 *= accs; f1 *= accs; }
+                if (a.bias) { f0 += bj[j].x; f1 += bj[j].y; }
+                if (a.relu) { f0 = fmaxf(f0, 0.f); f1 = fmaxf(f1, 0.f); }
+                if (kRangeCheck && ok) vmax[j & 1] = fmaxf(vmax[j & 1], fmaxf(fabsf(f0), fabsf(f1)));
+                if (FMT == 0) {
+                  const __half2 hv = __floats2half2_rn(f0, f1);
+                  hi[h][g][j] = *reinterpret_cast<const uint32_t*>(&hv);
+                  if (kSplitOut) {
+                    const float2 hf = __half22float2(hv);
+                    const __half2 lv = __floats2half2_rn(f0 - hf.x, f1 - hf.y);
+                    lo[h][g][j] = *reinterpret_cast<const uint32_t*>(&lv);
+                  }
+                } else {
+                  const __nv_bfloat162 hv = __floats2bfloat162_rn(f0, f1);
+                  hi[h][g][j] = *reinterpret_cast<const uint32_t*>(&hv);
+                }
+              }
+            }
+          }
+          // one count per warp and piece holding a value beyond the fp16 range in a row inside M
+          if (kRangeCheck && a.overflow != nullptr) {
+            const bool bad = __any_sync(0xffffffffu, !(fmaxf(vmax[0], vmax[1]) <= 65504.f));
+            if (bad && issuer) atomicAdd(a.overflow, 1);
+          }
+          auto stage_frags = [&](const uint32_t (&pk)[2][2][4], int colx) {
+            const uint32_t buf = begin_piece();
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+#pragma unroll
+              for (int jp = 0; jp < 2; ++jp)
+                stmatrix_x4(buf + (16 * h + sm_row) * 64 + (((2 * jp + sm_u) ^ sm_sw) << 4), pk[h][0][2 * jp],
+                            pk[h][1][2 * jp], pk[h][0][2 * jp + 1], pk[h][1][2 * jp + 1]);
+            }
+            end_piece(buf, colx);
+          };
+          stage_frags(hi, col0);
+          if (FMT == 0 && kSplitOut) stage_frags(lo, col0 + a.N);
+        } else {
+          // ---- backward epilogues, a row per lane
+          uint32_t v[32];
+          acc_rows<BLOCK_N / 2, 32>(acc, cc * 32, wb, v);
           uint32_t packed[16], packed_lo[kSplitOut ? 16 : 1];
-          float vm[4] = {0.f, 0.f, 0.f, 0.f};       // four independent max chains (one chain of 32 is latency bound)
           // EPI_MASK: the row's 32 stored activations (64 B), one 16-byte load per 8 columns
           const uint4* mp = reinterpret_cast<const uint4*>(a.mask + static_cast<int64_t>(row) * a.mask_ld + col0);
           uint4 mkw = make_uint4(0u, 0u, 0u, 0u);
 #pragma unroll
           for (int j4 = 0; j4 < 8; ++j4) {
-            float f[4] = {__uint_as_float(vv[4 * j4]), __uint_as_float(vv[4 * j4 + 1]),
-                          __uint_as_float(vv[4 * j4 + 2]), __uint_as_float(vv[4 * j4 + 3])};
+            float f[4] = {__uint_as_float(v[4 * j4]), __uint_as_float(v[4 * j4 + 1]),
+                          __uint_as_float(v[4 * j4 + 2]), __uint_as_float(v[4 * j4 + 3])};
             if (kSplitOut) {
 #pragma unroll
               for (int q = 0; q < 4; ++q) f[q] *= accs;
@@ -256,10 +371,6 @@ k_gemm_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
                 *reinterpret_cast<float4*>(reinterpret_cast<float*>(a.C) + static_cast<int64_t>(row) * a.ldc + col0 + 4 * j4) =
                     make_float4(f[0], f[1], f[2], f[3]);
             } else {
-              if (FMT == 0 && (EPI == EPI_PLAIN || EPI == EPI_SPLIT)) {
-#pragma unroll
-                for (int q = 0; q < 4; ++q) vm[q] = fmaxf(vm[q], fabsf(f[q]));
-              }
 #pragma unroll
               for (int q = 0; q < 2; ++q) {
                 if (FMT == 0) {
@@ -277,55 +388,23 @@ k_gemm_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
               }
             }
           }
-          if (FMT == 0 && (EPI == EPI_PLAIN || EPI == EPI_SPLIT)) {
-            const float vmax = fmaxf(fmaxf(vm[0], vm[1]), fmaxf(vm[2], vm[3]));
-            if (a.overflow != nullptr && row_ok && !(vmax <= 65504.f)) atomicAdd(a.overflow, 1);
-          }
-          // one [32 rows x 32 cols] piece at column colx of the (possibly doubled) output
-          auto store_piece = [&](const uint32_t* pk, int colx) {
-            if (use_tma) {
-              const uint32_t buf = stage0 + (piece & 1) * 2048;
-              const bool issuer = elect_one();                  // same lane every time: bulk groups are per thread
-              if (issuer) bulk_wait_read1();                    // the store issued two pieces ago has left this buffer
-              __syncwarp();
+          auto stage_row = [&](const uint32_t* pk, int colx) {
+            const uint32_t buf = begin_piece();
 #pragma unroll
-              for (int u = 0; u < 4; ++u)
-                st_shared_v4(buf + lane * 64 + ((static_cast<uint32_t>(u) ^ sw) << 4), pk[4 * u], pk[4 * u + 1],
-                             pk[4 * u + 2], pk[4 * u + 3]);
-              fence_proxy_async_smem();
-              __syncwarp();
-              if (issuer) {
-                // lanes 0..15 and 16..31 hold two 16-row runs of the tile (acc_row): two [16 x 32] panels
-#pragma unroll
-                for (int hh = 0; hh < 2; ++hh) {
-                  const int r0 = mb * Cfg::kBlockM + 64 * hh + 16 * quarter;
-                  if (a.chunk_rows_pad > 0)
-                    tma_store_2d(&tmC, buf + hh * 1024, colx & 63,
-                                 static_cast<int>((colx >> 6) * a.chunk_rows_pad + a.c_row0 + r0));
-                  else
-                    tma_store_2d(&tmC, buf + hh * 1024, colx, r0);
-                }
-                bulk_commit();
-              }
-              ++piece;
-            } else if (row_ok) {
-              uint16_t* dst = a.chunk_rows_pad > 0
-                                  ? reinterpret_cast<uint16_t*>(a.C) +
-                                        (static_cast<int64_t>(colx >> 6) * a.chunk_rows_pad + grow) * 64 + (colx & 63)
-                                  : crow + colx;
-              st_global_32b(dst, pk);            // 2 x 32 B: full sectors (16 B stores were half-used
-              st_global_32b(dst + 16, pk + 8);   // sectors)
-            }
+            for (int u = 0; u < 4; ++u)
+              st_shared_v4(buf + lane * 64 + ((static_cast<uint32_t>(u) ^ sw) << 4), pk[4 * u], pk[4 * u + 1],
+                           pk[4 * u + 2], pk[4 * u + 3]);
+            end_piece(buf, colx);
           };
           if (EPI != EPI_F32) {
-            store_piece(packed, col0);
-            if (FMT == 0 && kSplitOut) store_piece(packed_lo, col0 + a.N);
+            stage_row(packed, col0);
+            if (FMT == 0 && kSplitOut) stage_row(packed_lo, col0 + a.N);
           }
         }
       }
     }
   }
-  if (Cfg::kStoreBytes > 0 && a.tma_store && warp < 8 && elect_one()) bulk_wait0();
+  if (a.tma_store && warp < 8 && elect_one()) bulk_wait0();
   if (a.done_cnt != nullptr) signal_done(a.done_cnt, a.done_ok);   // includes __syncthreads
   else __syncthreads();
   if (threadIdx.x == 0) trace_write(a.trace, (100u + (a.K > 64 ? 1u : 0u)) | (a.trace_seq << 12), trace_t[0], trace_t[1], a.trace.rec ? gtime() : 0ull);
@@ -336,7 +415,7 @@ int g_num_sms = 0;
 template <int BLOCK_N, int FMT, int SMALL, int EPI = EPI_PLAIN>
 int launch_gemm_cfg(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC, const GemmTcArgs& a,
                     cudaStream_t st, bool pdl) {
-  using Cfg = GemmCfg<BLOCK_N, SMALL>;
+  using Cfg = GemmCfg<BLOCK_N, SMALL, EPI>;
   static bool attr_set = false;
   if (!attr_set) {
     NNC_CHECK_CUDA(cudaFuncSetAttribute(k_gemm_tc<BLOCK_N, FMT, SMALL, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize,

@@ -101,6 +101,18 @@ __device__ __forceinline__ void warpgroup_reg_alloc() {
 __device__ __forceinline__ void st_shared_v4(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
   asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
 }
+__device__ __forceinline__ void ld_shared_v4(uint32_t addr, uint32_t* v) {
+  asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]) : "r"(addr)
+               : "memory");
+}
+// Four 8x8 16-bit matrices from registers in the mma / wgmma accumulator layout (register i of lane l: row l / 4,
+// columns 2 (l % 4), + 1 of matrix i, two 16-bit values) to shared memory; lanes 8i .. 8i + 7 give the addresses of
+// the eight 16-byte rows of matrix i.
+__device__ __forceinline__ void stmatrix_x4(uint32_t addr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r0), "r"(r1),
+               "r"(r2), "r"(r3)
+               : "memory");
+}
 
 // One lane of a CONVERGED warp (elect.sync).  Role loops run on all 32 lanes and only issue through the elected
 // lane: operands computed in converged code are warp-uniform for the compiler (uniform registers), whereas
