@@ -263,14 +263,16 @@ int edge_features_rows(const Plan* P, const Weights* W, const float* edge_attr, 
   }
   if (nl == 1) {   // single Linear: h_last = edge_attr (padded)
     ProfScope ps(PK_LAYER1, st);
-    s = launch_edge_layer1(W->prec, edge_attr, P->perm, e_begin, E, W->dims[0], nullptr, nullptr, W->Kp, 1, h, st, hpad, 0);
+    s = launch_edge_layer1(W->prec, edge_attr, P->perm, e_begin, E, W->dims[0], nullptr, nullptr, W->Kp, 1, h, st, hpad, 0,
+                           overflow);
     if (launches) ++*launches;
     return s;
   }
   const size_t rowb = ef_row_bytes(W);
-  if (rowb == 0) {   // CUDA-core first layer straight into h (fp32 path, 2-layer MLP)
+  if (rowb == 0) {   // CUDA-core first layer straight into h (2-layer MLP: fp32, or k_in > 20 in 16 bits)
     ProfScope ps(PK_LAYER1, st);
-    s = launch_edge_layer1(W->prec, edge_attr, P->perm, e_begin, E, W->dims[0], W->W1, W->b1, W->kp[1], 0, h, st, hpad, 0);
+    s = launch_edge_layer1(W->prec, edge_attr, P->perm, e_begin, E, W->dims[0], W->W1, W->b1, W->kp[1], 0, h, st, hpad, 0,
+                           overflow);
     if (launches) ++*launches;
     return s;
   }
@@ -299,7 +301,7 @@ int edge_features_rows(const Plan* P, const Weights* W, const float* edge_attr, 
         if (launches) ++*launches;
       } else {
         s = launch_edge_layer1(W->prec, edge_attr, P->perm, e_begin + e0, n, W->dims[0], W->W1, W->b1, W->kp[1], 0, dst1,
-                               st, h_pad_l1, e0);
+                               st, h_pad_l1, e0, overflow);
       }
     }
     if (s) return s;
@@ -355,17 +357,25 @@ bool edge_kernels_supported(const Weights* W) {
          W->cout % 2 == 0 && W->n_layers >= 2;
 }
 
-size_t edge_kernels_bytes(const Plan* P, const Weights* W) {
-  return static_cast<size_t>(P->E > 0 ? P->E : 1) * W->cin * W->cout * 2 + 1024;
+// Kmat: the E matrices, then (the last 1024 bytes) the fp16 range counter of nnconv_edge_features_overflow
+static size_t edge_kernels_counter_offset(const Plan* P, const Weights* W) {
+  return static_cast<size_t>(P->E > 0 ? P->E : 1) * W->cin * W->cout * 2;
 }
+
+size_t edge_kernels_bytes(const Plan* P, const Weights* W) { return edge_kernels_counter_offset(P, W) + 1024; }
 
 int edge_kernels(const Plan* P, const Weights* W, const void* h, void* Kmat, cudaStream_t st) {
   NNC_REQUIRE(edge_kernels_supported(W), NNCONV_ERR_UNSUPPORTED, "per-edge kernel matrices: unsupported shape / precision");
+  // K_e = W_L h_e + b_L is rounded to 16 bits with b_L in it (formulation C keeps b_L in fp32): a large last-layer bias
+  // can leave the fp16 range although every h and Y is inside it, so the epilogue counts like the hidden layers'
+  int* overflow = reinterpret_cast<int*>(static_cast<char*>(Kmat) + edge_kernels_counter_offset(P, W));
+  NNC_CHECK_CUDA(cudaMemsetAsync(overflow, 0, sizeof(int), st));
   if (P->E == 0) return NNCONV_OK;
+  if (!options().overflow_check) overflow = nullptr;
   const int64_t hpad = round_up64(P->E, 128);
   const int NK = W->cin * W->cout;
   return launch_gemm_tc(W->prec, h, P->E, 0, static_cast<int>(P->E), W->Kp, W->W3n, NK, W->B3, 0, Kmat, NK, st, nullptr, 0, 0,
-                        0, nullptr, nullptr, 0, 0, hpad);
+                        0, overflow, nullptr, 0, 0, hpad);
 }
 
 int apply_edge(const Plan* P, const Weights* W, const void* Kmat, const float* x, const float* root, const float* bias,

@@ -21,7 +21,7 @@ int launch_transpose_pad(int prec, const float* src, int R, int C, void* dst, in
                          const float* scale = nullptr);
 int launch_edge_layer1(int prec, const float* edge_attr, const int* perm, int64_t e_begin, int64_t e_count, int k_in,
                        const float* W1, const float* b1, int kp1, int identity, void* out, cudaStream_t st,
-                       int64_t chunk_rows_pad = 0, int64_t out_row0 = 0);
+                       int64_t chunk_rows_pad = 0, int64_t out_row0 = 0, int* overflow = nullptr);
 int launch_build_a1(int prec, const float* edge_attr, const int* perm, int64_t e_begin, int64_t e_count, int k_in,
                     void* A1, cudaStream_t st);
 int launch_w1aug(int prec, const float* W1, const float* b1, int k1, int kp1, int k_in, void* dst, cudaStream_t st);

@@ -7,6 +7,8 @@
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
+#include <type_traits>
+
 #include "common.cuh"
 #include "kernels.h"
 
@@ -161,12 +163,16 @@ __global__ void k_transpose_pad_split3(const float* __restrict__ src, int R, int
 
 // First layer: h1[p, j] = relu(b1[j] + sum_c W1[j, c] * edge_attr[perm[p], c]),  j < kp1 (pad rows of W1/b1 are 0)
 // identity (single-Linear MLP): h[p, j] = edge_attr[perm[p], j] (zero padded), no ReLU.
+// overflow (fp16 output, nullable): +1 per block that wrote a value beyond the fp16 range or NaN.  Counted here, at the
+// writer: the next layer's GEMM would turn an inf into NaN, which its ReLU turns into 0 before its own range check.
 constexpr int kL1Edges = 32;
 template <typename T>
 __global__ void __launch_bounds__(256)
 k_edge_layer1(const float* __restrict__ edge_attr, const int* __restrict__ perm, int64_t e_begin, int64_t e_count,
               int k_in, const float* __restrict__ W1, const float* __restrict__ b1, int kp1, int identity,
-              T* __restrict__ out, int64_t chunk_rows_pad, int64_t out_row0) {
+              T* __restrict__ out, int64_t chunk_rows_pad, int64_t out_row0, int* __restrict__ overflow) {
+  constexpr bool kRangeCheck = std::is_same<T, __half>::value;
+  bool bad = false;
   extern __shared__ float sm[];
   float* s_ea = sm;                       // [kL1Edges][k_in]
   int64_t p0 = static_cast<int64_t>(blockIdx.x) * kL1Edges;
@@ -186,7 +192,11 @@ k_edge_layer1(const float* __restrict__ edge_attr, const int* __restrict__ perm,
   };
   for (int j = threadIdx.x; j < kp1; j += blockDim.x) {
     if (identity) {
-      for (int e = 0; e < ne; ++e) out[oidx(e, j)] = cvt<T>(j < k_in ? s_ea[e * k_in + j] : 0.f);
+      for (int e = 0; e < ne; ++e) {
+        const float v = j < k_in ? s_ea[e * k_in + j] : 0.f;
+        if (kRangeCheck) bad |= !(fabsf(v) <= 65504.f);
+        out[oidx(e, j)] = cvt<T>(v);
+      }
       continue;
     }
     float w[16];
@@ -205,8 +215,13 @@ k_edge_layer1(const float* __restrict__ edge_attr, const int* __restrict__ perm,
       } else {
         for (int c = 0; c < k_in; ++c) acc = fmaf(W1[static_cast<int64_t>(j) * k_in + c], s_ea[e * k_in + c], acc);
       }
-      out[oidx(e, j)] = cvt<T>(fmaxf(acc, 0.f));
+      const float v = fmaxf(acc, 0.f);
+      if (kRangeCheck) bad |= !(v <= 65504.f);
+      out[oidx(e, j)] = cvt<T>(v);
     }
+  }
+  if (kRangeCheck && overflow != nullptr) {
+    if (__syncthreads_or(bad) && threadIdx.x == 0) atomicAdd(overflow, 1);
   }
 }
 
@@ -802,19 +817,19 @@ int launch_transpose_pad(int prec, const float* src, int R, int C, void* dst, in
 
 int launch_edge_layer1(int prec, const float* edge_attr, const int* perm, int64_t e_begin, int64_t e_count, int k_in,
                        const float* W1, const float* b1, int kp1, int identity, void* out, cudaStream_t st,
-                       int64_t chunk_rows_pad, int64_t out_row0) {
+                       int64_t chunk_rows_pad, int64_t out_row0, int* overflow) {
   if (e_count <= 0) return NNCONV_OK;
   unsigned g = (unsigned)ceil_div64(e_count, kL1Edges);
   size_t sm = sizeof(float) * kL1Edges * k_in;
   if (prec == PREC_FP32)
     k_edge_layer1<float><<<g, 256, sm, st>>>(edge_attr, perm, e_begin, e_count, k_in, W1, b1, kp1, identity,
-                                             static_cast<float*>(out), chunk_rows_pad, out_row0);
+                                             static_cast<float*>(out), chunk_rows_pad, out_row0, nullptr);
   else if (prec == PREC_F16 || prec == PREC_F16X2)
     k_edge_layer1<__half><<<g, 256, sm, st>>>(edge_attr, perm, e_begin, e_count, k_in, W1, b1, kp1, identity,
-                                              static_cast<__half*>(out), chunk_rows_pad, out_row0);
+                                              static_cast<__half*>(out), chunk_rows_pad, out_row0, overflow);
   else
     k_edge_layer1<__nv_bfloat16><<<g, 256, sm, st>>>(edge_attr, perm, e_begin, e_count, k_in, W1, b1, kp1, identity,
-                                                     static_cast<__nv_bfloat16*>(out), chunk_rows_pad, out_row0);
+                                                     static_cast<__nv_bfloat16*>(out), chunk_rows_pad, out_row0, nullptr);
   NNC_CHECK_LAUNCH();
   return NNCONV_OK;
 }

@@ -588,17 +588,25 @@ class NNConv_old(torch.nn.Module):
         return st
 
     @staticmethod
+    def _overflow_count(prepared, counter, dev):
+        """One host sync: the fp16 range counter at the start of ``counter`` (0 when the check is off, during CUDA-graph
+        capture and for precisions without an fp16 range)."""
+        if not _OVERFLOW_CHECK or prepared.precision not in ('f16', 'fp16', 'f16x2') or \
+                torch.cuda.is_current_stream_capturing():
+            return 0
+        cnt = ctypes.c_int64(0)
+        _lib.check(_lib.lib().nnconv_edge_features_overflow(_ptr(counter), _stream_ptr(dev), ctypes.byref(cnt)))
+        return cnt.value
+
+    @staticmethod
     def _check_overflow(prepared, ws, dev):
         """One host sync: raise when edge-MLP activations written with ``ws`` left the fp16 range."""
-        if _OVERFLOW_CHECK and prepared.precision in ('f16', 'fp16', 'f16x2') and \
-                not torch.cuda.is_current_stream_capturing():
-            cnt = ctypes.c_int64(0)
-            _lib.check(_lib.lib().nnconv_edge_features_overflow(_ptr(ws), _stream_ptr(dev), ctypes.byref(cnt)))
-            if cnt.value:
-                raise FloatingPointError(
-                    'graph_pde_b200.NNConv: %d blocks of edge-MLP activations left the fp16 range (|h| > 65504 or '
-                    "NaN); use precision='bf16' or 'fp32' for this parameter scale (NNCONV_B200_OVERFLOW_CHECK=0 "
-                    'disables this check and its one host sync per edge-feature pass)' % cnt.value)
+        cnt = NNConv_old._overflow_count(prepared, ws, dev)
+        if cnt:
+            raise FloatingPointError(
+                'graph_pde_b200.NNConv: %d blocks of edge-MLP activations left the fp16 range (|h| > 65504 or '
+                "NaN); use precision='bf16' or 'fp32' for this parameter scale (NNCONV_B200_OVERFLOW_CHECK=0 "
+                'disables this check and its one host sync per edge-feature pass)' % cnt)
 
     def kept_acts(self, h):
         for ent in self._h_cache.values():
@@ -654,6 +662,10 @@ class NNConv_old(torch.nn.Module):
         _lib.check(L.nnconv_edge_kernels(plan.handle, prepared.handle, _ptr(h), _ptr(kmat), _stream_ptr(h.device)))
         stats['launches'] += 1
         stats['edge_kernel_passes'] = stats.get('edge_kernel_passes', 0) + 1
+        if self._overflow_count(prepared, kmat[nbytes.value - 1024:], h.device):
+            # K_e left the fp16 range (it holds b_L in 16 bits): formulation C, which keeps b_L in fp32 and whose h and
+            # Y passed their own checks, computes these edges instead
+            kmat = None
         self._k_cache = (h, kmat)
         return kmat
 

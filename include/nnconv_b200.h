@@ -142,7 +142,10 @@ int nnconv_apply_streamed(const nnconv_plan_t* plan, const nnconv_weights_t* w, 
  * MGKN_orthogonal_burgers1d.py has 2-4): K_e = W_L h_e + b_L ([in, out] 16-bit per edge, sorted edge order) is as
  * x-independent as h, so it is built ONCE per (edge_attr, parameters) from the h of nnconv_edge_features
  * (nn_conv.py:274) and every application is nnconv_apply_edge: out[dst] (+)= x_src @ K_e, one bandwidth-bound pass
- * (nn_conv.py:275-282 incl. root / bias / mean).  Same result as nnconv_apply up to 16-bit rounding of K_e. */
+ * (nn_conv.py:275-282 incl. root / bias / mean).  Same result as nnconv_apply up to 16-bit rounding of K_e.
+ * The last 1024 bytes of kmat hold the fp16 range counter of the build (nnconv_edge_features_overflow(kmat + bytes -
+ * 1024, ...)): K_e carries b_L in 16 bits, where nnconv_apply keeps it in fp32, so a last-layer bias beyond the
+ * fp16 range overflows here and not there. */
 int nnconv_edge_kernels_sizes(const nnconv_plan_t* plan, const nnconv_weights_t* w, size_t* bytes);
 int nnconv_edge_kernels(const nnconv_plan_t* plan, const nnconv_weights_t* w, const void* h, void* kmat, void* stream);
 int nnconv_apply_edge(const nnconv_plan_t* plan, const nnconv_weights_t* w, const void* kmat, const float* x,
