@@ -12,4 +12,4 @@ from . import _lib  # noqa: F401
 from .nn_conv import NNConv, NNConv_old, ECConv, stats, clear_caches  # noqa: F401
 
 __version__ = '0.1.0'
-from .capture import GraphedForward  # noqa: F401,E402
+from .capture import GraphedForward, GraphedTrainStep  # noqa: F401,E402

@@ -37,7 +37,7 @@ SYMBOLS = [
     'nnconv_backward_ex', 'nnconv_backward_mlp_ex',
     'nnconv_stream_split', 'nnconv_edge_features_prefix', 'nnconv_apply_streamed',
     'nnconv_backward_apply_streamed_sizes', 'nnconv_backward_apply_streamed', 'nnconv_backward_mlp_streamed_sizes',
-    'nnconv_backward_mlp_streamed', 'nnconv_backward_streamed_chunks',
+    'nnconv_backward_mlp_streamed', 'nnconv_backward_streamed_chunks', 'nnconv_overflow_accumulate',
 ]
 
 
@@ -98,6 +98,7 @@ def lib():
     L.nnconv_set_option.argtypes = [ctypes.c_char_p, c_int]
     L.nnconv_get_option.argtypes = [ctypes.c_char_p, P(c_int)]
     L.nnconv_edge_features_overflow.argtypes = [c_vp, c_vp, P(c_i64)]
+    L.nnconv_overflow_accumulate.argtypes = [c_vp, c_vp, c_vp]
     L.nnconv_debug_occupy.argtypes = [c_int, c_int, ctypes.c_longlong, c_vp]
     L.nnconv_backward_tc_supported.argtypes = [c_vp]
     L.nnconv_backward_apply_sizes.argtypes = [c_vp, c_vp, c_sz, P(c_sz)]

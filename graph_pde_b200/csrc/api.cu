@@ -1049,6 +1049,11 @@ int nnconv_edge_features_overflow(const void* ws, void* stream, int64_t* count) 
   return NNCONV_OK;
 }
 
+int nnconv_overflow_accumulate(const void* counter, int* sticky, void* stream) {
+  NNC_REQUIRE(counter && sticky, NNCONV_ERR_ARG, "null pointer");
+  return launch_overflow_accumulate(static_cast<const int*>(counter), sticky, static_cast<cudaStream_t>(stream));
+}
+
 int nnconv_edge_kernels_sizes(const nnconv_plan_t* plan, const nnconv_weights_t* w, size_t* bytes) {
   NNC_REQUIRE(plan && w && bytes, NNCONV_ERR_ARG, "null pointer");
   NNC_REQUIRE(edge_kernels_supported(&w->w), NNCONV_ERR_UNSUPPORTED, "per-edge kernel matrices: unsupported shape / precision");

@@ -11,6 +11,8 @@ int launch_w3p(int prec, const float* WL, int cin, int cout, int K, int Kp, int 
                const float* scale = nullptr);
 // scale2[0] = power of two s with max|src| * s in [0.5, 1), scale2[1] = 1 / s   (device floats)
 int launch_pow2_scale(const float* src, int64_t n, float* scale2, cudaStream_t st);
+// *sticky += *counter on the device (one thread; no host synchronisation, so it can be captured in a CUDA graph)
+int launch_overflow_accumulate(const int* counter, int* sticky, cudaStream_t st);
 int launch_pad_convert_split3(const float* src, int R, int C, void* dst, int Rp, int Cp, const float* scale, cudaStream_t st);
 // backward images of the last Linear: transposed == 0 -> W3q [Kp*cout, cin_p], 1 -> W3t [cin_p, Kp*cout]
 // (PREC_F16X2: the reduction dimension is tripled, [hi | lo | hi], and the values are multiplied by *scale first)

@@ -113,6 +113,11 @@ __global__ void k_pow2_from_max(float* scale2) {
   scale2[0] = s;
   scale2[1] = 1.f / s;
 }
+// *sticky += *counter: folds one pass's fp16 range counter into a word that outlives the pass's workspace
+__global__ void k_overflow_accumulate(const int* __restrict__ counter, int* __restrict__ sticky) {
+  const int v = *counter;
+  if (v != 0) atomicAdd(sticky, v);
+}
 __global__ void k_w3p_split3(const float* __restrict__ WL, int cin, int cout, int K, int Kp, int cin_p,
                              __half* __restrict__ dst, const float* __restrict__ scale) {
   int64_t idx = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
@@ -760,6 +765,12 @@ int launch_pow2_scale(const float* src, int64_t n, float* scale2, cudaStream_t s
     NNC_CHECK_LAUNCH();
   }
   k_pow2_from_max<<<1, 1, 0, st>>>(scale2);
+  NNC_CHECK_LAUNCH();
+  return NNCONV_OK;
+}
+
+int launch_overflow_accumulate(const int* counter, int* sticky, cudaStream_t st) {
+  k_overflow_accumulate<<<1, 1, 0, st>>>(counter, sticky);
   NNC_CHECK_LAUNCH();
   return NNCONV_OK;
 }

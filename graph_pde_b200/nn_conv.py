@@ -21,6 +21,7 @@ runs ``m_e = h_e . Y_src + c_src`` with the per-source matrix ``Y_src = x_src (x
 ``m_e / deg`` into the target rows.
 """
 import collections
+import contextlib
 import ctypes
 import math
 import os
@@ -70,6 +71,8 @@ _STREAM_TRAIN_MARGIN_BYTES = 4 << 30
 # default of NNConv_old(streamed_training=...): '1' lets training run on streamed edge features (see NNConv_old)
 _STREAMED_TRAINING = os.environ.get('NNCONV_B200_STREAMED_TRAINING', '0') == '1'
 _MLP_GROUP = 6                     # applications per deferred pass through the hidden layers
+# registered by capture.GraphedTrainStep while it captures a training step (see _CaptureSink), else None
+_CAPTURE_SINK = None
 
 
 def default_precision():
@@ -78,6 +81,28 @@ def default_precision():
 
 def clear_caches():
     _PLAN_CACHE.clear()
+
+
+class _CaptureSink(object):
+    """Where a CUDA-graph-captured training step reports fp16 overflow.  A captured pass cannot read its range counter
+    on the host, so while this sink is registered every counter site enqueues nnconv_overflow_accumulate instead: the
+    counter is added into ``words[0]``, and a K_e build's also into ``words[1]`` (the replay reads ``words[0]`` after
+    the step and ``words[1]`` only to word its error).  ``plans`` keeps the plans the captured launches read alive for
+    as long as the graph: an eviction from the plan cache would otherwise free buffers the graph still reads."""
+
+    def __init__(self, device):
+        self.words = torch.zeros(2, dtype=torch.int32, device=device)
+        self.plans = {}
+
+
+@contextlib.contextmanager
+def _capturing_into(sink):
+    global _CAPTURE_SINK
+    _CAPTURE_SINK = sink
+    try:
+        yield sink
+    finally:
+        _CAPTURE_SINK = None
 
 
 def _stream_ptr(device):
@@ -152,6 +177,8 @@ def get_plan(edge_index, n_nodes, flow='source_to_target'):
     plan = _PLAN_CACHE.get(key)
     if plan is not None:
         _PLAN_CACHE.move_to_end(key)
+        if _CAPTURE_SINK is not None:
+            _CAPTURE_SINK.plans[key] = plan
         return plan
     plan = _Plan(edge_index, n_nodes, flow)
     _PLAN_CACHE[key] = plan
@@ -359,6 +386,7 @@ class NNConv_old(torch.nn.Module):
         self._h_cache = collections.OrderedDict()
         self._h_cache_max = 1
         self._k_cache = None
+        self._kmat_overflowed = set()   # plan keys whose K_e build left the fp16 range in an eager pass
         self.reset_parameters()
 
     # -- reference: nn_conv.py:261-265 with torch_geometric.nn.inits.reset / uniform restated ----------
@@ -588,11 +616,20 @@ class NNConv_old(torch.nn.Module):
         return st
 
     @staticmethod
-    def _overflow_count(prepared, counter, dev):
+    def _overflow_count(prepared, counter, dev, edge_kernels=False):
         """One host sync: the fp16 range counter at the start of ``counter`` (0 when the check is off, during CUDA-graph
-        capture and for precisions without an fp16 range)."""
-        if not _OVERFLOW_CHECK or prepared.precision not in ('f16', 'fp16', 'f16x2') or \
-                torch.cuda.is_current_stream_capturing():
+        capture and for precisions without an fp16 range).  While a captured training step registers a _CaptureSink,
+        the counter is added into the sink on the device instead (``edge_kernels``: a K_e build's counter)."""
+        if not _OVERFLOW_CHECK or prepared.precision not in ('f16', 'fp16', 'f16x2'):
+            return 0
+        if torch.cuda.is_current_stream_capturing():
+            sink = _CAPTURE_SINK
+            if sink is not None:
+                L = _lib.lib()
+                for w in ((0, 1) if edge_kernels else (0,)):
+                    _lib.check(L.nnconv_overflow_accumulate(_ptr(counter), ctypes.c_void_p(sink.words[w].data_ptr()),
+                                                            _stream_ptr(dev)))
+                    stats['launches'] += 1
             return 0
         cnt = ctypes.c_int64(0)
         _lib.check(_lib.lib().nnconv_edge_features_overflow(_ptr(counter), _stream_ptr(dev), ctypes.byref(cnt)))
@@ -654,6 +691,8 @@ class NNConv_old(torch.nn.Module):
         hit = getattr(self, '_k_cache', None)
         if hit is not None and hit[0] is h:
             return hit[1]
+        if _CAPTURE_SINK is not None and plan.key in self._kmat_overflowed:
+            return None         # a captured step keeps the choice its eager warm-up made: formulation C
         L = _lib.lib()
         nbytes = ctypes.c_size_t()
         if L.nnconv_edge_kernels_sizes(plan.handle, prepared.handle, ctypes.byref(nbytes)) != _lib.OK:
@@ -662,10 +701,11 @@ class NNConv_old(torch.nn.Module):
         _lib.check(L.nnconv_edge_kernels(plan.handle, prepared.handle, _ptr(h), _ptr(kmat), _stream_ptr(h.device)))
         stats['launches'] += 1
         stats['edge_kernel_passes'] = stats.get('edge_kernel_passes', 0) + 1
-        if self._overflow_count(prepared, kmat[nbytes.value - 1024:], h.device):
+        if self._overflow_count(prepared, kmat[nbytes.value - 1024:], h.device, edge_kernels=True):
             # K_e left the fp16 range (it holds b_L in 16 bits): formulation C, which keeps b_L in fp32 and whose h and
             # Y passed their own checks, computes these edges instead
             kmat = None
+            self._kmat_overflowed.add(plan.key)
         self._k_cache = (h, kmat)
         return kmat
 

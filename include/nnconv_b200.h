@@ -121,6 +121,12 @@ int nnconv_edge_features_keep(const nnconv_plan_t* plan, const nnconv_weights_t*
  * Copies one int to the host and synchronises `stream`.  A non-zero count means h holds inf: use bf16 / fp32. */
 int nnconv_edge_features_overflow(const void* ws, void* stream, int64_t* count);
 
+/* The same counter without a host read: enqueues on `stream` one kernel that adds the int at `counter` (the first
+ * word of an edge-feature or nnconv_apply_streamed workspace, or the last 1024 bytes of kmat, as for
+ * nnconv_edge_features_overflow) into the device int `sticky`.  No host synchronisation: a CUDA graph can capture it,
+ * and the caller reads `sticky` once after any number of passes. */
+int nnconv_overflow_accumulate(const void* counter, int* sticky, void* stream);
+
 /* ---- partially resident edge features, for graphs whose h does not fit the device (16-bit precisions):
  * the h of the sorted edges [0, E_res) is cached as above, and every application recomputes the h of [E_res, E)
  * chunk by chunk (same bits as the cached pass) and contracts each chunk right after computing it.
