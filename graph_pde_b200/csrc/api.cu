@@ -394,7 +394,7 @@ int apply_edge(const Plan* P, const Weights* W, const void* Kmat, const float* x
 struct ApplyLayout {
   size_t off_Xc, off_cvec, off_xs, off_flags, off_Y, fixed_bytes, per_node;
 };
-constexpr int kMaxPipeBatches = 1 << 14;   // flags: cntY, cntC, okY, okC per batch
+constexpr int kMaxPipeBatches = 1 << 14;   // flags: cntY, cntC, okY, okC, cntU per batch
 
 static ApplyLayout layout_apply(const Plan* P, const Weights* W) {
   Carver c(nullptr, ~size_t(0));
@@ -460,167 +460,6 @@ static bool fused_geometry(const Weights* W, int64_t n_src, int64_t nodes_cap, i
   *ring_out = ring;
   *nb_out = nb;
   return ring >= 2;
-}
-
-int apply(const Plan* P, const Weights* W, const void* h, const float* x, const float* root, const float* bias,
-          int aggr_mean, float* out, void* ws, size_t ws_bytes, cudaStream_t st, int64_t* launches, unsigned node_flags) {
-  int s;
-  NNC_REQUIRE(!(node_flags & NNCONV_APPLY_RESIDUAL) || W->cin == W->cout, NNCONV_ERR_ARG,
-              "NNCONV_APPLY_RESIDUAL needs in_channels == out_channels");
-  if (P->E == 0 || P->n_src == 0) {
-    ProfScope ps(PK_NODE_PREP, st);
-    s = launch_out_init(x, root, bias, P->N, W->cin, W->cout, out, st, node_flags);
-    if (s == NNCONV_OK && launches) ++*launches;
-    return s;
-  }
-  const bool tc = tc_shapes_supported(W);
-  NNC_REQUIRE(tc || W->prec == PREC_FP32, NNCONV_ERR_UNSUPPORTED,
-              "shape not supported by the tensor-core path (out=%d, K=%d); use precision fp32", W->cout, W->K);
-  ApplyLayout L = layout_apply(P, W);
-  NNC_REQUIRE(ws != nullptr && ws_bytes >= L.fixed_bytes + L.per_node, NNCONV_ERR_WORKSPACE,
-              "apply: workspace too small (need >= %zu bytes)", L.fixed_bytes + L.per_node);
-  char* base = static_cast<char*>(ws);
-  void* Xc = base + L.off_Xc;
-  float* cvec = reinterpret_cast<float*>(base + L.off_cvec);
-  float* xs = reinterpret_cast<float*>(base + L.off_xs);
-  void* Y = base + L.off_Y;
-  int64_t nodes_cap = static_cast<int64_t>((ws_bytes - L.fixed_bytes) / L.per_node);
-  const Options& opt = options();
-  // fused persistent kernel (below): its batch geometry is needed here because the node-prep launch also clears its flags
-  int ring = 0;
-  int64_t nb = 0;
-  const bool fused = fused_geometry(W, P->n_src, nodes_cap, &ring, &nb) && ceil_div64(P->n_src, nb) <= kMaxPipeBatches;
-  int* flags = reinterpret_cast<int*>(base + L.off_flags);
-  if (fused) {
-    ProfScope ps(PK_NODE_PREP, st);
-    s = launch_node_prep(W->prec, x, root, bias, P->N, out, P->src_nodes, P->n_src, W->cin, W->cin_p, W->cout, W->B3, Xc,
-                         cvec, xs, flags, kMaxPipeBatches, static_cast<int>(ceil_div64(P->n_src, nb)), st, node_flags);
-    if (s) return s;
-    if (launches) ++*launches;
-  } else {
-    {
-      ProfScope ps(PK_NODE_PREP, st);
-      s = launch_out_init(x, root, bias, P->N, W->cin, W->cout, out, st, node_flags);
-    }
-    if (s) return s;
-    {
-      ProfScope ps(PK_NODE_PREP, st);
-      s = launch_src_prep(W->prec, x, P->src_nodes, P->n_src, W->cin, W->cin_p, W->cout, W->B3, Xc, cvec, xs, st, node_flags);
-    }
-    if (s) return s;
-    if (launches) *launches += 2;
-  }
-  // tile_ptr lives on the device; tile ranges per batch come from the host mirror kept in the plan handle
-  const int* h_tile_ptr = P->h_tile_ptr;
-  const int NY = W->cout * W->Kp;
-
-  if (W->prec == PREC_FP32) {   // CUDA-core path: plain stream order, one Y buffer
-    int64_t nb_max = nodes_cap > P->n_src ? P->n_src : nodes_cap;
-    for (int64_t c0 = 0; c0 < P->n_src; c0 += nb_max) {
-      const int nb = static_cast<int>((P->n_src - c0) < nb_max ? (P->n_src - c0) : nb_max);
-      const int tb = h_tile_ptr[c0], te = h_tile_ptr[c0 + nb];
-      {
-        ProfScope ps(PK_Y_GEMM, st);
-        s = launch_sgemm_store(reinterpret_cast<const float*>(Xc) + c0 * W->cin_p, W->cin_p,
-                               reinterpret_cast<const float*>(W->W3p), W->cin_p, static_cast<float*>(Y), NY, nb, NY,
-                               W->cin_p, nullptr, st);
-      }
-      if (s) return s;
-      {
-        ProfScope ps(PK_CONV, st);
-        s = launch_sgemm_scatter(P, static_cast<const float*>(h), W->Kp, static_cast<const float*>(Y), W->cout, tb,
-                                 te, static_cast<int>(c0), cvec, aggr_mean, out, st);
-      }
-      if (s) return s;
-      if (launches) *launches += 2;
-    }
-    return NNCONV_OK;
-  }
-
-  // Tensor-core path, default: ONE persistent kernel per application (apply_tc.cu) in which every CTA runs
-  // the Y GEMM pipeline and the contraction pipeline concurrently over a ring of L2-resident Y batches.
-  if (fused) {
-    {
-      ProfScope ps(PK_APPLY_FUSED, st);
-      s = launch_apply_tc(W->prec, P, W, h, Xc, Y, static_cast<int>(nb), ring, cvec, xs, aggr_mean, out, flags,
-                          kMaxPipeBatches, st);
-    }
-    if (s == NNCONV_OK) {
-      if (launches) ++*launches;
-      return NNCONV_OK;
-    }
-    // the driver cannot co-schedule one CTA per SM (MPS / green-context partition): per-batch kernels below
-    if (s != kApplyCannotCoSchedule) return s;
-  }
-  NNC_REQUIRE(!W->split, NNCONV_ERR_UNSUPPORTED,
-              "precision f16x2 runs in the fused persistent kernel only (shape or workspace not supported)");
-
-  // Fallback (NNCONV_NO_FUSE=1 or shapes the fused kernel does not cover): one Y GEMM + one contraction
-  // kernel per batch of sources.  Batches of sources sized so that the Y buffers stay L2 resident; kernel order
-  //   Y(0), Y(1), C(0), Y(2), C(1), ..., C(B-1)            (three Y buffers, b mod 3)
-  // launched with programmatic stream serialization, so CTAs of the next kernel start on SMs as CTAs of
-  // the running kernel retire; the true dependencies  C(b) <- Y(b)  and  Y(b) <- C(b-3) (buffer reuse)
-  // are completion flags in global memory.  Profiling mode (events between kernels) falls back to plain
-  // stream order so that per-kernel times are meaningful.
-  const bool no_pipe_env = opt.no_pipe != 0;   // measurement / debugging knob
-  const bool pipe = !prof_enabled() && !no_pipe_env && nodes_cap >= 3;
-  int64_t nb_max = pipe ? nodes_cap / 3 : nodes_cap;
-  if (nb_max > P->n_src) nb_max = P->n_src;
-  int64_t n_batches = ceil_div64(P->n_src, nb_max);
-  if (n_batches > kMaxPipeBatches) {   // keep the flag table bounded: grow batches past the L2 target
-    NNC_REQUIRE(false, NNCONV_ERR_WORKSPACE, "apply: workspace too small for %lld source batches", (long long)n_batches);
-  }
-  int* cntY = flags;
-  int* cntC = flags + kMaxPipeBatches;
-  int* okY = flags + 2 * kMaxPipeBatches;
-  int* okC = flags + 3 * kMaxPipeBatches;
-  if (pipe) NNC_CHECK_CUDA(cudaMemsetAsync(flags, 0, sizeof(int) * 4 * kMaxPipeBatches, st));
-  // three Y buffers: Y(b+2) is launched right after C(b) and reuses the buffer C(b-1) read, which has
-  // retired by then -- with two buffers Y(b+2) would have to wait for the kernel it directly follows
-  char* Ybuf[3] = {static_cast<char*>(Y), static_cast<char*>(Y) + (pipe ? nb_max * L.per_node : 0),
-                   static_cast<char*>(Y) + (pipe ? 2 * nb_max * L.per_node : 0)};
-
-  auto launch_y = [&](int64_t b) -> int {
-    const int64_t c0 = b * nb_max;
-    const int nb = static_cast<int>((P->n_src - c0) < nb_max ? (P->n_src - c0) : nb_max);
-    PipeFlags pf{};
-    pf.pdl = pipe && b > 0;
-    pf.small_footprint = true;
-    pf.wait_ok = (pipe && b >= 3) ? okC + (b - 3) : nullptr;
-    pf.done_cnt = pipe ? cntY + b : nullptr;
-    pf.done_ok = pipe ? okY + b : nullptr;
-    ProfScope ps(PK_Y_GEMM, st);
-    return launch_gemm_tc(W->prec, Xc, P->n_src, c0, nb, W->cin_p, W->W3p, NY, nullptr, 0, Ybuf[b % 3], NY, st, &pf);
-  };
-  auto launch_c = [&](int64_t b) -> int {
-    const int64_t c0 = b * nb_max;
-    const int nb = static_cast<int>((P->n_src - c0) < nb_max ? (P->n_src - c0) : nb_max);
-    const int tb = h_tile_ptr[c0], te = h_tile_ptr[c0 + nb];
-    PipeFlags pf{};
-    pf.pdl = pipe;
-    pf.wait_ok = pipe ? okY + b : nullptr;
-    pf.done_cnt = pipe ? cntC + b : nullptr;
-    pf.done_ok = pipe ? okC + b : nullptr;
-    if (pipe && b == n_batches - 1) {   // last kernel of the chain: join every earlier conv kernel
-      pf.join_ok = okC;
-      pf.join_n = static_cast<int>(n_batches - 1);
-    }
-    ProfScope ps(PK_CONV, st);
-    return launch_conv_tc(W->prec, P, h, W->Kp, Ybuf[b % 3], nb, W->cout, tb, te, static_cast<int>(c0), cvec, xs,
-                          aggr_mean, out, st, pipe ? &pf : nullptr);
-  };
-  s = launch_y(0);
-  if (s) return s;
-  for (int64_t b = 0; b < n_batches; ++b) {
-    if (b + 1 < n_batches) {
-      s = launch_y(b + 1);
-      if (s) return s;
-    }
-    s = launch_c(b);
-    if (s) return s;
-  }
-  if (launches) *launches += 2 * n_batches;
-  return NNCONV_OK;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -725,57 +564,274 @@ int stream_split(const Plan* P, const Weights* W, size_t resident_bytes, size_t 
   return NNCONV_OK;
 }
 
-// contraction of one unit range: the persistent kernel (flags at batch offset *boff), else per-batch kernels in
-// plain stream order
-static int contract_range(const Plan* P, const Weights* W, const UnitRange& R, int64_t e_hi, const void* h, bool fused, int ring,
-                          int64_t nb, int64_t nodes_cap, void* Xc, void* Y, const float* cvec, const float* xs,
-                          int aggr_mean, float* out, int* flags, int* boff, cudaStream_t st, int64_t* launches) {
-  if (fused) {
+// ------------------------------------------------------------------------------------------------
+// the application driver: every forward application of formulation C.  The cached h holds the sorted edges
+// [0, E_res) (a whole h: E_res = E); the h of the other edges is recomputed chunk by chunk into a chunk region and
+// contracted right after.  An application is a list of ranges -- [0, E_res), then chunks of at most `rows` edges that
+// end at unit boundaries -- and each range is one contraction: a persistent launch or one chain of per-batch kernels.
+// ------------------------------------------------------------------------------------------------
+
+// the application workspace (ApplyLayout)
+struct ApplyWs {
+  void* Xc;
+  float* cvec;
+  float* xs;
+  int* flags;          // cntY, cntC, okY, okC, cntU: kMaxPipeBatches each
+  void* Y;             // nodes_cap source matrices of per_node bytes
+  size_t per_node;
+  int64_t nodes_cap;
+};
+
+// the streamed edges [E_res, E): recomputed from edge_attr, `rows` at a time, into h (edge_features_rows scratch: ef)
+struct ChunkWs {
+  const float* edge_attr;
+  void* h;
+  void* ef;
+  size_t ef_bytes;
+  int64_t rows;
+  int* overflow;       // nullable
+};
+
+// how the ranges are contracted: the persistent kernel (ring slots of nb sources), else per-batch kernels of nb sources,
+// PDL-pipelined (pipe) or in plain stream order
+struct Schedule {
+  bool fused, pipe;
+  int ring;
+  int64_t nb;
+};
+
+// end of the range that starts at e
+static int64_t range_end(const Plan* P, int64_t e, int64_t E_res, int64_t rows) {
+  return e < E_res ? E_res : unit_floor(P, e + rows);
+}
+
+// flag batches of the ranges from the one that starts at e_from on, nb sources per batch
+static int64_t range_batches(const Plan* P, int64_t e_from, int64_t E_res, int64_t rows, int64_t nb) {
+  int64_t n = 0;
+  for (int64_t e = e_from; e < P->E;) {
+    const int64_t e2 = range_end(P, e, E_res, rows);
+    const UnitRange r = edge_range(P, e, e2);
+    n += ceil_div64(r.c_end - r.c_begin, nb);
+    e = e2;
+  }
+  return n;
+}
+
+// Contraction of the unit range R (sorted edges [R.e_base, e_hi), h holding exactly those rows), flag batches at
+// `flags`.  Fused: ONE persistent kernel (apply_tc.cu) in which every CTA runs the Y GEMM pipeline and the contraction
+// pipeline concurrently over a ring of L2-resident Y batches.  Otherwise one Y GEMM + one contraction kernel per batch
+// of the range's sources, batches sized so that the Y buffers stay L2 resident; kernel order
+//   Y(0), Y(1), C(0), Y(2), C(1), ..., C(B-1)            (three Y buffers, b mod 3)
+// launched with programmatic stream serialization, so CTAs of the next kernel start on SMs as CTAs of the running
+// kernel retire; the true dependencies  C(b) <- Y(b)  and  Y(b) <- C(b-3) (buffer reuse)  are completion flags in
+// global memory.  Without pipe the same kernels run in plain stream order with one Y buffer.
+static int contract_range(const Plan* P, const Weights* W, const UnitRange& R, int64_t e_hi, const void* h,
+                          const Schedule& S, const ApplyWs& A, int* flags, int aggr_mean, float* out, cudaStream_t st,
+                          int64_t* launches) {
+  if (S.fused) {
     int s;
     {
       ProfScope ps(PK_APPLY_FUSED, st);
-      s = launch_apply_tc(W->prec, P, W, h, Xc, Y, static_cast<int>(nb), ring, cvec, xs, aggr_mean, out, flags + *boff,
-                          kMaxPipeBatches, st, &R);
+      s = launch_apply_tc(W->prec, P, W, h, A.Xc, A.Y, static_cast<int>(S.nb), S.ring, A.cvec, A.xs, aggr_mean, out, flags,
+                          kMaxPipeBatches, st, R);
     }
-    *boff += static_cast<int>(ceil_div64(R.c_end - R.c_begin, nb));
-    if (s == NNCONV_OK) {
-      if (launches) ++*launches;
-      return NNCONV_OK;
-    }
-    if (s != kApplyCannotCoSchedule) return s;
+    if (s == NNCONV_OK && launches) ++*launches;
+    return s;
   }
-  NNC_REQUIRE(!W->split, NNCONV_ERR_UNSUPPORTED,
-              "precision f16x2 runs in the fused persistent kernel only (shape or workspace not supported)");
   const int NY = W->cout * W->Kp;
+  const int64_t n_batches = ceil_div64(R.c_end - R.c_begin, S.nb);
   const int t_lo = tile_at(P, R.e_base), t_hi = tile_at(P, e_hi);
-  for (int64_t c0 = R.c_begin; c0 < R.c_end; c0 += nodes_cap) {
-    const int nbat = static_cast<int>((R.c_end - c0) < nodes_cap ? (R.c_end - c0) : nodes_cap);
-    const int tb = P->h_tile_ptr[c0] > t_lo ? P->h_tile_ptr[c0] : t_lo;
-    const int te = P->h_tile_ptr[c0 + nbat] < t_hi ? P->h_tile_ptr[c0 + nbat] : t_hi;
+  int* cntY = flags;
+  int* cntC = flags + kMaxPipeBatches;
+  int* okY = flags + 2 * kMaxPipeBatches;
+  int* okC = flags + 3 * kMaxPipeBatches;
+  // three Y buffers: Y(b+2) is launched right after C(b) and reuses the buffer C(b-1) read, which has
+  // retired by then -- with two buffers Y(b+2) would have to wait for the kernel it directly follows
+  char* Ybuf[3] = {static_cast<char*>(A.Y), static_cast<char*>(A.Y) + (S.pipe ? S.nb * A.per_node : 0),
+                   static_cast<char*>(A.Y) + (S.pipe ? 2 * S.nb * A.per_node : 0)};
+  auto batch_size = [&](int64_t c0) { return static_cast<int>((R.c_end - c0) < S.nb ? (R.c_end - c0) : S.nb); };
+
+  auto launch_y = [&](int64_t b) -> int {
+    const int64_t c0 = R.c_begin + b * S.nb;
     PipeFlags pf{};
+    pf.pdl = S.pipe && b > 0;
     pf.small_footprint = true;
+    pf.wait_ok = (S.pipe && b >= 3) ? okC + (b - 3) : nullptr;
+    pf.done_cnt = S.pipe ? cntY + b : nullptr;
+    pf.done_ok = S.pipe ? okY + b : nullptr;
+    ProfScope ps(PK_Y_GEMM, st);
+    return launch_gemm_tc(W->prec, A.Xc, P->n_src, c0, batch_size(c0), W->cin_p, W->W3p, NY, nullptr, 0, Ybuf[b % 3], NY,
+                          st, &pf);
+  };
+  auto launch_c = [&](int64_t b) -> int {
+    const int64_t c0 = R.c_begin + b * S.nb;
+    const int nb = batch_size(c0);
+    const int tb = P->h_tile_ptr[c0] > t_lo ? P->h_tile_ptr[c0] : t_lo;
+    const int te = P->h_tile_ptr[c0 + nb] < t_hi ? P->h_tile_ptr[c0 + nb] : t_hi;
+    PipeFlags pf{};
+    pf.pdl = S.pipe;
+    pf.wait_ok = S.pipe ? okY + b : nullptr;
+    pf.done_cnt = S.pipe ? cntC + b : nullptr;
+    pf.done_ok = S.pipe ? okC + b : nullptr;
+    if (S.pipe && b == n_batches - 1) {   // last kernel of the chain: join every earlier conv kernel
+      pf.join_ok = okC;
+      pf.join_n = static_cast<int>(n_batches - 1);
+    }
+    ProfScope ps(PK_CONV, st);
+    return launch_conv_tc(W->prec, P, h, W->Kp, Ybuf[b % 3], nb, W->cout, tb, te, static_cast<int>(c0), A.cvec, A.xs,
+                          aggr_mean, out, st, S.pipe ? &pf : nullptr, R.e_base, R.h_rows);
+  };
+  int s = launch_y(0);
+  if (s) return s;
+  for (int64_t b = 0; b < n_batches; ++b) {
+    if (b + 1 < n_batches) {
+      s = launch_y(b + 1);
+      if (s) return s;
+    }
+    s = launch_c(b);
+    if (s) return s;
+  }
+  if (launches) *launches += 2 * n_batches;
+  return NNCONV_OK;
+}
+
+// precision fp32 (CUDA cores, whole h only): per batch of sources a Y GEMM and a contraction in plain stream order,
+// one Y buffer
+static int apply_fp32(const Plan* P, const Weights* W, const float* h, const float* x, const float* root,
+                      const float* bias, int aggr_mean, float* out, const ApplyWs& A, cudaStream_t st, int64_t* launches,
+                      unsigned node_flags) {
+  int s;
+  {
+    ProfScope ps(PK_NODE_PREP, st);
+    s = launch_out_init(x, root, bias, P->N, W->cin, W->cout, out, st, node_flags);
+  }
+  if (s) return s;
+  {
+    ProfScope ps(PK_NODE_PREP, st);
+    s = launch_src_prep(W->prec, x, P->src_nodes, P->n_src, W->cin, W->cin_p, W->cout, W->B3, A.Xc, A.cvec, A.xs, st,
+                        node_flags);
+  }
+  if (s) return s;
+  if (launches) *launches += 2;
+  const int NY = W->cout * W->Kp;
+  const int64_t nb_max = A.nodes_cap > P->n_src ? P->n_src : A.nodes_cap;
+  for (int64_t c0 = 0; c0 < P->n_src; c0 += nb_max) {
+    const int nb = static_cast<int>((P->n_src - c0) < nb_max ? (P->n_src - c0) : nb_max);
+    const int tb = P->h_tile_ptr[c0], te = P->h_tile_ptr[c0 + nb];
     {
       ProfScope ps(PK_Y_GEMM, st);
-      int s = launch_gemm_tc(W->prec, Xc, P->n_src, c0, nbat, W->cin_p, W->W3p, NY, nullptr, 0, Y, NY, st, &pf);
-      if (s) return s;
+      s = launch_sgemm_store(reinterpret_cast<const float*>(A.Xc) + c0 * W->cin_p, W->cin_p,
+                             reinterpret_cast<const float*>(W->W3p), W->cin_p, static_cast<float*>(A.Y), NY, nb, NY,
+                             W->cin_p, nullptr, st);
     }
+    if (s) return s;
     {
       ProfScope ps(PK_CONV, st);
-      int s = launch_conv_tc(W->prec, P, h, W->Kp, Y, nbat, W->cout, tb, te, static_cast<int>(c0), cvec, xs, aggr_mean,
-                             out, st, nullptr, R.e_base, R.h_rows);
-      if (s) return s;
+      s = launch_sgemm_scatter(P, h, W->Kp, static_cast<const float*>(A.Y), W->cout, tb, te, static_cast<int>(c0), A.cvec,
+                               aggr_mean, out, st);
     }
+    if (s) return s;
     if (launches) *launches += 2;
   }
   return NNCONV_OK;
 }
 
-int apply_streamed(const Plan* P, const Weights* W, const float* edge_attr, const void* h_res, int64_t E_res,
-                   const float* x, const float* root, const float* bias, int aggr_mean, float* out, void* ws,
-                   size_t ws_bytes, cudaStream_t st, int64_t* launches, unsigned node_flags) {
+// ws / ws_bytes: the application workspace; C: the chunk region, nullptr when E_res = E
+static int apply_ranges(const Plan* P, const Weights* W, const void* h_res, int64_t E_res, const ChunkWs* C,
+                        const float* x, const float* root, const float* bias, int aggr_mean, float* out, void* ws,
+                        size_t ws_bytes, cudaStream_t st, int64_t* launches, unsigned node_flags) {
   int s;
   NNC_REQUIRE(!(node_flags & NNCONV_APPLY_RESIDUAL) || W->cin == W->cout, NNCONV_ERR_ARG,
               "NNCONV_APPLY_RESIDUAL needs in_channels == out_channels");
+  if (P->E == 0 || P->n_src == 0) {
+    ProfScope ps(PK_NODE_PREP, st);
+    s = launch_out_init(x, root, bias, P->N, W->cin, W->cout, out, st, node_flags);
+    if (s == NNCONV_OK && launches) ++*launches;
+    return s;
+  }
+  NNC_REQUIRE(tc_shapes_supported(W) || W->prec == PREC_FP32, NNCONV_ERR_UNSUPPORTED,
+              "shape not supported by the tensor-core path (out=%d, K=%d); use precision fp32", W->cout, W->K);
+  const ApplyLayout L = layout_apply(P, W);
+  NNC_REQUIRE(ws != nullptr && ws_bytes >= L.fixed_bytes + L.per_node, NNCONV_ERR_WORKSPACE,
+              "apply: workspace too small (need >= %zu bytes)", L.fixed_bytes + L.per_node);
+  char* base = static_cast<char*>(ws);
+  const ApplyWs A{base + L.off_Xc, reinterpret_cast<float*>(base + L.off_cvec), reinterpret_cast<float*>(base + L.off_xs),
+                  reinterpret_cast<int*>(base + L.off_flags), base + L.off_Y, L.per_node,
+                  static_cast<int64_t>((ws_bytes - L.fixed_bytes) / L.per_node)};
+  if (W->prec == PREC_FP32)
+    return apply_fp32(P, W, static_cast<const float*>(h_res), x, root, bias, aggr_mean, out, A, st, launches, node_flags);
+
+  // the schedule, decided once: the persistent kernel when it has a geometry for this Y region and the flag batches of
+  // all ranges fit the table (every persistent launch has its own slice), else the per-batch chain
+  const int64_t rows = C ? C->rows : 0;
+  Schedule S{};
+  int64_t n_flag = 0;   // flag batches of the ranges still to run
+  auto use_chain = [&](int64_t e_from) -> int {
+    NNC_REQUIRE(!W->split, NNCONV_ERR_UNSUPPORTED,
+                "precision f16x2 runs in the fused persistent kernel only (shape or workspace not supported)");
+    S = Schedule{};
+    // profiling (events between kernels) runs in plain stream order so that per-kernel times are meaningful
+    S.pipe = !prof_enabled() && options().no_pipe == 0 && A.nodes_cap >= 3;
+    S.nb = S.pipe ? A.nodes_cap / 3 : A.nodes_cap;
+    if (S.nb > P->n_src) S.nb = P->n_src;
+    n_flag = range_batches(P, e_from, E_res, rows, S.nb);
+    NNC_REQUIRE(n_flag <= kMaxPipeBatches || C != nullptr, NNCONV_ERR_WORKSPACE,
+                "apply: workspace too small for %lld source batches", (long long)n_flag);
+    NNC_REQUIRE(n_flag <= kMaxPipeBatches, NNCONV_ERR_WORKSPACE,
+                "apply_streamed: %lld source batches over all chunks exceed %d: use larger chunks", (long long)n_flag,
+                kMaxPipeBatches);
+    return NNCONV_OK;
+  };
+  S.fused = fused_geometry(W, P->n_src, A.nodes_cap, &S.ring, &S.nb);
+  if (S.fused) n_flag = range_batches(P, 0, E_res, rows, S.nb);
+  if (!S.fused || n_flag > kMaxPipeBatches) {
+    s = use_chain(0);
+    if (s) return s;
+  }
+  // ONE launch initialises `out`, prepares the source rows and clears the flag batches [0, n_flag) of all ranges.
+  // Invariant: no launch of an application reads a flag slot that was not cleared in that application.
+  {
+    ProfScope ps(PK_NODE_PREP, st);
+    s = launch_node_prep(W->prec, x, root, bias, P->N, out, P->src_nodes, P->n_src, W->cin, W->cin_p, W->cout, W->B3, A.Xc,
+                         A.cvec, A.xs, A.flags, kMaxPipeBatches, static_cast<int>(n_flag), st, node_flags);
+  }
+  if (s) return s;
+  if (launches) ++*launches;
+  int64_t boff = 0;   // first flag batch of the next range
+  for (int64_t e = 0; e < P->E;) {
+    const int64_t e2 = range_end(P, e, E_res, rows);
+    const void* h = h_res;
+    if (e >= E_res) {
+      s = edge_features_rows(P, W, C->edge_attr, e, e2 - e, C->h, C->ef, C->ef_bytes, C->overflow, st, launches, nullptr);
+      if (s) return s;
+      h = C->h;
+    }
+    const UnitRange R = edge_range(P, e, e2);
+    s = contract_range(P, W, R, e2, h, S, A, A.flags + boff, aggr_mean, out, st, launches);
+    if (s == kApplyCannotCoSchedule) {
+      // the driver cannot co-schedule one CTA per SM (MPS / green-context partition): the chain runs this range and the
+      // rest, its flags numbered from 0 again over slots that the persistent launches before it have used
+      s = use_chain(e);
+      if (s) return s;
+      if (S.pipe) NNC_CHECK_CUDA(cudaMemsetAsync(A.flags, 0, sizeof(int) * 4 * kMaxPipeBatches, st));
+      boff = 0;
+      s = contract_range(P, W, R, e2, h, S, A, A.flags, aggr_mean, out, st, launches);
+    }
+    if (s) return s;
+    boff += ceil_div64(R.c_end - R.c_begin, S.nb);
+    e = e2;
+  }
+  return NNCONV_OK;
+}
+
+int apply(const Plan* P, const Weights* W, const void* h, const float* x, const float* root, const float* bias,
+          int aggr_mean, float* out, void* ws, size_t ws_bytes, cudaStream_t st, int64_t* launches, unsigned node_flags) {
+  return apply_ranges(P, W, h, P->E, nullptr, x, root, bias, aggr_mean, out, ws, ws_bytes, st, launches, node_flags);
+}
+
+int apply_streamed(const Plan* P, const Weights* W, const float* edge_attr, const void* h_res, int64_t E_res,
+                   const float* x, const float* root, const float* bias, int aggr_mean, float* out, void* ws,
+                   size_t ws_bytes, cudaStream_t st, int64_t* launches, unsigned node_flags) {
   NNC_REQUIRE(W->prec == PREC_F16 || W->prec == PREC_BF16 || W->prec == PREC_F16X2, NNCONV_ERR_UNSUPPORTED,
               "streamed edge features need precision f16, bf16 or f16x2");
   NNC_REQUIRE(tc_shapes_supported(W), NNCONV_ERR_UNSUPPORTED,
@@ -786,76 +842,14 @@ int apply_streamed(const Plan* P, const Weights* W, const float* edge_attr, cons
   char* base = static_cast<char*>(ws);
   int* overflow = reinterpret_cast<int*>(base);
   NNC_CHECK_CUDA(cudaMemsetAsync(overflow, 0, sizeof(int), st));
-  if (!options().overflow_check) overflow = nullptr;
-  if (P->E == 0 || P->n_src == 0) {
-    ProfScope ps(PK_NODE_PREP, st);
-    s = launch_out_init(x, root, bias, P->N, W->cin, W->cout, out, st, node_flags);
-    if (s == NNCONV_OK && launches) ++*launches;
-    return s;
-  }
   const StreamLayout SL = layout_stream(P, W, ws_bytes);
   NNC_REQUIRE(E_res == P->E || SL.rows >= kUnitEdges, NNCONV_ERR_WORKSPACE,
               "apply_streamed: workspace too small (use the size nnconv_stream_split returns)");
   NNC_REQUIRE(E_res == 0 || h_res != nullptr, NNCONV_ERR_ARG, "apply_streamed: null resident edge features");
-  const ApplyLayout L = layout_apply(P, W);
-  char* abase = base + SL.off_apply;
-  void* Xc = abase + L.off_Xc;
-  float* cvec = reinterpret_cast<float*>(abase + L.off_cvec);
-  float* xs = reinterpret_cast<float*>(abase + L.off_xs);
-  int* flags = reinterpret_cast<int*>(abase + L.off_flags);
-  void* Y = abase + L.off_Y;
-  const int64_t nodes_cap = static_cast<int64_t>((SL.apply_bytes - L.fixed_bytes) / L.per_node);
-  int ring = 0;
-  int64_t nb = 0;
-  const bool fused = fused_geometry(W, P->n_src, nodes_cap, &ring, &nb);
-  if (fused) {
-    // every persistent launch gets its own slice of the flag arrays: batches of all launches must fit the table
-    int64_t total = E_res > 0 ? ceil_div64(edge_range(P, 0, E_res).c_end, nb) : 0;
-    for (int64_t e = E_res; e < P->E;) {
-      const int64_t e2 = unit_floor(P, e + SL.rows);
-      const UnitRange r = edge_range(P, e, e2);
-      total += ceil_div64(r.c_end - r.c_begin, nb);
-      e = e2;
-    }
-    NNC_REQUIRE(total <= kMaxPipeBatches, NNCONV_ERR_WORKSPACE,
-                "apply_streamed: %lld source batches over all chunks exceed %d: use larger chunks", (long long)total,
-                kMaxPipeBatches);
-    NNC_CHECK_CUDA(cudaMemsetAsync(flags, 0, sizeof(int) * 5 * kMaxPipeBatches, st));
-    ProfScope ps(PK_NODE_PREP, st);
-    s = launch_node_prep(W->prec, x, root, bias, P->N, out, P->src_nodes, P->n_src, W->cin, W->cin_p, W->cout, W->B3, Xc,
-                         cvec, xs, flags, kMaxPipeBatches, 0, st, node_flags);
-    if (s) return s;
-    if (launches) ++*launches;
-  } else {
-    {
-      ProfScope ps(PK_NODE_PREP, st);
-      s = launch_out_init(x, root, bias, P->N, W->cin, W->cout, out, st, node_flags);
-    }
-    if (s) return s;
-    {
-      ProfScope ps(PK_NODE_PREP, st);
-      s = launch_src_prep(W->prec, x, P->src_nodes, P->n_src, W->cin, W->cin_p, W->cout, W->B3, Xc, cvec, xs, st, node_flags);
-    }
-    if (s) return s;
-    if (launches) *launches += 2;
-  }
-  int boff = 0;
-  if (E_res > 0) {
-    s = contract_range(P, W, edge_range(P, 0, E_res), E_res, h_res, fused, ring, nb, nodes_cap, Xc, Y, cvec, xs, aggr_mean, out,
-                       flags, &boff, st, launches);
-    if (s) return s;
-  }
-  void* hc = base + SL.off_h;
-  for (int64_t e = E_res; e < P->E;) {
-    const int64_t e2 = unit_floor(P, e + SL.rows);
-    s = edge_features_rows(P, W, edge_attr, e, e2 - e, hc, base + SL.off_ef, SL.ef_bytes, overflow, st, launches, nullptr);
-    if (s) return s;
-    s = contract_range(P, W, edge_range(P, e, e2), e2, hc, fused, ring, nb, nodes_cap, Xc, Y, cvec, xs, aggr_mean, out, flags,
-                       &boff, st, launches);
-    if (s) return s;
-    e = e2;
-  }
-  return NNCONV_OK;
+  const ChunkWs C{edge_attr, base + SL.off_h, base + SL.off_ef, SL.ef_bytes, SL.rows,
+                  options().overflow_check ? overflow : nullptr};
+  return apply_ranges(P, W, h_res, E_res, &C, x, root, bias, aggr_mean, out, base + SL.off_apply, SL.apply_bytes, st,
+                      launches, node_flags);
 }
 
 }  // namespace nnc

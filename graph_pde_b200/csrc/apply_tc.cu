@@ -628,7 +628,7 @@ int launch_variant(int grid, int smem_bytes, bool coop, cudaStream_t st, const H
   cudaError_t e = cudaLaunchKernelEx(&cfg, k_apply_tc<FMT, YBN, NC>, tmH, tmY, tmX, tmW, a);
   if (e == cudaErrorCooperativeLaunchTooLarge) {
     cudaGetLastError();
-    return kApplyCannotCoSchedule;   // handled by apply(): per-batch kernels instead
+    return kApplyCannotCoSchedule;   // handled by the application driver (api.cu): per-batch kernels instead
   }
   NNC_CHECK_CUDA(e);
   return NNCONV_OK;
@@ -637,7 +637,7 @@ int launch_variant(int grid, int smem_bytes, bool coop, cudaStream_t st, const H
 
 int launch_apply_tc(int prec, const Plan* P, const Weights* W, const void* h, const void* Xc, void* Yring, int nb,
                     int ring, const float* cvec, const float* xs, int aggr_mean, float* out, int* flags,
-                    int flags_stride, cudaStream_t st, const UnitRange* range) {
+                    int flags_stride, cudaStream_t st, const UnitRange& R) {
   int s = tc_init();
   if (s != NNCONV_OK) return s;
   const Options& opt = options();
@@ -648,8 +648,6 @@ int launch_apply_tc(int prec, const Plan* P, const Weights* W, const void* h, co
   NNC_REQUIRE(apply_shape(W->cout, eff_kp(W), ybn, y_num_kx(W), &as), NNCONV_ERR_UNSUPPORTED,
               "apply_tc: unsupported shape");
   if (opt.apply_stages >= 2 && opt.apply_stages < as.a_stages) as.a_stages = opt.apply_stages;
-  const UnitRange whole{0, P->n_units, 0, P->n_src, 0, round_up64(P->E, 128)};
-  const UnitRange& R = range ? *range : whole;
   const int64_t e_pad = R.h_rows;
   const int NY = W->cout * W->Kp;
   const int kmul = split ? 2 : 1;      // [hi | lo] activations / Y rows

@@ -84,9 +84,9 @@ int launch_apply_edge(int prec, const Plan* P, const Weights* W, const void* Kma
 int launch_gemm_tn(int prec, const void* A, int64_t lda, int a_col0, const void* B, int64_t ldb, int b_col0, int64_t R,
                    int M, int N, float* C, int64_t ldc, float alpha, const float* alpha_dev, cudaStream_t st);
 
-// Part of an application whose edge features are only partially resident (api.cu: apply_streamed): units
-// [u_begin, u_end) of sources [c_begin, c_end), with h holding the chunk-major rows of sorted edges [e_base, ...) in
-// panels of h_rows rows.  The whole graph is {0, n_units, 0, n_src, 0, round_up(E, 128)}.
+// The part of an application that one contraction covers (api.cu: contract_range): units [u_begin, u_end) of sources
+// [c_begin, c_end), with h holding the chunk-major rows of sorted edges [e_base, ...) in panels of h_rows rows.  A whole
+// cached h is the range {0, n_units, 0, n_src, 0, round_up(E, 128)}.
 struct UnitRange {
   int u_begin, u_end, c_begin, c_end;
   int64_t e_base, h_rows;
@@ -98,13 +98,13 @@ int launch_conv_tc(int prec, const Plan* P, const void* h, int Kp, const void* Y
                    int tile_begin, int tile_end, int c0, const float* cvec, const float* xs, int aggr_mean, float* out,
                    cudaStream_t st, const PipeFlags* pf = nullptr, int64_t e_base = 0, int64_t h_rows = 0);
 
-// ---- apply_tc.cu: ONE persistent kernel per application (Y GEMM + contraction pipelines in every CTA)
+// ---- apply_tc.cu: ONE persistent kernel per unit range (Y GEMM + contraction pipelines in every CTA); flags: the
+// range's batches of cntY, cntC, okY, okC, cntU at flags_stride
 constexpr int kApplyCannotCoSchedule = 1000;   // private status of launch_apply_tc: cooperative launch impossible
 bool apply_fused_supported(const Weights* W);
 int launch_apply_tc(int prec, const Plan* P, const Weights* W, const void* h, const void* Xc, void* Yring, int nb,
                     int ring, const float* cvec, const float* xs, int aggr_mean, float* out, int* flags,
-                    int flags_stride,
-                    cudaStream_t st, const UnitRange* range = nullptr);
+                    int flags_stride, cudaStream_t st, const UnitRange& R);
 
 // ---- graph_build.cu: ball graph (count / fill) on the device
 int ball_count(const double* pa, int64_t na, const double* pb, int64_t nb, double radius, int* counts, cudaStream_t st);

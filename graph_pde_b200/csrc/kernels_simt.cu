@@ -392,10 +392,11 @@ __global__ void k_src_prep(const float* __restrict__ x, const int* __restrict__ 
   src_prep_rows<T, SPLIT>(x, src_nodes, S, cin, cin_p, cout, B3, Xc, cvec, xs, node_flags, blockIdx.x, sx);
 }
 
-// One launch for everything a fused application needs before its persistent kernel: blocks [0, g_out) initialise the
-// output rows, blocks [g_out, g_out + g_src) prepare the source rows, and the first threads of the grid clear the batch
-// flags of the application (cntY / cntC / okY / okC [n_batches] at stride flags_stride, and the unit counter) -- in the
-// launch-bound MGKN regime (52 dependent applications per forward) every launch removed from the chain counts.
+// One launch for everything a 16-bit application needs before its contractions: blocks [0, g_out) initialise the
+// output rows, blocks [g_out, g_out + g_src) prepare the source rows, and the grid clears the batch flags of the
+// application (cntY / cntC / okY / okC / cntU [n_batches] at stride flags_stride; a grid-stride loop, because the
+// batches of many streamed chunks are not bounded by the source count that sizes the grid) -- in the launch-bound
+// MGKN regime (52 dependent applications per forward) every launch removed from the chain counts.
 template <typename T, int SPLIT = 0>
 __global__ void k_node_prep(const float* __restrict__ x, const float* __restrict__ root, const float* __restrict__ bias,
                             int64_t N, float* __restrict__ out, int g_out, const int* __restrict__ src_nodes, int S, int cin,
@@ -405,11 +406,11 @@ __global__ void k_node_prep(const float* __restrict__ x, const float* __restrict
   extern __shared__ float sx[];
   const int tid = threadIdx.y * blockDim.x + threadIdx.x;
   const int64_t gid = static_cast<int64_t>(blockIdx.x) * (blockDim.x * blockDim.y) + tid;
-  if (gid < n_batches) {
+  const int64_t n_threads = static_cast<int64_t>(gridDim.x) * (blockDim.x * blockDim.y);
+  for (int64_t i = gid; i < n_batches; i += n_threads) {
 #pragma unroll
-    for (int j = 0; j < 4; ++j) flags[j * flags_stride + gid] = 0;
+    for (int j = 0; j < 5; ++j) flags[j * flags_stride + i] = 0;
   }
-  if (gid == 0) flags[4 * flags_stride] = 0;
   if (static_cast<int>(blockIdx.x) < g_out)
     out_init_rows(x, root, bias, N, cin, cout, out, node_flags, blockIdx.x, sx);
   else
@@ -897,7 +898,7 @@ int launch_src_prep(int prec, const float* x, const int* src_nodes, int S, int c
   return NNCONV_OK;
 }
 
-// out_init + src_prep + the flag reset of one fused application as ONE launch (16-bit precisions)
+// out_init + src_prep + the flag reset of one application as ONE launch (16-bit precisions)
 int launch_node_prep(int prec, const float* x, const float* root, const float* bias, int64_t N, float* out,
                      const int* src_nodes, int S, int cin, int cin_p, int cout, const float* B3, void* Xc, float* cvec,
                      float* xs, int* flags, int flags_stride, int n_batches, cudaStream_t st, unsigned node_flags) {

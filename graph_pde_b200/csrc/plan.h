@@ -89,7 +89,7 @@ size_t edge_acts_offset(const Plan* P, const Weights* W, int l);
 int edge_features(const Plan* P, const Weights* W, const float* edge_attr, void* h, void* ws, size_t ws_bytes,
                   cudaStream_t st, int64_t* launches, void* acts = nullptr, int64_t n_edges = -1);
 
-// one conv application given h_last
+// one conv application given h_last of every edge: apply_streamed's application with E_res = E (one driver, api.cu)
 size_t apply_ws_bytes(const Plan* P, const Weights* W, size_t want_bytes);
 int apply(const Plan* P, const Weights* W, const void* h, const float* x, const float* root, const float* bias,
           int aggr_mean, float* out, void* ws, size_t ws_bytes, cudaStream_t st, int64_t* launches,
@@ -97,7 +97,7 @@ int apply(const Plan* P, const Weights* W, const void* h, const float* x, const 
 
 // partially resident edge features (16-bit precisions): the edge features of the sorted edges [0, E_res) are cached by
 // the caller (edge_features with n_edges = E_res), those of [E_res, E) are recomputed chunk by chunk inside every
-// application.  stream_split picks the largest unit-aligned E_res whose h fits resident_bytes and sizes the workspace
+// application, each chunk contracted as the resident prefix is.  stream_split picks the largest unit-aligned E_res whose h fits resident_bytes and sizes the workspace
 // of apply_streamed for chunks of chunk_ws_bytes (h rows + edge-feature workspace).
 int stream_split(const Plan* P, const Weights* W, size_t resident_bytes, size_t chunk_ws_bytes, int64_t* E_res,
                  size_t* h_res_bytes, size_t* ws_bytes, int64_t* n_chunks);

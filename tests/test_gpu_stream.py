@@ -209,7 +209,8 @@ def test_prefix_bits_equal_cached(dev, precision):
 
 
 def test_no_fuse_option(dev):
-    """The per-batch kernels (nnconv_set_option('no_fuse', 1)) over unit ranges with an edge base."""
+    """The per-batch kernels (nnconv_set_option('no_fuse', 1)) over unit ranges with an edge base, PDL-pipelined and
+    (no_pipe) in plain stream order."""
     from graph_pde_b200 import _lib
     w, T = 64, 2
     ei, ea = _hub_graph(dev)
@@ -217,16 +218,19 @@ def test_no_fuse_option(dev):
     conv = make_conv(_cls(), ws, bs, root, bias, 'mean', w, w, 'f16', dev)
     x0 = torch.randn(300, w, device=dev)
     ref, ins, _ = _stack(conv, x0, ei, ea, T, None)
-    _lib.set_option('no_fuse', 1)
-    try:
-        got, _, n = _stack(conv, x0, ei, ea, T, 0, ins)
-        got2, _, _ = _stack(conv, x0, ei, ea, T, _h_bytes(conv, ei, ea, 300) // 2, ins)
-    finally:
-        _lib.set_option('no_fuse', None)
-    assert n >= T
-    for k in range(T):
-        assert rel_err(got[k], ref[k]) < STREAM_TOL
-        assert rel_err(got2[k], ref[k]) < STREAM_TOL
+    for knobs in (('no_fuse',), ('no_fuse', 'no_pipe')):
+        for k in knobs:
+            _lib.set_option(k, 1)
+        try:
+            got, _, n = _stack(conv, x0, ei, ea, T, 0, ins)
+            got2, _, _ = _stack(conv, x0, ei, ea, T, _h_bytes(conv, ei, ea, 300) // 2, ins)
+        finally:
+            for k in knobs:
+                _lib.set_option(k, None)
+        assert n >= T, knobs
+        for k in range(T):
+            assert rel_err(got[k], ref[k]) < STREAM_TOL, knobs
+            assert rel_err(got2[k], ref[k]) < STREAM_TOL, knobs
 
 
 def test_residual_step_chain(dev):
