@@ -550,7 +550,10 @@ class NNConv_old(torch.nn.Module):
 
             e_res, h_res_b, chunk_ws_b, n_ch = split(0 if auto else budget)
             if auto:
-                free = torch.cuda.mem_get_info(dev)[0] + torch.cuda.memory_reserved(dev) - torch.cuda.memory_allocated(dev)
+                # the device's free memory only: the failed allocation above has already released the allocator's
+                # unused segments, and what it still holds unallocated are free parts of segments in use -- fragments
+                # that the 2 GiB workspaces below need not fit into
+                free = torch.cuda.mem_get_info(dev)[0]
                 work = chunk_ws_b + _STREAM_MARGIN_BYTES
                 if for_grad:
                     # the streamed backward's workspaces do not depend on where the prefix ends: sized at E_res = 0
