@@ -14,7 +14,7 @@ CSRC = os.path.join(_HERE, 'csrc')
 OK = 0
 ABI_VERSION = 2        # include/nnconv_b200.h: NNCONV_B200_ABI_VERSION this binding was written against
 PREC = {'fp32': 0, 'f16': 1, 'fp16': 1, 'bf16': 2, 'f16x2': 3}
-AGGR = {'add': 0, 'mean': 1}
+AGGR = {'add': 0, 'mean': 1, 'max': 2}     # max: through the nnconv_*_max entry points only
 APPLY_RELU_IN, APPLY_RESIDUAL = 1, 2        # include/nnconv_b200.h NNCONV_APPLY_*
 FLOW = {'source_to_target': 0, 'target_to_source': 1}
 
@@ -38,6 +38,8 @@ SYMBOLS = [
     'nnconv_stream_split', 'nnconv_edge_features_prefix', 'nnconv_apply_streamed',
     'nnconv_backward_apply_streamed_sizes', 'nnconv_backward_apply_streamed', 'nnconv_backward_mlp_streamed_sizes',
     'nnconv_backward_mlp_streamed', 'nnconv_backward_streamed_chunks', 'nnconv_overflow_accumulate',
+    'nnconv_apply_max_sizes', 'nnconv_apply_max', 'nnconv_backward_apply_max', 'nnconv_backward_mlp_max',
+    'nnconv_backward_max',
 ]
 
 
@@ -144,6 +146,15 @@ def lib():
     L.nnconv_backward_mlp_streamed.argtypes = [c_vp, c_vp, c_vp, c_vp, c_i64, c_int, P(c_vp), P(c_vp), c_int, P(c_vp),
                                                P(c_vp), c_vp, c_sz, c_vp, c_vp]
     L.nnconv_backward_streamed_chunks.argtypes = [c_vp, c_vp, c_i64, c_int, c_sz, P(c_i64)]
+    L.nnconv_apply_max_sizes.argtypes = [c_vp, c_vp, c_sz, P(c_sz)]
+    L.nnconv_apply_max.argtypes = [c_vp, c_vp, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, ctypes.c_uint, c_vp, c_vp, c_vp, c_sz,
+                                   c_vp, P(c_i64)]
+    L.nnconv_backward_apply_max.argtypes = [c_vp, c_vp, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
+                                            c_vp, c_vp, c_sz, c_vp, P(c_i64)]
+    L.nnconv_backward_mlp_max.argtypes = [c_vp, c_vp, c_vp, c_vp, c_i64, c_int, P(c_vp), P(c_vp), P(c_vp), P(c_vp),
+                                          P(c_vp), c_vp, c_sz, c_vp, c_vp, c_vp]
+    L.nnconv_backward_max.argtypes = [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, P(c_vp), P(c_vp), c_vp, c_vp, c_vp,
+                                      c_sz, c_vp, c_vp]
     for name in SYMBOLS:
         getattr(L, name)
     if L.nnconv_abi_version() != ABI_VERSION:

@@ -627,13 +627,13 @@ static int64_t range_batches(const Plan* P, int64_t e_from, int64_t E_res, int64
 // global memory.  Without pipe the same kernels run in plain stream order with one Y buffer.
 static int contract_range(const Plan* P, const Weights* W, const UnitRange& R, int64_t e_hi, const void* h,
                           const Schedule& S, const ApplyWs& A, int* flags, int aggr_mean, float* out, cudaStream_t st,
-                          int64_t* launches) {
+                          int64_t* launches, unsigned long long* max_keys) {
   if (S.fused) {
     int s;
     {
       ProfScope ps(PK_APPLY_FUSED, st);
       s = launch_apply_tc(W->prec, P, W, h, A.Xc, A.Y, static_cast<int>(S.nb), S.ring, A.cvec, A.xs, aggr_mean, out, flags,
-                          kMaxPipeBatches, st, R);
+                          kMaxPipeBatches, st, R, max_keys);
     }
     if (s == NNCONV_OK && launches) ++*launches;
     return s;
@@ -679,7 +679,7 @@ static int contract_range(const Plan* P, const Weights* W, const UnitRange& R, i
     }
     ProfScope ps(PK_CONV, st);
     return launch_conv_tc(W->prec, P, h, W->Kp, Ybuf[b % 3], nb, W->cout, tb, te, static_cast<int>(c0), A.cvec, A.xs,
-                          aggr_mean, out, st, S.pipe ? &pf : nullptr, R.e_base, R.h_rows);
+                          aggr_mean, out, st, S.pipe ? &pf : nullptr, R.e_base, R.h_rows, max_keys);
   };
   int s = launch_y(0);
   if (s) return s;
@@ -699,8 +699,10 @@ static int contract_range(const Plan* P, const Weights* W, const UnitRange& R, i
 // one Y buffer
 static int apply_fp32(const Plan* P, const Weights* W, const float* h, const float* x, const float* root,
                       const float* bias, int aggr_mean, float* out, const ApplyWs& A, cudaStream_t st, int64_t* launches,
-                      unsigned node_flags) {
+                      unsigned node_flags, unsigned long long* max_keys) {
   int s;
+  if (max_keys != nullptr)
+    NNC_CHECK_CUDA(cudaMemsetAsync(max_keys, 0, sizeof(unsigned long long) * P->N * W->cout, st));
   {
     ProfScope ps(PK_NODE_PREP, st);
     s = launch_out_init(x, root, bias, P->N, W->cin, W->cout, out, st, node_flags);
@@ -728,7 +730,7 @@ static int apply_fp32(const Plan* P, const Weights* W, const float* h, const flo
     {
       ProfScope ps(PK_CONV, st);
       s = launch_sgemm_scatter(P, h, W->Kp, static_cast<const float*>(A.Y), W->cout, tb, te, static_cast<int>(c0), A.cvec,
-                               aggr_mean, out, st);
+                               aggr_mean, out, st, max_keys);
     }
     if (s) return s;
     if (launches) *launches += 2;
@@ -736,15 +738,18 @@ static int apply_fp32(const Plan* P, const Weights* W, const float* h, const flo
   return NNCONV_OK;
 }
 
-// ws / ws_bytes: the application workspace; C: the chunk region, nullptr when E_res = E
-static int apply_ranges(const Plan* P, const Weights* W, const void* h_res, int64_t E_res, const ChunkWs* C,
-                        const float* x, const float* root, const float* bias, int aggr_mean, float* out, void* ws,
-                        size_t ws_bytes, cudaStream_t st, int64_t* launches, unsigned node_flags) {
+// the ranges of one application, contracted into out (aggr = max: into max_keys); see apply_ranges
+static int apply_contract(const Plan* P, const Weights* W, const void* h_res, int64_t E_res, const ChunkWs* C,
+                          const float* x, const float* root, const float* bias, int aggr_mean, float* out, void* ws,
+                          size_t ws_bytes, cudaStream_t st, int64_t* launches, unsigned node_flags,
+                          unsigned long long* max_keys) {
   int s;
   NNC_REQUIRE(!(node_flags & NNCONV_APPLY_RESIDUAL) || W->cin == W->cout, NNCONV_ERR_ARG,
               "NNCONV_APPLY_RESIDUAL needs in_channels == out_channels");
   if (P->E == 0 || P->n_src == 0) {
     ProfScope ps(PK_NODE_PREP, st);
+    if (max_keys != nullptr)   // no edge: every key stays empty
+      NNC_CHECK_CUDA(cudaMemsetAsync(max_keys, 0, sizeof(unsigned long long) * P->N * W->cout, st));
     s = launch_out_init(x, root, bias, P->N, W->cin, W->cout, out, st, node_flags);
     if (s == NNCONV_OK && launches) ++*launches;
     return s;
@@ -759,7 +764,8 @@ static int apply_ranges(const Plan* P, const Weights* W, const void* h_res, int6
                   reinterpret_cast<int*>(base + L.off_flags), base + L.off_Y, L.per_node,
                   static_cast<int64_t>((ws_bytes - L.fixed_bytes) / L.per_node)};
   if (W->prec == PREC_FP32)
-    return apply_fp32(P, W, static_cast<const float*>(h_res), x, root, bias, aggr_mean, out, A, st, launches, node_flags);
+    return apply_fp32(P, W, static_cast<const float*>(h_res), x, root, bias, aggr_mean, out, A, st, launches, node_flags,
+                      max_keys);
 
   // the schedule, decided once: the persistent kernel when it has a geometry for this Y region and the flag batches of
   // all ranges fit the table (every persistent launch has its own slice), else the per-batch chain
@@ -793,7 +799,7 @@ static int apply_ranges(const Plan* P, const Weights* W, const void* h_res, int6
   {
     ProfScope ps(PK_NODE_PREP, st);
     s = launch_node_prep(W->prec, x, root, bias, P->N, out, P->src_nodes, P->n_src, W->cin, W->cin_p, W->cout, W->B3, A.Xc,
-                         A.cvec, A.xs, A.flags, kMaxPipeBatches, static_cast<int>(n_flag), st, node_flags);
+                         A.cvec, A.xs, A.flags, kMaxPipeBatches, static_cast<int>(n_flag), st, node_flags, max_keys);
   }
   if (s) return s;
   if (launches) ++*launches;
@@ -807,7 +813,7 @@ static int apply_ranges(const Plan* P, const Weights* W, const void* h_res, int6
       h = C->h;
     }
     const UnitRange R = edge_range(P, e, e2);
-    s = contract_range(P, W, R, e2, h, S, A, A.flags + boff, aggr_mean, out, st, launches);
+    s = contract_range(P, W, R, e2, h, S, A, A.flags + boff, aggr_mean, out, st, launches, max_keys);
     if (s == kApplyCannotCoSchedule) {
       // the driver cannot co-schedule one CTA per SM (MPS / green-context partition): the chain runs this range and the
       // rest, its flags numbered from 0 again over slots that the persistent launches before it have used
@@ -815,7 +821,7 @@ static int apply_ranges(const Plan* P, const Weights* W, const void* h_res, int6
       if (s) return s;
       if (S.pipe) NNC_CHECK_CUDA(cudaMemsetAsync(A.flags, 0, sizeof(int) * 4 * kMaxPipeBatches, st));
       boff = 0;
-      s = contract_range(P, W, R, e2, h, S, A, A.flags, aggr_mean, out, st, launches);
+      s = contract_range(P, W, R, e2, h, S, A, A.flags, aggr_mean, out, st, launches, max_keys);
     }
     if (s) return s;
     boff += ceil_div64(R.c_end - R.c_begin, S.nb);
@@ -824,14 +830,30 @@ static int apply_ranges(const Plan* P, const Weights* W, const void* h_res, int6
   return NNCONV_OK;
 }
 
+// ws / ws_bytes: the application workspace; C: the chunk region, nullptr when E_res = E.  aggr = max: max_keys (N *
+// cout keys, else nullptr) and argmax [N, cout]; the application ends with the finalize launch
+static int apply_ranges(const Plan* P, const Weights* W, const void* h_res, int64_t E_res, const ChunkWs* C,
+                        const float* x, const float* root, const float* bias, int aggr_mean, float* out, void* ws,
+                        size_t ws_bytes, cudaStream_t st, int64_t* launches, unsigned node_flags,
+                        unsigned long long* max_keys, int* argmax) {
+  int s = apply_contract(P, W, h_res, E_res, C, x, root, bias, aggr_mean, out, ws, ws_bytes, st, launches, node_flags,
+                         max_keys);
+  if (s || max_keys == nullptr) return s;
+  s = launch_max_finalize(max_keys, P->N * W->cout, out, argmax, st);
+  if (s == NNCONV_OK && launches) ++*launches;
+  return s;
+}
+
 int apply(const Plan* P, const Weights* W, const void* h, const float* x, const float* root, const float* bias,
           int aggr_mean, float* out, void* ws, size_t ws_bytes, cudaStream_t st, int64_t* launches, unsigned node_flags) {
-  return apply_ranges(P, W, h, P->E, nullptr, x, root, bias, aggr_mean, out, ws, ws_bytes, st, launches, node_flags);
+  return apply_ranges(P, W, h, P->E, nullptr, x, root, bias, aggr_mean, out, ws, ws_bytes, st, launches, node_flags,
+                      nullptr, nullptr);
 }
 
 int apply_streamed(const Plan* P, const Weights* W, const float* edge_attr, const void* h_res, int64_t E_res,
                    const float* x, const float* root, const float* bias, int aggr_mean, float* out, void* ws,
-                   size_t ws_bytes, cudaStream_t st, int64_t* launches, unsigned node_flags) {
+                   size_t ws_bytes, cudaStream_t st, int64_t* launches, unsigned node_flags,
+                   unsigned long long* max_keys, int* argmax) {
   NNC_REQUIRE(W->prec == PREC_F16 || W->prec == PREC_BF16 || W->prec == PREC_F16X2, NNCONV_ERR_UNSUPPORTED,
               "streamed edge features need precision f16, bf16 or f16x2");
   NNC_REQUIRE(tc_shapes_supported(W), NNCONV_ERR_UNSUPPORTED,
@@ -849,7 +871,23 @@ int apply_streamed(const Plan* P, const Weights* W, const float* edge_attr, cons
   const ChunkWs C{edge_attr, base + SL.off_h, base + SL.off_ef, SL.ef_bytes, SL.rows,
                   options().overflow_check ? overflow : nullptr};
   return apply_ranges(P, W, h_res, E_res, &C, x, root, bias, aggr_mean, out, base + SL.off_apply, SL.apply_bytes, st,
-                      launches, node_flags);
+                      launches, node_flags, max_keys, argmax);
+}
+
+// aggr = max (nnconv_apply_max): ws = [keys (max_keys_bytes) | the workspace of the add / mean call]
+int apply_max(const Plan* P, const Weights* W, const float* edge_attr, const void* h_res, int64_t E_res, const float* x,
+              const float* root, const float* bias, float* out, int* argmax, void* ws, size_t ws_bytes, cudaStream_t st,
+              int64_t* launches, unsigned node_flags) {
+  const size_t kb = max_keys_bytes(P->N, W->cout);
+  NNC_REQUIRE(ws != nullptr && ws_bytes > kb, NNCONV_ERR_WORKSPACE,
+              "apply_max: workspace too small (use the size nnconv_apply_max_sizes returns)");
+  unsigned long long* keys = static_cast<unsigned long long*>(ws);
+  void* rest = static_cast<char*>(ws) + kb;
+  if (E_res == P->E)
+    return apply_ranges(P, W, h_res, P->E, nullptr, x, root, bias, 0, out, rest, ws_bytes - kb, st, launches, node_flags,
+                        keys, argmax);
+  return apply_streamed(P, W, edge_attr, h_res, E_res, x, root, bias, 0, out, rest, ws_bytes - kb, st, launches,
+                        node_flags, keys, argmax);
 }
 
 }  // namespace nnc
@@ -1014,7 +1052,7 @@ int nnconv_apply_streamed(const nnconv_plan_t* plan, const nnconv_weights_t* w, 
                           float* out, void* ws, size_t ws_bytes, void* stream, int64_t* launches) {
   NNC_REQUIRE(plan && w && x && out && (edge_attr || plan->p.E == 0), NNCONV_ERR_ARG, "null pointer");
   NNC_REQUIRE(aggr == NNCONV_AGGR_ADD || aggr == NNCONV_AGGR_MEAN, NNCONV_ERR_UNSUPPORTED,
-              "aggr must be add (0) or mean (1); 'max' is used by no call site of the reference and is not built");
+              "aggr must be add (0) or mean (1); aggr = max (2) runs through nnconv_apply_max");
   NNC_REQUIRE((flags & ~(NNCONV_APPLY_RELU_IN | NNCONV_APPLY_RESIDUAL)) == 0, NNCONV_ERR_ARG, "unknown apply flag");
   NNC_REQUIRE(x != out, NNCONV_ERR_ARG, "out must not alias x");
   return apply_streamed(&plan->p, &w->w, edge_attr, h_res, E_res, x, root, bias, aggr == NNCONV_AGGR_MEAN, out, ws,
@@ -1088,7 +1126,7 @@ int nnconv_apply(const nnconv_plan_t* plan, const nnconv_weights_t* w, const voi
                  int64_t* launches) {
   NNC_REQUIRE(plan && w && x && out && (h || plan->p.E == 0), NNCONV_ERR_ARG, "null pointer");
   NNC_REQUIRE(aggr == NNCONV_AGGR_ADD || aggr == NNCONV_AGGR_MEAN, NNCONV_ERR_UNSUPPORTED,
-              "aggr must be add (0) or mean (1); 'max' is used by no call site of the reference and is not built");
+              "aggr must be add (0) or mean (1); aggr = max (2) runs through nnconv_apply_max");
   return apply(&plan->p, &w->w, h, x, root, bias, aggr == NNCONV_AGGR_MEAN, out, ws, ws_bytes,
                static_cast<cudaStream_t>(stream), launches);
 }
@@ -1098,7 +1136,7 @@ int nnconv_apply_ex(const nnconv_plan_t* plan, const nnconv_weights_t* w, const 
                     void* stream, int64_t* launches) {
   NNC_REQUIRE(plan && w && x && out && (h || plan->p.E == 0), NNCONV_ERR_ARG, "null pointer");
   NNC_REQUIRE(aggr == NNCONV_AGGR_ADD || aggr == NNCONV_AGGR_MEAN, NNCONV_ERR_UNSUPPORTED,
-              "aggr must be add (0) or mean (1); 'max' is used by no call site of the reference and is not built");
+              "aggr must be add (0) or mean (1); aggr = max (2) runs through nnconv_apply_max");
   NNC_REQUIRE((flags & ~(NNCONV_APPLY_RELU_IN | NNCONV_APPLY_RESIDUAL)) == 0, NNCONV_ERR_ARG, "unknown apply flag");
   NNC_REQUIRE(x != out, NNCONV_ERR_ARG, "out must not alias x");
   return apply(&plan->p, &w->w, h, x, root, bias, aggr == NNCONV_AGGR_MEAN, out, ws, ws_bytes,
@@ -1125,7 +1163,8 @@ int nnconv_backward_ex(const nnconv_plan_t* plan, const nnconv_weights_t* w, con
                        float* const* grad_b, float* grad_root, float* grad_bias, void* ws, size_t ws_bytes,
                        void* stream, float* grad_edge_attr) {
   NNC_REQUIRE(plan && w && x && grad_out && grad_x && grad_W && grad_b, NNCONV_ERR_ARG, "null pointer");
-  NNC_REQUIRE(aggr == NNCONV_AGGR_ADD || aggr == NNCONV_AGGR_MEAN, NNCONV_ERR_UNSUPPORTED, "aggr must be add or mean");
+  NNC_REQUIRE(aggr == NNCONV_AGGR_ADD || aggr == NNCONV_AGGR_MEAN, NNCONV_ERR_UNSUPPORTED,
+              "aggr must be add or mean; aggr = max runs through nnconv_backward_max");
   NNC_REQUIRE((root == nullptr) == (grad_root == nullptr), NNCONV_ERR_ARG, "root / grad_root must both be given or both be NULL");
   NNC_REQUIRE(grad_edge_attr == nullptr || edge_attr != nullptr || plan->p.E == 0, NNCONV_ERR_ARG,
               "grad_edge_attr needs edge_attr");
@@ -1213,6 +1252,69 @@ int nnconv_backward_streamed_chunks(const nnconv_plan_t* plan, const nnconv_weig
               "backward_streamed_chunks: E_res = %lld is not a unit boundary of the plan", (long long)E_res);
   *n_chunks = backward_streamed_chunks(&plan->p, &w->w, n_apps, E_res, ws_bytes);
   return NNCONV_OK;
+}
+
+int nnconv_apply_max_sizes(const nnconv_plan_t* plan, const nnconv_weights_t* w, size_t ws_bytes, size_t* max_ws_bytes) {
+  NNC_REQUIRE(plan && w && max_ws_bytes, NNCONV_ERR_ARG, "null pointer");
+  *max_ws_bytes = max_keys_bytes(plan->p.N, w->w.cout) + ws_bytes;
+  return NNCONV_OK;
+}
+
+int nnconv_apply_max(const nnconv_plan_t* plan, const nnconv_weights_t* w, const float* edge_attr, const void* h_res,
+                     int64_t E_res, const float* x, const float* root, const float* bias, unsigned flags, float* out,
+                     int* argmax, void* ws, size_t ws_bytes, void* stream, int64_t* launches) {
+  NNC_REQUIRE(plan && w && x && out && argmax && (h_res || E_res == 0) && (edge_attr || E_res == plan->p.E),
+              NNCONV_ERR_ARG, "null pointer");
+  NNC_REQUIRE(is_unit_boundary(&plan->p, E_res), NNCONV_ERR_ARG,
+              "apply_max: E_res = %lld is not a unit boundary of the plan (use nnconv_stream_split)", (long long)E_res);
+  NNC_REQUIRE((flags & ~(NNCONV_APPLY_RELU_IN | NNCONV_APPLY_RESIDUAL)) == 0, NNCONV_ERR_ARG, "unknown apply flag");
+  NNC_REQUIRE(x != out, NNCONV_ERR_ARG, "out must not alias x");
+  return apply_max(&plan->p, &w->w, edge_attr, h_res, E_res, x, root, bias, out, argmax, ws, ws_bytes,
+                   static_cast<cudaStream_t>(stream), launches, flags);
+}
+
+int nnconv_backward_apply_max(const nnconv_plan_t* plan, const nnconv_weights_t* w, const float* edge_attr,
+                              const void* h_res, int64_t E_res, const float* x, const float* root, const int* argmax,
+                              const float* grad_out, float* grad_x, float* grad_W_last, float* grad_b_last,
+                              float* grad_root, float* grad_bias, void* ws, size_t ws_bytes, void* stream,
+                              int64_t* launches) {
+  NNC_REQUIRE(plan && w && x && argmax && grad_out && grad_x && grad_W_last && grad_b_last &&
+                  (edge_attr || E_res == plan->p.E) && (h_res || E_res == 0),
+              NNCONV_ERR_ARG, "null pointer");
+  NNC_REQUIRE((root == nullptr) == (grad_root == nullptr), NNCONV_ERR_ARG, "root / grad_root must both be given or both be NULL");
+  NNC_REQUIRE(is_unit_boundary(&plan->p, E_res), NNCONV_ERR_ARG,
+              "backward_apply_max: E_res = %lld is not a unit boundary of the plan (use nnconv_stream_split)",
+              (long long)E_res);
+  return backward_apply_tc(&plan->p, &w->w, edge_attr, h_res, E_res, x, root, 0, grad_out, grad_x, grad_W_last,
+                           grad_b_last, grad_root, grad_bias, ws, ws_bytes, static_cast<cudaStream_t>(stream), launches,
+                           argmax);
+}
+
+int nnconv_backward_mlp_max(const nnconv_plan_t* plan, const nnconv_weights_t* w, const float* edge_attr,
+                            const void* h_res, int64_t E_res, int n_apps, const float* const* grad_out,
+                            const float* const* x, const int* const* argmax, float* const* grad_W, float* const* grad_b,
+                            void* ws, size_t ws_bytes, void* stream, const void* acts, float* grad_edge_attr) {
+  NNC_REQUIRE(plan && w && grad_out && x && argmax && grad_W && grad_b && (edge_attr || plan->p.E == 0) &&
+                  (h_res || E_res == 0),
+              NNCONV_ERR_ARG, "null pointer");
+  NNC_REQUIRE(n_apps >= 1, NNCONV_ERR_ARG, "backward_mlp_max: n_apps >= 1");
+  for (int t = 0; t < n_apps; ++t) NNC_REQUIRE(argmax[t] != nullptr, NNCONV_ERR_ARG, "backward_mlp_max: null argmax");
+  NNC_REQUIRE(is_unit_boundary(&plan->p, E_res), NNCONV_ERR_ARG,
+              "backward_mlp_max: E_res = %lld is not a unit boundary of the plan (use nnconv_stream_split)",
+              (long long)E_res);
+  return backward_mlp_tc(&plan->p, &w->w, edge_attr, h_res, E_res, n_apps, grad_out, x, 0, grad_W, grad_b, ws, ws_bytes,
+                         static_cast<cudaStream_t>(stream), acts, grad_edge_attr, argmax);
+}
+
+int nnconv_backward_max(const nnconv_plan_t* plan, const nnconv_weights_t* w, const float* edge_attr, const float* x,
+                        const float* root, const int* argmax, const float* grad_out, float* grad_x,
+                        float* const* grad_W, float* const* grad_b, float* grad_root, float* grad_bias, void* ws,
+                        size_t ws_bytes, void* stream, float* grad_edge_attr) {
+  NNC_REQUIRE(plan && w && x && argmax && grad_out && grad_x && grad_W && grad_b, NNCONV_ERR_ARG, "null pointer");
+  NNC_REQUIRE((root == nullptr) == (grad_root == nullptr), NNCONV_ERR_ARG, "root / grad_root must both be given or both be NULL");
+  NNC_REQUIRE(edge_attr != nullptr || plan->p.E == 0, NNCONV_ERR_ARG, "backward_max: null edge_attr");
+  return backward_fp32(&plan->p, &w->w, edge_attr, x, root, 0, grad_out, grad_x, grad_W, grad_b, grad_root, grad_bias,
+                       ws, ws_bytes, static_cast<cudaStream_t>(stream), grad_edge_attr, argmax);
 }
 
 int nnconv_backward_mlp_sizes(const nnconv_plan_t* plan, const nnconv_weights_t* w, int n_apps, size_t want_bytes,

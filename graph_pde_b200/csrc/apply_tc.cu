@@ -40,6 +40,11 @@ constexpr int kQueue = 8;                  // unit queue between the scheduler a
 constexpr int kScatterPitch = 272;         // bytes per staged edge row (64 fp32 + 16 B)
 constexpr int kScatterRows = 16;           // staged rows per conv warp: its 32 rows go out as two halves
 constexpr int kScatterBytes = 8 * kScatterRows * kScatterPitch;
+// aggr = max: a staged row holds NC 8-byte keys (512 B at NC = 64); a warp's 32 rows go out in four trips of 8 rows
+// through the same staging slots
+constexpr int kKeyPitch = 64 * 8 + 16;
+constexpr int kKeyRows = 8;
+static_assert(kKeyRows * kKeyPitch <= kScatterRows * kScatterPitch, "key rows exceed a warp's scatter staging");
 constexpr int kMaxXBytes = 3 * kATileBytes;   // largest Xc tile (num_kx boxes) the Y GEMM keeps resident
 constexpr int kYStagingBytes = 4 * 32 * 128;   // Y epilogue: per Y warp, its 32 rows x 64 16-bit columns
 
@@ -83,6 +88,9 @@ struct ApplyArgs {
   int scatter_mode;                    // 1: rows staged in shared memory + cp.reduce.async.bulk (see options.h)
   int debug_scatter;      // timing experiments only (NNCONV_DEBUG_SCATTER): 1 = drop the scatter, 2 = plain stores
   TraceBuf trace;
+  // aggr = max (the MAX instantiation only): [N, cout] keys (common.cuh max_key) and the plan's perm (nullable)
+  unsigned long long* keys;
+  const int* perm;
 };
 
 struct HMaps {
@@ -97,10 +105,11 @@ __device__ __forceinline__ void raise_when_all(int* cnt, int* ok, int target) {
   }
 }
 
-template <int FMT, int kYBlockN, int NC>
-__global__ void __launch_bounds__(kThreads, 1)
-k_apply_tc(const __grid_constant__ HMaps tmH, const __grid_constant__ CUtensorMap tmY,
-           const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmW, ApplyArgs a) {
+// The kernel body, shared by k_apply_tc (aggr add / mean) and k_apply_tc_max.  MAX: aggr = max -- the epilogue
+// reduces each edge row's keys into a.keys with one bulk max.u64 request (DESIGN 4.1).
+template <int FMT, int kYBlockN, int NC, bool MAX>
+__device__ __forceinline__ void apply_tc_body(const HMaps& tmH, const CUtensorMap& tmY, const CUtensorMap& tmX,
+                                              const CUtensorMap& tmW, const ApplyArgs& a) {
   constexpr int kWBytes = kYBlockN * 64 * 2;   // one W3p box
   extern __shared__ __align__(1024) uint8_t smem[];
   if ((smem_u32(smem) & 1023u) != 0) __trap();
@@ -329,7 +338,33 @@ k_apply_tc(const __grid_constant__ HMaps tmH, const __grid_constant__ CUtensorMa
         fsc[i] = __shfl_sync(0xffffffffu, sc, L);
         fok[i] = __shfl_sync(0xffffffffu, ok ? 1 : 0, L) != 0;
       }
-      if (a.scatter_mode == 1) {
+      if constexpr (MAX) {
+        // the keys of the message add scatters (no degree scale), rows staged in shared memory, then ONE bulk
+        // .max.u64 reduction of NC * 8 bytes per row (its lane issues it); the warp's 32 rows go out in four trips of
+        // 8 -- rows 8 h + r (fragment i = h) in trip h -- through its scatter staging slots
+        const uint32_t ce = ok ? caller_edge(a.perm, a.tile_e0[en.x + g] + r) : 0u;
+        unsigned long long* krow = a.keys + static_cast<int64_t>(d) * NC;
+#pragma unroll
+        for (int h = 0; h < 4; ++h) {
+          const uint32_t ceh = __shfl_sync(0xffffffffu, ce, fr + 8 * h);
+          bulk_wait_read0();                               // this lane's previous row has left its staging slot
+          __syncwarp();
+#pragma unroll
+          for (int jj = 0; jj < NC / 8; ++jj) {
+            const float2 cq = __ldg(reinterpret_cast<const float2*>(cv + 8 * jj + fc));
+            const float* dv = acc.d[h >> 1] + 4 * jj + 2 * (h & 1);
+            const unsigned long long k0 = max_key(fmaf(dv[0], xsc, cq.x), ceh);
+            const unsigned long long k1 = max_key(fmaf(dv[1], xsc, cq.y), ceh);
+            const uint32_t addr = my_rows + static_cast<uint32_t>(fr * kKeyPitch + (8 * jj + fc) * 8);
+            asm volatile("st.shared.v2.u64 [%0], {%1, %2};" ::"r"(addr), "l"(k0), "l"(k1) : "memory");
+          }
+          fence_proxy_async_smem();                       // generic-proxy writes of the warp -> async proxy
+          __syncwarp();
+          if (ok && (lane >> 3) == h)
+            bulk_reduce_max_u64(krow, my_rows + static_cast<uint32_t>((lane & 7) * kKeyPitch), static_cast<uint32_t>(NC) * 8u);
+          bulk_commit();
+        }
+      } else if (a.scatter_mode == 1) {
         // rows staged in shared memory, then one bulk reduction per row (its lane issues it); the warp's 32 rows go
         // out as two halves of 16 through the same staging slots: rows 16 h + r (fragment i = 2 h, 2 h + 1) in half h
 #pragma unroll
@@ -374,7 +409,7 @@ k_apply_tc(const __grid_constant__ HMaps tmH, const __grid_constant__ CUtensorMa
         }
       }
     }
-    if (a.scatter_mode == 1) bulk_wait0();                  // every row has been added before the CTA retires
+    if (MAX || a.scatter_mode == 1) bulk_wait0();           // every row has been reduced before the CTA retires
   } else if (warp == kYProducer) {
     // ============================================================== Y GEMM: TMA producer (whole warp, elected lane)
     const int n_blocks = a.NY / kYBlockN;
@@ -539,17 +574,37 @@ k_apply_tc(const __grid_constant__ HMaps tmH, const __grid_constant__ CUtensorMa
   if (threadIdx.x == 0) trace_write(a.trace, 300u, tr0, tr0, a.trace.rec ? gtime() : 0ull);
 }
 
+template <int FMT, int kYBlockN, int NC>
+__global__ void __launch_bounds__(kThreads, 1)
+k_apply_tc(const __grid_constant__ HMaps tmH, const __grid_constant__ CUtensorMap tmY,
+           const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmW, ApplyArgs a) {
+  apply_tc_body<FMT, kYBlockN, NC, false>(tmH, tmY, tmX, tmW, a);
+}
+
+template <int FMT, int kYBlockN, int NC>
+__global__ void __launch_bounds__(kThreads, 1)
+k_apply_tc_max(const __grid_constant__ HMaps tmH, const __grid_constant__ CUtensorMap tmY,
+               const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmW, ApplyArgs a) {
+  apply_tc_body<FMT, kYBlockN, NC, true>(tmH, tmY, tmX, tmW, a);
+}
+
+template <int FMT, int YBN, int NC, bool MAX>
+struct ApplyKernel {
+  static constexpr auto fn = MAX ? k_apply_tc_max<FMT, YBN, NC> : k_apply_tc<FMT, YBN, NC>;
+};
+
 struct ApplyShape {
   int nb_slots, passes, a_stages, x_resident, y_bytes, smem_bytes;
 };
 
 // num_kx: 64-column boxes of the Y GEMM's K (the Xc tile of a 128-source m-block is num_kx * 16 KiB)
-bool apply_shape(int cout, int Kp, int ybn, int num_kx, ApplyShape* as) {
+// staging: the scatter staging is needed whatever scatter_mode says (aggr = max stages its key rows there)
+bool apply_shape(int cout, int Kp, int ybn, int num_kx, ApplyShape* as, bool staging = false) {
   const int w_bytes = ybn * 64 * 2;
   if (cout % 16 != 0 || cout < 16 || cout > 64 || Kp % 64 != 0) return false;
   const int num_kc = Kp / 64;
   const int b_stride = (cout * 128 + 1023) & ~1023;
-  const int bar_bytes = 1024 + kYStagingBytes + (options().scatter_mode == 1 ? kScatterBytes : 0);
+  const int bar_bytes = 1024 + kYStagingBytes + (options().scatter_mode == 1 || staging ? kScatterBytes : 0);
   // fewest passes that leave >= 7 A stages (the h stream needs the bytes in flight), else >= 5, else >= 3; at each
   // level a resident Xc tile (loaded once per m-block instead of once per n-block) first, where it fits
   const int forced = options().apply_passes;
@@ -597,17 +652,17 @@ bool apply_fused_supported(const Weights* W) {
 }
 
 namespace {
-template <int FMT, int YBN, int NC>
+template <int FMT, int YBN, int NC, bool MAX>
 int launch_variant(int grid, int smem_bytes, bool coop, cudaStream_t st, const HMaps& tmH, const CUtensorMap& tmY,
                    const CUtensorMap& tmX, const CUtensorMap& tmW, const ApplyArgs& a) {
   static bool attr_set = false;
   static int blocks_per_sm = -1;
   if (!attr_set) {
-    NNC_CHECK_CUDA(cudaFuncSetAttribute(k_apply_tc<FMT, YBN, NC>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    NNC_CHECK_CUDA(cudaFuncSetAttribute(ApplyKernel<FMT, YBN, NC, MAX>::fn, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     attr_set = true;
   }
   if (blocks_per_sm < 0)
-    NNC_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks_per_sm, k_apply_tc<FMT, YBN, NC>, kThreads,
+    NNC_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks_per_sm, ApplyKernel<FMT, YBN, NC, MAX>::fn, kThreads,
                                                                  smem_bytes));
   NNC_REQUIRE(blocks_per_sm >= 1, NNCONV_ERR_UNSUPPORTED, "apply_tc: the persistent kernel does not fit one SM");
   cudaLaunchConfig_t cfg{};
@@ -625,7 +680,7 @@ int launch_variant(int grid, int smem_bytes, bool coop, cudaStream_t st, const H
   attr[0].val.cooperative = 1;
   cfg.attrs = attr;
   cfg.numAttrs = coop ? 1 : 0;
-  cudaError_t e = cudaLaunchKernelEx(&cfg, k_apply_tc<FMT, YBN, NC>, tmH, tmY, tmX, tmW, a);
+  cudaError_t e = cudaLaunchKernelEx(&cfg, ApplyKernel<FMT, YBN, NC, MAX>::fn, tmH, tmY, tmX, tmW, a);
   if (e == cudaErrorCooperativeLaunchTooLarge) {
     cudaGetLastError();
     return kApplyCannotCoSchedule;   // handled by the application driver (api.cu): per-batch kernels instead
@@ -637,7 +692,7 @@ int launch_variant(int grid, int smem_bytes, bool coop, cudaStream_t st, const H
 
 int launch_apply_tc(int prec, const Plan* P, const Weights* W, const void* h, const void* Xc, void* Yring, int nb,
                     int ring, const float* cvec, const float* xs, int aggr_mean, float* out, int* flags,
-                    int flags_stride, cudaStream_t st, const UnitRange& R) {
+                    int flags_stride, cudaStream_t st, const UnitRange& R, unsigned long long* max_keys) {
   int s = tc_init();
   if (s != NNCONV_OK) return s;
   const Options& opt = options();
@@ -645,7 +700,7 @@ int launch_apply_tc(int prec, const Plan* P, const Weights* W, const void* h, co
   const int split = W->split ? 1 : 0;
   const int ybn = kYBN;
   ApplyShape as;
-  NNC_REQUIRE(apply_shape(W->cout, eff_kp(W), ybn, y_num_kx(W), &as), NNCONV_ERR_UNSUPPORTED,
+  NNC_REQUIRE(apply_shape(W->cout, eff_kp(W), ybn, y_num_kx(W), &as, max_keys != nullptr), NNCONV_ERR_UNSUPPORTED,
               "apply_tc: unsupported shape");
   if (opt.apply_stages >= 2 && opt.apply_stages < as.a_stages) as.a_stages = opt.apply_stages;
   const int64_t e_pad = R.h_rows;
@@ -689,6 +744,8 @@ int launch_apply_tc(int prec, const Plan* P, const Weights* W, const void* h, co
   a.debug_scatter = opt.debug_scatter;   // wrong results, timing only
   a.cntY = flags; a.cntC = flags + flags_stride; a.okY = flags + 2 * flags_stride; a.okC = flags + 3 * flags_stride;
   a.cntU = flags + 4 * flags_stride;
+  a.keys = max_keys;
+  a.perm = P->perm;
   {
     TraceHandle th = trace_get();
     a.trace = TraceBuf{th.rec, th.count, th.cap};
@@ -723,7 +780,10 @@ int launch_apply_tc(int prec, const Plan* P, const Weights* W, const void* h, co
   const int grid = tc_num_sms();
   const bool coop = opt.no_coop == 0;
   auto go = [&](auto fmt, auto nc) -> int {
-    return launch_variant<decltype(fmt)::value, kYBN, decltype(nc)::value>(grid, as.smem_bytes, coop, st,
+    if (max_keys != nullptr)
+      return launch_variant<decltype(fmt)::value, kYBN, decltype(nc)::value, true>(grid, as.smem_bytes, coop, st, tmH, tmY,
+                                                                                  tmX, tmW, a);
+    return launch_variant<decltype(fmt)::value, kYBN, decltype(nc)::value, false>(grid, as.smem_bytes, coop, st,
                                                                                            tmH, tmY, tmX, tmW, a);
   };
   auto by_cout = [&](auto fmt) -> int {

@@ -113,13 +113,21 @@ int gemm_any(const float* A, int64_t sa_m, int64_t sa_k, const float* B, int64_t
 }
 
 // G[p, o] = g[dst[p], o] * inv_deg[dst[p]]          (p local to the batch)
+// MAX (aggr = max): G[p, o] = g[dst[p], o] if argmax[dst[p], o] is the caller index of edge e0 + p, else 0
+template <bool MAX = false>
 __global__ void k_gather_g(const float* __restrict__ gout, const int* __restrict__ dst_sorted,
-                           const float* __restrict__ inv_deg, int e0, int ne, int cout, float* __restrict__ G) {
+                           const float* __restrict__ inv_deg, int e0, int ne, int cout, float* __restrict__ G,
+                           const int* __restrict__ argmax, const int* __restrict__ perm) {
   int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
   if (i >= static_cast<int64_t>(ne) * cout) return;
   const int p = static_cast<int>(i / cout), o = static_cast<int>(i % cout);
   const int d = dst_sorted[e0 + p];
-  G[i] = gout[static_cast<int64_t>(d) * cout + o] * (inv_deg ? inv_deg[d] : 1.f);
+  if constexpr (MAX) {
+    const int64_t k = static_cast<int64_t>(d) * cout + o;
+    G[i] = static_cast<uint32_t>(argmax[k]) == caller_edge(perm, e0 + p) ? gout[k] : 0.f;
+  } else {
+    G[i] = gout[static_cast<int64_t>(d) * cout + o] * (inv_deg ? inv_deg[d] : 1.f);
+  }
 }
 
 // Gs[c, o] = sum over the group's edges of G[p, o]
@@ -273,7 +281,7 @@ size_t backward_ws_bytes(const Plan* P, const Weights* W, size_t want_bytes) {
 
 int backward_fp32(const Plan* P, const Weights* W, const float* edge_attr, const float* x, const float* root,
                   int aggr_mean, const float* gout, float* dx, float* const* dWs, float* const* dbs, float* droot,
-                  float* dbias, void* ws, size_t ws_bytes, cudaStream_t st, float* grad_ea) {
+                  float* dbias, void* ws, size_t ws_bytes, cudaStream_t st, float* grad_ea, const int* argmax) {
   NNC_REQUIRE(W->prec == PREC_FP32, NNCONV_ERR_ARG, "backward needs weights prepared with precision fp32");
   const int nl = W->n_layers;
   const int cin = W->cin, cout = W->cout, Kp = W->Kp, cin_p = W->cin_p;
@@ -358,8 +366,12 @@ int backward_fp32(const Plan* P, const Weights* W, const float* edge_attr, const
                              Y, NY, nb, NY, cin_p, nullptr, st);
       if (s) return s;
       // ---- G, Gs
-      k_gather_g<<<(unsigned)ceil_div64(static_cast<int64_t>(ne) * cout, TB), TB, 0, st>>>(
-          gout, P->dst_sorted, aggr_mean ? P->inv_deg : nullptr, e0, ne, cout, G);
+      if (argmax != nullptr)
+        k_gather_g<true><<<(unsigned)ceil_div64(static_cast<int64_t>(ne) * cout, TB), TB, 0, st>>>(
+            gout, P->dst_sorted, nullptr, e0, ne, cout, G, argmax, P->perm);
+      else
+        k_gather_g<<<(unsigned)ceil_div64(static_cast<int64_t>(ne) * cout, TB), TB, 0, st>>>(
+            gout, P->dst_sorted, aggr_mean ? P->inv_deg : nullptr, e0, ne, cout, G, nullptr, nullptr);
       NNC_CHECK_LAUNCH();
       k_group_sum<<<nb, 64, 0, st>>>(G, P->group_ptr, c0, e0, nb, cout, Gs);
       NNC_CHECK_LAUNCH();

@@ -181,12 +181,14 @@ __global__ void k_colsum(const float* __restrict__ g, int64_t N, int C, float* _
 // G16[t*128 + r, o] = (g[dst, o] * inv_deg[dst]) / gs  for r < cnt_t, zero rows up to 128 (cout == 64)
 // and, in the same pass, Gs[c, o] += sum of the tile's UNSCALED G rows (Gs zero-initialised by the caller)
 // SPLIT (PREC_F16X2, T16 = __half): G16 holds the hi halves, the lo halves follow at row n_tiles*128 (one block per tile)
-template <typename T16, int SPLIT = 0>
+// MAX (aggr = max, inv_deg = nullptr): g[dst, o] only where argmax[dst, o] is the edge's caller index, else 0
+template <typename T16, int SPLIT = 0, bool MAX = false>
 __global__ void __launch_bounds__(256) k_gather_g16(const float* __restrict__ g, const int* __restrict__ dst_sorted,
                                                     const float* __restrict__ inv_deg, const int* __restrict__ tile_c,
                                                     const int* __restrict__ tile_e0,
                                                     const int* __restrict__ tile_cnt, const float* __restrict__ scal,
-                                                    T16* __restrict__ G16, float* __restrict__ Gs) {
+                                                    T16* __restrict__ G16, float* __restrict__ Gs,
+                                                    const int* __restrict__ argmax, const int* __restrict__ perm) {
   __shared__ float s_sum[32][65];
   const int t = blockIdx.x;
   const int e0 = tile_e0[t], cnt = tile_cnt[t];
@@ -200,8 +202,15 @@ __global__ void __launch_bounds__(256) k_gather_g16(const float* __restrict__ g,
       const int d = dst_sorted[e0 + r];
       const float dsc = inv_deg ? inv_deg[d] : 1.f;
       const float sc = dsc * inv_gs;
-      const float4 a = *reinterpret_cast<const float4*>(g + static_cast<int64_t>(d) * 64 + c0);
-      const float4 b = *reinterpret_cast<const float4*>(g + static_cast<int64_t>(d) * 64 + c0 + 4);
+      float4 a = *reinterpret_cast<const float4*>(g + static_cast<int64_t>(d) * 64 + c0);
+      float4 b = *reinterpret_cast<const float4*>(g + static_cast<int64_t>(d) * 64 + c0 + 4);
+      if constexpr (MAX) {
+        const int ce = static_cast<int>(caller_edge(perm, e0 + r));
+        const int4 ma = *reinterpret_cast<const int4*>(argmax + static_cast<int64_t>(d) * 64 + c0);
+        const int4 mb = *reinterpret_cast<const int4*>(argmax + static_cast<int64_t>(d) * 64 + c0 + 4);
+        a = make_float4(ma.x == ce ? a.x : 0.f, ma.y == ce ? a.y : 0.f, ma.z == ce ? a.z : 0.f, ma.w == ce ? a.w : 0.f);
+        b = make_float4(mb.x == ce ? b.x : 0.f, mb.y == ce ? b.y : 0.f, mb.z == ce ? b.z : 0.f, mb.w == ce ? b.w : 0.f);
+      }
       colsum[0] += a.x * dsc; colsum[1] += a.y * dsc; colsum[2] += a.z * dsc; colsum[3] += a.w * dsc;
       colsum[4] += b.x * dsc; colsum[5] += b.y * dsc; colsum[6] += b.z * dsc; colsum[7] += b.w * dsc;
       if (SPLIT) {
@@ -310,13 +319,19 @@ struct GatherGArgs {
   const float* xs[kMaxApps];    // [S] per-source power-of-two scale of the forward's Y operand
   int T;
 };
+// aggr = max: the argmax [N, 64] of every application's forward and the plan's perm (nullable)
+struct GatherMaxArgs {
+  const int* argmax[kMaxApps];
+  const int* perm;
+};
 // SPLIT (PREC_F16X2, T16 = __half): rows of 2 * T * 64, the hi halves in columns [0, T*64), the lo halves after them
-template <typename T16, int SPLIT = 0>
+// MAX (aggr = max, inv_deg = nullptr): application a's g[dst, o] only where its argmax[dst, o] is the edge's caller index
+template <typename T16, int SPLIT = 0, bool MAX = false>
 __global__ void __launch_bounds__(256) k_gather_ghat(GatherGArgs ga, const int* __restrict__ dst_sorted,
                                                      const float* __restrict__ inv_deg, const int* __restrict__ tile_c,
                                                      const int* __restrict__ tile_e0, const int* __restrict__ tile_cnt,
                                                      int tile0, int e_base, const float* __restrict__ scal,
-                                                     T16* __restrict__ Gh) {
+                                                     T16* __restrict__ Gh, GatherMaxArgs gm) {
   const int t = tile0 + blockIdx.x;
   const int e0 = tile_e0[t], cnt = tile_cnt[t], c = tile_c[t];
   const float inv_s = scal[17];
@@ -329,8 +344,16 @@ __global__ void __launch_bounds__(256) k_gather_ghat(GatherGArgs ga, const int* 
       if (r >= cnt) continue;
       const int d = dst_sorted[e0 + r];
       const float sc = (inv_deg ? inv_deg[d] : 1.f) * xsc;
-      const float4 p = *reinterpret_cast<const float4*>(g + static_cast<int64_t>(d) * 64 + c0);
-      const float4 q = *reinterpret_cast<const float4*>(g + static_cast<int64_t>(d) * 64 + c0 + 4);
+      float4 p = *reinterpret_cast<const float4*>(g + static_cast<int64_t>(d) * 64 + c0);
+      float4 q = *reinterpret_cast<const float4*>(g + static_cast<int64_t>(d) * 64 + c0 + 4);
+      if constexpr (MAX) {
+        const int ce = static_cast<int>(caller_edge(gm.perm, e0 + r));
+        const int* am = gm.argmax[a] + static_cast<int64_t>(d) * 64 + c0;
+        const int4 mp = *reinterpret_cast<const int4*>(am);
+        const int4 mq = *reinterpret_cast<const int4*>(am + 4);
+        p = make_float4(mp.x == ce ? p.x : 0.f, mp.y == ce ? p.y : 0.f, mp.z == ce ? p.z : 0.f, mp.w == ce ? p.w : 0.f);
+        q = make_float4(mq.x == ce ? q.x : 0.f, mq.y == ce ? q.y : 0.f, mq.z == ce ? q.z : 0.f, mq.w == ce ? q.w : 0.f);
+      }
       uint32_t w[4], wl[4];
       if (SPLIT) {
         pack2_split(p.x * sc, p.y * sc, w[0], wl[0]); pack2_split(p.z * sc, p.w * sc, w[1], wl[1]);
@@ -904,7 +927,7 @@ size_t backward_apply_ws_bytes(const Plan* P, const Weights* W, size_t want_byte
 int backward_apply_tc(const Plan* P, const Weights* W, const float* edge_attr, const void* h, int64_t E_res,
                       const float* x, const float* root, int aggr_mean, const float* gout, float* dx, float* dWL,
                       float* dbL, float* droot, float* dbias, void* ws, size_t ws_bytes, cudaStream_t st,
-                      int64_t* launches) {
+                      int64_t* launches, const int* argmax) {
   NNC_REQUIRE(backward_tc_supported(W), NNCONV_ERR_UNSUPPORTED, "tensor-core backward: unsupported shape / precision");
   const int cin = W->cin, cout = W->cout, Kp = W->Kp, cin_p = W->cin_p;
   const int64_t N = P->N;
@@ -968,12 +991,21 @@ int backward_apply_tc(const Plan* P, const Weights* W, const float* edge_attr, c
   k_apply_scales<<<1, 1, 0, st>>>(scal);
   NNC_CHECK_LAUNCH();
   NNC_CHECK_CUDA(cudaMemsetAsync(Gs, 0, sizeof(float) * static_cast<size_t>(S) * cout, st));
-  if (sp) k_gather_g16<__half, 1><<<P->n_tiles, 256, 0, st>>>(gout, P->dst_sorted, inv_deg, P->tile_c, P->tile_e0,
-                                                              P->tile_cnt, scal, static_cast<__half*>(G16), Gs);
-  else if (bf) k_gather_g16<__nv_bfloat16><<<P->n_tiles, 256, 0, st>>>(gout, P->dst_sorted, inv_deg, P->tile_c, P->tile_e0,
-                                                                       P->tile_cnt, scal, static_cast<__nv_bfloat16*>(G16), Gs);
-  else k_gather_g16<__half><<<P->n_tiles, 256, 0, st>>>(gout, P->dst_sorted, inv_deg, P->tile_c, P->tile_e0, P->tile_cnt, scal,
-                                                        static_cast<__half*>(G16), Gs);
+  {
+    auto gather = [&](auto t16, auto split, auto mx) {
+      using T16 = decltype(t16);
+      k_gather_g16<T16, decltype(split)::value, decltype(mx)::value><<<P->n_tiles, 256, 0, st>>>(
+          gout, P->dst_sorted, inv_deg, P->tile_c, P->tile_e0, P->tile_cnt, scal, static_cast<T16*>(G16), Gs, argmax,
+          P->perm);
+    };
+    auto by_max = [&](auto t16, auto split) {
+      if (argmax != nullptr) gather(t16, split, std::true_type());
+      else gather(t16, split, std::false_type());
+    };
+    if (sp) by_max(__half(), std::integral_constant<int, 1>());
+    else if (bf) by_max(__nv_bfloat16(), std::integral_constant<int, 0>());
+    else by_max(__half(), std::integral_constant<int, 0>());
+  }
   NNC_CHECK_LAUNCH();
   if (sp) k_prep_xg<__half, 1><<<(unsigned)ceil_div64(static_cast<int64_t>(S) * cin_p, 256), 256, 0, st>>>(
       x, P->src_nodes, S, cin, cin_p, scal, static_cast<__half*>(Xg));
@@ -1158,7 +1190,8 @@ size_t backward_mlp_ws_bytes(const Plan* P, const Weights* W, int T, size_t want
 
 int backward_mlp_tc(const Plan* P, const Weights* W, const float* edge_attr, const void* h, int64_t E_res, int T,
                     const float* const* gouts, const float* const* xs_in, int aggr_mean, float* const* dWs,
-                    float* const* dbs, void* ws, size_t ws_bytes, cudaStream_t st, const void* acts, float* grad_ea) {
+                    float* const* dbs, void* ws, size_t ws_bytes, cudaStream_t st, const void* acts, float* grad_ea,
+                    const int* const* argmax) {
   NNC_REQUIRE(backward_tc_supported(W), NNCONV_ERR_UNSUPPORTED, "tensor-core backward: unsupported shape / precision");
   const bool streamed = E_res < P->E;
   if (streamed || (acts != nullptr && edge_acts_bytes(P, W) == 0)) acts = nullptr;
@@ -1193,6 +1226,10 @@ int backward_mlp_tc(const Plan* P, const Weights* W, const float* edge_attr, con
   NNC_CHECK_CUDA(cudaMemsetAsync(base, 0, L.fixed, st));        // scales and every accumulator
   GatherGArgs ga{};
   ga.T = T;
+  GatherMaxArgs gm{};
+  gm.perm = P->perm;
+  if (argmax != nullptr)
+    for (int t = 0; t < T; ++t) gm.argmax[t] = argmax[t];
   float* cvec = reinterpret_cast<float*>(base + L.off_cvec);
   for (int t = 0; t < T; ++t) {
     void* Xc = base + L.off_Xc[t];
@@ -1307,13 +1344,19 @@ int backward_mlp_tc(const Plan* P, const Weights* W, const float* edge_attr, con
     // ---- Ghat rows of the batch
     {
       const int nt = htp[c1] - htp[c0];
-      if (sp) k_gather_ghat<__half, 1><<<nt, 256, 0, st>>>(ga, P->dst_sorted, inv_deg, P->tile_c, P->tile_e0, P->tile_cnt,
-                                                           htp[c0], e_base, scal, reinterpret_cast<__half*>(Gh));
-      else if (bf) k_gather_ghat<__nv_bfloat16><<<nt, 256, 0, st>>>(ga, P->dst_sorted, inv_deg, P->tile_c, P->tile_e0,
-                                                                     P->tile_cnt, htp[c0], e_base, scal,
-                                                                     reinterpret_cast<__nv_bfloat16*>(Gh));
-      else k_gather_ghat<__half><<<nt, 256, 0, st>>>(ga, P->dst_sorted, inv_deg, P->tile_c, P->tile_e0, P->tile_cnt, htp[c0],
-                                                     e_base, scal, reinterpret_cast<__half*>(Gh));
+      auto gather = [&](auto t16, auto split, auto mx) {
+        using T16 = decltype(t16);
+        k_gather_ghat<T16, decltype(split)::value, decltype(mx)::value><<<nt, 256, 0, st>>>(
+            ga, P->dst_sorted, inv_deg, P->tile_c, P->tile_e0, P->tile_cnt, htp[c0], e_base, scal,
+            reinterpret_cast<T16*>(Gh), gm);
+      };
+      auto by_max = [&](auto t16, auto split) {
+        if (argmax != nullptr) gather(t16, split, std::true_type());
+        else gather(t16, split, std::false_type());
+      };
+      if (sp) by_max(__half(), std::integral_constant<int, 1>());
+      else if (bf) by_max(__nv_bfloat16(), std::integral_constant<int, 0>());
+      else by_max(__half(), std::integral_constant<int, 0>());
       NNC_CHECK_LAUNCH();
     }
     // ---- dz_{L-1} = [h > 0] * (Ghat . Yt)

@@ -77,6 +77,9 @@ struct ConvTcArgs {
   int join_n;
   TraceBuf trace;
   unsigned int trace_seq;
+  // aggr = max (the MAX instantiation only): [N, cout] keys (common.cuh max_key) and the plan's perm (nullable)
+  unsigned long long* keys;
+  const int* perm;
 };
 
 // tmH.m[i] has a box of 16*(i+1) rows: the last tile of a source group only fetches the rows it owns
@@ -98,9 +101,10 @@ __device__ __forceinline__ bool next_unit(const ConvTcArgs& a, int t1, int& t, U
   return true;
 }
 
-template <int FMT, int NC>
-__global__ void __launch_bounds__(kThreads, NC <= 64 ? 2 : 1)
-k_conv_tc(const __grid_constant__ HMaps tmH, const __grid_constant__ CUtensorMap tmY, ConvTcArgs a) {
+// The kernel body, shared by k_conv_tc (aggr add / mean) and k_conv_tc_max.  MAX: aggr = max -- the epilogue reduces
+// one key per (edge row, channel) with red.global.max.u64 into a.keys.
+template <int FMT, int NC, bool MAX>
+__device__ __forceinline__ void conv_tc_body(const HMaps& tmH, const CUtensorMap& tmY, const ConvTcArgs& a) {
   extern __shared__ __align__(1024) uint8_t smem[];
   if ((smem_u32(smem) & 1023u) != 0) __trap();            // SWIZZLE_128B tiles need 1024 B alignment
   const int b_chunk_bytes = NC * 128;                 // [cout rows x 64 k] 16-bit
@@ -235,11 +239,24 @@ k_conv_tc(const __grid_constant__ HMaps tmH, const __grid_constant__ CUtensorMap
       const float* cv = a.cvec + static_cast<int64_t>(un.c) * NC;
       const float xsc = __ldg(a.xs + un.c);
       float* orow = a.out + static_cast<int64_t>(d) * NC;
+      const uint32_t ce = MAX && ok ? caller_edge(a.perm, a.tile_e0[un.t + g] + r) : 0u;
 #pragma unroll
       for (int cc = 0; cc < NC; cc += 16) {
         uint32_t v[16];
         acc_rows<NC, 16>(acc, cc, wb, v);
-        if (ok && !(a.debug & 1)) {
+        if constexpr (MAX) {
+          if (ok) {
+            unsigned long long* krow = a.keys + static_cast<int64_t>(d) * NC + cc;
+#pragma unroll
+            for (int q = 0; q < 4; ++q) {
+              const float4 cq = __ldg(reinterpret_cast<const float4*>(cv + cc) + q);
+              atomicMax(krow + 4 * q + 0, max_key(fmaf(__uint_as_float(v[4 * q + 0]), xsc, cq.x), ce));
+              atomicMax(krow + 4 * q + 1, max_key(fmaf(__uint_as_float(v[4 * q + 1]), xsc, cq.y), ce));
+              atomicMax(krow + 4 * q + 2, max_key(fmaf(__uint_as_float(v[4 * q + 2]), xsc, cq.z), ce));
+              atomicMax(krow + 4 * q + 3, max_key(fmaf(__uint_as_float(v[4 * q + 3]), xsc, cq.w), ce));
+            }
+          }
+        } else if (ok && !(a.debug & 1)) {
 #pragma unroll
           for (int q = 0; q < 4; ++q) {
             const float4 cq = __ldg(reinterpret_cast<const float4*>(cv + cc) + q);
@@ -258,6 +275,18 @@ k_conv_tc(const __grid_constant__ HMaps tmH, const __grid_constant__ CUtensorMap
   if (a.join_ok != nullptr && blockIdx.x == 0 && threadIdx.x == 0) {
     for (int i = 0; i < a.join_n; ++i) flag_wait(a.join_ok + i);
   }
+}
+
+template <int FMT, int NC>
+__global__ void __launch_bounds__(kThreads, NC <= 64 ? 2 : 1)
+k_conv_tc(const __grid_constant__ HMaps tmH, const __grid_constant__ CUtensorMap tmY, ConvTcArgs a) {
+  conv_tc_body<FMT, NC, false>(tmH, tmY, a);
+}
+
+template <int FMT, int NC>
+__global__ void __launch_bounds__(kThreads, NC <= 64 ? 2 : 1)
+k_conv_tc_max(const __grid_constant__ HMaps tmH, const __grid_constant__ CUtensorMap tmY, ConvTcArgs a) {
+  conv_tc_body<FMT, NC, true>(tmH, tmY, a);
 }
 
 struct ConvShape {
@@ -306,7 +335,7 @@ bool tc_shapes_supported(const Weights* W) {
 
 int launch_conv_tc(int prec, const Plan* P, const void* h, int Kp, const void* Y, int64_t y_nodes, int cout,
                    int tile_begin, int tile_end, int c0, const float* cvec, const float* xs, int aggr_mean, float* out,
-                   cudaStream_t st, const PipeFlags* pf, int64_t e_base, int64_t h_rows) {
+                   cudaStream_t st, const PipeFlags* pf, int64_t e_base, int64_t h_rows, unsigned long long* max_keys) {
   if (tile_end <= tile_begin) return NNCONV_OK;
   int s = tc_init();
   if (s != NNCONV_OK) return s;
@@ -344,6 +373,8 @@ int launch_conv_tc(int prec, const Plan* P, const void* h, int Kp, const void* Y
   a.done_ok = pf ? pf->done_ok : nullptr;
   a.join_ok = pf ? pf->join_ok : nullptr;
   a.join_n = pf ? pf->join_n : 0;
+  a.keys = max_keys;
+  a.perm = P->perm;
   const int tiles = tile_end - tile_begin;
   const int max_ctas = tc_num_sms() * cs.ctas_per_sm;
   const int grid = tiles < max_ctas ? tiles : max_ctas;
@@ -357,15 +388,21 @@ int launch_conv_tc(int prec, const Plan* P, const void* h, int Kp, const void* Y
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = (pf && pf->pdl) ? 1 : 0;
-  auto go = [&](auto fmt, auto nc) -> int {
+  auto go_v = [&](auto fmt, auto nc, auto mx) -> int {
     constexpr int F = decltype(fmt)::value, C = decltype(nc)::value;
+    constexpr bool M = decltype(mx)::value;
+    constexpr auto kern = M ? k_conv_tc_max<F, C> : k_conv_tc<F, C>;
     static bool attr_set = false;
     if (!attr_set) {
-      NNC_CHECK_CUDA(cudaFuncSetAttribute(k_conv_tc<F, C>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+      NNC_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
       attr_set = true;
     }
-    NNC_CHECK_CUDA(cudaLaunchKernelEx(&cfg, k_conv_tc<F, C>, tmH, tmY, a));
+    NNC_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kern, tmH, tmY, a));
     return NNCONV_OK;
+  };
+  auto go = [&](auto fmt, auto nc) -> int {
+    if (max_keys != nullptr) return go_v(fmt, nc, std::true_type());
+    return go_v(fmt, nc, std::false_type());
   };
   auto by_cout = [&](auto fmt) -> int {
     switch (cout) {

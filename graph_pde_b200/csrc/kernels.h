@@ -35,11 +35,18 @@ int launch_src_prep(int prec, const float* x, const int* src_nodes, int S, int c
                     const float* B3, void* Xc, float* cvec, float* xs, cudaStream_t st, unsigned node_flags = 0);
 int launch_node_prep(int prec, const float* x, const float* root, const float* bias, int64_t N, float* out,
                      const int* src_nodes, int S, int cin, int cin_p, int cout, const float* B3, void* Xc, float* cvec,
-                     float* xs, int* flags, int flags_stride, int n_batches, cudaStream_t st, unsigned node_flags);
+                     float* xs, int* flags, int flags_stride, int n_batches, cudaStream_t st, unsigned node_flags,
+                     unsigned long long* max_keys = nullptr);
 int launch_sgemm_store(const float* A, int64_t lda, const float* B, int64_t ldb, float* C, int64_t ldc, int M, int N,
                        int K, const float* bias_relu, cudaStream_t st);
 int launch_sgemm_scatter(const Plan* P, const float* h, int Kp, const float* Y, int cout, int tile_begin,
-                         int tile_end, int c0, const float* cvec, int aggr_mean, float* out, cudaStream_t st);
+                         int tile_end, int c0, const float* cvec, int aggr_mean, float* out, cudaStream_t st,
+                         unsigned long long* max_keys = nullptr);
+// aggr = max: max_keys (nullable everywhere above and below) are the [N, cout] keys of common.cuh max_key, which the
+// scatter epilogues reduce instead of adding into out; k_node_prep clears them.  After the last contraction of the
+// application launch_max_finalize adds the decoded max to out (nothing for a key 0) and writes the winning caller
+// edge index (-1 for a node without in-edges) to argmax.
+int launch_max_finalize(const unsigned long long* keys, int64_t n, float* out, int* argmax, cudaStream_t st);
 
 // CTA timeline tracing (NNCONV_TRACE=1; measurement only).  The buffer is the one place where the library
 // allocates device memory itself, and only when tracing is requested.
@@ -96,7 +103,8 @@ struct UnitRange {
 // rows of sorted edges [e_base, e_base + h_rows) (default: every edge)
 int launch_conv_tc(int prec, const Plan* P, const void* h, int Kp, const void* Y, int64_t y_nodes, int cout,
                    int tile_begin, int tile_end, int c0, const float* cvec, const float* xs, int aggr_mean, float* out,
-                   cudaStream_t st, const PipeFlags* pf = nullptr, int64_t e_base = 0, int64_t h_rows = 0);
+                   cudaStream_t st, const PipeFlags* pf = nullptr, int64_t e_base = 0, int64_t h_rows = 0,
+                   unsigned long long* max_keys = nullptr);
 
 // ---- apply_tc.cu: ONE persistent kernel per unit range (Y GEMM + contraction pipelines in every CTA); flags: the
 // range's batches of cntY, cntC, okY, okC, cntU at flags_stride
@@ -104,7 +112,7 @@ constexpr int kApplyCannotCoSchedule = 1000;   // private status of launch_apply
 bool apply_fused_supported(const Weights* W);
 int launch_apply_tc(int prec, const Plan* P, const Weights* W, const void* h, const void* Xc, void* Yring, int nb,
                     int ring, const float* cvec, const float* xs, int aggr_mean, float* out, int* flags,
-                    int flags_stride, cudaStream_t st, const UnitRange& R);
+                    int flags_stride, cudaStream_t st, const UnitRange& R, unsigned long long* max_keys = nullptr);
 
 // ---- graph_build.cu: ball graph (count / fill) on the device
 int ball_count(const double* pa, int64_t na, const double* pb, int64_t nb, double radius, int* counts, cudaStream_t st);

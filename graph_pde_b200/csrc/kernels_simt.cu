@@ -397,12 +397,13 @@ __global__ void k_src_prep(const float* __restrict__ x, const int* __restrict__ 
 // application (cntY / cntC / okY / okC / cntU [n_batches] at stride flags_stride; a grid-stride loop, because the
 // batches of many streamed chunks are not bounded by the source count that sizes the grid) -- in the launch-bound
 // MGKN regime (52 dependent applications per forward) every launch removed from the chain counts.
-template <typename T, int SPLIT = 0>
+// MAX (aggr = max): the same grid also clears the [N, cout] keys the scatter epilogues reduce into.
+template <typename T, int SPLIT = 0, bool MAX = false>
 __global__ void k_node_prep(const float* __restrict__ x, const float* __restrict__ root, const float* __restrict__ bias,
                             int64_t N, float* __restrict__ out, int g_out, const int* __restrict__ src_nodes, int S, int cin,
                             int cin_p, int cout, const float* __restrict__ B3, T* __restrict__ Xc, float* __restrict__ cvec,
                             float* __restrict__ xs, int* __restrict__ flags, int flags_stride, int n_batches,
-                            unsigned node_flags) {
+                            unsigned node_flags, unsigned long long* __restrict__ keys) {
   extern __shared__ float sx[];
   const int tid = threadIdx.y * blockDim.x + threadIdx.x;
   const int64_t gid = static_cast<int64_t>(blockIdx.x) * (blockDim.x * blockDim.y) + tid;
@@ -410,6 +411,9 @@ __global__ void k_node_prep(const float* __restrict__ x, const float* __restrict
   for (int64_t i = gid; i < n_batches; i += n_threads) {
 #pragma unroll
     for (int j = 0; j < 5; ++j) flags[j * flags_stride + i] = 0;
+  }
+  if constexpr (MAX) {
+    for (int64_t i = gid; i < N * cout; i += n_threads) keys[i] = 0ull;
   }
   if (static_cast<int>(blockIdx.x) < g_out)
     out_init_rows(x, root, bias, N, cin, cout, out, node_flags, blockIdx.x, sx);
@@ -421,7 +425,7 @@ __global__ void k_node_prep(const float* __restrict__ x, const float* __restrict
 // ------------------------------------------------------------------------------------------------
 // fp32 NT GEMM, 64x64x16 tiles, 256 threads, 4x4 register blocking.   C = A[M,K] * B[N,K]^T
 // ------------------------------------------------------------------------------------------------
-enum { EPI_STORE = 0, EPI_BIAS_RELU = 1, EPI_SCATTER = 2 };
+enum { EPI_STORE = 0, EPI_BIAS_RELU = 1, EPI_SCATTER = 2, EPI_SCATTER_MAX = 3 };
 
 struct SgemmArgs {
   const float* A;
@@ -437,6 +441,9 @@ struct SgemmArgs {
   const float *inv_deg, *cvec;
   int tile_begin, c0;
   int64_t y_stride;    // elements between consecutive sources in Y
+  // EPI_SCATTER_MAX (aggr = max): the rows reduce keys (common.cuh max_key) into keys [N, ldc] instead of adding to C
+  unsigned long long* keys;
+  const int* perm;
 };
 
 template <int EPI>
@@ -450,7 +457,7 @@ __global__ void __launch_bounds__(256) k_sgemm_nt(SgemmArgs a) {
   int n0 = blockIdx.y * 64;
   int c = 0, e0 = 0;
   int m_base = 0;
-  if (EPI == EPI_SCATTER) {
+  if (EPI == EPI_SCATTER || EPI == EPI_SCATTER_MAX) {
     int t = a.tile_begin + blockIdx.x / 2;
     c = a.tile_c[t];
     e0 = a.tile_e0[t];
@@ -489,7 +496,17 @@ __global__ void __launch_bounds__(256) k_sgemm_nt(SgemmArgs a) {
   for (int i = 0; i < 4; ++i) {
     int gm = m_base + ty * 4 + i;
     if (gm >= M) continue;
-    if (EPI == EPI_SCATTER) {
+    if (EPI == EPI_SCATTER_MAX) {
+      const int d = a.dst_sorted[e0 + gm];
+      const uint32_t ce = caller_edge(a.perm, e0 + gm);
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const int gn = n0 + tx * 4 + j;
+        if (gn < a.N)
+          atomicMax(&a.keys[static_cast<int64_t>(d) * a.ldc + gn],
+                    max_key(acc[i][j] + a.cvec[static_cast<int64_t>(c) * a.N + gn], ce));
+      }
+    } else if (EPI == EPI_SCATTER) {
       int d = a.dst_sorted[e0 + gm];
       float sc = a.inv_deg ? a.inv_deg[d] : 1.f;
 #pragma unroll
@@ -901,22 +918,29 @@ int launch_src_prep(int prec, const float* x, const int* src_nodes, int S, int c
 // out_init + src_prep + the flag reset of one application as ONE launch (16-bit precisions)
 int launch_node_prep(int prec, const float* x, const float* root, const float* bias, int64_t N, float* out,
                      const int* src_nodes, int S, int cin, int cin_p, int cout, const float* B3, void* Xc, float* cvec,
-                     float* xs, int* flags, int flags_stride, int n_batches, cudaStream_t st, unsigned node_flags) {
+                     float* xs, int* flags, int flags_stride, int n_batches, cudaStream_t st, unsigned node_flags,
+                     unsigned long long* max_keys) {
   dim3 b(64, 4);
   const int g_out = static_cast<int>(ceil_div64(N, b.y));
   const int g_src = ceil_div(S, (int)b.y);
   const unsigned g = static_cast<unsigned>(g_out + g_src);
   size_t sm = sizeof(float) * b.y * cin;
+  auto go = [&](auto t, auto split, auto mx) {
+    using T = decltype(t);
+    k_node_prep<T, decltype(split)::value, decltype(mx)::value><<<g, b, sm, st>>>(
+        x, root, bias, N, out, g_out, src_nodes, S, cin, cin_p, cout, B3, static_cast<T*>(Xc), cvec, xs, flags,
+        flags_stride, n_batches, node_flags, max_keys);
+  };
+  auto by_max = [&](auto t, auto split) {
+    if (max_keys != nullptr) go(t, split, std::true_type());
+    else go(t, split, std::false_type());
+  };
   if (prec == PREC_F16)
-    k_node_prep<__half><<<g, b, sm, st>>>(x, root, bias, N, out, g_out, src_nodes, S, cin, cin_p, cout, B3,
-                                          static_cast<__half*>(Xc), cvec, xs, flags, flags_stride, n_batches, node_flags);
+    by_max(__half(), std::integral_constant<int, 0>());
   else if (prec == PREC_F16X2)
-    k_node_prep<__half, 1><<<g, b, sm, st>>>(x, root, bias, N, out, g_out, src_nodes, S, cin, cin_p, cout, B3,
-                                             static_cast<__half*>(Xc), cvec, xs, flags, flags_stride, n_batches, node_flags);
+    by_max(__half(), std::integral_constant<int, 1>());
   else if (prec == PREC_BF16)
-    k_node_prep<__nv_bfloat16><<<g, b, sm, st>>>(x, root, bias, N, out, g_out, src_nodes, S, cin, cin_p, cout, B3,
-                                                 static_cast<__nv_bfloat16*>(Xc), cvec, xs, flags, flags_stride, n_batches,
-                                                 node_flags);
+    by_max(__nv_bfloat16(), std::integral_constant<int, 0>());
   else
     return NNCONV_ERR_UNSUPPORTED;
   NNC_CHECK_LAUNCH();
@@ -982,7 +1006,8 @@ int launch_sgemm_store(const float* A, int64_t lda, const float* B, int64_t ldb,
 }
 
 int launch_sgemm_scatter(const Plan* P, const float* h, int Kp, const float* Y, int cout, int tile_begin, int tile_end,
-                         int c0, const float* cvec, int aggr_mean, float* out, cudaStream_t st) {
+                         int c0, const float* cvec, int aggr_mean, float* out, cudaStream_t st,
+                         unsigned long long* max_keys) {
   int nt = tile_end - tile_begin;
   if (nt <= 0) return NNCONV_OK;
   SgemmArgs a{};
@@ -990,8 +1015,36 @@ int launch_sgemm_scatter(const Plan* P, const float* h, int Kp, const float* Y, 
   a.tile_c = P->tile_c; a.tile_e0 = P->tile_e0; a.tile_cnt = P->tile_cnt; a.dst_sorted = P->dst_sorted;
   a.inv_deg = aggr_mean ? P->inv_deg : nullptr; a.cvec = cvec; a.tile_begin = tile_begin; a.c0 = c0;
   a.y_stride = static_cast<int64_t>(cout) * Kp;
+  a.keys = max_keys; a.perm = P->perm;
   dim3 g(nt * 2, ceil_div(cout, 64));
-  k_sgemm_nt<EPI_SCATTER><<<g, 256, 0, st>>>(a);
+  if (max_keys != nullptr) k_sgemm_nt<EPI_SCATTER_MAX><<<g, 256, 0, st>>>(a);
+  else k_sgemm_nt<EPI_SCATTER><<<g, 256, 0, st>>>(a);
+  NNC_CHECK_LAUNCH();
+  return NNCONV_OK;
+}
+
+// aggr = max, after the last contraction of an application: out += the max the key encodes (nothing for key 0, the
+// empty neighbourhood), argmax = the winning caller edge index (-1 when empty)
+__global__ void k_max_finalize(const unsigned long long* __restrict__ keys, int64_t n, float* __restrict__ out,
+                               int* __restrict__ argmax) {
+  for (int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; i < n;
+       i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+    const unsigned long long k = keys[i];
+    if (k == 0ull) {
+      argmax[i] = -1;
+      continue;
+    }
+    const uint32_t hi = static_cast<uint32_t>(k >> 32);
+    const uint32_t u = (hi & 0x80000000u) ? (hi ^ 0x80000000u) : ~hi;
+    out[i] += __uint_as_float(u);
+    argmax[i] = static_cast<int>(0xFFFFFFFFu - static_cast<uint32_t>(k));
+  }
+}
+
+int launch_max_finalize(const unsigned long long* keys, int64_t n, float* out, int* argmax, cudaStream_t st) {
+  if (n <= 0) return NNCONV_OK;
+  const int64_t blocks = ceil_div64(n, 256);
+  k_max_finalize<<<static_cast<unsigned>(blocks < 4096 ? blocks : 4096), 256, 0, st>>>(keys, n, out, argmax);
   NNC_CHECK_LAUNCH();
   return NNCONV_OK;
 }

@@ -110,7 +110,14 @@ size_t ef_row_bytes(const Weights* W);
 size_t h_row_bytes(const Weights* W);      // bytes of one edge's cached h (16-bit: Kp * 2, twice that at f16x2)
 int apply_streamed(const Plan* P, const Weights* W, const float* edge_attr, const void* h_res, int64_t E_res,
                    const float* x, const float* root, const float* bias, int aggr_mean, float* out, void* ws,
-                   size_t ws_bytes, cudaStream_t st, int64_t* launches, unsigned node_flags);
+                   size_t ws_bytes, cudaStream_t st, int64_t* launches, unsigned node_flags,
+                   unsigned long long* max_keys = nullptr, int* argmax = nullptr);
+// aggr = max (DESIGN 5): the application of h_res / E_res (E_res = E: a whole h, else apply_streamed's chunks) with
+// ws = [max_keys_bytes(N, cout) of keys | the add / mean workspace]; writes out and argmax [N, cout] (caller edge
+// indices, -1 for a node without in-edges)
+int apply_max(const Plan* P, const Weights* W, const float* edge_attr, const void* h_res, int64_t E_res, const float* x,
+              const float* root, const float* bias, float* out, int* argmax, void* ws, size_t ws_bytes, cudaStream_t st,
+              int64_t* launches, unsigned node_flags);
 
 // tensor-core backward (backward_tc.cu): per application (dx, dW_L, db_L, droot, dbias) and, once per
 // (edge_attr, parameters) for all T applications of a shared conv, the pass through the hidden layers.
@@ -124,12 +131,12 @@ size_t backward_apply_ws_bytes(const Plan* P, const Weights* W, size_t want_byte
 int backward_apply_tc(const Plan* P, const Weights* W, const float* edge_attr, const void* h, int64_t E_res,
                       const float* x, const float* root, int aggr_mean, const float* gout, float* dx, float* dWL,
                       float* dbL, float* droot, float* dbias, void* ws, size_t ws_bytes, cudaStream_t st,
-                      int64_t* launches = nullptr);
+                      int64_t* launches = nullptr, const int* argmax = nullptr);
 size_t backward_mlp_ws_bytes(const Plan* P, const Weights* W, int T, size_t want_bytes, int64_t E_res = -1);
 int backward_mlp_tc(const Plan* P, const Weights* W, const float* edge_attr, const void* h, int64_t E_res, int T,
                     const float* const* gouts, const float* const* xs_in, int aggr_mean, float* const* dWs,
                     float* const* dbs, void* ws, size_t ws_bytes, cudaStream_t st, const void* acts = nullptr,
-                    float* grad_ea = nullptr);
+                    float* grad_ea = nullptr, const int* const* argmax = nullptr);
 // source batches whose edge features the call with this workspace recomputes (T = 0: backward_apply_tc)
 int64_t backward_streamed_chunks(const Plan* P, const Weights* W, int T, int64_t E_res, size_t ws_bytes);
 
@@ -140,10 +147,13 @@ int edge_kernels(const Plan* P, const Weights* W, const void* h, void* Kmat, cud
 int apply_edge(const Plan* P, const Weights* W, const void* Kmat, const float* x, const float* root, const float* bias,
                int aggr_mean, float* out, cudaStream_t st, unsigned node_flags = 0);
 
-// backward of one application (fp32 CUDA-core path), backward.cu; grad_ea as for backward_mlp_tc
+// backward of one application (fp32 CUDA-core path), backward.cu; grad_ea as for backward_mlp_tc.
+// aggr = max (all three backward calls): argmax [N, cout] of the forward (backward_mlp_tc: one per application) routes
+// each g[n, o] to the winning edge only, G_e[o] = g[dst_e, o] if argmax[dst_e, o] == caller index of e, else 0
 size_t backward_ws_bytes(const Plan* P, const Weights* W, size_t want_bytes);
 int backward_fp32(const Plan* P, const Weights* W, const float* edge_attr, const float* x, const float* root,
                   int aggr_mean, const float* gout, float* dx, float* const* dWs, float* const* dbs, float* droot,
-                  float* dbias, void* ws, size_t ws_bytes, cudaStream_t st, float* grad_ea = nullptr);
+                  float* dbias, void* ws, size_t ws_bytes, cudaStream_t st, float* grad_ea = nullptr,
+                  const int* argmax = nullptr);
 
 }  // namespace nnc

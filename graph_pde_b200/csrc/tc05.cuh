@@ -270,6 +270,11 @@ __device__ __forceinline__ void bulk_reduce_add_f32(float* gdst, uint32_t smem_s
                ::"l"(gdst), "r"(smem_src), "r"(bytes)
                : "memory");
 }
+__device__ __forceinline__ void bulk_reduce_max_u64(unsigned long long* gdst, uint32_t smem_src, uint32_t bytes) {
+  asm volatile("cp.reduce.async.bulk.global.shared::cta.bulk_group.max.u64 [%0], [%1], %2;"
+               ::"l"(gdst), "r"(smem_src), "r"(bytes)
+               : "memory");
+}
 
 // 32 bytes (one full sector) per thread as two 16-byte stores
 __device__ __forceinline__ void st_global_32b(void* addr, const uint32_t* v) {

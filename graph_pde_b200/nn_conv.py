@@ -283,13 +283,15 @@ class _NNConvFunction(torch.autograd.Function):
         ctx.module = module
         ctx.edge_index = edge_index
         ctx.save_for_backward(x, edge_attr)
-        return module._forward_impl(x, edge_index, edge_attr, for_grad=True)
+        out, ctx.argmax = module._forward_impl(x, edge_index, edge_attr, for_grad=True, with_argmax=True)
+        return out
 
     @staticmethod
     def backward(ctx, grad_out):
         module = ctx.module
         x, edge_attr = ctx.saved_tensors
-        grads = module._backward_impl(x, ctx.edge_index, edge_attr, grad_out, want_ea=ctx.needs_input_grad[3])
+        grads = module._backward_impl(x, ctx.edge_index, edge_attr, grad_out, want_ea=ctx.needs_input_grad[3],
+                                      argmax=ctx.argmax)
         # order of *params in forward(): list(module.parameters())
         by_id = {id(p): g for p, g in grads['params']}
         return (None, grads['x'] if ctx.needs_input_grad[1] else None, None, grads.get('edge_attr')) + tuple(
@@ -299,7 +301,8 @@ class _NNConvFunction(torch.autograd.Function):
 class _TrainState(object):
     """What the tensor-core backward shares between the applications of one conv on one (edge_attr, parameters):
     the plan, the prepared weights, the cached edge features (an _EdgeFeatures) and, filled during the backward sweep,
-    every application's (grad_out, x) for the ONE deferred pass through the hidden layers."""
+    every application's (grad_out, x, argmax) for the ONE deferred pass through the hidden layers (argmax: the
+    forward's winning edges under aggr='max', else None)."""
 
     def __init__(self, key, plan, prepared, ef):
         self.key, self.plan, self.prepared, self.ef = key, plan, prepared, ef
@@ -345,15 +348,16 @@ class _ApplyFn(torch.autograd.Function):
         x32 = _f32(x)
         ctx.save_for_backward(x32)
         ctx.x_dtype = x.dtype
-        return module._apply_impl(state.plan, state.prepared, state.ef, x32)
+        out, ctx.argmax = module._apply_impl(state.plan, state.prepared, state.ef, x32)
+        return out
 
     @staticmethod
     def backward(ctx, grad_out):
         (x32,) = ctx.saved_tensors
         module, state = ctx.module, ctx.state
         g32 = _f32(grad_out)
-        dx, dwl, dbl, droot, dbias = module._backward_apply_impl(state, x32, g32)
-        state.apps.append((g32, x32))
+        dx, dwl, dbl, droot, dbias = module._backward_apply_impl(state, x32, g32, ctx.argmax)
+        state.apps.append((g32, x32, ctx.argmax))
         return (None, None, dx.to(ctx.x_dtype) if ctx.needs_input_grad[2] else None, torch.zeros_like(state.token),
                 dwl, dbl, droot, dbias)
 
@@ -362,7 +366,9 @@ class NNConv_old(torch.nn.Module):
     r"""Edge-conditioned convolution  x'_i = Theta x_i + aggr_{j in N(i)} x_j . h_Theta(e_ij)
     (reference docstring: graph-neural-operator/nn_conv.py:198-232).
 
-    Args are the reference's (nn_conv.py:234-241).  Extra keyword ``precision`` in
+    Args are the reference's (nn_conv.py:234-241).  ``aggr`` in {'add', 'mean', 'max'}: 'max' takes the per-channel max
+    of the messages (ties: the smallest index in the caller's edge_index; a node without in-edges gets 0) and sends each
+    gradient entry to the winning edge only (DESIGN 5); it always runs formulation C.  Extra keyword ``precision`` in
     {'f16' (default), 'bf16', 'f16x2', 'fp32'} selects the tensor-core operand type: 'f16x2' carries every
     operand as an fp16 (hi, lo) pair -- fp32-grade results (tolerance 2e-5) on the tensor cores at ~2.4x the
     time of 'f16'; 'fp32' = CUDA-core path for arbitrary shapes.  ``flow`` is PyG's MessagePassing kwarg.
@@ -661,8 +667,6 @@ class NNConv_old(torch.nn.Module):
         _require_cuda(x, 'x')
         _require_cuda(edge_index, 'edge_index')
         _require_cuda(pseudo, 'edge_attr')
-        if self.aggr == 'max':
-            raise NotImplementedError("aggr='max' is used by no call site of the reference and is not built")
         if edge_index.dtype != torch.int64 or edge_index.dim() != 2 or edge_index.size(0) != 2:
             raise ValueError('edge_index must be an int64 tensor of shape [2, E]')
         if x.size(1) != self.in_channels:
@@ -680,8 +684,8 @@ class NNConv_old(torch.nn.Module):
         return plan, prepared, ea32, ef
 
     def _wants_edge_kernels(self, plan, prepared):
-        """The graph-shape policy of formulation B (see _edge_kernels)."""
-        if _EDGE_KERNELS == 'off' or prepared.precision not in ('f16', 'fp16', 'bf16') or plan.E == 0:
+        """The graph-shape policy of formulation B (see _edge_kernels).  aggr='max' always runs formulation C."""
+        if self.aggr == 'max' or _EDGE_KERNELS == 'off' or prepared.precision not in ('f16', 'fp16', 'bf16') or plan.E == 0:
             return False
         return _EDGE_KERNELS == 'on' or ((plan.E <= _EDGE_KERNELS_MAX_DEG * max(plan.n_src, 1) or
                                           plan.E <= _EDGE_KERNELS_MAX_EDGES) and
@@ -718,19 +722,35 @@ class NNConv_old(torch.nn.Module):
         """One application: on the per-edge kernel matrices (formulation B, nnconv_apply_edge_ex), else on the whole h
         (nnconv_apply_ex), else on the resident prefix with the other edges' h recomputed in chunks
         (nnconv_apply_streamed: no allocation inside the library and, besides the optional overflow check, no host
-        sync -- capturable by capture.GraphedForward)."""
+        sync -- capturable by capture.GraphedForward).  aggr='max' takes nnconv_apply_max for either residency.
+        Returns (out, argmax): argmax [N, out] int32 holds the winning caller edge of every (node, channel) under
+        aggr='max' (-1: no in-edge), else None."""
         L = _lib.lib()
         dev = x32.device
         kmat = self._edge_kernels(plan, prepared, ef)
+        keys_b = 0
         if kmat is None:
             ws_b = ctypes.c_size_t(ef.ws_bytes)         # a prefix: the size nnconv_stream_split gave it
             if not ef.streamed:
                 _lib.check(L.nnconv_apply_sizes(plan.handle, prepared.handle, _Y_BYTES, ctypes.byref(ws_b)))
+            if self.aggr == 'max':                      # the keys of the max precede the add / mean workspace
+                max_b = ctypes.c_size_t()
+                _lib.check(L.nnconv_apply_max_sizes(plan.handle, prepared.handle, ws_b.value, ctypes.byref(max_b)))
+                keys_b = max_b.value - ws_b.value
+                ws_b = max_b
             ws = torch.empty(ws_b.value, dtype=torch.uint8, device=dev)
         out = torch.empty(x32.size(0), self.out_channels, dtype=torch.float32, device=dev)
         root, bias = _f32(self.root), _f32(self.bias)
         aggr = _lib.AGGR[self.aggr]
-        if kmat is not None:
+        argmax = None
+        if self.aggr == 'max':
+            argmax = torch.empty(x32.size(0), self.out_channels, dtype=torch.int32, device=dev)
+            n_l = ctypes.c_int64(0)
+            _lib.check(L.nnconv_apply_max(plan.handle, prepared.handle, _ptr(ef.ea32), _ptr(ef.h), ef.E_res, _ptr(x32),
+                                          _ptr(root), _ptr(bias), flags, _ptr(out), _ptr(argmax), _ptr(ws), ws.numel(),
+                                          _stream_ptr(dev), ctypes.byref(n_l)))
+            stats['launches'] += n_l.value
+        elif kmat is not None:
             _lib.check(L.nnconv_apply_edge_ex(plan.handle, prepared.handle, _ptr(kmat), _ptr(x32), _ptr(root), _ptr(bias),
                                               aggr, flags, _ptr(out), _stream_ptr(dev)))
             stats['launches'] += 2
@@ -748,15 +768,17 @@ class NNConv_old(torch.nn.Module):
         stats['applies'] += 1
         if ef.n_chunks:
             stats['streamed_chunk_passes'] += ef.n_chunks
-            self._check_overflow(prepared, ws, dev)
-        return out
+            self._check_overflow(prepared, ws[keys_b:], dev)    # its first word: fp16 overflows of the chunks
+        return out, argmax
 
-    def _forward_impl(self, x, edge_index, pseudo, flags=0, for_grad=False):
+    def _forward_impl(self, x, edge_index, pseudo, flags=0, for_grad=False, with_argmax=False):
+        """One application on the cached edge features; with_argmax: returns (out, argmax) (see _apply_impl)."""
         self._check_inputs(x, edge_index, pseudo)
         with torch.cuda.device(x.device):
             x32 = _f32(x)
             plan, prepared, _, ef = self._prepare(x32, edge_index, pseudo, for_grad=for_grad)
-            return self._apply_impl(plan, prepared, ef, x32, flags)
+            out, argmax = self._apply_impl(plan, prepared, ef, x32, flags)
+            return (out, argmax) if with_argmax else out
 
     def residual_step(self, z, edge_index, edge_attr, relu_in=True):
         """One V-cycle step ``x <- relu(x + conv(x))`` (multipole-graph-neural-operator/neurips1_MGKN.py:76,81,84) on
@@ -800,9 +822,10 @@ class NNConv_old(torch.nn.Module):
                 self._tstate = st
             return st
 
-    def _backward_apply_impl(self, state, x32, g32):
+    def _backward_apply_impl(self, state, x32, g32, argmax=None):
         """Tensor-core backward of one application over the resident rows [0, E_res) of h; the other edges' h is
-        recomputed per source batch.  With E_res = E this is the call nnconv_backward_apply makes."""
+        recomputed per source batch.  With E_res = E this is the call nnconv_backward_apply makes.  argmax: the
+        forward's, under aggr='max' (nnconv_backward_apply_max routes every gradient to its winning edge)."""
         L = _lib.lib()
         dev = x32.device
         plan, prep, ef = state.plan, state.prepared, state.ef
@@ -821,10 +844,17 @@ class NNConv_old(torch.nn.Module):
                                                                   _EF_WS_BYTES, ctypes.byref(b)))
                 ws = torch.empty(b.value, dtype=torch.uint8, device=dev)
             n_l = ctypes.c_int64(0)
-            _lib.check(L.nnconv_backward_apply_streamed(plan.handle, prep.handle, _ptr(ef.ea32), _ptr(ef.h), ef.E_res,
-                                                        _ptr(x32), _ptr(root), _lib.AGGR[self.aggr], _ptr(g32), _ptr(dx),
-                                                        _ptr(dwl), _ptr(dbl), _ptr(droot), _ptr(dbias), _ptr(ws),
-                                                        ws.numel(), _stream_ptr(dev), ctypes.byref(n_l)))
+            if self.aggr == 'max':
+                _lib.check(L.nnconv_backward_apply_max(plan.handle, prep.handle, _ptr(ef.ea32), _ptr(ef.h), ef.E_res,
+                                                       _ptr(x32), _ptr(root), _ptr(argmax), _ptr(g32), _ptr(dx), _ptr(dwl),
+                                                       _ptr(dbl), _ptr(droot), _ptr(dbias), _ptr(ws), ws.numel(),
+                                                       _stream_ptr(dev), ctypes.byref(n_l)))
+            else:
+                _lib.check(L.nnconv_backward_apply_streamed(plan.handle, prep.handle, _ptr(ef.ea32), _ptr(ef.h),
+                                                            ef.E_res, _ptr(x32), _ptr(root), _lib.AGGR[self.aggr],
+                                                            _ptr(g32), _ptr(dx), _ptr(dwl), _ptr(dbl), _ptr(droot),
+                                                            _ptr(dbias), _ptr(ws), ws.numel(), _stream_ptr(dev),
+                                                            ctypes.byref(n_l)))
             stats['launches'] += n_l.value
             if ef.streamed:
                 stats['streamed_backward_chunk_passes'] += _streamed_chunks(plan, prep, ef.E_res, 0, ws.numel())
@@ -854,11 +884,17 @@ class NNConv_old(torch.nn.Module):
                 dws = [torch.empty_like(l.weight, dtype=torch.float32) for l in hidden]
                 dbs = [torch.empty_like(l.bias, dtype=torch.float32) for l in hidden]
                 gea = torch.empty(ef.ea32.shape, dtype=torch.float32, device=dev) if want_ea else None
-                gp = (ctypes.c_void_p * n)(*[g.data_ptr() for g, _ in apps])
-                xp = (ctypes.c_void_p * n)(*[x.data_ptr() for _, x in apps])
+                gp = (ctypes.c_void_p * n)(*[g.data_ptr() for g, _, _ in apps])
+                xp = (ctypes.c_void_p * n)(*[x.data_ptr() for _, x, _ in apps])
                 wp = (ctypes.c_void_p * len(hidden))(*[t.data_ptr() for t in dws])
                 bp = (ctypes.c_void_p * len(hidden))(*[t.data_ptr() for t in dbs])
-                if ef.acts is not None:
+                if self.aggr == 'max':
+                    # every application routed by its own forward's argmax
+                    ap = (ctypes.c_void_p * n)(*[am.data_ptr() for _, _, am in apps])
+                    _lib.check(L.nnconv_backward_mlp_max(plan.handle, prep.handle, _ptr(ef.ea32), _ptr(ef.h), ef.E_res, n,
+                                                         gp, xp, ap, wp, bp, _ptr(ws), ws.numel(), _stream_ptr(dev),
+                                                         _ptr(ef.acts), _ptr(gea)))
+                elif ef.acts is not None:
                     _lib.check(L.nnconv_backward_mlp_ex(plan.handle, prep.handle, _ptr(ef.ea32), _ptr(ef.h), n, gp, xp,
                                                         _lib.AGGR[self.aggr], wp, bp, _ptr(ws), ws.numel(),
                                                         _stream_ptr(dev), _ptr(ef.acts), _ptr(gea)))
@@ -879,9 +915,10 @@ class NNConv_old(torch.nn.Module):
                 gea_total = torch.zeros(ef.ea32.shape, dtype=torch.float32, device=dev)
         return total, gea_total
 
-    def _backward_impl(self, x, edge_index, pseudo, grad_out, want_ea=False):
+    def _backward_impl(self, x, edge_index, pseudo, grad_out, want_ea=False, argmax=None):
         """fp32 CUDA-core backward of one application; with ``want_ea`` also the gradient w.r.t. edge_attr
-        (returned under 'edge_attr' in pseudo's dtype)."""
+        (returned under 'edge_attr' in pseudo's dtype).  argmax: the forward's, under aggr='max' (whatever precision
+        that forward ran at, the gradients follow its winning edges)."""
         L = _lib.lib()
         with torch.cuda.device(x.device):
             x32 = _f32(x)
@@ -904,9 +941,14 @@ class NNConv_old(torch.nn.Module):
             bp = (ctypes.c_void_p * nl)(*[t.data_ptr() for t in dbs])
             root = _f32(self.root)
             gea = torch.empty_like(ea32) if want_ea else None
-            _lib.check(L.nnconv_backward_ex(plan.handle, prep.handle, _ptr(ea32), _ptr(x32), _ptr(root),
-                                            _lib.AGGR[self.aggr], _ptr(g32), _ptr(dx), wp, bp, _ptr(droot), _ptr(dbias),
-                                            _ptr(ws), ws_b.value, _stream_ptr(x.device), _ptr(gea)))
+            if self.aggr == 'max':
+                _lib.check(L.nnconv_backward_max(plan.handle, prep.handle, _ptr(ea32), _ptr(x32), _ptr(root), _ptr(argmax),
+                                                 _ptr(g32), _ptr(dx), wp, bp, _ptr(droot), _ptr(dbias), _ptr(ws),
+                                                 ws_b.value, _stream_ptr(x.device), _ptr(gea)))
+            else:
+                _lib.check(L.nnconv_backward_ex(plan.handle, prep.handle, _ptr(ea32), _ptr(x32), _ptr(root),
+                                                _lib.AGGR[self.aggr], _ptr(g32), _ptr(dx), wp, bp, _ptr(droot),
+                                                _ptr(dbias), _ptr(ws), ws_b.value, _stream_ptr(x.device), _ptr(gea)))
             stats['backwards'] += 1
         params = [(l.weight, dw) for l, dw in zip(linears, dws)] + [(l.bias, db) for l, db in zip(linears, dbs)]
         if self.root is not None:

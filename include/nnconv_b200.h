@@ -59,6 +59,9 @@ extern "C" {
 
 #define NNCONV_AGGR_ADD 0
 #define NNCONV_AGGR_MEAN 1
+/* per node and channel the largest message (ties: the smallest caller edge index), through the *_max entry points
+ * below only; the others refuse it */
+#define NNCONV_AGGR_MAX 2
 
 #define NNCONV_FLOW_SOURCE_TO_TARGET 0
 #define NNCONV_FLOW_TARGET_TO_SOURCE 1
@@ -259,6 +262,40 @@ int nnconv_backward_mlp_streamed(const nnconv_plan_t* plan, const nnconv_weights
                                  size_t ws_bytes, void* stream, float* grad_edge_attr /* nullable */);
 int nnconv_backward_streamed_chunks(const nnconv_plan_t* plan, const nnconv_weights_t* w, int64_t E_res, int n_apps,
                                     size_t ws_bytes, int64_t* n_chunks);
+
+/* ---- aggr = max (NNCONV_AGGR_MAX, formulation C only):
+ *   out[n, o] = max_{e: dst_e = n} m_e[o] + (x root + bias)[n, o]
+ * with m_e the message add scatters.  A node without in-edges gets 0 for the max term.  Ties go to the smallest index
+ * e in the caller's edge_index; -0 ties with +0; a NaN message wins (every NaN ties with every other NaN).
+ * argmax [N, out] int32 receives the winning caller edge index (-1: no in-edge).  The gradient of out[n, o] goes to
+ * the winning edge's message alone, so every backward takes the argmax of the forward it differentiates.
+ *   nnconv_apply_max_sizes: the workspace of nnconv_apply_max, given ws_bytes = the size the add / mean call would use
+ *     (nnconv_apply_sizes for a whole h, nnconv_stream_split for a prefix); the addition is N * out * 8 bytes of keys
+ *     (rounded up to 1 KiB) at the start of the workspace.
+ *   nnconv_apply_max: nnconv_apply_ex (E_res = E: h_res is the whole h, edge_attr may be NULL) or
+ *     nnconv_apply_streamed (E_res < E), flags as there; one more launch than they make.  No allocation, no host
+ *     synchronisation.  With E_res < E the first int after the keys counts fp16 overflows of the streamed chunks.
+ *   nnconv_backward_apply_max / nnconv_backward_mlp_max: nnconv_backward_apply_streamed / nnconv_backward_mlp_streamed
+ *     (same workspace sizes) given each application's argmax; acts as for nnconv_backward_mlp_ex (E_res = E only).
+ *   nnconv_backward_max: nnconv_backward_ex (fp32 CUDA-core weights) given the argmax. */
+int nnconv_apply_max_sizes(const nnconv_plan_t* plan, const nnconv_weights_t* w, size_t ws_bytes, size_t* max_ws_bytes);
+int nnconv_apply_max(const nnconv_plan_t* plan, const nnconv_weights_t* w, const float* edge_attr, const void* h_res,
+                     int64_t E_res, const float* x, const float* root, const float* bias, unsigned flags, float* out,
+                     int* argmax, void* ws, size_t ws_bytes, void* stream, int64_t* launches /*nullable*/);
+int nnconv_backward_apply_max(const nnconv_plan_t* plan, const nnconv_weights_t* w, const float* edge_attr,
+                              const void* h_res, int64_t E_res, const float* x, const float* root, const int* argmax,
+                              const float* grad_out, float* grad_x, float* grad_W_last, float* grad_b_last,
+                              float* grad_root, float* grad_bias, void* ws, size_t ws_bytes, void* stream,
+                              int64_t* launches /*nullable*/);
+int nnconv_backward_mlp_max(const nnconv_plan_t* plan, const nnconv_weights_t* w, const float* edge_attr,
+                            const void* h_res, int64_t E_res, int n_apps, const float* const* grad_out,
+                            const float* const* x, const int* const* argmax, float* const* grad_W, float* const* grad_b,
+                            void* ws, size_t ws_bytes, void* stream, const void* acts /* nullable */,
+                            float* grad_edge_attr /* nullable */);
+int nnconv_backward_max(const nnconv_plan_t* plan, const nnconv_weights_t* w, const float* edge_attr, const float* x,
+                        const float* root, const int* argmax, const float* grad_out, float* grad_x,
+                        float* const* grad_W, float* const* grad_b, float* grad_root, float* grad_bias, void* ws,
+                        size_t ws_bytes, void* stream, float* grad_edge_attr /* nullable */);
 
 /* ---- halo exchange of the node-range (strip) partition by peer stores over NVLink (no NCCL call, no host round
  * trip between applications).  `out` [n_local, channels] is the result of one application on this rank (owned rows
