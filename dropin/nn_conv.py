@@ -1,6 +1,7 @@
 """Drop-in for graph-neural-operator/nn_conv.py: put this directory FIRST on sys.path (or PYTHONPATH) and the
-reference scripts' ``from nn_conv import NNConv_old`` (UAI1_full_resolution.py:9) resolves to this library's op.
-Whole-module checkpoints pickled by the reference bind to the class path ``nn_conv.NNConv_old`` -- kept."""
+reference scripts' ``from nn_conv import NNConv_old`` (UAI1_full_resolution.py:9) and ``from nn_conv import NNConv,
+NNConv_old`` (neurips1_GKN.py:10, neurips5_GKN.py:10) resolve to this library's ops.  Whole-module checkpoints pickled
+by the reference bind to the class paths ``nn_conv.NNConv_old`` and ``nn_conv.NNConv`` -- kept."""
 import os
 import sys
 
@@ -10,13 +11,21 @@ if _ROOT not in sys.path:
 
 from graph_pde_b200.nn_conv import NNConv_old as _Base  # noqa: E402
 from graph_pde_b200.nn_conv import NNConv as _UpstreamNNConv  # noqa: E402
+from graph_pde_b200.nn_conv import DiagNNConv as _Diag  # noqa: E402
 
 
 class NNConv_old(_Base):
     pass
 
 
-# The reference's nn_conv.py also defines `NNConv` (a diagonal-kernel variant, nn_conv.py:8-96) and
-# `NNConv_Gaussian`; neither is instantiated by any script (SURVEY section 2), so they are not provided.
+class NNConv(_Diag):
+    """The reference's diagonal-kernel conv (nn_conv.py:8-96), imported by neurips1_GKN.py / neurips5_GKN.py."""
+    pass
+
+
+# The reference's nn_conv.py also defines `NNConv_Gaussian`, which no script instantiates: not provided.  Its ECConv
+# (nn_conv.py:288) names the diagonal class; here ECConv stays the upstream torch_geometric NNConv (INTEGRATION 1).
 NNConv_old.__module__ = 'nn_conv'
+NNConv.__module__ = 'nn_conv'
+NNConv.__qualname__ = 'NNConv'
 ECConv = _UpstreamNNConv

@@ -40,6 +40,9 @@ SYMBOLS = [
     'nnconv_backward_mlp_streamed', 'nnconv_backward_streamed_chunks', 'nnconv_overflow_accumulate',
     'nnconv_apply_max_sizes', 'nnconv_apply_max', 'nnconv_backward_apply_max', 'nnconv_backward_mlp_max',
     'nnconv_backward_max',
+    'nnconv_diag_weights_sizes', 'nnconv_diag_weights_create', 'nnconv_diag_weights_destroy', 'nnconv_diag_sizes',
+    'nnconv_diag_build', 'nnconv_apply_diag_sizes', 'nnconv_apply_diag', 'nnconv_backward_apply_diag',
+    'nnconv_backward_mlp_diag_sizes', 'nnconv_backward_mlp_diag',
 ]
 
 
@@ -155,6 +158,18 @@ def lib():
                                           P(c_vp), c_vp, c_sz, c_vp, c_vp, c_vp]
     L.nnconv_backward_max.argtypes = [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, P(c_vp), P(c_vp), c_vp, c_vp, c_vp,
                                       c_sz, c_vp, c_vp]
+    L.nnconv_diag_weights_sizes.argtypes = [c_int, P(c_int), c_int, c_int, P(c_sz)]
+    L.nnconv_diag_weights_create.argtypes = [c_int, P(c_int), c_int, c_int, P(c_vp), P(c_vp), c_vp, c_sz, c_vp, P(c_vp)]
+    L.nnconv_diag_weights_destroy.argtypes = [c_vp]
+    L.nnconv_diag_weights_destroy.restype = None
+    L.nnconv_diag_sizes.argtypes = [c_vp, c_vp, c_sz, P(c_sz), P(c_sz)]
+    L.nnconv_diag_build.argtypes = [c_vp, c_vp, c_vp, c_vp, c_vp, c_sz, c_vp, P(c_i64)]
+    L.nnconv_apply_diag_sizes.argtypes = [c_vp, c_vp, c_int, P(c_sz)]
+    L.nnconv_apply_diag.argtypes = [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_sz, c_vp, P(c_i64)]
+    L.nnconv_backward_apply_diag.argtypes = [c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
+                                             P(c_i64)]
+    L.nnconv_backward_mlp_diag_sizes.argtypes = [c_vp, c_vp, c_sz, P(c_sz)]
+    L.nnconv_backward_mlp_diag.argtypes = [c_vp, c_vp, c_vp, c_vp, P(c_vp), P(c_vp), c_vp, c_sz, c_vp, c_vp]
     for name in SYMBOLS:
         getattr(L, name)
     if L.nnconv_abi_version() != ABI_VERSION:

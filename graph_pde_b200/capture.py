@@ -16,7 +16,7 @@ loss, backward and the optimiser step together (see its docstring)."""
 import torch
 
 from . import nn_conv
-from .nn_conv import NNConv_old
+from .nn_conv import DiagNNConv, NNConv_old
 
 
 class GraphedForward(object):
@@ -69,7 +69,7 @@ class GraphedTrainStep(object):
     NNConv, so every replay recomputes them from the current parameters and edge attributes.  The gradients of the
     captured step live in the graph's memory: do not set them to None between replays.
 
-    After each replay the convs' caches are dropped (the step changed the parameters in place without bumping their
+    After each replay the convs' caches (NNConv_old, NNConv and DiagNNConv) are dropped (the step changed the parameters in place without bumping their
     version counters, so a later eager forward would otherwise use stale prepared weights), and the fp16 range counters
     that the step's edge-feature passes and K_e builds added up on the device are read with one 4-byte copy.  A
     non-zero count raises FloatingPointError.  The optimiser step has been applied by then: restore the parameters
@@ -92,7 +92,8 @@ class GraphedTrainStep(object):
                              'to be zeros: take one eager step before capturing' % (type(optimizer).__name__,
                                                                                      len(fresh)))
         self.loss_fn, self.model, self.optimizer, self.inputs = loss_fn, model, optimizer, static_inputs
-        self._convs = [m for m in model.modules() if isinstance(m, NNConv_old)]
+        # DiagNNConv keeps no edge features that could stream: only its prepared weights, d and training state
+        self._convs = [m for m in model.modules() if isinstance(m, (NNConv_old, DiagNNConv))]
         dev = params[0].device
 
         # snapshot, warm-up, restore in place
@@ -108,7 +109,7 @@ class GraphedTrainStep(object):
                 loss_fn(*static_inputs).backward()
                 optimizer.step()
         torch.cuda.current_stream(dev).wait_stream(side)
-        streamed = any(ef.streamed for c in self._convs for ef in c._h_cache.values())
+        streamed = any(ef.streamed for c in self._convs if isinstance(c, NNConv_old) for ef in c._h_cache.values())
         with torch.no_grad():
             for t, v in model_state:
                 t.copy_(v)

@@ -52,13 +52,20 @@ struct WeightsLayout {
   bool bwd;
 };
 
-static int fill_dims(Weights* W, int n_layers, const int* dims, int cin, int cout, int prec) {
+static int fill_dims(Weights* W, int n_layers, const int* dims, int cin, int cout, int prec, int diag = 0) {
   NNC_REQUIRE(n_layers >= 1 && n_layers <= kMaxLayers, NNCONV_ERR_ARG, "edge MLP must have 1..%d Linear layers", kMaxLayers);
   NNC_REQUIRE(prec >= PREC_FP32 && prec <= PREC_F16X2, NNCONV_ERR_ARG, "unknown precision %d", prec);
   NNC_REQUIRE(cin >= 1 && cout >= 1, NNCONV_ERR_ARG, "bad channel counts");
-  NNC_REQUIRE(dims[n_layers] == cin * cout, NNCONV_ERR_ARG,
-              "edge MLP output width %d != in_channels*out_channels = %d", dims[n_layers], cin * cout);
+  if (diag) {
+    NNC_REQUIRE(dims[n_layers] == cout && cin == cout, NNCONV_ERR_UNSUPPORTED,
+                "diagonal kernel: edge MLP output width %d, in_channels %d and out_channels %d must be equal",
+                dims[n_layers], cin, cout);
+  } else {
+    NNC_REQUIRE(dims[n_layers] == cin * cout, NNCONV_ERR_ARG,
+                "edge MLP output width %d != in_channels*out_channels = %d", dims[n_layers], cin * cout);
+  }
   memset(W, 0, sizeof(*W));
+  W->diag = diag;
   W->n_layers = n_layers;
   for (int l = 0; l <= n_layers; ++l) {
     NNC_REQUIRE(dims[l] >= 1, NNCONV_ERR_ARG, "bad layer width");
@@ -94,6 +101,12 @@ static WeightsLayout layout_weights(const Weights* W) {
     L.off_bh[l] = c.off; c.take<float>(W->kp[l]);
   }
   L.off_wscale = c.off; c.take<float>(2 * (kMaxLayers + 2));
+  if (W->diag) {   // W_L [cout, Kp] (16-bit for the tensor-core build of d, else fp32) and b_L
+    L.off_W3n = c.off; c.take<char>(static_cast<size_t>(W->cout) * W->Kp * (W->prec == PREC_F16 || W->prec == PREC_BF16 ? 2 : 4));
+    L.off_B3 = c.off; c.take<float>(W->cout);
+    L.bytes = c.off;
+    return L;
+  }
   L.off_W3p = c.off; c.take<char>(static_cast<size_t>(W->cout) * W->Kp * W->cin_p * W->esize * (W->split ? 3 : 1));
   L.off_B3 = c.off; c.take<float>(static_cast<size_t>(W->cin) * W->cout);
   // images for the tensor-core backward (same conditions as backward_tc_supported); PREC_F16X2: split [hi | lo | hi]
@@ -115,16 +128,16 @@ static WeightsLayout layout_weights(const Weights* W) {
   return L;
 }
 
-size_t weights_bytes(int n_layers, const int* dims, int cin, int cout, int prec) {
+size_t weights_bytes(int n_layers, const int* dims, int cin, int cout, int prec, int diag) {
   Weights W;
-  if (fill_dims(&W, n_layers, dims, cin, cout, prec) != NNCONV_OK) return 0;
+  if (fill_dims(&W, n_layers, dims, cin, cout, prec, diag) != NNCONV_OK) return 0;
   return layout_weights(&W).bytes;
 }
 
 int weights_prepare(Weights* W, int n_layers, const int* dims, int cin, int cout, int prec,
                     const float* const* Wsrc, const float* const* bsrc, void* buf, size_t buf_bytes,
-                    cudaStream_t st) {
-  int s = fill_dims(W, n_layers, dims, cin, cout, prec);
+                    cudaStream_t st, int diag) {
+  int s = fill_dims(W, n_layers, dims, cin, cout, prec, diag);
   if (s != NNCONV_OK) return s;
   WeightsLayout L = layout_weights(W);
   NNC_REQUIRE(buf != nullptr && L.bytes <= buf_bytes, NNCONV_ERR_WORKSPACE, "weights buffer too small (need %zu)", L.bytes);
@@ -163,6 +176,16 @@ int weights_prepare(Weights* W, int n_layers, const int* dims, int cin, int cout
     if (s) return s;
     W->Wh[l] = Wh;
     W->bh[l] = bh;
+  }
+  if (W->diag) {
+    const int p16 = prec == PREC_F16 || prec == PREC_BF16 ? prec : PREC_FP32;
+    s = launch_pad_convert(p16, Wsrc[nl - 1], cout, W->K, base + L.off_W3n, cout, W->Kp, st);
+    if (s) return s;
+    s = launch_pad_convert(PREC_FP32, bsrc[nl - 1], 1, cout, base + L.off_B3, 1, cout, st);
+    if (s) return s;
+    W->W3n = base + L.off_W3n;
+    W->B3 = reinterpret_cast<float*>(base + L.off_B3);
+    return NNCONV_OK;
   }
   void* W3p = base + L.off_W3p;
   float* B3 = reinterpret_cast<float*>(base + L.off_B3);
@@ -904,6 +927,9 @@ struct nnconv_plan {
 struct nnconv_weights {
   Weights w;
 };
+struct nnconv_diag_weights {
+  Weights w;
+};
 
 extern "C" {
 
@@ -1315,6 +1341,84 @@ int nnconv_backward_max(const nnconv_plan_t* plan, const nnconv_weights_t* w, co
   NNC_REQUIRE(edge_attr != nullptr || plan->p.E == 0, NNCONV_ERR_ARG, "backward_max: null edge_attr");
   return backward_fp32(&plan->p, &w->w, edge_attr, x, root, 0, grad_out, grad_x, grad_W, grad_b, grad_root, grad_bias,
                        ws, ws_bytes, static_cast<cudaStream_t>(stream), grad_edge_attr, argmax);
+}
+
+int nnconv_diag_weights_sizes(int n_layers, const int* dims, int channels, int precision, size_t* bytes) {
+  NNC_REQUIRE(bytes && dims, NNCONV_ERR_ARG, "null pointer");
+  Weights W;
+  int s = fill_dims(&W, n_layers, dims, channels, channels, precision, 1);
+  if (s) return s;
+  *bytes = layout_weights(&W).bytes;
+  return NNCONV_OK;
+}
+
+int nnconv_diag_weights_create(int n_layers, const int* dims, int channels, int precision, const float* const* W,
+                               const float* const* b, void* buf, size_t buf_bytes, void* stream,
+                               nnconv_diag_weights_t** out) {
+  NNC_REQUIRE(out && dims && W && b, NNCONV_ERR_ARG, "null pointer");
+  *out = nullptr;
+  nnconv_diag_weights* h = new (std::nothrow) nnconv_diag_weights();
+  NNC_REQUIRE(h != nullptr, NNCONV_ERR_ARG, "out of host memory");
+  int s = weights_prepare(&h->w, n_layers, dims, channels, channels, precision, W, b, buf, buf_bytes,
+                          static_cast<cudaStream_t>(stream), 1);
+  if (s != NNCONV_OK) { delete h; return s; }
+  *out = h;
+  return NNCONV_OK;
+}
+
+void nnconv_diag_weights_destroy(nnconv_diag_weights_t* w) { delete w; }
+
+int nnconv_diag_sizes(const nnconv_plan_t* plan, const nnconv_diag_weights_t* w, size_t want_ws_bytes, size_t* d_bytes,
+                      size_t* ws_bytes) {
+  NNC_REQUIRE(plan && w && d_bytes && ws_bytes, NNCONV_ERR_ARG, "null pointer");
+  *d_bytes = static_cast<size_t>(plan->p.E > 0 ? plan->p.E : 1) * w->w.cout * sizeof(float);
+  *ws_bytes = diag_ws_bytes(&plan->p, &w->w, want_ws_bytes);
+  return NNCONV_OK;
+}
+
+int nnconv_diag_build(const nnconv_plan_t* plan, const nnconv_diag_weights_t* w, const float* edge_attr, float* d,
+                      void* ws, size_t ws_bytes, void* stream, int64_t* launches) {
+  NNC_REQUIRE(plan && w && d && (edge_attr || plan->p.E == 0), NNCONV_ERR_ARG, "null pointer");
+  return diag_build(&plan->p, &w->w, edge_attr, d, ws, ws_bytes, static_cast<cudaStream_t>(stream), launches);
+}
+
+int nnconv_apply_diag_sizes(const nnconv_plan_t* plan, const nnconv_diag_weights_t* w, int aggr, size_t* ws_bytes) {
+  NNC_REQUIRE(plan && w && ws_bytes, NNCONV_ERR_ARG, "null pointer");
+  *ws_bytes = aggr == NNCONV_AGGR_MAX ? max_keys_bytes(plan->p.N, w->w.cout) : 1024;
+  return NNCONV_OK;
+}
+
+int nnconv_apply_diag(const nnconv_plan_t* plan, const nnconv_diag_weights_t* w, const float* d, const float* x,
+                      const float* root, const float* bias, int aggr, float* out, int* argmax, void* ws, size_t ws_bytes,
+                      void* stream, int64_t* launches) {
+  NNC_REQUIRE(plan && w && x && out && (d || plan->p.E == 0), NNCONV_ERR_ARG, "null pointer");
+  NNC_REQUIRE(x != out, NNCONV_ERR_ARG, "out must not alias x");
+  return apply_diag(&plan->p, &w->w, d, x, root, bias, aggr, out, argmax, ws, ws_bytes, static_cast<cudaStream_t>(stream),
+                    launches);
+}
+
+int nnconv_backward_apply_diag(const nnconv_plan_t* plan, const nnconv_diag_weights_t* w, const float* d, const float* x,
+                               const float* root, int aggr, const int* argmax, const float* grad_out, float* grad_x,
+                               float* grad_root, float* grad_bias, float* grad_d, void* stream, int64_t* launches) {
+  NNC_REQUIRE(plan && w && x && grad_out && grad_x && (d || plan->p.E == 0), NNCONV_ERR_ARG, "null pointer");
+  NNC_REQUIRE((root == nullptr) == (grad_root == nullptr), NNCONV_ERR_ARG, "root / grad_root must both be given or both be NULL");
+  return backward_apply_diag(&plan->p, &w->w, d, x, root, aggr, argmax, grad_out, grad_x, grad_root, grad_bias, grad_d,
+                             static_cast<cudaStream_t>(stream), launches);
+}
+
+int nnconv_backward_mlp_diag_sizes(const nnconv_plan_t* plan, const nnconv_diag_weights_t* w, size_t want_bytes,
+                                   size_t* ws_bytes) {
+  NNC_REQUIRE(plan && w && ws_bytes, NNCONV_ERR_ARG, "null pointer");
+  *ws_bytes = backward_mlp_diag_ws_bytes(&plan->p, &w->w, want_bytes);
+  return NNCONV_OK;
+}
+
+int nnconv_backward_mlp_diag(const nnconv_plan_t* plan, const nnconv_diag_weights_t* w, const float* edge_attr,
+                             const float* grad_d, float* const* grad_W, float* const* grad_b, void* ws, size_t ws_bytes,
+                             void* stream, float* grad_edge_attr) {
+  NNC_REQUIRE(plan && w && grad_W && grad_b && ((edge_attr && grad_d) || plan->p.E == 0), NNCONV_ERR_ARG, "null pointer");
+  return backward_mlp_diag(&plan->p, &w->w, edge_attr, grad_d, grad_W, grad_b, ws, ws_bytes,
+                           static_cast<cudaStream_t>(stream), grad_edge_attr);
 }
 
 int nnconv_backward_mlp_sizes(const nnconv_plan_t* plan, const nnconv_weights_t* w, int n_apps, size_t want_bytes,

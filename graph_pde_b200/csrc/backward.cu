@@ -234,6 +234,64 @@ __global__ void k_colsum_rows(const float* __restrict__ g, int64_t N, int C, flo
   }
 }
 
+// dh = the gradient w.r.t. h_{L-1} of the sorted edges [e0, e0 + ne) in cur ([ne, Kp] fp32; nxt: a buffer of the same
+// size): back through the hidden layers with the ReLU masks of act[1 .. L-1] (recomputed fp32 activations), adding into
+// the padded accumulators dW[l], db[l], and, with grad_ea, the gradient w.r.t. the batch's edge_attr rows.  ea: scratch
+// of ne * k_in floats.
+int mlp_backward_rows(const Plan* P, const Weights* W, const float* edge_attr, int e0, int ne, float* const* act, float* ea,
+                      float* cur, float* nxt, float* const* dW, float* const* db, float* grad_ea, cudaStream_t st) {
+  const int nl = W->n_layers;
+  const int TB = 256;
+  int s;
+  if (nl >= 2) {
+    k_gather_ea<<<(unsigned)ceil_div64(static_cast<int64_t>(ne) * W->kp[0], TB), TB, 0, st>>>(
+        edge_attr, P->perm, e0, ne, W->kp[0], ea);
+    NNC_CHECK_LAUNCH();
+  }
+  for (int l = nl - 1; l >= 1; --l) {
+    k_relu_mask_colsum<<<ceil_div(W->kp[l], 32), dim3(32, 8), 0, st>>>(cur, act[l], ne, W->kp[l], db[l]);
+    NNC_CHECK_LAUNCH();
+    const float* prev = l == 1 ? ea : act[l - 1];
+    const int kprev = W->kp[l - 1];
+    // dW_l += dz^T prev
+    s = gemm_any(cur, 1, W->kp[l], prev, kprev, 1, dW[l], kprev, W->kp[l], kprev, ne, 1.f, st);
+    if (s) return s;
+    if (l > 1) {   // dh_{l-1} = dz W_l
+      s = gemm_any(cur, W->kp[l], 1, reinterpret_cast<const float*>(W->Wh[l]), kprev, 1, nxt, kprev, ne, kprev,
+                   W->kp[l], 0.f, st);
+      if (s) return s;
+      float* t = cur; cur = nxt; nxt = t;
+    }
+  }
+  // ---- cur = dz_1 (masked, [ne, kp1]) or, for a single Linear, dh ([ne, Kp]): edge_attr rows of the batch
+  if (grad_ea != nullptr) {
+    k_ea_grad_fp32<<<(unsigned)ceil_div64(static_cast<int64_t>(ne) * W->dims[0], TB), TB, 0, st>>>(
+        cur, ne, nl >= 2 ? W->kp[1] : W->Kp, nl >= 2 ? W->W1 : nullptr, nl >= 2 ? W->dims[1] : 0, W->dims[0], P->perm,
+        e0, grad_ea);
+    NNC_CHECK_LAUNCH();
+  }
+  return NNCONV_OK;
+}
+
+// recomputes the fp32 activations act[1 .. L-1] of the sorted edges [e0, e0 + ne) (a single Linear: the identity
+// features into hid) and returns h_{L-1}
+const float* recompute_acts_fp32(const Plan* P, const Weights* W, const float* edge_attr, int e0, int ne, float* const* act,
+                                 float* hid, cudaStream_t st, int* status) {
+  const int nl = W->n_layers;
+  int s;
+  if (nl == 1) {
+    s = launch_edge_layer1(PREC_FP32, edge_attr, P->perm, e0, ne, W->dims[0], nullptr, nullptr, W->Kp, 1, hid, st);
+    *status = s;
+    return hid;
+  }
+  s = launch_edge_layer1(PREC_FP32, edge_attr, P->perm, e0, ne, W->dims[0], W->W1, W->b1, W->kp[1], 0, act[1], st);
+  for (int l = 2; l <= nl - 1 && s == NNCONV_OK; ++l)
+    s = launch_sgemm_store(act[l - 1], W->kp[l - 1], reinterpret_cast<const float*>(W->Wh[l]), W->kp[l - 1], act[l],
+                           W->kp[l], ne, W->kp[l], W->kp[l - 1], W->bh[l], st);
+  *status = s;
+  return act[nl - 1];
+}
+
 struct BwdLayout {
   // persistent over the call (padded fp32 gradient accumulators)
   size_t off_dW[kMaxLayers + 1], off_db[kMaxLayers + 1], off_dW3p, off_dB3, off_Xc, off_cvec;
@@ -346,21 +404,8 @@ int backward_fp32(const Plan* P, const Weights* W, const float* edge_attr, const
       float* dXc = cv.take<float>(static_cast<size_t>(nb) * cin_p);
       NNC_REQUIRE(cv.ok(), NNCONV_ERR_WORKSPACE, "backward: workspace carve overflow");
       // ---- recompute the edge features of this batch (fp32)
-      const float* h = nullptr;
-      if (nl == 1) {
-        s = launch_edge_layer1(PREC_FP32, edge_attr, P->perm, e0, ne, W->dims[0], nullptr, nullptr, Kp, 1, hid, st);
-        if (s) return s;
-        h = hid;
-      } else {
-        s = launch_edge_layer1(PREC_FP32, edge_attr, P->perm, e0, ne, W->dims[0], W->W1, W->b1, W->kp[1], 0, act[1], st);
-        if (s) return s;
-        for (int l = 2; l <= nl - 1; ++l) {
-          s = launch_sgemm_store(act[l - 1], W->kp[l - 1], reinterpret_cast<const float*>(W->Wh[l]), W->kp[l - 1],
-                                 act[l], W->kp[l], ne, W->kp[l], W->kp[l - 1], W->bh[l], st);
-          if (s) return s;
-        }
-        h = act[nl - 1];
-      }
+      const float* h = recompute_acts_fp32(P, W, edge_attr, e0, ne, act, hid, st, &s);
+      if (s) return s;
       // ---- Y of the batch
       s = launch_sgemm_store(Xc + static_cast<int64_t>(c0) * cin_p, cin_p, reinterpret_cast<const float*>(W->W3p), cin_p,
                              Y, NY, nb, NY, cin_p, nullptr, st);
@@ -411,37 +456,14 @@ int backward_fp32(const Plan* P, const Weights* W, const float* edge_attr, const
           NNC_CHECK_LAUNCH();
         }
         // ---- MLP backward through the hidden layers
-        if (nl >= 2) {
-          k_gather_ea<<<(unsigned)ceil_div64(static_cast<int64_t>(ne) * W->kp[0], TB), TB, 0, st>>>(
-              edge_attr, P->perm, e0, ne, W->kp[0], ea);
-          NNC_CHECK_LAUNCH();
+        float* dWp[kMaxLayers + 1] = {nullptr};
+        float* dbp[kMaxLayers + 1] = {nullptr};
+        for (int l = 1; l <= nl - 1; ++l) {
+          dWp[l] = reinterpret_cast<float*>(base + L.off_dW[l]);
+          dbp[l] = reinterpret_cast<float*>(base + L.off_db[l]);
         }
-        float* cur = dhA;
-        float* nxt = dhB;
-        for (int l = nl - 1; l >= 1; --l) {
-          float* dWl = reinterpret_cast<float*>(base + L.off_dW[l]);
-          float* dbl = reinterpret_cast<float*>(base + L.off_db[l]);
-          k_relu_mask_colsum<<<ceil_div(W->kp[l], 32), dim3(32, 8), 0, st>>>(cur, act[l], ne, W->kp[l], dbl);
-          NNC_CHECK_LAUNCH();
-          const float* prev = l == 1 ? ea : act[l - 1];
-          const int kprev = W->kp[l - 1];
-          // dW_l += dz^T prev
-          s = gemm_any(cur, 1, W->kp[l], prev, kprev, 1, dWl, kprev, W->kp[l], kprev, ne, 1.f, st);
-          if (s) return s;
-          if (l > 1) {   // dh_{l-1} = dz W_l
-            s = gemm_any(cur, W->kp[l], 1, reinterpret_cast<const float*>(W->Wh[l]), kprev, 1, nxt, kprev, ne, kprev,
-                         W->kp[l], 0.f, st);
-            if (s) return s;
-            float* t = cur; cur = nxt; nxt = t;
-          }
-        }
-        // ---- cur = dz_1 (masked, [ne, kp1]) or, for a single Linear, dh ([ne, Kp]): edge_attr rows of the batch
-        if (grad_ea != nullptr) {
-          k_ea_grad_fp32<<<(unsigned)ceil_div64(static_cast<int64_t>(ne) * W->dims[0], TB), TB, 0, st>>>(
-              cur, ne, nl >= 2 ? W->kp[1] : Kp, nl >= 2 ? W->W1 : nullptr, nl >= 2 ? W->dims[1] : 0, W->dims[0], P->perm,
-              e0, grad_ea);
-          NNC_CHECK_LAUNCH();
-        }
+        s = mlp_backward_rows(P, W, edge_attr, e0, ne, act, ea, dhA, dhB, dWp, dbp, grad_ea, st);
+        if (s) return s;
       }
       c0 = c1;
     }
@@ -459,6 +481,200 @@ int backward_fp32(const Plan* P, const Weights* W, const float* edge_attr, const
       dW3p, cin, cout, W->K, Kp, cin_p, dWs[nl - 1]);
   NNC_CHECK_LAUNCH();
   NNC_CHECK_CUDA(cudaMemcpyAsync(dbs[nl - 1], dB3, sizeof(float) * cin * cout, cudaMemcpyDeviceToDevice, st));
+  return NNCONV_OK;
+}
+
+// ------------------------------------------------------------------------------------------------
+// diagonal-kernel conv (formulation D, diag.cu).  Per application, with G_e = g[dst_e] * inv_deg[dst_e] (mean), g[dst_e]
+// (add) or g[dst_e] masked by the forward's argmax (max):
+//   dx_n = g_n root^T + sum_{e: src_e = n} G_e * d_e          dd_e += x_src(e) * G_e   (summed over the applications)
+// and once per (edge_attr, parameters): dW_L = dd^T h, db_L = sum_e dd_e, dh = dd W_L, then the hidden layers.
+// ------------------------------------------------------------------------------------------------
+namespace {
+
+// one warp per plan tile (one source): lane o of each 32-channel block keeps x_src[o] and the tile's dx sum in registers
+// (dd nullable: no gradient reaches the edge network)
+template <int AGGR>
+__global__ void __launch_bounds__(256) k_bwd_diag_edges(const float* __restrict__ d, const float* __restrict__ x,
+                                                        const float* __restrict__ gout, int cout, int n_tiles,
+                                                        const int* __restrict__ tile_c, const int* __restrict__ tile_e0,
+                                                        const int* __restrict__ tile_cnt, const int* __restrict__ src_nodes,
+                                                        const int* __restrict__ dst_sorted,
+                                                        const float* __restrict__ inv_deg, const int* __restrict__ argmax,
+                                                        const int* __restrict__ perm, float* __restrict__ dx,
+                                                        float* __restrict__ dd) {
+  const int t = static_cast<int>((blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x) >> 5);
+  const int lane = threadIdx.x & 31;
+  if (t >= n_tiles) return;
+  const int e0 = tile_e0[t], cnt = tile_cnt[t];
+  const int64_t s = src_nodes[tile_c[t]];
+  for (int o = lane; o < cout; o += 32) {
+    const float xv = x[s * cout + o];
+    float acc = 0.f;
+    for (int p = 0; p < cnt; ++p) {
+      const int64_t e = e0 + p;
+      const int dn = dst_sorted[e];
+      const int64_t k = static_cast<int64_t>(dn) * cout + o;
+      float g = gout[k];
+      if (AGGR == 1) g *= inv_deg[dn];
+      if (AGGR == 2 && static_cast<uint32_t>(argmax[k]) != caller_edge(perm, e)) g = 0.f;
+      acc = fmaf(g, d[e * cout + o], acc);
+      if (dd != nullptr) dd[e * cout + o] += xv * g;
+    }
+    atomicAdd(dx + s * cout + o, acc);
+  }
+}
+
+// out[c] += sum_n g[n, c]
+__global__ void k_colsum_rows_add(const float* __restrict__ g, int64_t N, int C, float* __restrict__ out) {
+  __shared__ float red[8][33];
+  const int col = blockIdx.x * 32 + threadIdx.x;
+  float s = 0.f;
+  for (int64_t n = threadIdx.y; n < N; n += 8)
+    if (col < C) s += g[n * C + col];
+  red[threadIdx.y][threadIdx.x] = s;
+  __syncthreads();
+  if (threadIdx.y == 0 && col < C) {
+    float t = 0.f;
+    for (int r = 0; r < 8; ++r) t += red[r][threadIdx.x];
+    out[col] += t;
+  }
+}
+
+constexpr size_t kDiagCarveSlack = 16 * 1024;
+
+struct DiagBwdLayout {
+  size_t off_dW[kMaxLayers + 1], off_db[kMaxLayers + 1], off_dWL, off_dbL, fixed, per_edge;
+};
+
+DiagBwdLayout diag_bwd_layout(const Weights* W) {
+  Carver c(nullptr, ~size_t(0));
+  DiagBwdLayout L{};
+  const int nl = W->n_layers;
+  for (int l = 1; l <= nl - 1; ++l) {
+    L.off_dW[l] = c.off; c.take<float>(static_cast<size_t>(W->kp[l]) * W->kp[l - 1]);
+    L.off_db[l] = c.off; c.take<float>(W->kp[l]);
+  }
+  L.off_dWL = c.off; c.take<float>(static_cast<size_t>(W->cout) * W->Kp);
+  L.off_dbL = c.off; c.take<float>(W->cout);
+  L.fixed = c.off;
+  size_t acts = 0;
+  int maxkp = W->Kp;
+  for (int l = 1; l <= nl - 1; ++l) { acts += W->kp[l]; maxkp = W->kp[l] > maxkp ? W->kp[l] : maxkp; }
+  if (nl == 1) acts = W->Kp;
+  // activations of every hidden layer + two dh ping-pong buffers + gathered edge_attr
+  L.per_edge = sizeof(float) * (acts + 2 * static_cast<size_t>(maxkp) + W->kp[0]);
+  return L;
+}
+
+}  // namespace
+
+int backward_apply_diag(const Plan* P, const Weights* W, const float* d, const float* x, const float* root, int aggr,
+                        const int* argmax, const float* gout, float* dx, float* droot, float* dbias, float* dd,
+                        cudaStream_t st, int64_t* launches) {
+  NNC_REQUIRE(W->diag, NNCONV_ERR_ARG, "backward_apply_diag: weights not prepared as a diagonal kernel");
+  NNC_REQUIRE(aggr >= 0 && aggr <= 2 && (aggr != 2 || argmax != nullptr), NNCONV_ERR_ARG,
+              "backward_apply_diag: aggr %d (max needs the forward's argmax)", aggr);
+  const int C = W->cout;
+  const int64_t N = P->N;
+  int64_t n_l = 0;
+  int s;
+  if (dbias) {
+    k_colsum_rows<<<ceil_div(C, 32), dim3(32, 8), 0, st>>>(gout, N, C, dbias);
+    NNC_CHECK_LAUNCH();
+    ++n_l;
+  }
+  if (root != nullptr) {
+    s = gemm_any(x, 1, C, gout, C, 1, droot, C, C, C, static_cast<int>(N), 0.f, st);   // droot = x^T g
+    if (s) return s;
+    s = gemm_any(gout, C, 1, root, 1, C, dx, C, static_cast<int>(N), C, C, 0.f, st);   // dx = g root^T
+    if (s) return s;
+    n_l += 2;
+  } else {
+    NNC_CHECK_CUDA(cudaMemsetAsync(dx, 0, sizeof(float) * N * C, st));
+  }
+  if (P->E > 0 && P->n_tiles > 0) {
+    const unsigned grid = static_cast<unsigned>(ceil_div64(static_cast<int64_t>(P->n_tiles) * 32, 256));
+#define NNC_DIAG_BWD(A)                                                                                               \
+  k_bwd_diag_edges<A><<<grid, 256, 0, st>>>(d, x, gout, C, P->n_tiles, P->tile_c, P->tile_e0, P->tile_cnt, P->src_nodes, \
+                                            P->dst_sorted, P->inv_deg, argmax, P->perm, dx, dd)
+    if (aggr == 0) NNC_DIAG_BWD(0);
+    else if (aggr == 1) NNC_DIAG_BWD(1);
+    else NNC_DIAG_BWD(2);
+#undef NNC_DIAG_BWD
+    NNC_CHECK_LAUNCH();
+    ++n_l;
+  }
+  if (launches) *launches += n_l;
+  return NNCONV_OK;
+}
+
+size_t backward_mlp_diag_ws_bytes(const Plan* P, const Weights* W, size_t want_bytes) {
+  const DiagBwdLayout L = diag_bwd_layout(W);
+  const size_t need_min = L.fixed + L.per_edge * 128 + kDiagCarveSlack;
+  const size_t all = L.fixed + L.per_edge * static_cast<size_t>(P->E > 0 ? P->E : 1) + kDiagCarveSlack;
+  size_t w = want_bytes < need_min ? need_min : want_bytes;
+  return w < all ? w : all;
+}
+
+int backward_mlp_diag(const Plan* P, const Weights* W, const float* edge_attr, const float* dd, float* const* dWs,
+                      float* const* dbs, void* ws, size_t ws_bytes, cudaStream_t st, float* grad_ea) {
+  NNC_REQUIRE(W->diag && W->prec == PREC_FP32, NNCONV_ERR_ARG,
+              "backward_mlp_diag: needs diagonal weights prepared with precision fp32");
+  const int nl = W->n_layers, C = W->cout, Kp = W->Kp;
+  const DiagBwdLayout L = diag_bwd_layout(W);
+  NNC_REQUIRE(ws != nullptr && ws_bytes >= L.fixed + L.per_edge * 128 + kDiagCarveSlack, NNCONV_ERR_WORKSPACE,
+              "backward_mlp_diag: workspace too small");
+  char* base = static_cast<char*>(ws);
+  NNC_CHECK_CUDA(cudaMemsetAsync(base, 0, L.fixed, st));
+  float* dWL = reinterpret_cast<float*>(base + L.off_dWL);
+  float* dbL = reinterpret_cast<float*>(base + L.off_dbL);
+  float* dWp[kMaxLayers + 1] = {nullptr};
+  float* dbp[kMaxLayers + 1] = {nullptr};
+  for (int l = 1; l <= nl - 1; ++l) {
+    dWp[l] = reinterpret_cast<float*>(base + L.off_dW[l]);
+    dbp[l] = reinterpret_cast<float*>(base + L.off_db[l]);
+  }
+  const size_t avail = ws_bytes - L.fixed;
+  int64_t rows = static_cast<int64_t>((avail - kDiagCarveSlack) / L.per_edge);   // slack: the carver's 1 KiB rounding
+  if (rows > P->E) rows = P->E;
+  int s;
+  for (int64_t e0 = 0; e0 < P->E; e0 += rows) {
+    const int ne = static_cast<int>(P->E - e0 < rows ? P->E - e0 : rows);
+    Carver cv(base + L.fixed, avail);
+    float* act[kMaxLayers + 1] = {nullptr};
+    for (int l = 1; l <= nl - 1; ++l) act[l] = cv.take<float>(static_cast<size_t>(ne) * W->kp[l]);
+    int maxkp = Kp;
+    for (int l = 1; l <= nl - 1; ++l) maxkp = W->kp[l] > maxkp ? W->kp[l] : maxkp;
+    float* hid = nl == 1 ? cv.take<float>(static_cast<size_t>(ne) * Kp) : nullptr;
+    float* dhA = cv.take<float>(static_cast<size_t>(ne) * maxkp);
+    float* dhB = cv.take<float>(static_cast<size_t>(ne) * maxkp);
+    float* ea = cv.take<float>(static_cast<size_t>(ne) * W->kp[0]);
+    NNC_REQUIRE(cv.ok(), NNCONV_ERR_WORKSPACE, "backward_mlp_diag: workspace carve overflow");
+    const float* h = recompute_acts_fp32(P, W, edge_attr, static_cast<int>(e0), ne, act, hid, st, &s);
+    if (s) return s;
+    const float* ddb = dd + e0 * C;
+    // dW_L += dd^T h ; db_L += sum_e dd_e ; dh = dd W_L
+    s = gemm_any(ddb, 1, C, h, Kp, 1, dWL, Kp, C, Kp, ne, 1.f, st);
+    if (s) return s;
+    k_colsum_rows_add<<<ceil_div(C, 32), dim3(32, 8), 0, st>>>(ddb, ne, C, dbL);
+    NNC_CHECK_LAUNCH();
+    s = gemm_any(ddb, C, 1, static_cast<const float*>(W->W3n), Kp, 1, dhA, Kp, ne, Kp, C, 0.f, st);
+    if (s) return s;
+    s = mlp_backward_rows(P, W, edge_attr, static_cast<int>(e0), ne, act, ea, dhA, dhB, dWp, dbp, grad_ea, st);
+    if (s) return s;
+  }
+  const int TB = 256;
+  for (int l = 1; l <= nl - 1; ++l) {
+    const int R = W->dims[l], Cl = W->dims[l - 1];
+    k_unpad<<<(unsigned)ceil_div64(static_cast<int64_t>(R) * Cl, TB), TB, 0, st>>>(dWp[l], W->kp[l - 1], dWs[l - 1], R, Cl);
+    NNC_CHECK_LAUNCH();
+    k_unpad<<<ceil_div(R, TB), TB, 0, st>>>(dbp[l], R, dbs[l - 1], 1, R);
+    NNC_CHECK_LAUNCH();
+  }
+  k_unpad<<<(unsigned)ceil_div64(static_cast<int64_t>(C) * W->K, TB), TB, 0, st>>>(dWL, Kp, dWs[nl - 1], C, W->K);
+  NNC_CHECK_LAUNCH();
+  NNC_CHECK_CUDA(cudaMemcpyAsync(dbs[nl - 1], dbL, sizeof(float) * C, cudaMemcpyDeviceToDevice, st));
   return NNCONV_OK;
 }
 

@@ -72,12 +72,16 @@ struct Weights {
   const void* W3q;              // [Kp*cout, cin_p]:  W3q[(k*cout + o), i] = W_L[i*cout + o, k]   (Y^T rows per source; split: 3*cin_p)
   const void* W3t;              // [cin_p, Kp*cout]:  W3t[i, (k*cout + o)] = W_L[i*cout + o, k]   (dx = dY : W_L; split: 3*Kp*cout)
   const void* WhT[kMaxLayers];  // hidden layers l = 2 .. L-1 transposed: [kp[l-1], kp[l]]  (dz_{l-1} = dz_l W_l; split: 3*kp[l])
+  // diagonal-kernel conv (formulation D, DESIGN 4.7): the last Linear maps h to one value per channel, d_e = W_L h_e +
+  // b_L with cin == cout == dims[L].  Only the hidden layers, W3n and B3 are prepared: W3n = W_L [cout, Kp] zero padded,
+  // 16-bit at f16 / bf16 (tensor-core build of d), fp32 at f16x2 and fp32 (CUDA-core build); B3 = b_L [cout] fp32.
+  int diag;
 };
 
-size_t weights_bytes(int n_layers, const int* dims, int cin, int cout, int prec);
+size_t weights_bytes(int n_layers, const int* dims, int cin, int cout, int prec, int diag = 0);
 int weights_prepare(Weights* W, int n_layers, const int* dims, int cin, int cout, int prec,
                     const float* const* Wsrc, const float* const* bsrc, void* buf, size_t buf_bytes,
-                    cudaStream_t st);
+                    cudaStream_t st, int diag = 0);
 
 // edge features: h_last[p, :] for every sorted edge p  (x-independent prefix of the edge MLP)
 size_t edge_features_ws_bytes(const Plan* P, const Weights* W, size_t want_bytes);
@@ -146,6 +150,25 @@ bool edge_kernels_supported(const Weights* W);
 int edge_kernels(const Plan* P, const Weights* W, const void* h, void* Kmat, cudaStream_t st);
 int apply_edge(const Plan* P, const Weights* W, const void* Kmat, const float* x, const float* root, const float* bias,
                int aggr_mean, float* out, cudaStream_t st, unsigned node_flags = 0);
+
+// diagonal-kernel conv (formulation D, diag.cu; weights prepared with diag = 1):
+//   out_n = aggr_{e: dst_e = n} (x_src(e) * d_e) + x_n root + bias,   d_e = W_L h_e + b_L   (fp32 [E, cout], sorted order)
+// diag_build computes d chunk by chunk from edge_attr (only d is kept); ws: diag_ws_bytes, its header holds the fp16
+// range counter of the chunks' hidden activations (nnconv_edge_features_overflow).  apply_diag: aggr 0 add, 1 mean,
+// 2 max (ws: max_keys_bytes of keys, argmax written).  backward_apply_diag: dx, droot, dbias of one application, and
+// dd_e += x_src(e) * G_e accumulated over the applications; backward_mlp_diag (weights prepared at fp32): every
+// Linear's gradient from dd, the activations recomputed in fp32 batch by batch.
+size_t diag_ws_bytes(const Plan* P, const Weights* W, size_t want_bytes);
+int diag_build(const Plan* P, const Weights* W, const float* edge_attr, float* d, void* ws, size_t ws_bytes, cudaStream_t st,
+               int64_t* launches);
+int apply_diag(const Plan* P, const Weights* W, const float* d, const float* x, const float* root, const float* bias,
+               int aggr, float* out, int* argmax, void* ws, size_t ws_bytes, cudaStream_t st, int64_t* launches);
+int backward_apply_diag(const Plan* P, const Weights* W, const float* d, const float* x, const float* root, int aggr,
+                        const int* argmax, const float* gout, float* dx, float* droot, float* dbias, float* dd,
+                        cudaStream_t st, int64_t* launches);
+size_t backward_mlp_diag_ws_bytes(const Plan* P, const Weights* W, size_t want_bytes);
+int backward_mlp_diag(const Plan* P, const Weights* W, const float* edge_attr, const float* dd, float* const* dWs,
+                      float* const* dbs, void* ws, size_t ws_bytes, cudaStream_t st, float* grad_ea);
 
 // backward of one application (fp32 CUDA-core path), backward.cu; grad_ea as for backward_mlp_tc.
 // aggr = max (all three backward calls): argmax [N, cout] of the forward (backward_mlp_tc: one per application) routes

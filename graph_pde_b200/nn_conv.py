@@ -32,7 +32,7 @@ from torch.nn import Parameter
 
 from . import _lib
 
-__all__ = ['NNConv_old', 'NNConv', 'ECConv', 'stats', 'clear_caches', 'default_precision']
+__all__ = ['NNConv_old', 'NNConv', 'ECConv', 'DiagNNConv', 'stats', 'clear_caches', 'default_precision']
 
 stats = {'launches': 0, 'plans_built': 0, 'edge_feature_passes': 0, 'edge_kernel_passes': 0, 'applies': 0,
          'weight_preps': 0, 'backwards': 0, 'mlp_backwards': 0, 'streamed_chunk_passes': 0,
@@ -964,9 +964,296 @@ class NNConv_old(torch.nn.Module):
 class NNConv(NNConv_old):
     """Drop-in for upstream ``torch_geometric.nn.NNConv`` as the MGKN scripts use it
     (multipole-graph-neural-operator/neurips1_MGKN.py:41,49,57; MGKN_general_darcy2d.py:45,53,61;
-    MGKN_orthogonal_burgers1d.py:37).  NOTE: graph-neural-operator/nn_conv.py:8-96 also defines a class
-    called NNConv (diagonal-kernel variant) which no script instantiates; it is out of scope."""
+    MGKN_orthogonal_burgers1d.py:37).  graph-neural-operator/nn_conv.py:8-96 also defines a class called NNConv, the
+    diagonal-kernel variant: that one is DiagNNConv (and ``nn_conv.NNConv`` of the drop-in directory)."""
     pass
 
 
 ECConv = NNConv
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# diagonal-kernel conv (formulation D, DESIGN 4.7)
+# ---------------------------------------------------------------------------------------------------------------------
+_DIAG_WS_BYTES = 1 << 30         # edge-network chunk of the d build (h rows + hidden activations)
+
+
+class _DiagWeights(object):
+    """nnconv_diag_weights_t: padded / down-converted snapshot of the edge network of a DiagNNConv."""
+
+    def __init__(self, linears, channels, precision):
+        L = _lib.lib()
+        _lib.check(L.nnconv_init())
+        n = len(linears)
+        dims = [linears[0].in_features] + [l.out_features for l in linears]
+        c_dims = (ctypes.c_int * (n + 1))(*dims)
+        nbytes = ctypes.c_size_t()
+        prec = _lib.PREC[precision]
+        _lib.check(L.nnconv_diag_weights_sizes(n, c_dims, channels, prec, ctypes.byref(nbytes)))
+        dev = linears[0].weight.device
+        self.buf = torch.empty(nbytes.value, dtype=torch.uint8, device=dev)
+        ws = [l.weight.detach().contiguous().float() for l in linears]
+        bs = [l.bias.detach().contiguous().float() for l in linears]
+        wp = (ctypes.c_void_p * n)(*[w.data_ptr() for w in ws])
+        bp = (ctypes.c_void_p * n)(*[b.data_ptr() for b in bs])
+        h = ctypes.c_void_p()
+        _lib.check(L.nnconv_diag_weights_create(n, c_dims, channels, prec, wp, bp, _ptr(self.buf), nbytes.value,
+                                                _stream_ptr(dev), ctypes.byref(h)))
+        self._keep = (ws, bs)
+        self.handle = h
+        self.precision = precision
+        stats['weight_preps'] += 1
+        self._finalizer = weakref.finalize(self, L.nnconv_diag_weights_destroy, h)
+
+
+class _DiagFeatures(object):
+    """d = W_L h + b_L of one (plan, weights, edge_attr): fp32 [E, out] in the plan's sorted edge order.  ``ea32`` is
+    held so that its address cannot be recycled while it keys the cache."""
+
+    def __init__(self, d, ea32):
+        self.d, self.ea32 = d, ea32
+
+
+class _DiagState(object):
+    """What the applications of one DiagNNConv on one (edge_attr, parameters) share in training: the plan, d, and, when
+    a gradient reaches the edge network (``for_mlp``), grad_d [E, out], into which every application's backward adds
+    x_src * G_e before the ONE pass through the edge network (_DiagMlpFn, whose output is ``token``).  Without it dd and
+    token stay None and the backward computes only the gradients of x, root and bias."""
+
+    def __init__(self, key, plan, feats, out_channels, for_mlp):
+        self.key, self.plan, self.feats = key, plan, feats
+        self.dd = (torch.zeros(max(plan.E, 1), out_channels, dtype=torch.float32, device=feats.ea32.device)
+                   if for_mlp else None)
+        self.consumed = False
+        self.token = None
+
+
+class _DiagMlpFn(torch.autograd.Function):
+    """Autograd node of d = nn(edge_attr): a 1-element token stands for d (which lives in the module's cache); every
+    application returns a dummy gradient for it, so this backward runs once, after all of them, on their summed
+    grad_d."""
+
+    @staticmethod
+    def forward(ctx, module, state, edge_attr, *mlp_params):
+        ctx.module, ctx.state = module, state
+        ctx.ea_dtype = edge_attr.dtype
+        return torch.zeros(1, device=edge_attr.device)
+
+    @staticmethod
+    def backward(ctx, _):
+        state = ctx.state
+        grads, gea = ctx.module._backward_mlp_impl(state, want_ea=ctx.needs_input_grad[2])
+        state.consumed = True
+        state.dd = None
+        return (None, None, gea.to(ctx.ea_dtype) if gea is not None else None) + tuple(grads)
+
+
+class _DiagApplyFn(torch.autograd.Function):
+    """One DiagNNConv application given d."""
+
+    @staticmethod
+    def forward(ctx, module, state, x, token, root, bias):
+        ctx.module, ctx.state = module, state
+        x32 = _f32(x)
+        ctx.save_for_backward(x32)
+        ctx.x_dtype = x.dtype
+        out, ctx.argmax = module._apply_impl(state.plan, state.feats, x32)
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        (x32,) = ctx.saved_tensors
+        state = ctx.state
+        dx, droot, dbias = ctx.module._backward_apply_impl(state, x32, _f32(grad_out), ctx.argmax)
+        return (None, None, dx.to(ctx.x_dtype) if ctx.needs_input_grad[2] else None,
+                torch.zeros_like(state.token) if state.token is not None else None, droot, dbias)
+
+
+class DiagNNConv(torch.nn.Module):
+    r"""The diagonal-kernel edge-conditioned convolution of graph-neural-operator/nn_conv.py:8-96 (class ``NNConv``
+    there):  x'_i = x_i root + bias + aggr_{j in N(i)} x_j * nn(e_ij), channel by channel.
+
+    Same signature, attributes, state-dict keys and initialisation as NNConv_old (reference :47-73): the edge network
+    ``nn`` is a Linear (ReLU Linear)* chain whose output width is ``out_channels``.  The reference multiplies x_j by
+    ``diag_embed(nn(e)).view(-1, in, out)``, which is the diagonal matrix only when nn's output width, in_channels and
+    out_channels are equal; any other shape raises NotImplementedError.  ``aggr`` in {'add', 'mean', 'max'} ('max':
+    the rules of NNConv_old), ``precision`` in {'f16' (default), 'bf16', 'f16x2', 'fp32'} selects the edge network's
+    operand type, ``flow`` is PyG's MessagePassing kwarg.
+
+    d_e = nn(e) is x-independent: it is computed once per (edge_attr, parameters), chunk by chunk so that the hidden
+    activations of the edge network are never held for the whole graph, and kept in fp32 (4 * out bytes per edge).
+    Each application is one pass over d.  The backward computes every gradient on the CUDA cores in fp32, recomputing
+    the edge network's activations from edge_attr once per backward pass for all applications of a shared conv.  Cache
+    rules are NNConv_old's: ``invalidate()`` after parameter writes that bypass autograd's version counter.
+    """
+
+    def __init__(self, in_channels, out_channels, nn, aggr='add', root_weight=True, bias=True, **kwargs):
+        super(DiagNNConv, self).__init__()
+        self.precision = kwargs.pop('precision', None)
+        self.flow = kwargs.pop('flow', 'source_to_target')
+        if kwargs:
+            raise TypeError('unexpected keyword arguments %s' % sorted(kwargs))
+        if aggr not in ('add', 'mean', 'max'):
+            raise ValueError("aggr must be 'add', 'mean' or 'max'")
+        if self.flow not in _lib.FLOW:
+            raise ValueError('flow must be source_to_target or target_to_source')
+        self.in_channels = in_channels
+        self.out_channels = out_channels
+        self.nn = nn
+        self.aggr = aggr
+        if root_weight:
+            self.root = Parameter(torch.Tensor(in_channels, out_channels))
+        else:
+            self.register_parameter('root', None)
+        if bias:
+            self.bias = Parameter(torch.Tensor(out_channels))
+        else:
+            self.register_parameter('bias', None)
+        self._prepared = {}             # slot ('forward' / 'backward') -> (key, _DiagWeights)
+        self._d_cache = {}              # at most one entry: cache key -> _DiagFeatures
+        self._tstate = None             # _DiagState of the current training step
+        self.reset_parameters()
+
+    reset_parameters = NNConv_old.reset_parameters
+    __repr__ = NNConv_old.__repr__
+
+    def invalidate(self):
+        """Drop the prepared-weight snapshots and the cached d."""
+        self._prepared.clear()
+        self._d_cache.clear()
+
+    def train(self, mode=True):
+        self.invalidate()
+        return super(DiagNNConv, self).train(mode)
+
+    def _load_from_state_dict(self, *args, **kwargs):
+        self.invalidate()
+        return super(DiagNNConv, self)._load_from_state_dict(*args, **kwargs)
+
+    def _check_shape(self):
+        lin = _linear_chain(self.nn)
+        k = lin[-1].out_features
+        if not (k == self.in_channels == self.out_channels):
+            raise NotImplementedError(
+                'DiagNNConv: the diagonal kernel needs nn output width == in_channels == out_channels; got nn output '
+                '%d, in_channels %d, out_channels %d' % (k, self.in_channels, self.out_channels))
+        return lin
+
+    # -- reference: nn_conv.py:79-84 -----------------------------------------------------------------------------
+    def forward(self, x, edge_index, edge_attr):
+        x = x.unsqueeze(-1) if x.dim() == 1 else x
+        pseudo = edge_attr.unsqueeze(-1) if edge_attr.dim() == 1 else edge_attr
+        lin = self._check_shape()
+        NNConv_old._check_inputs(self, x, edge_index, pseudo)
+        needs_grad = torch.is_grad_enabled() and (
+            x.requires_grad or pseudo.requires_grad or any(p.requires_grad for p in self.parameters()))
+        with torch.cuda.device(x.device):
+            plan = get_plan(edge_index, x.size(0), self.flow)
+            ea32 = _f32(pseudo)
+            feats = self._features(plan, ea32)
+            if not needs_grad:
+                return self._apply_impl(plan, feats, _f32(x))[0]
+            params = [t for l in lin for t in (l.weight, l.bias)]
+            for_mlp = pseudo.requires_grad or any(p.requires_grad for p in params)
+            key = (plan.key, ea32.data_ptr(), tuple(ea32.shape), ea32._version, id(feats), pseudo.requires_grad, for_mlp)
+            st = self._tstate
+            if st is None or st.key != key or st.consumed:
+                st = _DiagState(key, plan, feats, self.out_channels, for_mlp)
+                if for_mlp:
+                    st.token = _DiagMlpFn.apply(self, st, pseudo, *params)
+                self._tstate = st
+            return _DiagApplyFn.apply(self, st, x, st.token, self.root, self.bias)
+
+    # -- host-side sequencing ------------------------------------------------------------------------------------
+    def _get_prepared(self, precision, slot='forward'):
+        linears = _linear_chain(self.nn)
+        key = (precision,) + tuple((l.weight.data_ptr(), l.weight._version, l.bias.data_ptr(), l.bias._version)
+                                   for l in linears)
+        hit = self._prepared.get(slot)
+        if hit is None or hit[0] != key:
+            hit = self._prepared[slot] = (key, _DiagWeights(linears, self.out_channels, precision))
+            if slot == 'forward':
+                self._d_cache.clear()
+        return hit[1]
+
+    def _features(self, plan, ea32):
+        """The cached d of this (plan, parameters, edge_attr), built by nnconv_diag_build on a miss."""
+        prepared = self._get_prepared(self.precision or default_precision())
+        key = (plan.key, ea32.data_ptr(), tuple(ea32.shape), ea32._version, id(prepared))
+        hit = self._d_cache.get(key)
+        if hit is not None:
+            return hit
+        self._d_cache.clear()
+        L = _lib.lib()
+        d_b, ws_b = ctypes.c_size_t(), ctypes.c_size_t()
+        _lib.check(L.nnconv_diag_sizes(plan.handle, prepared.handle, _DIAG_WS_BYTES, ctypes.byref(d_b), ctypes.byref(ws_b)))
+        dev = ea32.device
+        d = torch.empty(d_b.value // 4, dtype=torch.float32, device=dev)
+        ws = torch.empty(ws_b.value, dtype=torch.uint8, device=dev)
+        n_l = ctypes.c_int64(0)
+        _lib.check(L.nnconv_diag_build(plan.handle, prepared.handle, _ptr(ea32), _ptr(d), _ptr(ws), ws_b.value,
+                                       _stream_ptr(dev), ctypes.byref(n_l)))
+        stats['launches'] += n_l.value
+        stats['edge_feature_passes'] += 1
+        NNConv_old._check_overflow(prepared, ws, dev)
+        feats = _DiagFeatures(d, ea32)
+        feats.prepared = prepared
+        self._d_cache[key] = feats
+        return feats
+
+    def _apply_impl(self, plan, feats, x32):
+        """One application (nnconv_apply_diag); returns (out, argmax), argmax None unless aggr='max'."""
+        L = _lib.lib()
+        dev = x32.device
+        aggr = _lib.AGGR[self.aggr]
+        ws_b = ctypes.c_size_t()
+        _lib.check(L.nnconv_apply_diag_sizes(plan.handle, feats.prepared.handle, aggr, ctypes.byref(ws_b)))
+        ws = torch.empty(ws_b.value, dtype=torch.uint8, device=dev)
+        out = torch.empty(x32.size(0), self.out_channels, dtype=torch.float32, device=dev)
+        argmax = torch.empty(x32.size(0), self.out_channels, dtype=torch.int32, device=dev) if self.aggr == 'max' else None
+        n_l = ctypes.c_int64(0)
+        _lib.check(L.nnconv_apply_diag(plan.handle, feats.prepared.handle, _ptr(feats.d), _ptr(x32), _ptr(_f32(self.root)),
+                                       _ptr(_f32(self.bias)), aggr, _ptr(out), _ptr(argmax), _ptr(ws), ws_b.value,
+                                       _stream_ptr(dev), ctypes.byref(n_l)))
+        stats['launches'] += n_l.value
+        stats['applies'] += 1
+        return out, argmax
+
+    def _backward_apply_impl(self, state, x32, g32, argmax):
+        """dx, droot, dbias of one application; adds its share into state.dd (when the edge network needs it)."""
+        L = _lib.lib()
+        dev = x32.device
+        with torch.cuda.device(dev):
+            dx = torch.empty_like(x32)
+            droot = torch.empty_like(self.root, dtype=torch.float32) if self.root is not None else None
+            dbias = torch.empty_like(self.bias, dtype=torch.float32) if self.bias is not None else None
+            n_l = ctypes.c_int64(0)
+            _lib.check(L.nnconv_backward_apply_diag(state.plan.handle, state.feats.prepared.handle, _ptr(state.feats.d),
+                                                    _ptr(x32), _ptr(_f32(self.root)), _lib.AGGR[self.aggr], _ptr(argmax),
+                                                    _ptr(g32), _ptr(dx), _ptr(droot), _ptr(dbias), _ptr(state.dd),
+                                                    _stream_ptr(dev), ctypes.byref(n_l)))
+            stats['launches'] += n_l.value
+            stats['backwards'] += 1
+        return dx, droot, dbias
+
+    def _backward_mlp_impl(self, state, want_ea=False):
+        """Gradients of every Linear of the edge network (weight, bias, in order) from the summed grad_d, and with
+        ``want_ea`` the fp32 gradient w.r.t. edge_attr."""
+        L = _lib.lib()
+        ea32 = state.feats.ea32
+        dev = ea32.device
+        linears = _linear_chain(self.nn)
+        with torch.cuda.device(dev):
+            prep = self._get_prepared('fp32', 'backward')
+            ws_b = ctypes.c_size_t()
+            _lib.check(L.nnconv_backward_mlp_diag_sizes(state.plan.handle, prep.handle, _BWD_WS_BYTES, ctypes.byref(ws_b)))
+            ws = torch.empty(ws_b.value, dtype=torch.uint8, device=dev)
+            dws = [torch.empty_like(l.weight, dtype=torch.float32) for l in linears]
+            dbs = [torch.empty_like(l.bias, dtype=torch.float32) for l in linears]
+            gea = torch.empty_like(ea32) if want_ea else None
+            wp = (ctypes.c_void_p * len(linears))(*[t.data_ptr() for t in dws])
+            bp = (ctypes.c_void_p * len(linears))(*[t.data_ptr() for t in dbs])
+            _lib.check(L.nnconv_backward_mlp_diag(state.plan.handle, prep.handle, _ptr(ea32), _ptr(state.dd), wp, bp,
+                                                  _ptr(ws), ws_b.value, _stream_ptr(dev), _ptr(gea)))
+            stats['mlp_backwards'] += 1
+        return [t for pair in zip(dws, dbs) for t in pair], gea

@@ -68,6 +68,7 @@ extern "C" {
 
 typedef struct nnconv_plan nnconv_plan_t;       /* per edge_index: source grouping, tiles, degrees */
 typedef struct nnconv_weights nnconv_weights_t; /* per parameter version: padded/permuted MLP weights */
+typedef struct nnconv_diag_weights nnconv_diag_weights_t; /* the same for the diagonal-kernel conv (see below) */
 
 const char* nnconv_last_error(void);
 int nnconv_abi_version(void);
@@ -296,6 +297,47 @@ int nnconv_backward_max(const nnconv_plan_t* plan, const nnconv_weights_t* w, co
                         const float* root, const int* argmax, const float* grad_out, float* grad_x,
                         float* const* grad_W, float* const* grad_b, float* grad_root, float* grad_bias, void* ws,
                         size_t ws_bytes, void* stream, float* grad_edge_attr /* nullable */);
+
+/* ---- diagonal-kernel conv (graph-neural-operator/nn_conv.py:8-96, formulation D of DESIGN 4.7): the edge network
+ * ends in `channels` outputs k_e and the message is x_src(e) * k_e channel by channel (in == out == channels):
+ *   out[n] = aggr_{e: dst_e = n} x_src(e) * d_e + x_n root + bias,   d_e = W_L h_e + b_L
+ * aggr as NNCONV_AGGR_* (max: the rules of nnconv_apply_max, argmax written).  d is x-independent: fp32 [E, channels]
+ * in the plan's sorted edge order, built once per (edge_attr, parameters).
+ *   nnconv_diag_weights_*: dims[n_layers] == channels.  Precision f16 / bf16 need 64 or 128 channels, f16x2 at most 64
+ *     (the channel counts its split-precision edge network accepts at in == out), each with the tensor-core edge
+ *     network's hidden widths; fp32 takes any shape.  The backward calls need weights prepared at fp32.  Shapes the
+ *     build does not cover fail in nnconv_diag_build with NNCONV_ERR_UNSUPPORTED.
+ *   nnconv_diag_sizes / nnconv_diag_build: d (d_bytes) from edge_attr in chunks of about want_ws_bytes of workspace;
+ *     the whole h is never held.  The first int of ws counts fp16 overflows of the chunks' activations
+ *     (nnconv_edge_features_overflow).
+ *   nnconv_apply_diag_sizes / nnconv_apply_diag: one application (ws: the max keys; argmax NULL unless aggr is max).
+ *   nnconv_backward_apply_diag: grad_x, grad_root, grad_bias of one application and grad_d += x_src * G_e, where G_e
+ *     is the gradient that reaches the edge's message; grad_d [E, channels] fp32 (sorted order) is zeroed by the
+ *     caller and shared by every application of the conv (NULL: no gradient is needed beyond x, root and bias).
+ *   nnconv_backward_mlp_diag_sizes / nnconv_backward_mlp_diag: the gradients of every Linear of the edge network
+ *     (grad_W[l] [dims[l+1], dims[l]], grad_b[l]) and optionally of edge_attr, from grad_d, in one pass.
+ * No allocation; no host synchronisation. */
+int nnconv_diag_weights_sizes(int n_layers, const int* dims, int channels, int precision, size_t* bytes);
+int nnconv_diag_weights_create(int n_layers, const int* dims, int channels, int precision, const float* const* W,
+                               const float* const* b, void* buf, size_t buf_bytes, void* stream,
+                               nnconv_diag_weights_t** out);
+void nnconv_diag_weights_destroy(nnconv_diag_weights_t* w);
+int nnconv_diag_sizes(const nnconv_plan_t* plan, const nnconv_diag_weights_t* w, size_t want_ws_bytes, size_t* d_bytes,
+                      size_t* ws_bytes);
+int nnconv_diag_build(const nnconv_plan_t* plan, const nnconv_diag_weights_t* w, const float* edge_attr, float* d,
+                      void* ws, size_t ws_bytes, void* stream, int64_t* launches);
+int nnconv_apply_diag_sizes(const nnconv_plan_t* plan, const nnconv_diag_weights_t* w, int aggr, size_t* ws_bytes);
+int nnconv_apply_diag(const nnconv_plan_t* plan, const nnconv_diag_weights_t* w, const float* d, const float* x,
+                      const float* root, const float* bias, int aggr, float* out, int* argmax, void* ws, size_t ws_bytes,
+                      void* stream, int64_t* launches);
+int nnconv_backward_apply_diag(const nnconv_plan_t* plan, const nnconv_diag_weights_t* w, const float* d, const float* x,
+                               const float* root, int aggr, const int* argmax, const float* grad_out, float* grad_x,
+                               float* grad_root, float* grad_bias, float* grad_d, void* stream, int64_t* launches);
+int nnconv_backward_mlp_diag_sizes(const nnconv_plan_t* plan, const nnconv_diag_weights_t* w, size_t want_bytes,
+                                   size_t* ws_bytes);
+int nnconv_backward_mlp_diag(const nnconv_plan_t* plan, const nnconv_diag_weights_t* w, const float* edge_attr,
+                             const float* grad_d, float* const* grad_W, float* const* grad_b, void* ws, size_t ws_bytes,
+                             void* stream, float* grad_edge_attr /* nullable */);
 
 /* ---- halo exchange of the node-range (strip) partition by peer stores over NVLink (no NCCL call, no host round
  * trip between applications).  `out` [n_local, channels] is the result of one application on this rank (owned rows
