@@ -89,6 +89,88 @@ def asymmetric_graph(n_nodes=200, n_edges=3000, seed=7):
     return torch.stack([src[keep], dst[keep]])
 
 
+POW2_DEGREES = (1, 2, 4, 8, 16, 32, 64)
+POW2_WEIGHTS = (.08, .10, .14, .20, .22, .18, .08)         # mean in-degree ~17, as in mixed_graph
+
+
+def _pow2_choice(rng, size, max_in):
+    """``size`` in-degrees drawn from POW2_DEGREES up to ``max_in`` (one number for size None)."""
+    k = sum(d <= max_in for d in POW2_DEGREES)
+    w = np.array(POW2_WEIGHTS[:k])
+    return rng.choice(POW2_DEGREES[:k], size, p=w / w.sum())
+
+
+def _pow2_layout(indeg, srcs_of_slots, rng):
+    """One dst slot per in-edge of ``indeg`` (shuffled), paired with the sources ``srcs_of_slots(E)`` returns."""
+    dst = np.repeat(np.arange(indeg.size), indeg)
+    rng.shuffle(dst)
+    return srcs_of_slots(dst), dst
+
+
+def pow2_indegree_graph(n_nodes=300, hub=700, hub_in=256, seed=5, flow='source_to_target', max_in=64):
+    """Every in-degree 0 or a power of two, so that aggr='mean' scales by exact 1/deg.  Unsorted, directed: a hub
+    source (node 7, ``hub`` out-edges), a hub target (node n/2, ``hub_in`` in-edges), ten copies of one edge, 40
+    self-loops, targets 0..9 without in-edges, and nodes n-10..n-1 isolated; the sources are random, so a node's
+    out-degree differs from its in-degree at most nodes.  Built in (src, dst) terms; under ``flow='target_to_source'``
+    the rows are stored swapped, so that the library reads the same (src, dst) pairs.  The other targets' in-degrees
+    are powers of two up to ``max_in``."""
+    rng = np.random.RandomState(seed)
+    indeg = np.zeros(n_nodes, dtype=np.int64)
+    targets = np.arange(10, n_nodes - 10)
+    indeg[targets] = _pow2_choice(rng, targets.size, max_in)
+    hub_t, dup_t, dup_s = n_nodes // 2, n_nodes // 3, 20
+    indeg[hub_t], indeg[dup_t] = hub_in, 16
+    indeg[dup_t] -= 10                                      # ten of its slots are the copies, laid out below
+    src, dst = _pow2_layout(indeg, lambda d: rng.randint(0, n_nodes - 20, d.size), rng)
+    src[:hub] = 7
+    loops = np.arange(hub, hub + 40)
+    src[loops] = dst[loops]                                 # self-loops
+    src = np.concatenate([src, np.full(10, dup_s)])
+    dst = np.concatenate([dst, np.full(10, dup_t)])
+    perm = rng.permutation(src.size)
+    src, dst = torch.from_numpy(src[perm]), torch.from_numpy(dst[perm])
+    return torch.stack([dst, src] if flow == 'target_to_source' else [src, dst])
+
+
+def pow2_degree_graph(out_degrees, n_nodes, seed, max_in=64):
+    """Source i has out_degrees[i] out-edges; every target's in-degree is a power of two up to ``max_in`` (the
+    remainder in its binary digits), edges in random order."""
+    rng = np.random.RandomState(seed)
+    E = int(sum(out_degrees))
+    indeg = np.zeros(n_nodes, dtype=np.int64)
+    left, order = E, rng.permutation(n_nodes)
+    for n in order:
+        if left == 0:
+            break
+        d = int(_pow2_choice(rng, None, max_in))
+        d = d if d <= left else 1 << (left.bit_length() - 1)
+        indeg[n], left = d, left - d
+    assert left == 0, 'too few nodes for %d edges' % E
+
+    def sources(d):
+        s = np.repeat(np.arange(len(out_degrees)), out_degrees)
+        rng.shuffle(s)
+        return s
+    src, dst = _pow2_layout(indeg, sources, rng)
+    return torch.stack([torch.from_numpy(src), torch.from_numpy(dst)])
+
+
+def pow2_low_degree_graph(n_src, seed):
+    """Formulation B's shape with power-of-two in-degrees: 2-4 out-edges per source, in-degrees in {1, 2, 4, 8}."""
+    rng = np.random.RandomState(seed)
+    indeg = rng.choice([1, 2, 4, 8], n_src, p=[.25, .25, .4, .1])
+    out = np.full(n_src, 3)
+    delta = int(indeg.sum()) - 3 * n_src
+    out[rng.permutation(n_src)[:abs(delta)]] += 1 if delta > 0 else -1
+
+    def sources(d):
+        s = np.repeat(np.arange(n_src), out)
+        rng.shuffle(s)
+        return s
+    src, dst = _pow2_layout(indeg, sources, rng)
+    return torch.stack([torch.from_numpy(src), torch.from_numpy(dst)])
+
+
 def block_diagonal(graphs_and_sizes):
     """Disjoint union of (edge_index, n_nodes) pairs, node ids offset: a batch of graphs."""
     eis, off = [], 0
@@ -130,13 +212,15 @@ WIDE = 2048        # x = b + WIDE * a: 12 significant bits, so an f16x2 pair has
 
 
 def make_probe(ei, n_nodes, layers, cin, cout, *, seed=0, T=1, grad=False, wide_ea=False, wide_x=False, wide_g=False,
-               flow='source_to_target', y_density=1 / 16., g_density=1 / 8., g_rows=1.0, root_bias=True):
+               flow='source_to_target', y_density=1 / 16., g_density=1 / 8., g_rows=1.0, root_bias=True, g_in=None):
     """An exact probe on the graph ``ei`` (any device; the edge attributes are made on its device) for an edge network
     of widths ``layers`` (``layers[-1] == cin * cout``), with T inputs and, with ``grad``, T output gradients.
     ``wide_x`` / ``wide_g``: a quarter of the entries of x (channels >= 1) / of the non-zero output gradients get
     +-2048 added, so that they need 12 significant bits: the f16x2 pairs of Xc, Y, x, G, Ghat, dY and dz then have
     non-zero lo halves (one operand of every product keeps at most 11 bits, so lo * lo stays zero).  ``g_rows``: the
-    fraction of nodes whose output-gradient rows may be non-zero."""
+    fraction of nodes whose output-gradient rows may be non-zero; ``g_in``: if given, the in-degrees (under ``flow``)
+    of the nodes whose output-gradient rows may be non-zero (aggr='mean': a narrow range of 1/deg keeps the 16-bit
+    gradient buffers exact)."""
     assert layers[-1] == cin * cout
     rng = np.random.RandomState(seed)
     k_in = layers[0]
@@ -190,6 +274,9 @@ def make_probe(ei, n_nodes, layers, cin, cout, *, seed=0, T=1, grad=False, wide_
                 g = g * (rng.rand(n_nodes, 1) < g_rows)
             if wide_g:
                 g = g + WIDE * (g != 0) * rng.choice([-1, 0, 0, 0, 0, 0, 0, 1], (n_nodes, cout))
+            if g_in is not None:
+                deg = torch.bincount(dst.cpu(), minlength=n_nodes).numpy()
+                g = g * np.isin(deg, g_in)[:, None]
             gouts.append(torch.from_numpy(g.astype(np.float64)))
     return Probe(ei=ei, n_nodes=n_nodes, flow=flow, layers=list(layers), cin=cin, cout=cout, ea=ea, ws=ws, bs=bs,
                  root=root, bias=bias, x=xs, grad_out=gouts, wide_ea=wide_ea)
@@ -236,9 +323,14 @@ def roundtrip(v, precision):
     return hi
 
 
-def check_16bit(name, v, precision, normalise=False, fp16_range=True):
+FP16_MIN_NORMAL = 2.0 ** -14
+
+
+def check_16bit(name, v, precision, normalise=False, fp16_range=True, normal=False):
     """Every entry of ``v`` is stored unchanged by a 16-bit buffer (after the kernels' power-of-two normalisation by
-    the largest magnitude, if ``normalise``), and inside the fp16 range where a raw fp16 value is stored."""
+    the largest magnitude, if ``normalise``), and inside the fp16 range where a raw fp16 value is stored.  ``normal``:
+    no fp16 value (hi or lo half of an f16x2 pair) is subnormal -- the probes do not rely on every 16-bit writer and
+    every MMA keeping fp16 subnormals."""
     if precision == 'fp32':
         return
     v = v.double()
@@ -250,13 +342,23 @@ def check_16bit(name, v, precision, normalise=False, fp16_range=True):
     if bool(bad.any()):
         raise NotExact('%s: %d of %d values are not exact in %s (e.g. %r)'
                        % (name, int(bad.sum()), v.numel(), precision, float(v[bad][0])))
+    if normal and precision != 'bf16':
+        halves = v.to(torch.float16).double().flatten()
+        small = (halves != 0) & (halves.abs() < FP16_MIN_NORMAL)
+        if bool(small.any()):
+            raise NotExact('%s: %d values are fp16 subnormals (e.g. %r)' % (name, int(small.sum()),
+                                                                           float(halves[small][0])))
 
 
 def check_sum(name, abs_sum, quantum):
-    """A sum whose terms have absolute values adding up to ``abs_sum``, each a multiple of ``quantum``."""
+    """A sum whose terms have absolute values adding up to ``abs_sum``, each a multiple of ``quantum`` (a number, or
+    a tensor of quanta that broadcasts against ``abs_sum``: one per sum)."""
     if abs_sum.numel() == 0:
         return
-    worst = float(abs_sum.max()) / quantum
+    if torch.is_tensor(quantum):
+        worst = float((abs_sum / quantum).max())
+    else:
+        worst = float(abs_sum.max()) / quantum
     if worst > SUM_QUANTA:
         raise NotExact('%s: a sum reaches %.4g quanta, more than 2^22' % (name, worst))
 
@@ -303,16 +405,38 @@ def _split(v, precision):
     return hi, v - hi
 
 
-def assert_exact(probe, precision, kmat=None):
+def in_degree_scale(probe, aggr):
+    """Per-node factor of aggr ('add': 1, 'mean': 1 / max(in-degree, 1)) under the probe's flow, fp64 [N]."""
+    if aggr == 'add':
+        return torch.ones(probe.n_nodes, dtype=torch.float64)
+    deg = torch.bincount(probe.src_dst()[1].cpu(), minlength=probe.n_nodes)
+    return 1.0 / deg.clamp(min=1).double()
+
+
+def assert_exact(probe, precision, kmat=None, aggr='add'):
     """Raise NotExact (naming the buffer) unless every kernel path computes ``probe`` without rounding at
-    ``precision`` ('f16', 'bf16', 'f16x2' or 'fp32').  ``kmat``: also prove formulation B (per-edge kernel matrices;
-    default: when the graph is small enough for the library to build them).  Returns the forward bounds used by the
-    tests: a dict with the per-edge message bound ``msg`` [E] and the largest node sum ``node_sum``."""
+    ``precision`` ('f16', 'bf16', 'f16x2' or 'fp32') and aggregation ``aggr`` ('add' or 'mean').  ``kmat``: also
+    prove formulation B (per-edge kernel matrices; default: when the graph is small enough for the library to build
+    them).  Returns the forward bounds used by the tests: a dict with the per-edge message bound ``msg`` [E] and the
+    largest node sum ``node_sum``.
+
+    aggr='mean' multiplies every message into node n by inv_deg[n] = 1 / deg(n) (and the backward every G and Ghat
+    row of an edge into n): exact only when every in-degree is a power of two, and then a node's sum has quantum
+    q * inv_deg[n].  Every fp16 value of a normalised buffer must also be normal (see ``check_16bit``)."""
     p = probe
     ws, bs = p.ws, p.bs
     ea = p.ea.double().cpu()
     src, dst = (t.cpu() for t in p.src_dst())
     E, N = ea.size(0), p.n_nodes
+    if aggr not in ('add', 'mean'):
+        raise ValueError(aggr)
+    if aggr == 'mean':
+        deg = torch.bincount(dst, minlength=N)
+        odd = torch.nonzero((deg & (deg - 1)) != 0).flatten()
+        if odd.numel():
+            raise NotExact('in-degree: node %d has %d in-edges, not a power of two, so 1/deg is inexact (aggr=mean)'
+                           % (int(odd[0]), int(deg[odd[0]])))
+    inv_deg = in_degree_scale(p, aggr)
     n_lin = len(ws)
     single = n_lin == 1
     if kmat is None:
@@ -370,38 +494,47 @@ def assert_exact(probe, precision, kmat=None):
         init = init + xmax * p.root.abs().sum(0).max()
     if p.bias is not None:
         init = init + p.bias.abs().max()
-    node_sum = init.index_add(0, dst, msg)
-    check_sum('scatter into out[dst] (root, bias and every in-edge)', node_sum, quantum)
+    node_sum = init.index_add(0, dst, msg * inv_deg[dst])
+    # node n's terms are multiples of quantum * inv_deg[n] (root and bias: of quantum)
+    check_sum('scatter into out[dst] (root, bias and every in-edge)', node_sum,
+              quantum * inv_deg if aggr == 'mean' else quantum)
     if kmat and precision in ('f16', 'bf16'):
         for c0 in range(0, h.size(0), 4096):
             kc = h[c0:c0 + 4096] @ wl.t() + bl
             check_16bit('K_e (formulation B)', kc, precision)
             check_sum('K_e build', h[c0:c0 + 4096].abs() @ wl.abs().t() + bl.abs(), _lowest_bit(h))
     if p.grad_out is not None:
-        _assert_exact_backward(p, precision, src, dst, inv, hs, quantum)
+        _assert_exact_backward(p, precision, src, dst, inv, hs, quantum, aggr, inv_deg)
     return {'msg': msg, 'node_sum': node_sum}
 
 
-def _assert_exact_backward(p, precision, src, dst, inv, hs_u, q_fwd):
+def _assert_exact_backward(p, precision, src, dst, inv, hs_u, q_fwd, aggr, inv_deg):
     """The tensor-core backward's 16-bit buffers and fp32 sums, edge by edge (nn_conv / backward_tc.cu):
-    G_e = g[dst_e]; dY_c = sum_{e in c} h_e (x) G_e; dx, dW_L, db_L, droot, dbias; the MLP pass's
-    Ghat_e[t] = g_t[dst_e] * xs_t[src_e] with Y_t = Xc_t W_L, dh_e = sum_t Ghat_e[t] . Y_t[src_e], dz_{L-1} = dh * mask,
-    dz_{l-1} = (dz_l W_l) * mask, dW_l = dz_l^T h_{l-1}, dW_1 against A1, d edge_attr = dz_1 W_1."""
+    G_e = g[dst_e] * s_e; dY_c = sum_{e in c} h_e (x) G_e; dx, dW_L, db_L, droot, dbias; the MLP pass's
+    Ghat_e[t] = g_t[dst_e] * s_e * xs_t[src_e] with Y_t = Xc_t W_L, dh_e = sum_t Ghat_e[t] . Y_t[src_e],
+    dz_{L-1} = dh * mask, dz_{l-1} = (dz_l W_l) * mask, dW_l = dz_l^T h_{l-1}, dW_1 against A1,
+    d edge_attr = dz_1 W_1.  s_e = inv_deg[dst_e] (1 for add): a sum over one source's edges (dY, dx) has the
+    quantum of that source's smallest s_e, a sum over one edge's row (dh, dz W) that of its s_e, and a sum over every
+    edge (dW_L, db_L, dW_l, db_l) that of the smallest s_e."""
     ws, bs = p.ws, p.bs
     cin, cout = p.cin, p.cout
+    mean = aggr == 'mean'
     # an edge whose target has a zero gradient row in every application adds exact zeros to every buffer and sum below
     active = torch.stack([(g[dst] != 0).any(1) for g in p.grad_out]).any(0)
     src, dst, inv = src[active], dst[active], inv[active]
+    s_e = inv_deg[dst]                                             # [E]
+    s_min = float(s_e.min()) if s_e.numel() else 1.0
     hs = [a[inv] for a in hs_u]                                   # per active edge
     h = hs[-1]
     wl = ws[-1]
     order = torch.argsort(src, stable=True)
     counts = torch.bincount(src, minlength=p.n_nodes)
+    s_src = torch.ones(p.n_nodes, dtype=torch.float64).scatter_reduce(0, src, s_e, 'amin')   # per source
     E = h.size(0)
     gq = min(_lowest_bit(g) for g in p.grad_out)
     for t, (x, g) in enumerate(zip(p.x, p.grad_out)):
-        G = g[dst]
-        check_16bit('G (gathered output gradient), application %d' % t, G, precision, normalise=True)
+        G = g[dst] * s_e.unsqueeze(1)
+        check_16bit('G (gathered output gradient), application %d' % t, G, precision, normalise=True, normal=mean)
         # dY_c = h_c^T G_c  per source (in groups of sources), and the sums that read it
         if not bool(active.any()):
             continue
@@ -416,34 +549,36 @@ def _assert_exact_backward(p, precision, src, dst, inv, hs_u, q_fwd):
                               G[order[int(starts[c]):int(starts[c] + counts[c])]] for c in cs])    # [S, K, cout]
             dyabs = torch.stack([h[order[int(starts[c]):int(starts[c] + counts[c])]].abs().t() @
                                  G[order[int(starts[c]):int(starts[c] + counts[c])]].abs() for c in cs])
-            check_sum('dY (k_dy), application %d' % t, dyabs, _lowest_bit(h) * gq)
-            check_16bit('dY, application %d' % t, dY, precision, normalise=True)
+            q_dy = _lowest_bit(h) * gq * (s_src[torch.tensor(cs)].view(-1, 1, 1) if mean else 1.0)
+            check_sum('dY (k_dy), application %d' % t, dyabs, q_dy)
+            check_16bit('dY, application %d' % t, dY, precision, normalise=True, normal=mean)
             # dx_c[i] = sum_{k,o} dY_c[k,o] W_L[i*cout+o, k]
             check_sum('dx = dY : W_L, application %d' % t, torch.einsum('sko,iok->si', dyabs, wl3),
-                      _lowest_bit(h) * gq)
+                      q_dy.view(-1, 1) if mean else q_dy)
             check_product('dx GEMM', dY, wl, precision)
             check_product('dW_L GEMM', x, dY, precision)
             dwl_abs += torch.einsum('si,sko->iok', x[torch.tensor(cs)].abs(), dyabs)
-        check_16bit('x rows of dW_L, application %d' % t, x, precision, normalise=True)
-        check_sum('dW_L = x (x) dY, application %d' % t, dwl_abs, _lowest_bit(x) * _lowest_bit(h) * gq)
-        check_sum('db_L, application %d' % t, x[src].abs().t() @ G.abs(), _lowest_bit(x) * gq)
+        check_16bit('x rows of dW_L, application %d' % t, x, precision, normalise=True, normal=mean)
+        check_sum('dW_L = x (x) dY, application %d' % t, dwl_abs, _lowest_bit(x) * _lowest_bit(h) * gq * s_min)
+        check_sum('db_L, application %d' % t, x[src].abs().t() @ G.abs(), _lowest_bit(x) * gq * s_min)
     # MLP pass, all applications together
     xs_scale = [torch.tensor([_pow2_ge(float(v)) for v in x.abs().max(1).values]) for x in p.x]
-    ghat = torch.cat([g[dst] * s[src].unsqueeze(1) for g, s in zip(p.grad_out, xs_scale)], 1)
-    check_16bit('Ghat (MLP pass)', ghat, precision, normalise=True)
+    ghat = torch.cat([g[dst] * (s_e * s[src]).unsqueeze(1) for g, s in zip(p.grad_out, xs_scale)], 1)
+    check_16bit('Ghat (MLP pass)', ghat, precision, normalise=True, normal=mean)
     dh = torch.zeros_like(h)
     dh_abs = torch.zeros_like(h)
     for x, g in zip(p.x, p.grad_out):
-        P = (x[src].unsqueeze(2) * g[dst].unsqueeze(1)).reshape(E, cin * cout)
+        P = (x[src].unsqueeze(2) * (g[dst] * s_e.unsqueeze(1)).unsqueeze(1)).reshape(E, cin * cout)
         dh += P @ wl
         dh_abs += P.abs() @ wl.abs()
-    check_sum('dh = Ghat . Y^T (k_dh)', dh_abs, min(_lowest_bit(x) for x in p.x) * gq * _lowest_bit(wl))
+    row_q = s_e.unsqueeze(1) if mean else 1.0                      # every term of edge e's row carries s_e
+    check_sum('dh = Ghat . Y^T (k_dh)', dh_abs, min(_lowest_bit(x) for x in p.x) * gq * _lowest_bit(wl) * row_q)
     check_product('k_dh Ghat . Y^T', ghat, torch.cat(p.x), precision)
     n_lin = len(ws)
     if n_lin == 1:
         return
     dz = dh * (h > 0)
-    check_16bit('dz %d' % (n_lin - 1), dz, precision, normalise=True)
+    check_16bit('dz %d' % (n_lin - 1), dz, precision, normalise=True, normal=mean)
     for l in range(n_lin - 1, 0, -1):                              # dz is the gradient at layer l's pre-activation
         a = hs[l - 1]
         if l == 1 and p.layers[0] <= 20:
@@ -456,11 +591,12 @@ def _assert_exact_backward(p, precision, src, dst, inv, hs_u, q_fwd):
         check_sum('db_%d' % l, dz.abs().sum(0, keepdim=True), qz)
         check_product('dW_%d GEMM' % l, dz, a, precision)
         w = ws[l - 1]
-        check_sum('d input of layer %d = dz W' % l, dz.abs() @ w.abs(), qz * _lowest_bit(w))
+        qz_row = _lowest_bit(dz / row_q) * row_q if mean else qz
+        check_sum('d input of layer %d = dz W' % l, dz.abs() @ w.abs(), qz_row * _lowest_bit(w))
         if l > 1:
             check_product('dz_%d GEMM' % (l - 1), dz, w, precision)
             dz = (dz @ w) * (a > 0)
-            check_16bit('dz %d' % (l - 1), dz, precision, normalise=True)
+            check_16bit('dz %d' % (l - 1), dz, precision, normalise=True, normal=mean)
 
 
 # ---- the probes of the GPU tests (tests/test_probe_exactness.py proves every one of them) ------------------------------
@@ -493,6 +629,26 @@ def graph(name):
         return low_degree_graph(4096, 1), 4096
     if name == 'low_degree_256':
         return low_degree_graph(256, 2), 256
+    # power-of-two in-degrees (aggr='mean'), every graph in the (src, dst) rows of flow source_to_target but the t2s
+    # one; suffix '_in32': in-degrees up to 32 (hub target included), for the probes with 12-bit x or g
+    if name.startswith('pow2_'):
+        base, max_in = (name[:-5], 32) if name.endswith('_in32') else (name, 64)
+        hub_in, sfx = (256, '') if max_in == 64 else (max_in, '_in32')
+        if base == 'pow2_mixed':
+            return pow2_indegree_graph(hub_in=hub_in, max_in=max_in), 300
+        if base == 'pow2_t2s':                   # another graph of the same kind, rows stored (dst, src)
+            return pow2_indegree_graph(hub_in=hub_in, seed=6, flow='target_to_source', max_in=max_in), 300
+        if base == 'pow2_partial_tiles':
+            return pow2_degree_graph(PARTIAL_TILE_DEGREES, 600, seed=9, max_in=max_in), 600
+        if base == 'pow2_hub_batches':           # a hub of 2,500 out-edges among ~380 sources
+            return pow2_indegree_graph(400, hub=2500, hub_in=hub_in, seed=17, max_in=max_in), 400
+        if base == 'pow2_batch':                 # a union keeps every in-degree
+            return block_diagonal([graph('pow2_mixed' + sfx), (graph('pow2_t2s' + sfx)[0].flip(0), 300),
+                                   (pow2_degree_graph([3, 130, 1, 257], 50, seed=4, max_in=max_in), 50)])
+        if base == 'pow2_low_degree_4096':
+            return pow2_low_degree_graph(4096, 1), 4096
+        if base == 'pow2_low_degree_256':
+            return pow2_low_degree_graph(256, 2), 256
     if name == 'darcy241':
         from oracle import nnconv_oracle as O
         return torch.from_numpy(O.ball_connectivity(241, 0.05)), 241 * 241
@@ -556,9 +712,62 @@ WIDE_F16X2 = {
 }
 
 
+# aggr='mean' probes: every in-degree under the probe's flow is 0 or a power of two (graphs 'pow2_*'), so that 1/deg
+# is exact and the library must equal the fp64 mean bit for bit, as for add.
+MEAN_FORWARD = {
+    'mixed': ('pow2_mixed', [6, 64, 128, 64 * 64], 64, 64, {}, ('f16', 'bf16', 'f16x2', 'fp32')),
+    't2s': ('pow2_t2s', [6, 64, 128, 64 * 64], 64, 64, {'flow': 'target_to_source'}, ('f16', 'bf16', 'f16x2')),
+    'batch': ('pow2_batch', [6, 64, 128, 64 * 64], 64, 64, {}, ('f16', 'bf16', 'f16x2')),
+    'hub_batches': ('pow2_hub_batches', [6, 64, 256, 64 * 64], 64, 64, {}, ('f16', 'bf16', 'f16x2')),
+    'partial_tiles': ('pow2_partial_tiles', [6, 32, 128, 64 * 64], 64, 64, {}, ('f16', 'bf16', 'f16x2')),
+    'edge_v64_src': ('pow2_low_degree_4096', [4, 64, 64, 64 * 64], 64, 64, {}, ('f16', 'bf16')),
+    'edge_v64': ('pow2_low_degree_256', [4, 64, 64, 64 * 64], 64, 64, {}, ('f16', 'bf16')),
+    'edge_v32': ('pow2_low_degree_256', [4, 64, 64, 32 * 32], 32, 32, {}, ('f16', 'bf16')),
+    'edge_scalar_src': ('pow2_low_degree_4096', [4, 64, 64, 16 * 64], 16, 64, {}, ('f16', 'bf16')),
+    'edge_scalar': ('pow2_low_degree_256', [4, 64, 64, 48 * 48], 48, 48, {}, ('f16', 'bf16')),
+}
+
+MEAN_BACKWARD = {
+    'mixed': ('pow2_mixed', [6, 64, 128, 64 * 64], 64, 64, {'T': 2}, ('f16', 'bf16', 'f16x2', 'fp32')),
+    'mixed_T1': ('pow2_mixed', [6, 64, 128, 64 * 64], 64, 64, {'T': 1}, ('f16', 'bf16', 'f16x2')),
+    'mixed_T7': ('pow2_mixed', [6, 64, 128, 64 * 64], 64, 64, {'T': 7}, ('f16', 'bf16')),
+    'mixed_T13': ('pow2_mixed', [6, 64, 128, 64 * 64], 64, 64, {'T': 13}, ('f16', 'bf16', 'f16x2')),
+    't2s': ('pow2_t2s', [6, 64, 128, 64 * 64], 64, 64, {'T': 2, 'flow': 'target_to_source'},
+            ('f16', 'bf16', 'f16x2', 'fp32')),
+    't2s_T1': ('pow2_t2s', [6, 64, 128, 64 * 64], 64, 64, {'T': 1, 'flow': 'target_to_source'}, ('f16', 'bf16', 'f16x2')),
+    't2s_T7': ('pow2_t2s', [6, 64, 128, 64 * 64], 64, 64, {'T': 7, 'flow': 'target_to_source'}, ('f16', 'bf16')),
+    't2s_T13': ('pow2_t2s', [6, 64, 128, 64 * 64], 64, 64, {'T': 13, 'flow': 'target_to_source'},
+                ('f16', 'bf16', 'f16x2')),
+    'batch': ('pow2_batch', [6, 64, 128, 64 * 64], 64, 64, {'T': 2}, ('f16', 'bf16')),
+    'cuda_core_out32': ('pow2_mixed', [6, 64, 128, 32 * 32], 32, 32, {'T': 2}, ('f16', 'fp32')),
+    'cuda_core_in128': ('pow2_mixed', [6, 64, 128, 128 * 64], 128, 64, {'T': 2}, ('f16', 'fp32')),
+}
+
+# Per-precision make_probe options of the mean probes.  A dY entry of the 700-edge hub source mixes terms scaled by
+# 1/1 .. 1/256, and the 16-bit dY must hold it: at f16 the gradient rows are non-zero only at targets of in-degree 8 to
+# 256, at half the density; at bf16 (8 bits) only at targets of in-degree 16.  At f16x2, x carries 12-bit values
+# (lo halves) on the '_in32' graphs (in-degrees up to 32: a 256-edge hub target's message sum of 12-bit x leaves the
+# 2^22 budget), and the gradient rows are non-zero at an eighth of the targets of in-degree 16, so that dz stays in the
+# fp16 normal range.  12-bit output gradients do not fit at mean: the hub source's dY then spans more than the fp16
+# normal range.
+MEAN_OPTIONS = {
+    'forward': {'f16x2': {'wide_x': True, 'graph': '_in32'}},
+    'backward': {'f16': {'g_in': (8, 16, 32, 64, 256), 'g_density': 1 / 16.}, 'bf16': {'g_in': (16,)},
+                 'f16x2': {'wide_x': True, 'g_rows': 0.125, 'g_in': (16,), 'graph': '_in32'}},
+}
+MEAN_PLAIN = ('edge_v64_src', 'edge_v64', 'edge_v32', 'edge_scalar_src', 'edge_scalar', 'cuda_core_out32',
+              'cuda_core_in128')                 # formulation B and the CUDA-core shapes: the table's options only
+MEAN_PLAIN_F16X2_FORWARD = ('batch', 'hub_batches', 'partial_tiles')    # small-integer x: 12-bit x leaves the budget
+
+
 def wide_options(table, name, precision, wide='x'):
     """make_probe options of the f16x2 variant of a probe (``wide``: 'x' or 'g', the backward operand that carries the
-    lo halves), else {}."""
+    lo halves), else {}; for a probe of ``MEAN_FORWARD`` or ``MEAN_BACKWARD``, its options at ``precision``
+    (``MEAN_OPTIONS``, where 'graph' is the suffix of the graph to use)."""
+    if table is MEAN_FORWARD or table is MEAN_BACKWARD:
+        if name in MEAN_PLAIN or (table is MEAN_FORWARD and name in MEAN_PLAIN_F16X2_FORWARD):
+            return {}
+        return dict(MEAN_OPTIONS['forward' if table is MEAN_FORWARD else 'backward'].get(precision, {}))
     if precision != 'f16x2':
         return {}
     if table is FORWARD:
@@ -567,9 +776,10 @@ def wide_options(table, name, precision, wide='x'):
 
 
 def probe(table, name, device='cpu', precision=None, wide='x'):
-    """The probe ``name`` of ``FORWARD`` or ``BACKWARD`` with its graph on ``device``; at precision 'f16x2' the variant
-    with lo halves where the budget allows (``wide``: which backward operand carries them, 'x' or 'g')."""
+    """The probe ``name`` of ``FORWARD``, ``BACKWARD``, ``MEAN_FORWARD`` or ``MEAN_BACKWARD`` with its graph on
+    ``device``; at precision 'f16x2' the variant with lo halves where the budget allows (``wide``: which backward
+    operand carries them, 'x' or 'g')."""
     gname, layers, cin, cout, opts, _ = table[name]
-    ei, n = graph(gname)
     opts = dict(opts, **wide_options(table, name, precision, wide))
-    return make_probe(ei.to(device), n, layers, cin, cout, grad=table is BACKWARD, **opts)
+    ei, n = graph(gname + opts.pop('graph', ''))
+    return make_probe(ei.to(device), n, layers, cin, cout, grad=table is BACKWARD or table is MEAN_BACKWARD, **opts)

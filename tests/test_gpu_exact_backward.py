@@ -28,13 +28,15 @@ def _cls():
 _REF = {}
 
 
-def _reference(p, key):
-    """fp64 autograd on the CPU of sum_t sum(conv(x_t) * g_t) (aggr='add')."""
+def _reference(p, key, aggr='add'):
+    """fp64 autograd on the CPU of sum_t sum(conv(x_t) * g_t)."""
     if key in _REF:
         return _REF[key]
     src, dst = (t.cpu() for t in p.src_dst())
-    # only edges whose target has a non-zero gradient row contribute (exact zeros elsewhere): autograd on those
+    # only edges whose target has a non-zero gradient row contribute (exact zeros elsewhere): autograd on those, with
+    # the mean's in-degrees counted over every edge
     active = torch.stack([(g[dst] != 0).any(1) for g in p.grad_out]).any(0)
+    inv_deg = P.in_degree_scale(p, aggr).unsqueeze(1)
     src, dst = src[active], dst[active]
     leaves = {'ea': p.ea.double().cpu()[active], 'root': p.root.clone(), 'bias': p.bias.clone()}
     for i, (w, b) in enumerate(zip(p.ws, p.bs)):
@@ -45,8 +47,13 @@ def _reference(p, key):
     n = len(p.ws)
     loss = 0
     for x, g in zip(xs, p.grad_out):
-        out = O.nnconv_forward(x, torch.stack([src, dst]), leaves['ea'], [leaves['w%d' % i] for i in range(n)],
-                               [leaves['b%d' % i] for i in range(n)], leaves['root'], leaves['bias'], 'add')
+        ws, bs = [leaves['w%d' % i] for i in range(n)], [leaves['b%d' % i] for i in range(n)]
+        if aggr == 'add':
+            out = O.nnconv_forward(x, torch.stack([src, dst]), leaves['ea'], ws, bs, leaves['root'], leaves['bias'],
+                                   'add')
+        else:                   # the active edges are every in-edge of a node with a gradient row
+            out = O.nnconv_forward(x, torch.stack([src, dst]), leaves['ea'], ws, bs, None, None, 'add') * inv_deg
+            out = out + x @ leaves['root'] + leaves['bias']
         loss = loss + (out * g).sum()
     loss.backward()
     ref = {k: v.grad for k, v in leaves.items()}
@@ -56,8 +63,8 @@ def _reference(p, key):
     return ref
 
 
-def _library(p, precision, with_conv=False, **kw):
-    conv = p.conv(_cls(), precision, 'add', DEV, **kw)
+def _library(p, precision, with_conv=False, aggr='add', **kw):
+    conv = p.conv(_cls(), precision, aggr, DEV, **kw)
     ea = p.ea.to(DEV).requires_grad_()
     ei = p.ei.to(DEV)
     xs = [x.float().to(DEV).requires_grad_() for x in p.x]
