@@ -43,7 +43,10 @@ SYMBOLS = [
     'nnconv_diag_weights_sizes', 'nnconv_diag_weights_create', 'nnconv_diag_weights_destroy', 'nnconv_diag_sizes',
     'nnconv_diag_build', 'nnconv_apply_diag_sizes', 'nnconv_apply_diag', 'nnconv_backward_apply_diag',
     'nnconv_backward_mlp_diag_sizes', 'nnconv_backward_mlp_diag',
+    'nnconv_gcn_graph_sizes', 'nnconv_gcn_graph_create', 'nnconv_gcn_graph_destroy', 'nnconv_gcn_apply_sizes',
+    'nnconv_gcn_apply', 'nnconv_gcn_backward_sizes', 'nnconv_gcn_backward',
 ]
+GCN_IMPROVED, GCN_NO_SELF_LOOPS, GCN_NO_NORMALIZE = 1, 2, 4   # include/nnconv_b200.h NNCONV_GCN_*
 
 
 class NNConvLibraryError(RuntimeError):
@@ -170,6 +173,15 @@ def lib():
                                              P(c_i64)]
     L.nnconv_backward_mlp_diag_sizes.argtypes = [c_vp, c_vp, c_sz, P(c_sz)]
     L.nnconv_backward_mlp_diag.argtypes = [c_vp, c_vp, c_vp, c_vp, P(c_vp), P(c_vp), c_vp, c_sz, c_vp, c_vp]
+    L.nnconv_gcn_graph_sizes.argtypes = [c_i64, c_i64, P(c_sz), P(c_sz)]
+    L.nnconv_gcn_graph_create.argtypes = [c_vp, c_vp, c_i64, c_i64, c_int, c_int, c_vp, c_sz, c_vp, c_sz, c_vp, P(c_vp)]
+    L.nnconv_gcn_graph_destroy.argtypes = [c_vp]
+    L.nnconv_gcn_graph_destroy.restype = None
+    L.nnconv_gcn_apply_sizes.argtypes = [c_vp, c_int, c_int, c_int, P(c_sz)]
+    L.nnconv_gcn_apply.argtypes = [c_vp, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_sz, c_vp, P(c_i64)]
+    L.nnconv_gcn_backward_sizes.argtypes = [c_vp, c_int, c_int, c_int, P(c_sz)]
+    L.nnconv_gcn_backward.argtypes = [c_vp, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_sz, c_vp,
+                                      P(c_i64)]
     for name in SYMBOLS:
         getattr(L, name)
     if L.nnconv_abi_version() != ABI_VERSION:

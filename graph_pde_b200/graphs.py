@@ -238,3 +238,20 @@ def multi_pole_grid1d(theta, s, is_periodic=False, levels=None, device='cpu'):
         ei_list.append(e)
         ea_list.append(attr(e))
     return X_list, ei_list, ea_list
+
+
+def grid_edge(n_x, n_y, device='cpu'):
+    """The lattice of MGNO/utilities.py:1480-1520 (``grid_edge(n_x, n_y)``, a = None), vectorised: returns
+    (grid [n_x n_y, 2] fp32, edge_index [2, E] int64).  Node i = y n_x + x sits at (x / (n_x - 1), y / (n_y - 1)); node
+    by node in that order, the edges are (i, i+1), (i+1, i) unless x is the last column, then (i, i+n_x), (i+n_x, i)
+    unless y is the last row -- the reference's edge order."""
+    xs = torch.linspace(0.0, 1.0, n_x, dtype=torch.float64)
+    ys = torch.linspace(0.0, 1.0, n_y, dtype=torch.float64)
+    gy, gx = torch.meshgrid(ys, xs, indexing='ij')
+    grid = torch.stack([gx.reshape(-1), gy.reshape(-1)], dim=1).float().to(device)
+    i = torch.arange(n_x * n_y, dtype=torch.int64, device=device)
+    x, y = i % n_x, i // n_x
+    pairs = torch.stack([torch.stack([i, i + 1], 1), torch.stack([i + 1, i], 1),
+                         torch.stack([i, i + n_x], 1), torch.stack([i + n_x, i], 1)], dim=1)   # [N, 4, 2]
+    ok = torch.stack([x != n_x - 1, x != n_x - 1, y != n_y - 1, y != n_y - 1], dim=1)       # [N, 4]
+    return grid, pairs[ok].t().contiguous()

@@ -8,6 +8,7 @@ scripts so that their checkpoints / training loops carry over:
 * ``MKGN``          -- multipole-graph-neural-operator/MGKN_general_darcy2d.py:21-94 (mid conv with root,
                        level-sliced node ranges)
 * ``MGKN``          -- multipole-graph-neural-operator/MGKN_orthogonal_burgers1d.py:21-86
+* ``GCN_Net``       -- multipole-graph-neural-operator/neurips4_GCN.py:20-53 (the GCN baseline, GCNConv)
 
 Only the conv applications run in the CUDA library; the pointwise lifts / projections (fc*) stay
 torch.nn.Linear exactly as in the reference (they are not on the hot path, SURVEY 8(a)).
@@ -18,6 +19,7 @@ import numpy as np
 import torch
 import torch.nn.functional as F
 
+from .gcn import GCNConv
 from .nn_conv import NNConv, NNConv_old
 
 # NNCONV_B200_FUSED_STEPS=0: KernelInduced inference runs the reference's op sequence (conv, add, ReLU as separate kernels)
@@ -243,3 +245,30 @@ class MGKN(torch.nn.Module):
                     x = F.relu(x + self.conv_list[0](phi[0], edge_index_list[0], edge_attr_list[0]))
         x = F.relu(self.fc2(x))
         return self.fc3(x)
+
+
+class GCN_Net(torch.nn.Module):
+    """neurips4_GCN.py:20-53: fc_in, four GCNConv(width, width) applied ``depth`` times with ReLUs, fc_out1, fc_out2."""
+
+    def __init__(self, width, ker_width, depth, in_width=1, out_width=1, precision=None):
+        super(GCN_Net, self).__init__()
+        self.depth = depth
+        self.width = width
+        self.fc_in = torch.nn.Linear(in_width, width)
+        self.conv1 = GCNConv(width, width, precision=precision)
+        self.conv2 = GCNConv(width, width, precision=precision)
+        self.conv3 = GCNConv(width, width, precision=precision)
+        self.conv4 = GCNConv(width, width, precision=precision)
+        self.fc_out1 = torch.nn.Linear(width, ker_width)
+        self.fc_out2 = torch.nn.Linear(ker_width, 1)      # the reference ignores out_width here
+
+    def forward(self, data):
+        x, edge_index = data.x, data.edge_index
+        x = self.fc_in(x)
+        for _ in range(self.depth):
+            x = F.relu(self.conv1(x, edge_index))
+            x = F.relu(self.conv2(x, edge_index))
+            x = F.relu(self.conv3(x, edge_index))
+            x = F.relu(self.conv4(x, edge_index))
+        x = F.relu(self.fc_out1(x))
+        return self.fc_out2(x)

@@ -82,6 +82,8 @@ def default_precision():
 
 def clear_caches():
     _PLAN_CACHE.clear()
+    from . import gcn          # the GCNConv graphs (gcn imports this module, so not at the top)
+    gcn._GRAPH_CACHE.clear()
 
 
 class _CaptureSink(object):

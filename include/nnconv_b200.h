@@ -339,6 +339,39 @@ int nnconv_backward_mlp_diag(const nnconv_plan_t* plan, const nnconv_diag_weight
                              const float* grad_d, float* const* grad_W, float* const* grad_b, void* ws, size_t ws_bytes,
                              void* stream, float* grad_edge_attr /* nullable */);
 
+/* ---- GCNConv (PyG 1.x GCNConv, the reference's neurips4_GCN.py baseline; DESIGN 4.8):
+ *   out = A_hat x W + bias,   A_hat = D^-1/2 (A + I_fill) D^-1/2
+ * with A[dst, src] counting every caller edge (duplicates once each) except self loops; every node gets one loop of
+ * weight 1 if the caller's list had one, else `fill` (2 with NNCONV_GCN_IMPROVED, else 1); D sums the weights at the
+ * target.  deg^-1/2 is 0 for a zero degree.  NNCONV_GCN_NO_SELF_LOOPS: no loop is added (a caller's loops count with
+ * weight 1); NNCONV_GCN_NO_NORMALIZE: A_hat = A including the caller's loops.  flow as for nnconv_plan_create.
+ *   nnconv_gcn_graph_sizes / _create / _destroy: the graph of one edge_index (CSRs by target and by source, per-entry
+ *     norm, per-node diagonal).  Creation checks the indices and synchronises; nothing after it does.
+ *   nnconv_gcn_apply_sizes / nnconv_gcn_apply: out [N, out] = A_hat x W + bias (bias nullable); x [N, in], W [in, out]
+ *     fp32.  Precision f16 / bf16 / f16x2 need in and out multiples of 16 in [16, 128] (NNCONV_ERR_UNSUPPORTED
+ *     otherwise) and 16-byte aligned x, out; fp32 takes any shape.
+ *   nnconv_gcn_backward_sizes / nnconv_gcn_backward: grad_x = A_hat^T g W^T, grad_weight = x^T A_hat^T g and
+ *     grad_bias = sum_n g_n (nullable), all WRITTEN.
+ * Results are bitwise reproducible run to run (no atomics).  No allocation. */
+#define NNCONV_GCN_IMPROVED 1
+#define NNCONV_GCN_NO_SELF_LOOPS 2
+#define NNCONV_GCN_NO_NORMALIZE 4
+typedef struct nnconv_gcn_graph nnconv_gcn_graph_t;
+int nnconv_gcn_graph_sizes(int64_t E, int64_t N, size_t* ws_bytes, size_t* tmp_bytes);
+int nnconv_gcn_graph_create(const int64_t* row0, const int64_t* row1, int64_t E, int64_t N, int flow, int flags, void* ws,
+                            size_t ws_bytes, void* tmp, size_t tmp_bytes, void* stream, nnconv_gcn_graph_t** out);
+void nnconv_gcn_graph_destroy(nnconv_gcn_graph_t* graph);
+int nnconv_gcn_apply_sizes(const nnconv_gcn_graph_t* graph, int precision, int in_channels, int out_channels,
+                           size_t* ws_bytes);
+int nnconv_gcn_apply(const nnconv_gcn_graph_t* graph, int precision, int in_channels, int out_channels, const float* x,
+                     const float* weight, const float* bias, float* out, void* ws, size_t ws_bytes, void* stream,
+                     int64_t* launches);
+int nnconv_gcn_backward_sizes(const nnconv_gcn_graph_t* graph, int precision, int in_channels, int out_channels,
+                              size_t* ws_bytes);
+int nnconv_gcn_backward(const nnconv_gcn_graph_t* graph, int precision, int in_channels, int out_channels, const float* x,
+                        const float* weight, const float* grad_out, float* grad_x, float* grad_weight,
+                        float* grad_bias /* nullable */, void* ws, size_t ws_bytes, void* stream, int64_t* launches);
+
 /* ---- halo exchange of the node-range (strip) partition by peer stores over NVLink (no NCCL call, no host round
  * trip between applications).  `out` [n_local, channels] is the result of one application on this rank (owned rows
  * [own_lo, own_hi) valid); the call writes relu?(out) of the owned rows into this rank's next-application buffer
