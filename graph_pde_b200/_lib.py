@@ -17,6 +17,8 @@ PREC = {'fp32': 0, 'f16': 1, 'fp16': 1, 'bf16': 2, 'f16x2': 3}
 AGGR = {'add': 0, 'mean': 1, 'max': 2}     # max: through the nnconv_*_max entry points only
 APPLY_RELU_IN, APPLY_RESIDUAL = 1, 2        # include/nnconv_b200.h NNCONV_APPLY_*
 FLOW = {'source_to_target': 0, 'target_to_source': 1}
+# hidden activation of the edge MLP, include/nnconv_b200.h NNCONV_ACT_*
+ACT = {'relu': 0, 'leaky_relu': 1, 'elu': 2, 'tanh': 3, 'sigmoid': 4}
 
 # every symbol include/nnconv_b200.h declares (tests/test_cabi_symbols.py checks the .so exports them)
 SYMBOLS = [
@@ -45,6 +47,7 @@ SYMBOLS = [
     'nnconv_backward_mlp_diag_sizes', 'nnconv_backward_mlp_diag',
     'nnconv_gcn_graph_sizes', 'nnconv_gcn_graph_create', 'nnconv_gcn_graph_destroy', 'nnconv_gcn_apply_sizes',
     'nnconv_gcn_apply', 'nnconv_gcn_backward_sizes', 'nnconv_gcn_backward',
+    'nnconv_weights_create_act', 'nnconv_diag_weights_create_act',
 ]
 GCN_IMPROVED, GCN_NO_SELF_LOOPS, GCN_NO_NORMALIZE = 1, 2, 4   # include/nnconv_b200.h NNCONV_GCN_*
 
@@ -90,6 +93,8 @@ def lib():
     L.nnconv_weights_sizes.argtypes = [c_int, P(c_int), c_int, c_int, c_int, P(c_sz)]
     L.nnconv_weights_create.argtypes = [c_int, P(c_int), c_int, c_int, c_int, P(c_vp), P(c_vp), c_vp, c_sz, c_vp,
                                         P(c_vp)]
+    L.nnconv_weights_create_act.argtypes = [c_int, P(c_int), c_int, c_int, c_int, c_int, ctypes.c_float, P(c_vp), P(c_vp),
+                                            c_vp, c_sz, c_vp, P(c_vp)]
     L.nnconv_weights_destroy.argtypes = [c_vp]
     L.nnconv_weights_destroy.restype = None
     L.nnconv_weights_tc_supported.argtypes = [c_vp]
@@ -163,6 +168,8 @@ def lib():
                                       c_sz, c_vp, c_vp]
     L.nnconv_diag_weights_sizes.argtypes = [c_int, P(c_int), c_int, c_int, P(c_sz)]
     L.nnconv_diag_weights_create.argtypes = [c_int, P(c_int), c_int, c_int, P(c_vp), P(c_vp), c_vp, c_sz, c_vp, P(c_vp)]
+    L.nnconv_diag_weights_create_act.argtypes = [c_int, P(c_int), c_int, c_int, c_int, ctypes.c_float, P(c_vp), P(c_vp),
+                                                 c_vp, c_sz, c_vp, P(c_vp)]
     L.nnconv_diag_weights_destroy.argtypes = [c_vp]
     L.nnconv_diag_weights_destroy.restype = None
     L.nnconv_diag_sizes.argtypes = [c_vp, c_vp, c_sz, P(c_sz), P(c_sz)]

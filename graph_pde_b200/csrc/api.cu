@@ -295,7 +295,7 @@ int edge_features_rows(const Plan* P, const Weights* W, const float* edge_attr, 
   if (rowb == 0) {   // CUDA-core first layer straight into h (2-layer MLP: fp32, or k_in > 20 in 16 bits)
     ProfScope ps(PK_LAYER1, st);
     s = launch_edge_layer1(W->prec, edge_attr, P->perm, e_begin, E, W->dims[0], W->W1, W->b1, W->kp[1], 0, h, st, hpad, 0,
-                           overflow);
+                           overflow, act_of(W));
     if (launches) ++*launches;
     return s;
   }
@@ -320,11 +320,11 @@ int edge_features_rows(const Plan* P, const Weights* W, const float* edge_attr, 
         if (s) return s;
         s = launch_gemm_tc(W->prec, a1, n, 0, static_cast<int>(n), 64, W->W1aug, W->kp[1], nullptr, 1, dst1,
                            static_cast<int64_t>(amul) * W->kp[1], st, nullptr, h_pad_l1, e0,
-                           W->split ? GEMM_C_SPLIT : 0, overflow);
+                           W->split ? GEMM_C_SPLIT : 0, overflow, nullptr, 0, 0, 0, nullptr, act_of(W));
         if (launches) ++*launches;
       } else {
         s = launch_edge_layer1(W->prec, edge_attr, P->perm, e_begin + e0, n, W->dims[0], W->W1, W->b1, W->kp[1], 0, dst1,
-                               st, h_pad_l1, e0, overflow);
+                               st, h_pad_l1, e0, overflow, act_of(W));
       }
     }
     if (s) return s;
@@ -339,12 +339,12 @@ int edge_features_rows(const Plan* P, const Weights* W, const float* edge_attr, 
       if (W->prec == PREC_FP32) {
         s = launch_sgemm_store(reinterpret_cast<const float*>(cur), W->kp[l - 1],
                                reinterpret_cast<const float*>(W->Wh[l]), W->kp[l - 1], static_cast<float*>(dst),
-                               W->kp[l], static_cast<int>(n), W->kp[l], W->kp[l - 1], W->bh[l], st);
+                               W->kp[l], static_cast<int>(n), W->kp[l], W->kp[l - 1], W->bh[l], st, act_of(W));
       } else {
         s = launch_gemm_tc(W->prec, cur, n, 0, static_cast<int>(n), kmul * W->kp[l - 1], W->Wh[l], W->kp[l], W->bh[l], 1,
                            dst, static_cast<int64_t>(amul) * W->kp[l], st, nullptr, last ? hpad : 0, e0,
                            W->split ? (GEMM_A_SPLIT | GEMM_C_SPLIT) : 0, overflow, nullptr, 0, 0, 0,
-                           W->split ? W->wscale + 2 * l + 1 : nullptr);
+                           W->split ? W->wscale + 2 * l + 1 : nullptr, act_of(W));
       }
       if (s) return s;
       if (launches) ++*launches;
@@ -931,6 +931,16 @@ struct nnconv_diag_weights {
   Weights w;
 };
 
+// the backward takes f'(z) from the output y = f(z): for a negative LeakyReLU slope or ELU alpha y no longer tells the
+// sign of z
+static int check_act(int activation, float act_param) {
+  NNC_REQUIRE(activation >= NNCONV_ACT_RELU && activation <= NNCONV_ACT_SIGMOID, NNCONV_ERR_ARG,
+              "unknown edge-network activation %d", activation);
+  NNC_REQUIRE(!(activation == NNCONV_ACT_LEAKY_RELU || activation == NNCONV_ACT_ELU) || act_param >= 0.f, NNCONV_ERR_UNSUPPORTED,
+              "edge-network activation: a negative LeakyReLU slope / ELU alpha (%g) is not supported", act_param);
+  return NNCONV_OK;
+}
+
 extern "C" {
 
 const char* nnconv_last_error(void) { return nnc::g_err; }
@@ -1028,13 +1038,24 @@ int nnconv_weights_sizes(int n_layers, const int* dims, int in_channels, int out
 int nnconv_weights_create(int n_layers, const int* dims, int in_channels, int out_channels, int precision,
                           const float* const* W, const float* const* b, void* buf, size_t buf_bytes, void* stream,
                           nnconv_weights_t** out) {
+  return nnconv_weights_create_act(n_layers, dims, in_channels, out_channels, precision, NNCONV_ACT_RELU, 0.f, W, b, buf,
+                                   buf_bytes, stream, out);
+}
+
+int nnconv_weights_create_act(int n_layers, const int* dims, int in_channels, int out_channels, int precision,
+                              int activation, float act_param, const float* const* W, const float* const* b, void* buf,
+                              size_t buf_bytes, void* stream, nnconv_weights_t** out) {
   NNC_REQUIRE(out && dims && W && b, NNCONV_ERR_ARG, "null pointer");
   *out = nullptr;
+  int s = check_act(activation, act_param);
+  if (s) return s;
   nnconv_weights* h = new (std::nothrow) nnconv_weights();
   NNC_REQUIRE(h != nullptr, NNCONV_ERR_ARG, "out of host memory");
-  int s = weights_prepare(&h->w, n_layers, dims, in_channels, out_channels, precision, W, b, buf, buf_bytes,
-                          static_cast<cudaStream_t>(stream));
+  s = weights_prepare(&h->w, n_layers, dims, in_channels, out_channels, precision, W, b, buf, buf_bytes,
+                      static_cast<cudaStream_t>(stream));
   if (s != NNCONV_OK) { delete h; return s; }
+  h->w.act = activation;
+  h->w.act_param = act_param;
   *out = h;
   return NNCONV_OK;
 }
@@ -1355,13 +1376,24 @@ int nnconv_diag_weights_sizes(int n_layers, const int* dims, int channels, int p
 int nnconv_diag_weights_create(int n_layers, const int* dims, int channels, int precision, const float* const* W,
                                const float* const* b, void* buf, size_t buf_bytes, void* stream,
                                nnconv_diag_weights_t** out) {
+  return nnconv_diag_weights_create_act(n_layers, dims, channels, precision, NNCONV_ACT_RELU, 0.f, W, b, buf, buf_bytes,
+                                        stream, out);
+}
+
+int nnconv_diag_weights_create_act(int n_layers, const int* dims, int channels, int precision, int activation,
+                                   float act_param, const float* const* W, const float* const* b, void* buf,
+                                   size_t buf_bytes, void* stream, nnconv_diag_weights_t** out) {
   NNC_REQUIRE(out && dims && W && b, NNCONV_ERR_ARG, "null pointer");
   *out = nullptr;
+  int s = check_act(activation, act_param);
+  if (s) return s;
   nnconv_diag_weights* h = new (std::nothrow) nnconv_diag_weights();
   NNC_REQUIRE(h != nullptr, NNCONV_ERR_ARG, "out of host memory");
-  int s = weights_prepare(&h->w, n_layers, dims, channels, channels, precision, W, b, buf, buf_bytes,
-                          static_cast<cudaStream_t>(stream), 1);
+  s = weights_prepare(&h->w, n_layers, dims, channels, channels, precision, W, b, buf, buf_bytes,
+                      static_cast<cudaStream_t>(stream), 1);
   if (s != NNCONV_OK) { delete h; return s; }
+  h->w.act = activation;
+  h->w.act_param = act_param;
   *out = h;
   return NNCONV_OK;
 }

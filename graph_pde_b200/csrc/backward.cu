@@ -13,6 +13,7 @@
 //   d ea_e  = dz_1[e, :] . W_1             (on request; dh_e[:k_in] for a single-Linear edge network).
 // Sources are processed in batches (contiguous sorted edges) so that activations are recomputed and freed
 // batch by batch; parameter gradients accumulate across batches.
+#include "act.cuh"
 #include "kernels.h"
 
 namespace nnc {
@@ -143,16 +144,18 @@ __global__ void k_group_sum(const float* __restrict__ G, const int* __restrict__
   }
 }
 
-// dz = dh * (act > 0), in place; column sums accumulate into db (one block per 32 columns)
-__global__ void k_relu_mask_colsum(float* __restrict__ dh, const float* __restrict__ act, int ne, int kp,
-                                   float* __restrict__ db) {
+// dz = dh * (act > 0), in place; column sums accumulate into db (one block per 32 columns).  k_act_grad_colsum<ACT>
+// multiplies by f'(act) of another hidden activation (act.cuh) instead.
+template <int ACT>
+__device__ __forceinline__ void act_grad_colsum(float* __restrict__ dh, const float* __restrict__ act, int ne, int kp,
+                                                float* __restrict__ db, float act_param) {
   __shared__ float red[8][33];
   const int col = blockIdx.x * 32 + threadIdx.x;
   float s = 0.f;
   for (int p = threadIdx.y; p < ne; p += 8) {
     if (col < kp) {
       const int64_t i = static_cast<int64_t>(p) * kp + col;
-      const float v = act[i] > 0.f ? dh[i] : 0.f;
+      const float v = ACT == ACT_RELU ? (act[i] > 0.f ? dh[i] : 0.f) : dh[i] * act_grad<ACT>(act[i], act_param);
       dh[i] = v;
       s += v;
     }
@@ -164,6 +167,17 @@ __global__ void k_relu_mask_colsum(float* __restrict__ dh, const float* __restri
     for (int r = 0; r < 8; ++r) t += red[r][threadIdx.x];
     db[col] += t;
   }
+}
+
+__global__ void k_relu_mask_colsum(float* __restrict__ dh, const float* __restrict__ act, int ne, int kp,
+                                   float* __restrict__ db) {
+  act_grad_colsum<ACT_RELU>(dh, act, ne, kp, db, 0.f);
+}
+
+template <int ACT>
+__global__ void k_act_grad_colsum(float* __restrict__ dh, const float* __restrict__ act, int ne, int kp,
+                                  float* __restrict__ db, float act_param) {
+  act_grad_colsum<ACT>(dh, act, ne, kp, db, act_param);
 }
 
 __global__ void k_gather_ea(const float* __restrict__ edge_attr, const int* __restrict__ perm, int e0, int ne,
@@ -235,7 +249,8 @@ __global__ void k_colsum_rows(const float* __restrict__ g, int64_t N, int C, flo
 }
 
 // dh = the gradient w.r.t. h_{L-1} of the sorted edges [e0, e0 + ne) in cur ([ne, Kp] fp32; nxt: a buffer of the same
-// size): back through the hidden layers with the ReLU masks of act[1 .. L-1] (recomputed fp32 activations), adding into
+// size): back through the hidden layers with the activation derivatives f'(act[1 .. L-1]) (recomputed fp32
+// activations; the ReLU mask for ReLU), adding into
 // the padded accumulators dW[l], db[l], and, with grad_ea, the gradient w.r.t. the batch's edge_attr rows.  ea: scratch
 // of ne * k_in floats.
 int mlp_backward_rows(const Plan* P, const Weights* W, const float* edge_attr, int e0, int ne, float* const* act, float* ea,
@@ -249,7 +264,13 @@ int mlp_backward_rows(const Plan* P, const Weights* W, const float* edge_attr, i
     NNC_CHECK_LAUNCH();
   }
   for (int l = nl - 1; l >= 1; --l) {
-    k_relu_mask_colsum<<<ceil_div(W->kp[l], 32), dim3(32, 8), 0, st>>>(cur, act[l], ne, W->kp[l], db[l]);
+    if (W->act == ACT_RELU)
+      k_relu_mask_colsum<<<ceil_div(W->kp[l], 32), dim3(32, 8), 0, st>>>(cur, act[l], ne, W->kp[l], db[l]);
+    else
+      act_dispatch(W->act, [&](auto k) {
+        k_act_grad_colsum<decltype(k)::value><<<ceil_div(W->kp[l], 32), dim3(32, 8), 0, st>>>(cur, act[l], ne, W->kp[l],
+                                                                                              db[l], W->act_param);
+      });
     NNC_CHECK_LAUNCH();
     const float* prev = l == 1 ? ea : act[l - 1];
     const int kprev = W->kp[l - 1];
@@ -284,10 +305,11 @@ const float* recompute_acts_fp32(const Plan* P, const Weights* W, const float* e
     *status = s;
     return hid;
   }
-  s = launch_edge_layer1(PREC_FP32, edge_attr, P->perm, e0, ne, W->dims[0], W->W1, W->b1, W->kp[1], 0, act[1], st);
+  s = launch_edge_layer1(PREC_FP32, edge_attr, P->perm, e0, ne, W->dims[0], W->W1, W->b1, W->kp[1], 0, act[1], st, 0, 0,
+                         nullptr, act_of(W));
   for (int l = 2; l <= nl - 1 && s == NNCONV_OK; ++l)
     s = launch_sgemm_store(act[l - 1], W->kp[l - 1], reinterpret_cast<const float*>(W->Wh[l]), W->kp[l - 1], act[l],
-                           W->kp[l], ne, W->kp[l], W->kp[l - 1], W->bh[l], st);
+                           W->kp[l], ne, W->kp[l], W->kp[l - 1], W->bh[l], st, act_of(W));
   *status = s;
   return act[nl - 1];
 }

@@ -31,6 +31,7 @@
 #include <algorithm>
 #include <type_traits>
 
+#include "act.cuh"
 #include "kernels.h"
 #include "tc05.cuh"
 #include "tmap.h"
@@ -537,6 +538,7 @@ struct DhArgs {
   // transpose and accumulated in a per-warp shared array; needs 4 * (4224 + 4 * Kp) extra bytes of shared memory.
   float* colsum;
   int colsum_stride;
+  float act_param;          // LeakyReLU slope / ELU alpha of MODE's activation
 };
 
 constexpr int kDhScratch = 4 * acc_scratch_bytes<32>();
@@ -546,9 +548,12 @@ __host__ __device__ constexpr int dh_pipe_bytes(int split, int BN, int T) {
   return split ? kDhBStages * (2 * kDhAChunk + 2 * BN * 128) : T * kDhAChunk + kDhBStages * BN * 128;
 }
 
-template <int FMT, int BN, int SPLIT = 0>
+// MODE = SPLIT | ACT << 1: ACT is the hidden activation (act.cuh).  ReLU (ACT 0) masks with h > 0 as above; another
+// activation multiplies by act_grad<ACT>(h) (SPLIT: of h's hi + lo halves), so the ReLU kernels keep their names.
+template <int FMT, int BN, int MODE = 0>
 __global__ void __launch_bounds__(160, 1)
 k_dh(const __grid_constant__ Maps8 tmA, const __grid_constant__ CUtensorMap tmB, DhArgs a) {
+  constexpr int SPLIT = MODE & 1, kAct = MODE >> 1;
   extern __shared__ __align__(1024) uint8_t smem[];
   if ((smem_u32(smem) & 1023u) != 0) __trap();
   const int b_stage_bytes = BN * 128;
@@ -681,10 +686,27 @@ k_dh(const __grid_constant__ Maps8 tmA, const __grid_constant__ CUtensorMap tmB,
             for (int q = 0; q < 4; ++q) {
               const uint4 mk = __ldg(reinterpret_cast<const uint4*>(hp) + q);
               const uint32_t mw[4] = {mk.x, mk.y, mk.z, mk.w};
+              uint32_t lw[4] = {0u, 0u, 0u, 0u};
+              if (SPLIT && kAct != ACT_RELU) {   // the lo panels follow the Kp / 64 hi panels
+                const uint4 ml = __ldg(reinterpret_cast<const uint4*>(hp + static_cast<int64_t>(a.Kp) * a.h_rows) + q);
+                lw[0] = ml.x; lw[1] = ml.y; lw[2] = ml.z; lw[3] = ml.w;
+              }
 #pragma unroll
               for (int j = 0; j < 4; ++j) {
-                const float f0 = (mw[j] & 0x7FFFu) ? __uint_as_float(v[8 * q + 2 * j]) : 0.f;
-                const float f1 = (mw[j] & 0x7FFF0000u) ? __uint_as_float(v[8 * q + 2 * j + 1]) : 0.f;
+                float f0, f1;
+                if (kAct == ACT_RELU) {
+                  f0 = (mw[j] & 0x7FFFu) ? __uint_as_float(v[8 * q + 2 * j]) : 0.f;
+                  f1 = (mw[j] & 0x7FFF0000u) ? __uint_as_float(v[8 * q + 2 * j + 1]) : 0.f;
+                } else {
+                  float2 y = unpack2<FMT>(mw[j]);
+                  if (SPLIT) {
+                    const float2 yl = unpack2<FMT>(lw[j]);
+                    y.x += yl.x;
+                    y.y += yl.y;
+                  }
+                  f0 = __uint_as_float(v[8 * q + 2 * j]) * act_grad<kAct>(y.x, a.act_param);
+                  f1 = __uint_as_float(v[8 * q + 2 * j + 1]) * act_grad<kAct>(y.y, a.act_param);
+                }
                 if (SPLIT) pack2_split(f0, f1, pk[4 * q + j], pl[4 * q + j]);
                 else pk[4 * q + j] = pack2<FMT>(f0, f1);
                 v[8 * q + 2 * j] = __float_as_uint(f0);
@@ -720,6 +742,19 @@ k_dh(const __grid_constant__ Maps8 tmA, const __grid_constant__ CUtensorMap tmB,
       }
     }
   }
+}
+
+// k_dh with another hidden activation (the ReLU launches below set their attributes once, together)
+template <int FMT, int BN, int MODE>
+int launch_dh(const Maps8& tmA, const CUtensorMap& tmB, const DhArgs& a, int grid, int smem, cudaStream_t st) {
+  static bool attr_set = false;
+  if (!attr_set) {
+    NNC_CHECK_CUDA(cudaFuncSetAttribute(k_dh<FMT, BN, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    attr_set = true;
+  }
+  k_dh<FMT, BN, MODE><<<grid, 160, smem, st>>>(tmA, tmB, a);
+  NNC_CHECK_LAUNCH();
+  return NNCONV_OK;
 }
 
 // =====================================================================================================
@@ -1308,12 +1343,12 @@ int backward_mlp_tc(const Plan* P, const Weights* W, const float* edge_attr, con
       if (r) return r;
       if (nl >= 3 && acts == nullptr) {
         r = launch_gemm_tc(W->prec, A1, n, 0, n, 64, W->W1aug, W->kp[1], nullptr, 1, act[1], pm * W->kp[1], st, nullptr, 0, 0,
-                           sp ? GEMM_C_SPLIT : 0);
+                           sp ? GEMM_C_SPLIT : 0, nullptr, nullptr, 0, 0, 0, nullptr, act_of(W));
         if (r) return r;
         for (int l = 2; l <= nl - 2; ++l) {
           r = launch_gemm_tc(W->prec, act[l - 1], n, 0, n, kmul * W->kp[l - 1], W->Wh[l], W->kp[l], W->bh[l], 1, act[l],
                              pm * W->kp[l], st, nullptr, 0, 0, sp ? (GEMM_A_SPLIT | GEMM_C_SPLIT) : 0, nullptr, nullptr, 0, 0,
-                             0, sp ? W->wscale + 2 * l + 1 : nullptr);
+                             0, sp ? W->wscale + 2 * l + 1 : nullptr, act_of(W));
           if (r) return r;
         }
       }
@@ -1326,11 +1361,11 @@ int backward_mlp_tc(const Plan* P, const Weights* W, const float* edge_attr, con
       const int64_t hpad = round_up64(n, 128);
       if (nl == 2)
         s = launch_gemm_tc(W->prec, A1, n, 0, n, 64, W->W1aug, W->kp[1], nullptr, 1, hb, pm * W->kp[1], st, nullptr, hpad, 0,
-                           sp ? GEMM_C_SPLIT : 0);
+                           sp ? GEMM_C_SPLIT : 0, nullptr, nullptr, 0, 0, 0, nullptr, act_of(W));
       else
         s = launch_gemm_tc(W->prec, act[nl - 2], n, 0, n, kmul * W->kp[nl - 2], W->Wh[nl - 1], W->kp[nl - 1], W->bh[nl - 1], 1,
                            hb, pm * W->kp[nl - 1], st, nullptr, hpad, 0, sp ? (GEMM_A_SPLIT | GEMM_C_SPLIT) : 0, nullptr,
-                           nullptr, 0, 0, 0, sp ? W->wscale + 2 * (nl - 1) + 1 : nullptr);
+                           nullptr, 0, 0, 0, sp ? W->wscale + 2 * (nl - 1) + 1 : nullptr, act_of(W));
       if (s) return s;
     }
     // ---- Y^T of the batch for every application: Yt[t][(c, k), o] = sum_i Xc_t[c, i] W_L[i*out + o, k]
@@ -1380,7 +1415,18 @@ int backward_mlp_tc(const Plan* P, const Weights* W, const float* edge_attr, con
       a.colsum_stride = 64;
       const int tiles = a.tile1 - a.tile0;
       const int grid = tiles < tc_num_sms() ? tiles : tc_num_sms();
-      if (sp) {
+      a.act_param = W->act_param;
+      if (W->act != ACT_RELU) {
+        s = act_dispatch(W->act, [&](auto k) {
+          constexpr int M = decltype(k)::value << 1;
+          if (sp) return BN == 128 ? launch_dh<0, 128, M | 1>(tmA, tmB, a, grid, dh_smem, st)
+                                   : launch_dh<0, 64, M | 1>(tmA, tmB, a, grid, dh_smem, st);
+          if (BN == 128) return bf ? launch_dh<1, 128, M>(tmA, tmB, a, grid, dh_smem, st)
+                                   : launch_dh<0, 128, M>(tmA, tmB, a, grid, dh_smem, st);
+          return bf ? launch_dh<1, 64, M>(tmA, tmB, a, grid, dh_smem, st) : launch_dh<0, 64, M>(tmA, tmB, a, grid, dh_smem, st);
+        });
+        if (s) return s;
+      } else if (sp) {
         if (BN == 128) k_dh<0, 128, 1><<<grid, 160, dh_smem, st>>>(tmA, tmB, a);
         else k_dh<0, 64, 1><<<grid, 160, dh_smem, st>>>(tmA, tmB, a);
       } else if (BN == 128) {
@@ -1412,10 +1458,11 @@ int backward_mlp_tc(const Plan* P, const Weights* W, const float* edge_attr, con
         s = gemm_tn_pairs(W, cur, pm * W->kp[l], W->kp[l], act[l - 1], pm * W->kp[l - 1], W->kp[l - 1], n, W->kp[l],
                           W->kp[l - 1], dWl, W->kp[l - 1], st);
         if (s) return s;
-        // dz_{l-1} = (dz_l W_l) * [h_{l-1} > 0]   (PREC_F16X2: the mask is the hi half of the activation pair)
+        // dz_{l-1} = (dz_l W_l) * [h_{l-1} > 0]   (PREC_F16X2: the mask is the hi half of the activation pair); another
+        // activation multiplies by f'(h_{l-1}) instead (PREC_F16X2: of hi + lo)
         s = launch_gemm_tc(W->prec, cur, n, 0, n, kmul * W->kp[l], W->WhT[l], W->kp[l - 1], nullptr, 0, nxt,
                            pm * W->kp[l - 1], st, nullptr, 0, 0, sp ? (GEMM_A_SPLIT | GEMM_C_SPLIT) : 0, nullptr, act[l - 1],
-                           pm * W->kp[l - 1], 0, 0, sp ? W->wscale + 2 * l + 1 : nullptr);
+                           pm * W->kp[l - 1], 0, 0, sp ? W->wscale + 2 * l + 1 : nullptr, act_of(W));
         if (s) return s;
         uint16_t* tmp = cur; cur = nxt; nxt = tmp;
       }

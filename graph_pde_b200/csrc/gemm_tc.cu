@@ -13,6 +13,7 @@
 // configuration keeps a single producer warp (9 warps) so that two CTAs share an SM.  Operands are K-major
 // 128B-swizzled tiles [128 x 64] / [BLOCK_N x 64] staged by TMA in a ring of kStages, so the producer runs ahead
 // into the next tile while the warpgroups run the epilogue of this one.
+#include "act.cuh"
 #include "kernels.h"
 #include "options.h"
 #include "tc05.cuh"
@@ -63,6 +64,7 @@ struct GemmTcArgs {
   int out_f32;
   TraceBuf trace;
   unsigned int trace_seq;
+  float act_param;     // LeakyReLU slope / ELU alpha of the activation epi_act(EPI)
 };
 
 // EPI selects the epilogue at COMPILE time (runtime flags inside the 32-column inner loop cut it into dozens of
@@ -71,11 +73,20 @@ struct GemmTcArgs {
 //   EPI_MASK  ReLU-derivative mask from a stored activation (backward)     EPI_F32 fp32 output, plain stores
 //   EPI_NOCHECK = EPI_PLAIN without the fp16 range tracking (bf16 outputs, option overflow_check = 0, test hooks)
 //   EPI_MASK_SPLIT = EPI_MASK with acc_scale, written as (hi, lo) pairs (PREC_F16X2 backward; the mask is the hi half)
+// The hidden activation (act.cuh) rides in the bits above: EPI = base | ACT << 3.  ReLU is ACT 0, so the ReLU
+// instantiations keep their names and code; for the other activations the forward epilogues apply act_fwd<ACT> where
+// ReLU applies the max, and the mask epilogues multiply by act_grad<ACT>(y) of the stored activation y (the split
+// form reads y = hi + lo, the lo half at column c + N of the mask row).
 // The forward epilogues (PLAIN, NOCHECK, SPLIT) work on the accumulator fragments and write the 16-bit staging with
 // stmatrix; the backward ones first transpose the fragments through a per-warp fp32 scratch (acc_rows: lane = row),
 // because their mask is read and their fp32 output written a row at a time.
 enum { EPI_PLAIN = 0, EPI_SPLIT = 1, EPI_MASK = 2, EPI_F32 = 3, EPI_NOCHECK = 4, EPI_MASK_SPLIT = 5 };
-constexpr bool epi_uses_rows(int epi) { return epi == EPI_MASK || epi == EPI_MASK_SPLIT || epi == EPI_F32; }
+constexpr int epi_base(int epi) { return epi & 7; }
+constexpr int epi_act(int epi) { return epi >> 3; }
+constexpr int epi_with_act(int epi, int act) { return epi | act << 3; }
+constexpr bool epi_uses_rows(int epi) {
+  return epi_base(epi) == EPI_MASK || epi_base(epi) == EPI_MASK_SPLIT || epi_base(epi) == EPI_F32;
+}
 
 // SMALL = 1: a 2-stage, BLOCK_N = 128, 288-thread footprint (~100 KB smem) that can share an SM with a
 // contraction CTA or a second GEMM CTA -- used for the per-source Y GEMM, which is store bound and runs
@@ -109,10 +120,11 @@ __global__ void __launch_bounds__(GemmCfg<BLOCK_N, SMALL, EPI>::kThreads, SMALL 
 k_gemm_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
           const __grid_constant__ CUtensorMap tmC, GemmTcArgs a) {
   using Cfg = GemmCfg<BLOCK_N, SMALL, EPI>;
-  constexpr bool kSplitOut = EPI == EPI_SPLIT || EPI == EPI_MASK_SPLIT;
-  constexpr bool kMask = EPI == EPI_MASK || EPI == EPI_MASK_SPLIT;
+  constexpr int kEpi = epi_base(EPI), kAct = epi_act(EPI);
+  constexpr bool kSplitOut = kEpi == EPI_SPLIT || kEpi == EPI_MASK_SPLIT;
+  constexpr bool kMask = kEpi == EPI_MASK || kEpi == EPI_MASK_SPLIT;
   constexpr bool kRows = epi_uses_rows(EPI);
-  constexpr bool kRangeCheck = FMT == 0 && (EPI == EPI_PLAIN || EPI == EPI_SPLIT);
+  constexpr bool kRangeCheck = FMT == 0 && (kEpi == EPI_PLAIN || kEpi == EPI_SPLIT);
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
   uint8_t* smem = smem_raw + (((raw + 1023u) & ~1023u) - raw);
@@ -292,8 +304,20 @@ k_gemm_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
                 float f0 = acc.d[h][4 * (4 * cc + j) + 2 * g], f1 = acc.d[h][4 * (4 * cc + j) + 2 * g + 1];
                 if (kSplitOut) { f0 *= accs; f1 *= accs; }
                 if (a.bias) { f0 += bj[j].x; f1 += bj[j].y; }
-                if (a.relu) { f0 = fmaxf(f0, 0.f); f1 = fmaxf(f1, 0.f); }
-                if (kRangeCheck && ok) vmax[j & 1] = fmaxf(vmax[j & 1], fmaxf(fabsf(f0), fabsf(f1)));
+                if (kAct == ACT_RELU) {
+                  if (a.relu) { f0 = fmaxf(f0, 0.f); f1 = fmaxf(f1, 0.f); }
+                  if (kRangeCheck && ok) vmax[j & 1] = fmaxf(vmax[j & 1], fmaxf(fabsf(f0), fabsf(f1)));
+                } else {
+                  float r0 = fabsf(f0), r1 = fabsf(f1);
+                  if (a.relu) {
+                    const float y0 = act_fwd<kAct>(f0, a.act_param), y1 = act_fwd<kAct>(f1, a.act_param);
+                    r0 = act_range<kAct>(f0, y0);
+                    r1 = act_range<kAct>(f1, y1);
+                    f0 = y0;
+                    f1 = y1;
+                  }
+                  if (kRangeCheck && ok) vmax[j & 1] = fmaxf(vmax[j & 1], fmaxf(r0, r1));
+                }
                 if (FMT == 0) {
                   const __half2 hv = __floats2half2_rn(f0, f1);
                   hi[h][g][j] = *reinterpret_cast<const uint32_t*>(&hv);
@@ -335,6 +359,7 @@ k_gemm_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
           // EPI_MASK: the row's 32 stored activations (64 B), one 16-byte load per 8 columns
           const uint4* mp = reinterpret_cast<const uint4*>(a.mask + static_cast<int64_t>(row) * a.mask_ld + col0);
           uint4 mkw = make_uint4(0u, 0u, 0u, 0u);
+          uint4 mkl = make_uint4(0u, 0u, 0u, 0u);   // split form, other activations: the lo half of the same columns
 #pragma unroll
           for (int j4 = 0; j4 < 8; ++j4) {
             float f[4] = {__uint_as_float(v[4 * j4]), __uint_as_float(v[4 * j4 + 1]),
@@ -354,9 +379,30 @@ k_gemm_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
             }
             if (a.relu) {
 #pragma unroll
-              for (int q = 0; q < 4; ++q) f[q] = fmaxf(f[q], 0.f);
+              for (int q = 0; q < 4; ++q) f[q] = act_fwd<kAct>(f[q], a.act_param);
             }
-            if (kMask) {
+            if (kMask && kAct != ACT_RELU) {
+              // f'(y) from the stored activation: y = hi (+ lo at column c + N for the split form)
+              if (row_ok) {
+                if (j4 % 2 == 0) {
+                  mkw = __ldg(mp + j4 / 2);
+                  if (kSplitOut) mkl = __ldg(reinterpret_cast<const uint4*>(reinterpret_cast<const uint16_t*>(mp) + a.N) + j4 / 2);
+                }
+                const uint32_t mw[2] = {j4 % 2 ? mkw.z : mkw.x, j4 % 2 ? mkw.w : mkw.y};
+                const uint32_t lw[2] = {j4 % 2 ? mkl.z : mkl.x, j4 % 2 ? mkl.w : mkl.y};
+#pragma unroll
+                for (int q = 0; q < 2; ++q) {
+                  float2 y = unpack2<FMT>(mw[q]);
+                  if (kSplitOut) {
+                    const float2 yl = unpack2<FMT>(lw[q]);
+                    y.x += yl.x;
+                    y.y += yl.y;
+                  }
+                  f[2 * q] *= act_grad<kAct>(y.x, a.act_param);
+                  f[2 * q + 1] *= act_grad<kAct>(y.y, a.act_param);
+                }
+              }
+            } else if (kMask) {
               if (row_ok) {
                 if (j4 % 2 == 0) mkw = __ldg(mp + j4 / 2);
                 const uint32_t mx = j4 % 2 ? mkw.z : mkw.x, my = j4 % 2 ? mkw.w : mkw.y;
@@ -366,7 +412,7 @@ k_gemm_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
                 if ((my & 0x7FFF0000u) == 0u) f[3] = 0.f;
               }
             }
-            if (EPI == EPI_F32) {
+            if (kEpi == EPI_F32) {
               if (row_ok)
                 *reinterpret_cast<float4*>(reinterpret_cast<float*>(a.C) + static_cast<int64_t>(row) * a.ldc + col0 + 4 * j4) =
                     make_float4(f[0], f[1], f[2], f[3]);
@@ -396,7 +442,7 @@ k_gemm_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
                            pk[4 * u + 2], pk[4 * u + 3]);
             end_piece(buf, colx);
           };
-          if (EPI != EPI_F32) {
+          if (kEpi != EPI_F32) {
             stage_row(packed, col0);
             if (FMT == 0 && kSplitOut) stage_row(packed_lo, col0 + a.N);
           }
@@ -439,6 +485,47 @@ int launch_gemm_cfg(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtens
   return NNCONV_OK;
 }
 
+// the launch of launch_gemm_tc's configuration with the hidden activation ACT (ACT_RELU: the original instantiations)
+template <int ACT>
+int dispatch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC, const GemmTcArgs& a,
+                  cudaStream_t st, bool pdl, int BN, int bf, bool small, int out_f32, bool mask_split, bool has_mask,
+                  bool c_split) {
+  // backward / split epilogues (never pipelined, never the small-footprint configuration)
+#define NNC_GEMM_EPI(E)                                                                                              \
+  do {                                                                                                               \
+    if (BN == 256) return bf ? launch_gemm_cfg<256, 1, 0, E>(tmA, tmB, tmC, a, st, pdl) : launch_gemm_cfg<256, 0, 0, E>(tmA, tmB, tmC, a, st, pdl); \
+    if (BN == 128) return bf ? launch_gemm_cfg<128, 1, 0, E>(tmA, tmB, tmC, a, st, pdl) : launch_gemm_cfg<128, 0, 0, E>(tmA, tmB, tmC, a, st, pdl); \
+    return bf ? launch_gemm_cfg<64, 1, 0, E>(tmA, tmB, tmC, a, st, pdl) : launch_gemm_cfg<64, 0, 0, E>(tmA, tmB, tmC, a, st, pdl); \
+  } while (0)
+  if constexpr (ACT == ACT_RELU) {    // fp32 output and the small footprint never apply the activation
+    if (out_f32) { NNC_REQUIRE(!small && !c_split && !has_mask, NNCONV_ERR_ARG, "gemm_tc: fp32 output excludes split / mask"); NNC_GEMM_EPI(EPI_F32); }
+  }
+  if (mask_split) {
+    NNC_REQUIRE(!small && !bf, NNCONV_ERR_ARG, "gemm_tc: split mask epilogue is fp16 only");
+    if (BN == 128) return launch_gemm_cfg<128, 0, 0, epi_with_act(EPI_MASK_SPLIT, ACT)>(tmA, tmB, tmC, a, st, pdl);
+    return launch_gemm_cfg<64, 0, 0, epi_with_act(EPI_MASK_SPLIT, ACT)>(tmA, tmB, tmC, a, st, pdl);
+  }
+  if (has_mask) { NNC_REQUIRE(!small, NNCONV_ERR_ARG, "gemm_tc: mask excludes the small-footprint configuration"); NNC_GEMM_EPI(epi_with_act(EPI_MASK, ACT)); }
+  if (c_split) {
+    NNC_REQUIRE(!small, NNCONV_ERR_ARG, "gemm_tc: split output excludes the small-footprint configuration");
+    if (BN == 256) return launch_gemm_cfg<256, 0, 0, epi_with_act(EPI_SPLIT, ACT)>(tmA, tmB, tmC, a, st, pdl);
+    if (BN == 128) return launch_gemm_cfg<128, 0, 0, epi_with_act(EPI_SPLIT, ACT)>(tmA, tmB, tmC, a, st, pdl);
+    return launch_gemm_cfg<64, 0, 0, epi_with_act(EPI_SPLIT, ACT)>(tmA, tmB, tmC, a, st, pdl);
+  }
+#undef NNC_GEMM_EPI
+  if (!bf && !small && a.overflow == nullptr) {      // fp16 output nobody wants range-checked
+    if (BN == 256) return launch_gemm_cfg<256, 0, 0, epi_with_act(EPI_NOCHECK, ACT)>(tmA, tmB, tmC, a, st, pdl);
+    if (BN == 128) return launch_gemm_cfg<128, 0, 0, epi_with_act(EPI_NOCHECK, ACT)>(tmA, tmB, tmC, a, st, pdl);
+    return launch_gemm_cfg<64, 0, 0, epi_with_act(EPI_NOCHECK, ACT)>(tmA, tmB, tmC, a, st, pdl);
+  }
+  if constexpr (ACT == ACT_RELU) {
+    if (small) return bf ? launch_gemm_cfg<128, 1, 1>(tmA, tmB, tmC, a, st, pdl) : launch_gemm_cfg<128, 0, 1>(tmA, tmB, tmC, a, st, pdl);
+  }
+  if (BN == 256) return bf ? launch_gemm_cfg<256, 1, 0, epi_with_act(EPI_PLAIN, ACT)>(tmA, tmB, tmC, a, st, pdl) : launch_gemm_cfg<256, 0, 0, epi_with_act(EPI_PLAIN, ACT)>(tmA, tmB, tmC, a, st, pdl);
+  if (BN == 128) return bf ? launch_gemm_cfg<128, 1, 0, epi_with_act(EPI_PLAIN, ACT)>(tmA, tmB, tmC, a, st, pdl) : launch_gemm_cfg<128, 0, 0, epi_with_act(EPI_PLAIN, ACT)>(tmA, tmB, tmC, a, st, pdl);
+  return bf ? launch_gemm_cfg<64, 1, 0, epi_with_act(EPI_PLAIN, ACT)>(tmA, tmB, tmC, a, st, pdl) : launch_gemm_cfg<64, 0, 0, epi_with_act(EPI_PLAIN, ACT)>(tmA, tmB, tmC, a, st, pdl);
+}
+
 }  // namespace
 
 int tc_init() {
@@ -460,7 +547,7 @@ int tc_num_sms() { return g_num_sms; }
 int launch_gemm_tc(int prec, const void* A_base, int64_t a_rows_total, int64_t a_row0, int M, int K, const void* B,
                    int N, const float* bias, int relu, void* C, int64_t ldc, cudaStream_t st, const PipeFlags* pf,
                    int64_t chunk_rows_pad, int64_t c_row0, int split_flags, int* overflow, const void* mask,
-                   int64_t mask_ld, int out_f32, int64_t a_chunk_rows_pad, const float* acc_scale) {
+                   int64_t mask_ld, int out_f32, int64_t a_chunk_rows_pad, const float* acc_scale, Act act) {
   if (M <= 0 || N <= 0) return NNCONV_OK;
   int s = tc_init();
   if (s != NNCONV_OK) return s;
@@ -535,36 +622,14 @@ int launch_gemm_tc(int prec, const void* A_base, int64_t a_rows_total, int64_t a
   a.done_cnt = pf ? pf->done_cnt : nullptr;
   a.done_ok = pf ? pf->done_ok : nullptr;
   const bool pdl = pf && pf->pdl;
-  // backward / split epilogues (never pipelined, never the small-footprint configuration)
-#define NNC_GEMM_EPI(E)                                                                                              \
-  do {                                                                                                               \
-    if (BN == 256) return bf ? launch_gemm_cfg<256, 1, 0, E>(tmA, tmB, tmC, a, st, pdl) : launch_gemm_cfg<256, 0, 0, E>(tmA, tmB, tmC, a, st, pdl); \
-    if (BN == 128) return bf ? launch_gemm_cfg<128, 1, 0, E>(tmA, tmB, tmC, a, st, pdl) : launch_gemm_cfg<128, 0, 0, E>(tmA, tmB, tmC, a, st, pdl); \
-    return bf ? launch_gemm_cfg<64, 1, 0, E>(tmA, tmB, tmC, a, st, pdl) : launch_gemm_cfg<64, 0, 0, E>(tmA, tmB, tmC, a, st, pdl); \
-  } while (0)
-  if (out_f32) { NNC_REQUIRE(!small && !c_split && mask == nullptr, NNCONV_ERR_ARG, "gemm_tc: fp32 output excludes split / mask"); NNC_GEMM_EPI(EPI_F32); }
-  if (mask_split) {
-    NNC_REQUIRE(!small && !bf, NNCONV_ERR_ARG, "gemm_tc: split mask epilogue is fp16 only");
-    if (BN == 128) return launch_gemm_cfg<128, 0, 0, EPI_MASK_SPLIT>(tmA, tmB, tmC, a, st, pdl);
-    return launch_gemm_cfg<64, 0, 0, EPI_MASK_SPLIT>(tmA, tmB, tmC, a, st, pdl);
-  }
-  if (mask != nullptr) { NNC_REQUIRE(!small, NNCONV_ERR_ARG, "gemm_tc: mask excludes the small-footprint configuration"); NNC_GEMM_EPI(EPI_MASK); }
-  if (c_split) {
-    NNC_REQUIRE(!small, NNCONV_ERR_ARG, "gemm_tc: split output excludes the small-footprint configuration");
-    if (BN == 256) return launch_gemm_cfg<256, 0, 0, EPI_SPLIT>(tmA, tmB, tmC, a, st, pdl);
-    if (BN == 128) return launch_gemm_cfg<128, 0, 0, EPI_SPLIT>(tmA, tmB, tmC, a, st, pdl);
-    return launch_gemm_cfg<64, 0, 0, EPI_SPLIT>(tmA, tmB, tmC, a, st, pdl);
-  }
-#undef NNC_GEMM_EPI
-  if (!bf && !small && a.overflow == nullptr) {      // fp16 output nobody wants range-checked
-    if (BN == 256) return launch_gemm_cfg<256, 0, 0, EPI_NOCHECK>(tmA, tmB, tmC, a, st, pdl);
-    if (BN == 128) return launch_gemm_cfg<128, 0, 0, EPI_NOCHECK>(tmA, tmB, tmC, a, st, pdl);
-    return launch_gemm_cfg<64, 0, 0, EPI_NOCHECK>(tmA, tmB, tmC, a, st, pdl);
-  }
-  if (small) return bf ? launch_gemm_cfg<128, 1, 1>(tmA, tmB, tmC, a, st, pdl) : launch_gemm_cfg<128, 0, 1>(tmA, tmB, tmC, a, st, pdl);
-  if (BN == 256) return bf ? launch_gemm_cfg<256, 1, 0>(tmA, tmB, tmC, a, st, pdl) : launch_gemm_cfg<256, 0, 0>(tmA, tmB, tmC, a, st, pdl);
-  if (BN == 128) return bf ? launch_gemm_cfg<128, 1, 0>(tmA, tmB, tmC, a, st, pdl) : launch_gemm_cfg<128, 0, 0>(tmA, tmB, tmC, a, st, pdl);
-  return bf ? launch_gemm_cfg<64, 1, 0>(tmA, tmB, tmC, a, st, pdl) : launch_gemm_cfg<64, 0, 0>(tmA, tmB, tmC, a, st, pdl);
+  // the activation matters only where it is applied (relu) or differentiated (mask); every other launch is the ReLU
+  // instantiation, as it always was
+  a.act_param = act.param;
+  if (act.kind == ACT_RELU || (!relu && mask == nullptr)) return dispatch_gemm<ACT_RELU>(tmA, tmB, tmC, a, st, pdl, BN, bf, small, out_f32, mask_split, mask != nullptr, c_split);
+  NNC_REQUIRE(!out_f32 && !small, NNCONV_ERR_ARG, "gemm_tc: the activation excludes fp32 output / the small-footprint configuration");
+  return act_dispatch(act.kind, [&](auto k) {
+    return dispatch_gemm<decltype(k)::value>(tmA, tmB, tmC, a, st, pdl, BN, bf, small, out_f32, mask_split, mask != nullptr, c_split);
+  });
 }
 
 }  // namespace nnc

@@ -23,7 +23,7 @@ int launch_transpose_pad(int prec, const float* src, int R, int C, void* dst, in
                          const float* scale = nullptr);
 int launch_edge_layer1(int prec, const float* edge_attr, const int* perm, int64_t e_begin, int64_t e_count, int k_in,
                        const float* W1, const float* b1, int kp1, int identity, void* out, cudaStream_t st,
-                       int64_t chunk_rows_pad = 0, int64_t out_row0 = 0, int* overflow = nullptr);
+                       int64_t chunk_rows_pad = 0, int64_t out_row0 = 0, int* overflow = nullptr, Act act = Act{});
 int launch_build_a1(int prec, const float* edge_attr, const int* perm, int64_t e_begin, int64_t e_count, int k_in,
                     void* A1, cudaStream_t st);
 int launch_w1aug(int prec, const float* W1, const float* b1, int k1, int kp1, int k_in, void* dst, cudaStream_t st);
@@ -38,7 +38,7 @@ int launch_node_prep(int prec, const float* x, const float* root, const float* b
                      float* xs, int* flags, int flags_stride, int n_batches, cudaStream_t st, unsigned node_flags,
                      unsigned long long* max_keys = nullptr);
 int launch_sgemm_store(const float* A, int64_t lda, const float* B, int64_t ldb, float* C, int64_t ldc, int M, int N,
-                       int K, const float* bias_relu, cudaStream_t st);
+                       int K, const float* bias_relu, cudaStream_t st, Act act = Act{});
 int launch_sgemm_scatter(const Plan* P, const float* h, int Kp, const float* Y, int cout, int tile_begin,
                          int tile_end, int c0, const float* cvec, int aggr_mean, float* out, cudaStream_t st,
                          unsigned long long* max_keys = nullptr);
@@ -73,13 +73,14 @@ struct PipeFlags {
 // tensor A_base[a_rows_total, K]; K, N multiples of 64.  bias == nullptr -> no bias, relu flag separate.
 // split_flags (PREC_F16X2): GEMM_A_SPLIT -> A is [hi | lo] with 2K/3 columns and B is [hi | lo | hi] with K columns;
 // GEMM_C_SPLIT -> C receives [hi | lo] pairs (2N columns / 2N/64 chunks).  overflow: device counter of output
-// pieces that left the fp16 range (nullable).
+// pieces that left the fp16 range (nullable).  act: the edge network's hidden activation, applied where relu != 0 and
+// differentiated where mask != nullptr (C = acc * f'(mask), the ReLU mask for act.kind = NNCONV_ACT_RELU).
 enum { GEMM_A_SPLIT = 1, GEMM_C_SPLIT = 2 };
 int launch_gemm_tc(int prec, const void* A_base, int64_t a_rows_total, int64_t a_row0, int M, int K,
                    const void* B, int N, const float* bias, int relu, void* C, int64_t ldc, cudaStream_t st,
                    const PipeFlags* pf = nullptr, int64_t chunk_rows_pad = 0, int64_t c_row0 = 0,
                    int split_flags = 0, int* overflow = nullptr, const void* mask = nullptr, int64_t mask_ld = 0,
-                   int out_f32 = 0, int64_t a_chunk_rows_pad = 0, const float* acc_scale = nullptr);
+                   int out_f32 = 0, int64_t a_chunk_rows_pad = 0, const float* acc_scale = nullptr, Act act = Act{});
 
 // ---- per-edge kernel matrices (formulation B, for graphs with few out-edges per source): K_e = W_L h_e + b_L once per
 // (edge_attr, parameters), then out[dst] += x_src . K_e per application (kernels_simt.cu)

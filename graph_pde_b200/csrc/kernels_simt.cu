@@ -9,6 +9,7 @@
 
 #include <type_traits>
 
+#include "act.cuh"
 #include "common.cuh"
 #include "kernels.h"
 
@@ -170,12 +171,15 @@ __global__ void k_transpose_pad_split3(const float* __restrict__ src, int R, int
 // identity (single-Linear MLP): h[p, j] = edge_attr[perm[p], j] (zero padded), no ReLU.
 // overflow (fp16 output, nullable): +1 per block that wrote a value beyond the fp16 range or NaN.  Counted here, at the
 // writer: the next layer's GEMM would turn an inf into NaN, which its ReLU turns into 0 before its own range check.
+// k_edge_layer1 is the ReLU kernel; k_edge_layer1_act<ACT> applies another hidden activation (act.cuh, act_range for
+// the range check) in its place.
 constexpr int kL1Edges = 32;
-template <typename T>
-__global__ void __launch_bounds__(256)
-k_edge_layer1(const float* __restrict__ edge_attr, const int* __restrict__ perm, int64_t e_begin, int64_t e_count,
-              int k_in, const float* __restrict__ W1, const float* __restrict__ b1, int kp1, int identity,
-              T* __restrict__ out, int64_t chunk_rows_pad, int64_t out_row0, int* __restrict__ overflow) {
+template <int ACT, typename T>
+__device__ __forceinline__ void edge_layer1(const float* __restrict__ edge_attr, const int* __restrict__ perm,
+                                            int64_t e_begin, int64_t e_count, int k_in, const float* __restrict__ W1,
+                                            const float* __restrict__ b1, int kp1, int identity, T* __restrict__ out,
+                                            int64_t chunk_rows_pad, int64_t out_row0, int* __restrict__ overflow,
+                                            float act_param) {
   constexpr bool kRangeCheck = std::is_same<T, __half>::value;
   bool bad = false;
   extern __shared__ float sm[];
@@ -220,14 +224,38 @@ k_edge_layer1(const float* __restrict__ edge_attr, const int* __restrict__ perm,
       } else {
         for (int c = 0; c < k_in; ++c) acc = fmaf(W1[static_cast<int64_t>(j) * k_in + c], s_ea[e * k_in + c], acc);
       }
-      const float v = fmaxf(acc, 0.f);
-      if (kRangeCheck) bad |= !(v <= 65504.f);
-      out[oidx(e, j)] = cvt<T>(v);
+      if (ACT == ACT_RELU) {
+        const float v = fmaxf(acc, 0.f);
+        if (kRangeCheck) bad |= !(v <= 65504.f);
+        out[oidx(e, j)] = cvt<T>(v);
+      } else {
+        const float v = act_fwd<ACT>(acc, act_param);
+        if (kRangeCheck) bad |= !(act_range<ACT>(acc, v) <= 65504.f);
+        out[oidx(e, j)] = cvt<T>(v);
+      }
     }
   }
   if (kRangeCheck && overflow != nullptr) {
     if (__syncthreads_or(bad) && threadIdx.x == 0) atomicAdd(overflow, 1);
   }
+}
+
+template <typename T>
+__global__ void __launch_bounds__(256)
+k_edge_layer1(const float* __restrict__ edge_attr, const int* __restrict__ perm, int64_t e_begin, int64_t e_count,
+              int k_in, const float* __restrict__ W1, const float* __restrict__ b1, int kp1, int identity,
+              T* __restrict__ out, int64_t chunk_rows_pad, int64_t out_row0, int* __restrict__ overflow) {
+  edge_layer1<ACT_RELU>(edge_attr, perm, e_begin, e_count, k_in, W1, b1, kp1, identity, out, chunk_rows_pad, out_row0,
+                        overflow, 0.f);
+}
+
+template <int ACT, typename T>
+__global__ void __launch_bounds__(256)
+k_edge_layer1_act(const float* __restrict__ edge_attr, const int* __restrict__ perm, int64_t e_begin, int64_t e_count,
+                  int k_in, const float* __restrict__ W1, const float* __restrict__ b1, int kp1, T* __restrict__ out,
+                  int64_t chunk_rows_pad, int64_t out_row0, int* __restrict__ overflow, float act_param) {
+  edge_layer1<ACT>(edge_attr, perm, e_begin, e_count, k_in, W1, b1, kp1, 0, out, chunk_rows_pad, out_row0, overflow,
+                   act_param);
 }
 
 // ---- first edge-MLP layer on the tensor cores with fp32-grade inputs -------------------------------
@@ -425,7 +453,8 @@ __global__ void k_node_prep(const float* __restrict__ x, const float* __restrict
 // ------------------------------------------------------------------------------------------------
 // fp32 NT GEMM, 64x64x16 tiles, 256 threads, 4x4 register blocking.   C = A[M,K] * B[N,K]^T
 // ------------------------------------------------------------------------------------------------
-enum { EPI_STORE = 0, EPI_BIAS_RELU = 1, EPI_SCATTER = 2, EPI_SCATTER_MAX = 3 };
+// EPI_BIAS_ACT + ACT: bias and another hidden activation (act.cuh) where EPI_BIAS_RELU applies the ReLU
+enum { EPI_STORE = 0, EPI_BIAS_RELU = 1, EPI_SCATTER = 2, EPI_SCATTER_MAX = 3, EPI_BIAS_ACT = 8 };
 
 struct SgemmArgs {
   const float* A;
@@ -435,7 +464,7 @@ struct SgemmArgs {
   float* C;
   int64_t ldc;
   int M, N, K;
-  const float* bias;   // EPI_BIAS_RELU
+  const float* bias;   // EPI_BIAS_RELU, EPI_BIAS_ACT + ACT
   // EPI_SCATTER (grid.x = tile): A rows = h rows of the tile, B = Y of the tile's source
   const int *tile_c, *tile_e0, *tile_cnt, *dst_sorted;
   const float *inv_deg, *cvec;
@@ -444,6 +473,7 @@ struct SgemmArgs {
   // EPI_SCATTER_MAX (aggr = max): the rows reduce keys (common.cuh max_key) into keys [N, ldc] instead of adding to C
   unsigned long long* keys;
   const int* perm;
+  float act_param;     // EPI_BIAS_ACT + ACT
 };
 
 template <int EPI>
@@ -524,6 +554,7 @@ __global__ void __launch_bounds__(256) k_sgemm_nt(SgemmArgs a) {
         if (gn < a.N) {
           float v = acc[i][j];
           if (EPI == EPI_BIAS_RELU) v = fmaxf(v + a.bias[gn], 0.f);
+          if constexpr (EPI > EPI_BIAS_ACT) v = act_fwd<EPI - EPI_BIAS_ACT>(v + a.bias[gn], a.act_param);
           a.C[static_cast<int64_t>(gm) * a.ldc + gn] = v;
         }
       }
@@ -846,11 +877,27 @@ int launch_transpose_pad(int prec, const float* src, int R, int C, void* dst, in
 
 int launch_edge_layer1(int prec, const float* edge_attr, const int* perm, int64_t e_begin, int64_t e_count, int k_in,
                        const float* W1, const float* b1, int kp1, int identity, void* out, cudaStream_t st,
-                       int64_t chunk_rows_pad, int64_t out_row0, int* overflow) {
+                       int64_t chunk_rows_pad, int64_t out_row0, int* overflow, Act act) {
   if (e_count <= 0) return NNCONV_OK;
   unsigned g = (unsigned)ceil_div64(e_count, kL1Edges);
   size_t sm = sizeof(float) * kL1Edges * k_in;
-  if (prec == PREC_FP32)
+  if (!identity && act.kind != ACT_RELU) {
+    act_dispatch(act.kind, [&](auto k) {
+      constexpr int A = decltype(k)::value;
+      if (prec == PREC_FP32)
+        k_edge_layer1_act<A, float><<<g, 256, sm, st>>>(edge_attr, perm, e_begin, e_count, k_in, W1, b1, kp1,
+                                                         static_cast<float*>(out), chunk_rows_pad, out_row0, nullptr,
+                                                         act.param);
+      else if (prec == PREC_F16 || prec == PREC_F16X2)
+        k_edge_layer1_act<A, __half><<<g, 256, sm, st>>>(edge_attr, perm, e_begin, e_count, k_in, W1, b1, kp1,
+                                                          static_cast<__half*>(out), chunk_rows_pad, out_row0, overflow,
+                                                          act.param);
+      else
+        k_edge_layer1_act<A, __nv_bfloat16><<<g, 256, sm, st>>>(edge_attr, perm, e_begin, e_count, k_in, W1, b1, kp1,
+                                                                 static_cast<__nv_bfloat16*>(out), chunk_rows_pad,
+                                                                 out_row0, nullptr, act.param);
+    });
+  } else if (prec == PREC_FP32)
     k_edge_layer1<float><<<g, 256, sm, st>>>(edge_attr, perm, e_begin, e_count, k_in, W1, b1, kp1, identity,
                                              static_cast<float*>(out), chunk_rows_pad, out_row0, nullptr);
   else if (prec == PREC_F16 || prec == PREC_F16X2)
@@ -994,12 +1041,15 @@ int launch_apply_edge(int prec, const Plan* P, const Weights* W, const void* Kma
 }
 
 int launch_sgemm_store(const float* A, int64_t lda, const float* B, int64_t ldb, float* C, int64_t ldc, int M, int N,
-                       int K, const float* bias_relu, cudaStream_t st) {
+                       int K, const float* bias_relu, cudaStream_t st, Act act) {
   if (M <= 0 || N <= 0) return NNCONV_OK;
   SgemmArgs a{};
   a.A = A; a.lda = lda; a.B = B; a.ldb = ldb; a.C = C; a.ldc = ldc; a.M = M; a.N = N; a.K = K; a.bias = bias_relu;
+  a.act_param = act.param;
   dim3 g(ceil_div(M, 64), ceil_div(N, 64));
-  if (bias_relu) k_sgemm_nt<EPI_BIAS_RELU><<<g, 256, 0, st>>>(a);
+  if (bias_relu && act.kind != ACT_RELU)
+    act_dispatch(act.kind, [&](auto k) { k_sgemm_nt<EPI_BIAS_ACT + decltype(k)::value><<<g, 256, 0, st>>>(a); });
+  else if (bias_relu) k_sgemm_nt<EPI_BIAS_RELU><<<g, 256, 0, st>>>(a);
   else k_sgemm_nt<EPI_STORE><<<g, 256, 0, st>>>(a);
   NNC_CHECK_LAUNCH();
   return NNCONV_OK;

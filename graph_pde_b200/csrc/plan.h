@@ -44,6 +44,12 @@ void plan_sizes(int64_t E, int64_t N, size_t* ws_bytes, size_t* tmp_bytes);
 int plan_build(Plan* P, const int64_t* row0, const int64_t* row1, int64_t E, int64_t N, int flow, void* ws, size_t ws_bytes,
                void* tmp, size_t tmp_bytes, cudaStream_t st);
 
+// hidden activation of the edge MLP: kind = NNCONV_ACT_* (0 = ReLU), param = LeakyReLU slope / ELU alpha
+struct Act {
+  int kind;
+  float param;
+};
+
 // Prepared (padded / permuted / down-converted) snapshot of the edge-MLP parameters.
 struct Weights {
   int n_layers;                 // Linear layers of the edge MLP (DenseNet)
@@ -76,7 +82,12 @@ struct Weights {
   // b_L with cin == cout == dims[L].  Only the hidden layers, W3n and B3 are prepared: W3n = W_L [cout, Kp] zero padded,
   // 16-bit at f16 / bf16 (tensor-core build of d), fp32 at f16x2 and fp32 (CUDA-core build); B3 = b_L [cout] fp32.
   int diag;
+  // hidden activation of the edge MLP (NNCONV_ACT_*) and its parameter (LeakyReLU slope / ELU alpha), see act.cuh
+  int act;
+  float act_param;
 };
+
+inline Act act_of(const Weights* W) { return Act{W->act, W->act_param}; }
 
 size_t weights_bytes(int n_layers, const int* dims, int cin, int cout, int prec, int diag = 0);
 int weights_prepare(Weights* W, int n_layers, const int* dims, int cin, int cout, int prec,

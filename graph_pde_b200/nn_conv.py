@@ -216,37 +216,93 @@ def get_plan(edge_index, n_nodes, flow='source_to_target'):
     return plan
 
 
-def _linear_chain(nn_module):
-    """The edge network must be the reference's DenseNet shape: Linear (ReLU Linear)* with no output
-    nonlinearity (graph-neural-operator/utilities.py:201-227; every call site passes torch.nn.ReLU,
-    normalize=False)."""
+# hidden activations the library runs: each has a derivative that is a function of its output (include/nnconv_b200.h
+# NNCONV_ACT_*), so the backward needs nothing beyond the activations it keeps for ReLU
+def _act_spec(m):
+    """('relu' | 'leaky_relu' | 'elu' | 'tanh' | 'sigmoid', parameter) of an activation module, None for any other
+    module; raises NotImplementedError for an activation the library does not run, naming the reason."""
+    if isinstance(m, torch.nn.ReLU):
+        return ('relu', 0.0)
+    if isinstance(m, torch.nn.LeakyReLU):
+        if m.negative_slope < 0:
+            raise NotImplementedError('edge network: LeakyReLU with a negative slope (%g) is not supported: its '
+                                      'derivative is not a function of its output' % m.negative_slope)
+        return ('leaky_relu', float(m.negative_slope))
+    if isinstance(m, torch.nn.ELU):
+        if m.alpha < 0:
+            raise NotImplementedError('edge network: ELU with a negative alpha (%g) is not supported: its derivative '
+                                      'is not a function of its output' % m.alpha)
+        return ('elu', float(m.alpha))
+    if isinstance(m, torch.nn.Tanh):
+        return ('tanh', 0.0)
+    if isinstance(m, torch.nn.Sigmoid):
+        return ('sigmoid', 0.0)
+    if isinstance(m, (torch.nn.GELU, torch.nn.SiLU, torch.nn.Softplus, torch.nn.Mish, torch.nn.Hardswish)):
+        raise NotImplementedError('edge network: %s is not supported: its derivative is not a function of its '
+                                  'output, so the backward would have to recompute the pre-activations'
+                                  % type(m).__name__)
+    if isinstance(m, torch.nn.modules.batchnorm._BatchNorm):
+        raise NotImplementedError('edge network: normalize=True (%s between the layers) is not supported'
+                                  % type(m).__name__)
+    return None
+
+
+def _edge_network(nn_module):
+    """The edge network must be the reference's DenseNet shape (graph-neural-operator/utilities.py:201-227):
+    Linear (act Linear)* with one hidden activation ``act`` in {ReLU, LeakyReLU(s >= 0), ELU(alpha >= 0), Tanh,
+    Sigmoid} after every Linear but the last, no output nonlinearity and normalize=False.  Returns (the Linear
+    layers, the activation spec (kind, parameter)); a single Linear has the spec ('relu', 0.0), which it never uses."""
+    if type(nn_module).__name__ == 'DenseNet_sin':
+        raise NotImplementedError('edge network: DenseNet_sin (torch.sin between the layers) is not supported: the '
+                                  'derivative of sin is not a function of its output')
     mods = [m for m in nn_module.modules() if len(list(m.children())) == 0]
     lin = []
+    act = None
     expect_linear = True
     for m in mods:
         if isinstance(m, torch.nn.Linear):
             if not expect_linear:
-                raise NotImplementedError('edge network: two Linear layers without a ReLU in between')
+                raise NotImplementedError('edge network: two Linear layers without an activation in between (an '
+                                          'activation applied inside forward(), like torch.sin, is not supported)')
             if m.bias is None:
                 raise NotImplementedError('edge network: Linear without bias is not supported')
             lin.append(m)
             expect_linear = False
-        elif isinstance(m, torch.nn.ReLU):
-            if expect_linear:
-                raise NotImplementedError('edge network: ReLU must follow a Linear layer')
-            expect_linear = True
-        else:
-            raise NotImplementedError('edge network: only Linear/ReLU chains (DenseNet) are supported, found %s'
-                                      % type(m).__name__)
+            continue
+        spec = _act_spec(m)
+        if spec is None:
+            raise NotImplementedError('edge network: only Linear chains with ReLU, LeakyReLU, ELU, Tanh or Sigmoid '
+                                      'between them (DenseNet) are supported, found %s' % type(m).__name__)
+        if expect_linear:
+            if lin:
+                raise NotImplementedError('edge network: two activations in a row (%s after an activation)'
+                                          % type(m).__name__)
+            raise NotImplementedError('edge network: %s must follow a Linear layer' % type(m).__name__)
+        if act is not None and act != spec:
+            raise NotImplementedError('edge network: mixed activations (%s and %s): one activation must follow every '
+                                      'hidden Linear, as DenseNet builds it' % (act, spec))
+        act = spec
+        expect_linear = True
     if not lin or expect_linear:
-        raise NotImplementedError('edge network must end with a Linear layer (no output nonlinearity)')
+        raise NotImplementedError('edge network must end with a Linear layer (no output nonlinearity: '
+                                  'out_nonlinearity is not supported)')
+    return lin, act if act is not None else ('relu', 0.0)
+
+
+def _linear_chain(nn_module):
+    """The Linear layers of a ReLU edge network, Linear (ReLU Linear)*; any other edge network raises
+    NotImplementedError.  The library's own code reads the network with _edge_network, which also accepts the other
+    hidden activations."""
+    lin, act = _edge_network(nn_module)
+    if act[0] != 'relu':
+        raise NotImplementedError('edge network: _linear_chain reads ReLU chains only, found %s' % (act,))
     return lin
 
 
 class _Prepared(object):
     """nnconv_weights_t: padded / permuted / down-converted snapshot of the edge-MLP parameters."""
 
-    def __init__(self, linears, cin, cout, precision):
+    def __init__(self, linears, cin, cout, precision, act=('relu', 0.0)):
         L = _lib.lib()
         _lib.check(L.nnconv_init())
         n = len(linears)
@@ -262,12 +318,13 @@ class _Prepared(object):
         wp = (ctypes.c_void_p * n)(*[w.data_ptr() for w in ws])
         bp = (ctypes.c_void_p * n)(*[b.data_ptr() for b in bs])
         h = ctypes.c_void_p()
-        _lib.check(L.nnconv_weights_create(n, c_dims, cin, cout, prec, wp, bp, _ptr(self.buf), nbytes.value,
-                                           _stream_ptr(dev), ctypes.byref(h)))
+        _lib.check(L.nnconv_weights_create_act(n, c_dims, cin, cout, prec, _lib.ACT[act[0]], act[1], wp, bp,
+                                               _ptr(self.buf), nbytes.value, _stream_ptr(dev), ctypes.byref(h)))
         self._keep = (ws, bs)
         self.handle = h
         self.dims = dims
         self.precision = precision
+        self.act = act
         self.tc = bool(L.nnconv_weights_tc_supported(h))
         self.bwd_tc = bool(L.nnconv_backward_tc_supported(h))
         stats['weight_preps'] += 1
@@ -449,7 +506,7 @@ class NNConv_old(torch.nn.Module):
         if needs_grad:
             state = self._train_state(x, edge_index, pseudo)
             if state is not None:            # tensor-core backward (csrc/backward_tc.cu)
-                lin = _linear_chain(self.nn)[-1]
+                lin = _edge_network(self.nn)[0][-1]
                 return _ApplyFn.apply(self, state, x, state.token, lin.weight, lin.bias, self.root, self.bias)
             return _NNConvFunction.apply(self, x, edge_index, pseudo, *list(self.parameters()))
         return self._forward_impl(x, edge_index, pseudo)
@@ -477,12 +534,12 @@ class NNConv_old(torch.nn.Module):
         """Weight snapshot at ``precision``, cached per parameter versions in one of two slots: 'forward' (the
         edge-feature pass and the applications; a new snapshot drops the edge features of the old one) and 'backward'
         (the fp32 CUDA-core backward, whatever precision the forward runs at)."""
-        linears = _linear_chain(self.nn)
-        key = (precision,) + tuple((l.weight.data_ptr(), l.weight._version, l.bias.data_ptr(), l.bias._version)
-                                   for l in linears)
+        linears, act = _edge_network(self.nn)
+        key = (precision, act) + tuple((l.weight.data_ptr(), l.weight._version, l.bias.data_ptr(), l.bias._version)
+                                       for l in linears)
         hit = self._prepared.get(slot)
         if hit is None or hit[0] != key:
-            hit = self._prepared[slot] = (key, _Prepared(linears, self.in_channels, self.out_channels, precision))
+            hit = self._prepared[slot] = (key, _Prepared(linears, self.in_channels, self.out_channels, precision, act))
             if slot == 'forward':
                 self._h_cache.clear()
         return hit[1]
@@ -818,7 +875,7 @@ class NNConv_old(torch.nn.Module):
             if st is None or st.key != key or st.consumed or st.ef is not ef:
                 st = _TrainState(key, plan, prepared, ef)
                 hidden = []
-                for l in _linear_chain(self.nn)[:-1]:
+                for l in _edge_network(self.nn)[0][:-1]:
                     hidden += [l.weight, l.bias]
                 st.token = _EdgeFeaturesFn.apply(self, st, pseudo, *hidden)
                 self._tstate = st
@@ -831,7 +888,7 @@ class NNConv_old(torch.nn.Module):
         L = _lib.lib()
         dev = x32.device
         plan, prep, ef = state.plan, state.prepared, state.ef
-        lin = _linear_chain(self.nn)[-1]
+        lin = _edge_network(self.nn)[0][-1]
         with torch.cuda.device(dev):
             dx = torch.empty_like(x32)
             dwl = torch.empty_like(lin.weight, dtype=torch.float32)
@@ -869,7 +926,7 @@ class NNConv_old(torch.nn.Module):
         ([E, k_in], summed over the groups; else None)."""
         L = _lib.lib()
         plan, prep, ef = state.plan, state.prepared, state.ef
-        hidden = _linear_chain(self.nn)[:-1]
+        hidden = _edge_network(self.nn)[0][:-1]
         dev = ef.ea32.device
         total = None
         gea_total = None
@@ -928,7 +985,7 @@ class NNConv_old(torch.nn.Module):
             g32 = _f32(grad_out)
             n = x32.size(0)
             plan = get_plan(edge_index, n, self.flow)
-            linears = _linear_chain(self.nn)
+            linears = _edge_network(self.nn)[0]
             prep = self._get_prepared('fp32', 'backward')
             ws_b = ctypes.c_size_t()
             _lib.check(L.nnconv_backward_sizes(plan.handle, prep.handle, _BWD_WS_BYTES, ctypes.byref(ws_b)))
@@ -983,7 +1040,7 @@ _DIAG_WS_BYTES = 1 << 30         # edge-network chunk of the d build (h rows + h
 class _DiagWeights(object):
     """nnconv_diag_weights_t: padded / down-converted snapshot of the edge network of a DiagNNConv."""
 
-    def __init__(self, linears, channels, precision):
+    def __init__(self, linears, channels, precision, act=('relu', 0.0)):
         L = _lib.lib()
         _lib.check(L.nnconv_init())
         n = len(linears)
@@ -999,8 +1056,8 @@ class _DiagWeights(object):
         wp = (ctypes.c_void_p * n)(*[w.data_ptr() for w in ws])
         bp = (ctypes.c_void_p * n)(*[b.data_ptr() for b in bs])
         h = ctypes.c_void_p()
-        _lib.check(L.nnconv_diag_weights_create(n, c_dims, channels, prec, wp, bp, _ptr(self.buf), nbytes.value,
-                                                _stream_ptr(dev), ctypes.byref(h)))
+        _lib.check(L.nnconv_diag_weights_create_act(n, c_dims, channels, prec, _lib.ACT[act[0]], act[1], wp, bp,
+                                                    _ptr(self.buf), nbytes.value, _stream_ptr(dev), ctypes.byref(h)))
         self._keep = (ws, bs)
         self.handle = h
         self.precision = precision
@@ -1076,7 +1133,8 @@ class DiagNNConv(torch.nn.Module):
     there):  x'_i = x_i root + bias + aggr_{j in N(i)} x_j * nn(e_ij), channel by channel.
 
     Same signature, attributes, state-dict keys and initialisation as NNConv_old (reference :47-73): the edge network
-    ``nn`` is a Linear (ReLU Linear)* chain whose output width is ``out_channels``.  The reference multiplies x_j by
+    ``nn`` is a Linear (act Linear)* chain (act: ReLU, LeakyReLU, ELU, Tanh or Sigmoid, see _edge_network) whose output
+    width is ``out_channels``.  The reference multiplies x_j by
     ``diag_embed(nn(e)).view(-1, in, out)``, which is the diagonal matrix only when nn's output width, in_channels and
     out_channels are equal; any other shape raises NotImplementedError.  ``aggr`` in {'add', 'mean', 'max'} ('max':
     the rules of NNConv_old), ``precision`` in {'f16' (default), 'bf16', 'f16x2', 'fp32'} selects the edge network's
@@ -1133,7 +1191,7 @@ class DiagNNConv(torch.nn.Module):
         return super(DiagNNConv, self)._load_from_state_dict(*args, **kwargs)
 
     def _check_shape(self):
-        lin = _linear_chain(self.nn)
+        lin = _edge_network(self.nn)[0]
         k = lin[-1].out_features
         if not (k == self.in_channels == self.out_channels):
             raise NotImplementedError(
@@ -1168,12 +1226,12 @@ class DiagNNConv(torch.nn.Module):
 
     # -- host-side sequencing ------------------------------------------------------------------------------------
     def _get_prepared(self, precision, slot='forward'):
-        linears = _linear_chain(self.nn)
-        key = (precision,) + tuple((l.weight.data_ptr(), l.weight._version, l.bias.data_ptr(), l.bias._version)
-                                   for l in linears)
+        linears, act = _edge_network(self.nn)
+        key = (precision, act) + tuple((l.weight.data_ptr(), l.weight._version, l.bias.data_ptr(), l.bias._version)
+                                       for l in linears)
         hit = self._prepared.get(slot)
         if hit is None or hit[0] != key:
-            hit = self._prepared[slot] = (key, _DiagWeights(linears, self.out_channels, precision))
+            hit = self._prepared[slot] = (key, _DiagWeights(linears, self.out_channels, precision, act))
             if slot == 'forward':
                 self._d_cache.clear()
         return hit[1]
@@ -1244,7 +1302,7 @@ class DiagNNConv(torch.nn.Module):
         L = _lib.lib()
         ea32 = state.feats.ea32
         dev = ea32.device
-        linears = _linear_chain(self.nn)
+        linears = _edge_network(self.nn)[0]
         with torch.cuda.device(dev):
             prep = self._get_prepared('fp32', 'backward')
             ws_b = ctypes.c_size_t()

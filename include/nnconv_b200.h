@@ -104,6 +104,25 @@ int nnconv_weights_create(int n_layers, const int* dims, int in_channels, int ou
                           nnconv_weights_t** out);
 void nnconv_weights_destroy(nnconv_weights_t* w);
 int nnconv_weights_tc_supported(const nnconv_weights_t* w);
+/* hidden activation of the edge MLP (the `nonlinearity` of utilities.py:201, applied after every Linear but the
+ * last).  Each has a derivative that is a function of its OUTPUT y = f(z), so every backward multiplies by f'(y) taken
+ * from the activations it already keeps or recomputes:
+ *   RELU        max(z, 0)                     f' = y > 0 ? 1 : 0
+ *   LEAKY_RELU  z > 0 ? z : s z   (s >= 0)    f' = y > 0 ? 1 : s
+ *   ELU         z > 0 ? z : a (e^z - 1) (a>=0) f' = y > 0 ? 1 : y + a
+ *   TANH        tanh z                        f' = 1 - y^2
+ *   SIGMOID     1 / (1 + e^-z)                f' = y (1 - y)
+ * act_param is s (LEAKY_RELU) or a (ELU) and is ignored otherwise.  The activation is stored in the handle and every
+ * entry point that runs or differentiates the edge MLP reads it from there; nnconv_weights_create is
+ * nnconv_weights_create_act with NNCONV_ACT_RELU. */
+#define NNCONV_ACT_RELU 0
+#define NNCONV_ACT_LEAKY_RELU 1
+#define NNCONV_ACT_ELU 2
+#define NNCONV_ACT_TANH 3
+#define NNCONV_ACT_SIGMOID 4
+int nnconv_weights_create_act(int n_layers, const int* dims, int in_channels, int out_channels, int precision,
+                              int activation, float act_param, const float* const* W, const float* const* b, void* buf,
+                              size_t buf_bytes, void* stream, nnconv_weights_t** out);
 
 /* ---- hoisted, x-independent part of message(): h_e for every edge (utilities.py:223-227 minus the
  * last Linear).  Valid as long as edge_attr and the weights are unchanged, i.e. for all T applications
@@ -321,6 +340,10 @@ int nnconv_diag_weights_sizes(int n_layers, const int* dims, int channels, int p
 int nnconv_diag_weights_create(int n_layers, const int* dims, int channels, int precision, const float* const* W,
                                const float* const* b, void* buf, size_t buf_bytes, void* stream,
                                nnconv_diag_weights_t** out);
+/* the same with the edge network's hidden activation (NNCONV_ACT_*, see nnconv_weights_create_act) */
+int nnconv_diag_weights_create_act(int n_layers, const int* dims, int channels, int precision, int activation,
+                                   float act_param, const float* const* W, const float* const* b, void* buf,
+                                   size_t buf_bytes, void* stream, nnconv_diag_weights_t** out);
 void nnconv_diag_weights_destroy(nnconv_diag_weights_t* w);
 int nnconv_diag_sizes(const nnconv_plan_t* plan, const nnconv_diag_weights_t* w, size_t want_ws_bytes, size_t* d_bytes,
                       size_t* ws_bytes);
