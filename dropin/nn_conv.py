@@ -1,7 +1,8 @@
 """Drop-in for graph-neural-operator/nn_conv.py: put this directory FIRST on sys.path (or PYTHONPATH) and the
 reference scripts' ``from nn_conv import NNConv_old`` (UAI1_full_resolution.py:9) and ``from nn_conv import NNConv,
-NNConv_old`` (neurips1_GKN.py:10, neurips5_GKN.py:10) resolve to this library's ops.  Whole-module checkpoints pickled
-by the reference bind to the class paths ``nn_conv.NNConv_old`` and ``nn_conv.NNConv`` -- kept."""
+NNConv_old`` (neurips1_GKN.py:10, neurips5_GKN.py:10) resolve to this library's ops, and so does the module's third
+class, ``NNConv_Gaussian``.  Whole-module checkpoints pickled by the reference bind to the class paths
+``nn_conv.NNConv_old``, ``nn_conv.NNConv`` and ``nn_conv.NNConv_Gaussian`` -- kept."""
 import os
 import sys
 
@@ -12,6 +13,7 @@ if _ROOT not in sys.path:
 from graph_pde_b200.nn_conv import NNConv_old as _Base  # noqa: E402
 from graph_pde_b200.nn_conv import NNConv as _UpstreamNNConv  # noqa: E402
 from graph_pde_b200.nn_conv import DiagNNConv as _Diag  # noqa: E402
+from graph_pde_b200.gauss import GaussianNNConv as _Gauss  # noqa: E402
 
 
 class NNConv_old(_Base):
@@ -23,9 +25,15 @@ class NNConv(_Diag):
     pass
 
 
-# The reference's nn_conv.py also defines `NNConv_Gaussian`, which no script instantiates: not provided.  Its ECConv
-# (nn_conv.py:288) names the diagonal class; here ECConv stays the upstream torch_geometric NNConv (INTEGRATION 1).
+class NNConv_Gaussian(_Gauss):
+    """The reference's Gaussian-kernel conv (nn_conv.py:99-194)."""
+    pass
+
+
+# The reference's ECConv (nn_conv.py:288) names the diagonal class; here ECConv stays the upstream torch_geometric
+# NNConv (INTEGRATION 1).
 NNConv_old.__module__ = 'nn_conv'
 NNConv.__module__ = 'nn_conv'
 NNConv.__qualname__ = 'NNConv'
+NNConv_Gaussian.__module__ = 'nn_conv'
 ECConv = _UpstreamNNConv

@@ -48,6 +48,7 @@ SYMBOLS = [
     'nnconv_gcn_graph_sizes', 'nnconv_gcn_graph_create', 'nnconv_gcn_graph_destroy', 'nnconv_gcn_apply_sizes',
     'nnconv_gcn_apply', 'nnconv_gcn_backward_sizes', 'nnconv_gcn_backward',
     'nnconv_weights_create_act', 'nnconv_diag_weights_create_act',
+    'nnconv_gauss_apply_sizes', 'nnconv_gauss_apply', 'nnconv_gauss_backward',
 ]
 GCN_IMPROVED, GCN_NO_SELF_LOOPS, GCN_NO_NORMALIZE = 1, 2, 4   # include/nnconv_b200.h NNCONV_GCN_*
 
@@ -189,6 +190,11 @@ def lib():
     L.nnconv_gcn_backward_sizes.argtypes = [c_vp, c_int, c_int, c_int, P(c_sz)]
     L.nnconv_gcn_backward.argtypes = [c_vp, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_sz, c_vp,
                                       P(c_i64)]
+    L.nnconv_gauss_apply_sizes.argtypes = [c_vp, c_int, c_int, P(c_sz)]
+    L.nnconv_gauss_apply.argtypes = [c_vp, c_vp, c_int, c_vp, c_int, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_sz, c_vp,
+                                     P(c_i64)]
+    L.nnconv_gauss_backward.argtypes = [c_vp, c_vp, c_int, c_vp, c_int, c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp,
+                                        c_vp, c_vp, c_vp, P(c_i64)]
     for name in SYMBOLS:
         getattr(L, name)
     if L.nnconv_abi_version() != ABI_VERSION:

@@ -1453,6 +1453,31 @@ int nnconv_backward_mlp_diag(const nnconv_plan_t* plan, const nnconv_diag_weight
                            static_cast<cudaStream_t>(stream), grad_edge_attr);
 }
 
+int nnconv_gauss_apply_sizes(const nnconv_plan_t* plan, int channels, int aggr, size_t* ws_bytes) {
+  NNC_REQUIRE(plan && ws_bytes, NNCONV_ERR_ARG, "null pointer");
+  *ws_bytes = gauss_apply_ws_bytes(&plan->p, channels, aggr);
+  return NNCONV_OK;
+}
+
+int nnconv_gauss_apply(const nnconv_plan_t* plan, const float* edge_attr, int k_in, const float* sigma, int channels,
+                       const float* x, const float* root, const float* bias, int aggr, float* out, int* argmax, void* ws,
+                       size_t ws_bytes, void* stream, int64_t* launches) {
+  NNC_REQUIRE(plan && x && out && sigma && (edge_attr || plan->p.E == 0), NNCONV_ERR_ARG, "null pointer");
+  NNC_REQUIRE(x != out, NNCONV_ERR_ARG, "out must not alias x");
+  return apply_gauss(&plan->p, edge_attr, k_in, sigma, channels, x, root, bias, aggr, out, argmax, ws, ws_bytes,
+                     static_cast<cudaStream_t>(stream), launches);
+}
+
+int nnconv_gauss_backward(const nnconv_plan_t* plan, const float* edge_attr, int k_in, const float* sigma, int channels,
+                          const float* x, const float* root, int aggr, const int* argmax, const float* grad_out,
+                          float* grad_x, float* grad_root, float* grad_bias, float* grad_sigma, float* grad_edge_attr,
+                          void* stream, int64_t* launches) {
+  NNC_REQUIRE(plan && x && sigma && grad_out && grad_x && (edge_attr || plan->p.E == 0), NNCONV_ERR_ARG, "null pointer");
+  NNC_REQUIRE((root == nullptr) == (grad_root == nullptr), NNCONV_ERR_ARG, "root / grad_root must both be given or both be NULL");
+  return backward_gauss(&plan->p, edge_attr, k_in, sigma, channels, x, root, aggr, argmax, grad_out, grad_x, grad_root,
+                        grad_bias, grad_sigma, grad_edge_attr, static_cast<cudaStream_t>(stream), launches);
+}
+
 int nnconv_backward_mlp_sizes(const nnconv_plan_t* plan, const nnconv_weights_t* w, int n_apps, size_t want_bytes,
                               size_t* ws_bytes) {
   NNC_REQUIRE(plan && w && ws_bytes && n_apps >= 1, NNCONV_ERR_ARG, "bad arguments");

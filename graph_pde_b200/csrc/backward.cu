@@ -591,6 +591,25 @@ DiagBwdLayout diag_bwd_layout(const Weights* W) {
 
 }  // namespace
 
+int backward_node_terms(const float* x, const float* root, const float* gout, int64_t N, int C, float* dx, float* droot,
+                        float* dbias, cudaStream_t st, int64_t* launches) {
+  if (dbias) {
+    k_colsum_rows<<<ceil_div(C, 32), dim3(32, 8), 0, st>>>(gout, N, C, dbias);
+    NNC_CHECK_LAUNCH();
+    ++*launches;
+  }
+  if (root != nullptr) {
+    int s = gemm_any(x, 1, C, gout, C, 1, droot, C, C, C, static_cast<int>(N), 0.f, st);   // droot = x^T g
+    if (s) return s;
+    s = gemm_any(gout, C, 1, root, 1, C, dx, C, static_cast<int>(N), C, C, 0.f, st);       // dx = g root^T
+    if (s) return s;
+    *launches += 2;
+  } else {
+    NNC_CHECK_CUDA(cudaMemsetAsync(dx, 0, sizeof(float) * N * C, st));
+  }
+  return NNCONV_OK;
+}
+
 int backward_apply_diag(const Plan* P, const Weights* W, const float* d, const float* x, const float* root, int aggr,
                         const int* argmax, const float* gout, float* dx, float* droot, float* dbias, float* dd,
                         cudaStream_t st, int64_t* launches) {
@@ -598,23 +617,9 @@ int backward_apply_diag(const Plan* P, const Weights* W, const float* d, const f
   NNC_REQUIRE(aggr >= 0 && aggr <= 2 && (aggr != 2 || argmax != nullptr), NNCONV_ERR_ARG,
               "backward_apply_diag: aggr %d (max needs the forward's argmax)", aggr);
   const int C = W->cout;
-  const int64_t N = P->N;
   int64_t n_l = 0;
-  int s;
-  if (dbias) {
-    k_colsum_rows<<<ceil_div(C, 32), dim3(32, 8), 0, st>>>(gout, N, C, dbias);
-    NNC_CHECK_LAUNCH();
-    ++n_l;
-  }
-  if (root != nullptr) {
-    s = gemm_any(x, 1, C, gout, C, 1, droot, C, C, C, static_cast<int>(N), 0.f, st);   // droot = x^T g
-    if (s) return s;
-    s = gemm_any(gout, C, 1, root, 1, C, dx, C, static_cast<int>(N), C, C, 0.f, st);   // dx = g root^T
-    if (s) return s;
-    n_l += 2;
-  } else {
-    NNC_CHECK_CUDA(cudaMemsetAsync(dx, 0, sizeof(float) * N * C, st));
-  }
+  const int s = backward_node_terms(x, root, gout, P->N, C, dx, droot, dbias, st, &n_l);
+  if (s) return s;
   if (P->E > 0 && P->n_tiles > 0) {
     const unsigned grid = static_cast<unsigned>(ceil_div64(static_cast<int64_t>(P->n_tiles) * 32, 256));
 #define NNC_DIAG_BWD(A)                                                                                               \

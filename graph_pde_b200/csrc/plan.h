@@ -181,6 +181,25 @@ size_t backward_mlp_diag_ws_bytes(const Plan* P, const Weights* W, size_t want_b
 int backward_mlp_diag(const Plan* P, const Weights* W, const float* edge_attr, const float* dd, float* const* dWs,
                       float* const* dbs, void* ws, size_t ws_bytes, cudaStream_t st, float* grad_ea);
 
+// node-level gradients of an application whose message is channel by channel (in == out == C), backward.cu:
+// dbias = sum_n g_n (dbias nullable), droot = x^T g and dx = g root^T (root NULL: dx = 0)
+int backward_node_terms(const float* x, const float* root, const float* gout, int64_t N, int C, float* dx, float* droot,
+                        float* dbias, cudaStream_t st, int64_t* launches);
+
+// Gaussian-kernel conv (gauss.cu, DESIGN 4.9): d_ec = exp(-p_e0^2 / sigma_c^2) / sqrt(|p_e1 p_e2|) computed in registers
+//   out_n = aggr_{e: dst_e = n} x_src(e) * d_e + x_n root + bias          (C == in == out, 1 <= C <= kGaussMaxChannels)
+// edge_attr [E, k_in] (k_in >= 3) in the caller's order, sigma [C].  apply_gauss: aggr 0 add, 1 mean, 2 max (ws:
+// max_keys_bytes of keys, argmax written).  backward_gauss: dx, droot, dbias, and the nullable dsigma [C] and dea
+// [E, k_in] (written, columns 3 and up 0) of one application.
+constexpr int kGaussMaxChannels = 4096;
+size_t gauss_apply_ws_bytes(const Plan* P, int C, int aggr);
+int apply_gauss(const Plan* P, const float* edge_attr, int k_in, const float* sigma, int C, const float* x,
+                const float* root, const float* bias, int aggr, float* out, int* argmax, void* ws, size_t ws_bytes,
+                cudaStream_t st, int64_t* launches);
+int backward_gauss(const Plan* P, const float* edge_attr, int k_in, const float* sigma, int C, const float* x,
+                   const float* root, int aggr, const int* argmax, const float* gout, float* dx, float* droot,
+                   float* dbias, float* dsigma, float* dea, cudaStream_t st, int64_t* launches);
+
 // backward of one application (fp32 CUDA-core path), backward.cu; grad_ea as for backward_mlp_tc.
 // aggr = max (all three backward calls): argmax [N, cout] of the forward (backward_mlp_tc: one per application) routes
 // each g[n, o] to the winning edge only, G_e[o] = g[dst_e, o] if argmax[dst_e, o] == caller index of e, else 0

@@ -9,6 +9,8 @@
  * and, through the same entry points, upstream torch_geometric.nn.NNConv as used by
  *   multipole-graph-neural-operator/neurips1_MGKN.py:41,49,57, MGKN_general_darcy2d.py:45,53,61,
  *   MGKN_orthogonal_burgers1d.py:37.
+ * The same module's diagonal-kernel NNConv (nn_conv.py:8-96) and NNConv_Gaussian (nn_conv.py:99-194), and PyG 1.x
+ * GCNConv, have entry points of their own below.
  *
  * Conventions
  *   - every function returns 0 on success or an NNCONV_ERR_* code; nnconv_last_error() returns a
@@ -361,6 +363,27 @@ int nnconv_backward_mlp_diag_sizes(const nnconv_plan_t* plan, const nnconv_diag_
 int nnconv_backward_mlp_diag(const nnconv_plan_t* plan, const nnconv_diag_weights_t* w, const float* edge_attr,
                              const float* grad_d, float* const* grad_W, float* const* grad_b, void* ws, size_t ws_bytes,
                              void* stream, float* grad_edge_attr /* nullable */);
+
+/* ---- Gaussian-kernel conv (graph-neural-operator/nn_conv.py:99-194 NNConv_Gaussian, DESIGN 4.9): with p_e the
+ * first three columns of edge_attr row e and a width-`channels` vector sigma (in == out == channels):
+ *   d_ec = exp(-p_e0^2 / sigma_c^2) / sqrt(|p_e1 p_e2|)
+ *   out[n] = aggr_{e: dst_e = n} x_src(e) * d_e + x_n root + bias
+ * aggr as NNCONV_AGGR_* (max: the rules of nnconv_apply_max, argmax written).  d is computed inside the kernels and
+ * never stored, so nothing per edge outlives a call.  edge_attr [E, k_in] fp32 (k_in >= 3) in the caller's edge order,
+ * sigma [channels] fp32, 1 <= channels <= 4096.  fp32 throughout; root and bias nullable.
+ *   nnconv_gauss_apply_sizes / nnconv_gauss_apply: one application (ws: the max keys; argmax NULL unless aggr is max).
+ *   nnconv_gauss_backward: grad_x, grad_root, grad_bias of one application and, when not NULL, grad_sigma [channels]
+ *     and grad_edge_attr [E, k_in] (caller's order; columns 3 and up are 0), all WRITTEN.  Gradients on edges with
+ *     p_e1 p_e2 = 0 or channels with sigma_c = 0 are not finite.
+ * No allocation; no host synchronisation. */
+int nnconv_gauss_apply_sizes(const nnconv_plan_t* plan, int channels, int aggr, size_t* ws_bytes);
+int nnconv_gauss_apply(const nnconv_plan_t* plan, const float* edge_attr, int k_in, const float* sigma, int channels,
+                       const float* x, const float* root, const float* bias, int aggr, float* out, int* argmax, void* ws,
+                       size_t ws_bytes, void* stream, int64_t* launches);
+int nnconv_gauss_backward(const nnconv_plan_t* plan, const float* edge_attr, int k_in, const float* sigma, int channels,
+                          const float* x, const float* root, int aggr, const int* argmax, const float* grad_out,
+                          float* grad_x, float* grad_root, float* grad_bias, float* grad_sigma /* nullable */,
+                          float* grad_edge_attr /* nullable */, void* stream, int64_t* launches);
 
 /* ---- GCNConv (PyG 1.x GCNConv, the reference's neurips4_GCN.py baseline; DESIGN 4.8):
  *   out = A_hat x W + bias,   A_hat = D^-1/2 (A + I_fill) D^-1/2
