@@ -49,6 +49,7 @@ SYMBOLS = [
     'nnconv_gcn_apply', 'nnconv_gcn_backward_sizes', 'nnconv_gcn_backward',
     'nnconv_weights_create_act', 'nnconv_diag_weights_create_act',
     'nnconv_gauss_apply_sizes', 'nnconv_gauss_apply', 'nnconv_gauss_backward',
+    'nnconv_plan_sizes_bipartite', 'nnconv_plan_create_bipartite', 'nnconv_root_term', 'nnconv_root_term_backward',
 ]
 GCN_IMPROVED, GCN_NO_SELF_LOOPS, GCN_NO_NORMALIZE = 1, 2, 4   # include/nnconv_b200.h NNCONV_GCN_*
 
@@ -88,6 +89,11 @@ def lib():
     L.nnconv_init.restype = c_int
     L.nnconv_plan_sizes.argtypes = [c_i64, c_i64, P(c_sz), P(c_sz)]
     L.nnconv_plan_create.argtypes = [c_vp, c_vp, c_i64, c_i64, c_int, c_vp, c_sz, c_vp, c_sz, c_vp, P(c_vp)]
+    L.nnconv_plan_sizes_bipartite.argtypes = [c_i64, c_i64, c_i64, P(c_sz), P(c_sz)]
+    L.nnconv_plan_create_bipartite.argtypes = [c_vp, c_vp, c_i64, c_i64, c_i64, c_int, c_vp, c_sz, c_vp, c_sz, c_vp,
+                                               P(c_vp)]
+    L.nnconv_root_term.argtypes = [c_vp, c_vp, c_vp, c_i64, c_int, c_int, c_vp, c_vp]
+    L.nnconv_root_term_backward.argtypes = [c_vp, c_vp, c_vp, c_i64, c_int, c_int, c_vp, c_vp, c_vp, c_vp, P(c_i64)]
     L.nnconv_plan_destroy.argtypes = [c_vp]
     L.nnconv_plan_destroy.restype = None
     L.nnconv_plan_info.argtypes = [c_vp, P(c_i64), c_int]

@@ -405,7 +405,9 @@ int apply_edge(const Plan* P, const Weights* W, const void* Kmat, const float* x
                int aggr_mean, float* out, cudaStream_t st, unsigned node_flags) {
   NNC_REQUIRE(!(node_flags & NNCONV_APPLY_RESIDUAL) || W->cin == W->cout, NNCONV_ERR_ARG,
               "NNCONV_APPLY_RESIDUAL needs in_channels == out_channels");
-  int s = launch_out_init(x, root, bias, P->N, W->cin, W->cout, out, st, node_flags);
+  int s = check_bipartite_root(P, root, node_flags);
+  if (s) return s;
+  s = launch_out_init(x, root, bias, P->N_dst, W->cin, W->cout, out, st, node_flags);
   if (s) return s;
   if (P->E == 0 || P->n_src == 0) return NNCONV_OK;
   return launch_apply_edge(W->prec, P, W, Kmat, x, aggr_mean, out, st, node_flags);
@@ -452,7 +454,7 @@ static size_t default_y_bytes(const Plan* P, const Weights* W) {
   }
   const size_t l2 = static_cast<size_t>(l2_bytes[dev] > 0 ? l2_bytes[dev] : 50 << 20);
   const size_t per_node = layout_apply(P, W).per_node;
-  const size_t used = static_cast<size_t>(P->N) * W->cout * sizeof(float) + l2 / kL2HeadroomDiv;
+  const size_t used = static_cast<size_t>(P->N_dst) * W->cout * sizeof(float) + l2 / kL2HeadroomDiv;
   const size_t fit = l2 > used ? l2 - used : 0;
   size_t floor_bytes = static_cast<size_t>(options().ring) * 128 * per_node;
   if (floor_bytes > l2) floor_bytes = l2;
@@ -725,10 +727,10 @@ static int apply_fp32(const Plan* P, const Weights* W, const float* h, const flo
                       unsigned node_flags, unsigned long long* max_keys) {
   int s;
   if (max_keys != nullptr)
-    NNC_CHECK_CUDA(cudaMemsetAsync(max_keys, 0, sizeof(unsigned long long) * P->N * W->cout, st));
+    NNC_CHECK_CUDA(cudaMemsetAsync(max_keys, 0, sizeof(unsigned long long) * P->N_dst * W->cout, st));
   {
     ProfScope ps(PK_NODE_PREP, st);
-    s = launch_out_init(x, root, bias, P->N, W->cin, W->cout, out, st, node_flags);
+    s = launch_out_init(x, root, bias, P->N_dst, W->cin, W->cout, out, st, node_flags);
   }
   if (s) return s;
   {
@@ -769,11 +771,13 @@ static int apply_contract(const Plan* P, const Weights* W, const void* h_res, in
   int s;
   NNC_REQUIRE(!(node_flags & NNCONV_APPLY_RESIDUAL) || W->cin == W->cout, NNCONV_ERR_ARG,
               "NNCONV_APPLY_RESIDUAL needs in_channels == out_channels");
+  s = check_bipartite_root(P, root, node_flags);
+  if (s) return s;
   if (P->E == 0 || P->n_src == 0) {
     ProfScope ps(PK_NODE_PREP, st);
     if (max_keys != nullptr)   // no edge: every key stays empty
-      NNC_CHECK_CUDA(cudaMemsetAsync(max_keys, 0, sizeof(unsigned long long) * P->N * W->cout, st));
-    s = launch_out_init(x, root, bias, P->N, W->cin, W->cout, out, st, node_flags);
+      NNC_CHECK_CUDA(cudaMemsetAsync(max_keys, 0, sizeof(unsigned long long) * P->N_dst * W->cout, st));
+    s = launch_out_init(x, root, bias, P->N_dst, W->cin, W->cout, out, st, node_flags);
     if (s == NNCONV_OK && launches) ++*launches;
     return s;
   }
@@ -821,7 +825,7 @@ static int apply_contract(const Plan* P, const Weights* W, const void* h_res, in
   // Invariant: no launch of an application reads a flag slot that was not cleared in that application.
   {
     ProfScope ps(PK_NODE_PREP, st);
-    s = launch_node_prep(W->prec, x, root, bias, P->N, out, P->src_nodes, P->n_src, W->cin, W->cin_p, W->cout, W->B3, A.Xc,
+    s = launch_node_prep(W->prec, x, root, bias, P->N_dst, out, P->src_nodes, P->n_src, W->cin, W->cin_p, W->cout, W->B3, A.Xc,
                          A.cvec, A.xs, A.flags, kMaxPipeBatches, static_cast<int>(n_flag), st, node_flags, max_keys);
   }
   if (s) return s;
@@ -862,7 +866,7 @@ static int apply_ranges(const Plan* P, const Weights* W, const void* h_res, int6
   int s = apply_contract(P, W, h_res, E_res, C, x, root, bias, aggr_mean, out, ws, ws_bytes, st, launches, node_flags,
                          max_keys);
   if (s || max_keys == nullptr) return s;
-  s = launch_max_finalize(max_keys, P->N * W->cout, out, argmax, st);
+  s = launch_max_finalize(max_keys, P->N_dst * W->cout, out, argmax, st);
   if (s == NNCONV_OK && launches) ++*launches;
   return s;
 }
@@ -901,7 +905,7 @@ int apply_streamed(const Plan* P, const Weights* W, const float* edge_attr, cons
 int apply_max(const Plan* P, const Weights* W, const float* edge_attr, const void* h_res, int64_t E_res, const float* x,
               const float* root, const float* bias, float* out, int* argmax, void* ws, size_t ws_bytes, cudaStream_t st,
               int64_t* launches, unsigned node_flags) {
-  const size_t kb = max_keys_bytes(P->N, W->cout);
+  const size_t kb = max_keys_bytes(P->N_dst, W->cout);
   NNC_REQUIRE(ws != nullptr && ws_bytes > kb, NNCONV_ERR_WORKSPACE,
               "apply_max: workspace too small (use the size nnconv_apply_max_sizes returns)");
   unsigned long long* keys = static_cast<unsigned long long*>(ws);
@@ -966,19 +970,34 @@ int nnconv_get_option(const char* name, int* value) {
 int nnconv_plan_sizes(int64_t E, int64_t N, size_t* ws_bytes, size_t* tmp_bytes) {
   NNC_REQUIRE(ws_bytes && tmp_bytes, NNCONV_ERR_ARG, "null output pointer");
   NNC_REQUIRE(E >= 0 && N >= 1, NNCONV_ERR_ARG, "need E >= 0, N >= 1");
-  plan_sizes(E, N, ws_bytes, tmp_bytes);
+  plan_sizes(E, N, N, ws_bytes, tmp_bytes);
+  return NNCONV_OK;
+}
+
+int nnconv_plan_sizes_bipartite(int64_t E, int64_t n_src, int64_t n_dst, size_t* ws_bytes, size_t* tmp_bytes) {
+  NNC_REQUIRE(ws_bytes && tmp_bytes, NNCONV_ERR_ARG, "null output pointer");
+  NNC_REQUIRE(E >= 0, NNCONV_ERR_ARG, "plan_sizes_bipartite: need E >= 0 (got %lld)", (long long)E);
+  NNC_REQUIRE(n_src >= 1, NNCONV_ERR_ARG, "plan_sizes_bipartite: need n_src >= 1 (got %lld)", (long long)n_src);
+  NNC_REQUIRE(n_dst >= 1, NNCONV_ERR_ARG, "plan_sizes_bipartite: need n_dst >= 1 (got %lld)", (long long)n_dst);
+  plan_sizes(E, n_src, n_dst, ws_bytes, tmp_bytes);
   return NNCONV_OK;
 }
 
 int nnconv_plan_create(const int64_t* row0, const int64_t* row1, int64_t E, int64_t N, int flow, void* ws, size_t ws_bytes,
                        void* tmp, size_t tmp_bytes, void* stream, nnconv_plan_t** out) {
+  return nnconv_plan_create_bipartite(row0, row1, E, N, N, flow, ws, ws_bytes, tmp, tmp_bytes, stream, out);
+}
+
+int nnconv_plan_create_bipartite(const int64_t* row0, const int64_t* row1, int64_t E, int64_t n_src, int64_t n_dst,
+                                 int flow, void* ws, size_t ws_bytes, void* tmp, size_t tmp_bytes, void* stream,
+                                 nnconv_plan_t** out) {
   NNC_REQUIRE(out != nullptr, NNCONV_ERR_ARG, "null output pointer");
   *out = nullptr;
   nnconv_plan* h = new (std::nothrow) nnconv_plan();
   NNC_REQUIRE(h != nullptr, NNCONV_ERR_ARG, "out of host memory");
   h->h_tile_ptr_storage = nullptr;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  int s = plan_build(&h->p, row0, row1, E, N, flow, ws, ws_bytes, tmp, tmp_bytes, st);
+  int s = plan_build(&h->p, row0, row1, E, n_src, n_dst, flow, ws, ws_bytes, tmp, tmp_bytes, st);
   if (s != NNCONV_OK) { delete h; return s; }
   // host mirror of tile_ptr (S+1 ints) so that batch tile ranges need no device read later
   const int S = h->p.n_src;
@@ -1016,13 +1035,48 @@ void nnconv_plan_destroy(nnconv_plan_t* plan) {
 int nnconv_plan_info(const nnconv_plan_t* plan, int64_t* info, int n_info) {
   NNC_REQUIRE(plan && info && n_info >= 7, NNCONV_ERR_ARG, "plan_info: need a plan and >= 7 slots");
   info[0] = plan->p.E;
-  info[1] = plan->p.N;
+  info[1] = plan->p.N_src;
   info[2] = plan->p.n_src;
   info[3] = plan->p.n_tiles;
   info[4] = plan->p.max_out_deg;
   info[5] = plan->p.src_sorted;
   info[6] = plan->p.flow;
+  if (n_info >= 8) info[7] = plan->p.N_dst;
   return NNCONV_OK;
+}
+
+int nnconv_root_term(const float* x, const float* root, const float* bias, int64_t n, int in_channels, int out_channels,
+                     float* out, void* stream) {
+  NNC_REQUIRE(out != nullptr && (root == nullptr || x != nullptr), NNCONV_ERR_ARG, "root_term: null pointer");
+  NNC_REQUIRE(n >= 0 && in_channels >= 1 && out_channels >= 1, NNCONV_ERR_ARG,
+              "root_term: need n >= 0 and channels >= 1 (got n=%lld, in=%d, out=%d)", (long long)n, in_channels,
+              out_channels);
+  NNC_REQUIRE(x != out, NNCONV_ERR_ARG, "root_term: out must not alias x");
+  return root_term(x, root, bias, n, in_channels, out_channels, out, static_cast<cudaStream_t>(stream));
+}
+
+int nnconv_root_term_backward(const float* x, const float* root, const float* grad_out, int64_t n, int in_channels,
+                              int out_channels, float* grad_x, float* grad_root, float* grad_bias, void* stream,
+                              int64_t* launches) {
+  NNC_REQUIRE(grad_out != nullptr, NNCONV_ERR_ARG, "root_term_backward: null grad_out");
+  NNC_REQUIRE(root == nullptr || (x && grad_x && grad_root), NNCONV_ERR_ARG,
+              "root_term_backward: root needs x, grad_x and grad_root");
+  NNC_REQUIRE(n >= 0 && in_channels >= 1 && out_channels >= 1, NNCONV_ERR_ARG,
+              "root_term_backward: need n >= 0 and channels >= 1 (got n=%lld, in=%d, out=%d)", (long long)n,
+              in_channels, out_channels);
+  int64_t n_l = 0;
+  int s = NNCONV_OK;
+  if (n > 0) {
+    s = node_terms_rows(x, root, grad_out, n, in_channels, out_channels, root ? grad_x : nullptr, grad_root, grad_bias,
+                        static_cast<cudaStream_t>(stream), &n_l);
+  } else if (grad_bias != nullptr) {
+    NNC_CHECK_CUDA(cudaMemsetAsync(grad_bias, 0, sizeof(float) * out_channels, static_cast<cudaStream_t>(stream)));
+  }
+  if (root != nullptr && n == 0)
+    NNC_CHECK_CUDA(cudaMemsetAsync(grad_root, 0, sizeof(float) * in_channels * out_channels,
+                                   static_cast<cudaStream_t>(stream)));
+  if (launches) *launches += n_l;
+  return s;
 }
 
 int nnconv_weights_sizes(int n_layers, const int* dims, int in_channels, int out_channels, int precision,
@@ -1303,7 +1357,7 @@ int nnconv_backward_streamed_chunks(const nnconv_plan_t* plan, const nnconv_weig
 
 int nnconv_apply_max_sizes(const nnconv_plan_t* plan, const nnconv_weights_t* w, size_t ws_bytes, size_t* max_ws_bytes) {
   NNC_REQUIRE(plan && w && max_ws_bytes, NNCONV_ERR_ARG, "null pointer");
-  *max_ws_bytes = max_keys_bytes(plan->p.N, w->w.cout) + ws_bytes;
+  *max_ws_bytes = max_keys_bytes(plan->p.N_dst, w->w.cout) + ws_bytes;
   return NNCONV_OK;
 }
 
@@ -1416,7 +1470,7 @@ int nnconv_diag_build(const nnconv_plan_t* plan, const nnconv_diag_weights_t* w,
 
 int nnconv_apply_diag_sizes(const nnconv_plan_t* plan, const nnconv_diag_weights_t* w, int aggr, size_t* ws_bytes) {
   NNC_REQUIRE(plan && w && ws_bytes, NNCONV_ERR_ARG, "null pointer");
-  *ws_bytes = aggr == NNCONV_AGGR_MAX ? max_keys_bytes(plan->p.N, w->w.cout) : 1024;
+  *ws_bytes = aggr == NNCONV_AGGR_MAX ? max_keys_bytes(plan->p.N_dst, w->w.cout) : 1024;
   return NNCONV_OK;
 }
 

@@ -365,9 +365,10 @@ int backward_fp32(const Plan* P, const Weights* W, const float* edge_attr, const
   NNC_REQUIRE(W->prec == PREC_FP32, NNCONV_ERR_ARG, "backward needs weights prepared with precision fp32");
   const int nl = W->n_layers;
   const int cin = W->cin, cout = W->cout, Kp = W->Kp, cin_p = W->cin_p;
-  const int64_t N = P->N;
+  const int64_t N = P->N_dst;   // rows of gout; dx has N_src rows (square plans: the same)
   const int NY = cout * Kp;
-  int s;
+  int s = check_bipartite_root(P, root, 0);
+  if (s) return s;
   const int TB = 256;
   // ---- node-level terms: dbias, droot, dx = g root^T
   if (dbias) {
@@ -382,7 +383,7 @@ int backward_fp32(const Plan* P, const Weights* W, const float* edge_attr, const
     s = gemm_any(gout, cout, 1, root, 1, cout, dx, cin, static_cast<int>(N), cin, cout, 0.f, st);
     if (s) return s;
   } else {
-    NNC_CHECK_CUDA(cudaMemsetAsync(dx, 0, sizeof(float) * N * cin, st));
+    NNC_CHECK_CUDA(cudaMemsetAsync(dx, 0, sizeof(float) * P->N_src * cin, st));
   }
   BwdLayout L = bwd_layout(P, W);
   NNC_REQUIRE(ws != nullptr && ws_bytes >= L.fixed, NNCONV_ERR_WORKSPACE, "backward: workspace too small");
@@ -591,21 +592,21 @@ DiagBwdLayout diag_bwd_layout(const Weights* W) {
 
 }  // namespace
 
-int backward_node_terms(const float* x, const float* root, const float* gout, int64_t N, int C, float* dx, float* droot,
-                        float* dbias, cudaStream_t st, int64_t* launches) {
+int backward_node_terms(const float* x, const float* root, const float* gout, int64_t N, int cin, int cout, float* dx,
+                        float* droot, float* dbias, cudaStream_t st, int64_t* launches) {
   if (dbias) {
-    k_colsum_rows<<<ceil_div(C, 32), dim3(32, 8), 0, st>>>(gout, N, C, dbias);
+    k_colsum_rows<<<ceil_div(cout, 32), dim3(32, 8), 0, st>>>(gout, N, cout, dbias);
     NNC_CHECK_LAUNCH();
     ++*launches;
   }
   if (root != nullptr) {
-    int s = gemm_any(x, 1, C, gout, C, 1, droot, C, C, C, static_cast<int>(N), 0.f, st);   // droot = x^T g
+    int s = gemm_any(x, 1, cin, gout, cout, 1, droot, cout, cin, cout, static_cast<int>(N), 0.f, st);   // droot = x^T g
     if (s) return s;
-    s = gemm_any(gout, C, 1, root, 1, C, dx, C, static_cast<int>(N), C, C, 0.f, st);       // dx = g root^T
+    s = gemm_any(gout, cout, 1, root, 1, cout, dx, cin, static_cast<int>(N), cin, cout, 0.f, st);       // dx = g root^T
     if (s) return s;
     *launches += 2;
-  } else {
-    NNC_CHECK_CUDA(cudaMemsetAsync(dx, 0, sizeof(float) * N * C, st));
+  } else if (dx != nullptr) {
+    NNC_CHECK_CUDA(cudaMemsetAsync(dx, 0, sizeof(float) * N * cin, st));
   }
   return NNCONV_OK;
 }
@@ -618,7 +619,8 @@ int backward_apply_diag(const Plan* P, const Weights* W, const float* d, const f
               "backward_apply_diag: aggr %d (max needs the forward's argmax)", aggr);
   const int C = W->cout;
   int64_t n_l = 0;
-  const int s = backward_node_terms(x, root, gout, P->N, C, dx, droot, dbias, st, &n_l);
+  if (int sq = check_square(P, "backward_apply_diag")) return sq;
+  const int s = backward_node_terms(x, root, gout, P->N_dst, C, C, dx, droot, dbias, st, &n_l);
   if (s) return s;
   if (P->E > 0 && P->n_tiles > 0) {
     const unsigned grid = static_cast<unsigned>(ceil_div64(static_cast<int64_t>(P->n_tiles) * 32, 256));

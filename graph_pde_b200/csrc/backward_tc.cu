@@ -941,6 +941,30 @@ int apply_stream_batch_end(const Plan* P, const Weights* W, const ApplyBwdLayout
 
 }  // namespace
 
+int node_terms_rows(const float* x, const float* root, const float* gout, int64_t N, int cin, int cout, float* dx,
+                    float* droot, float* dbias, cudaStream_t st, int64_t* launches) {
+  const size_t smem_xtv = sizeof(float) * 32 * (cin + cout), smem_rootT = sizeof(float) * cin * (cout + 1);
+  if (smem_xtv > 48 * 1024 || smem_rootT > 48 * 1024)
+    return backward_node_terms(x, root, gout, N, cin, cout, dx, droot, dbias, st, launches);
+  if (dbias) {
+    NNC_CHECK_CUDA(cudaMemsetAsync(dbias, 0, sizeof(float) * cout, st));
+    k_colsum<<<dim3(ceil_div(cout, 32), 64), dim3(32, 8), 0, st>>>(gout, N, cout, dbias);
+    NNC_CHECK_LAUNCH();
+    ++*launches;
+  }
+  if (root != nullptr) {
+    NNC_CHECK_CUDA(cudaMemsetAsync(droot, 0, sizeof(float) * cin * cout, st));
+    k_xtv<<<(unsigned)ceil_div64(N, 32), 256, smem_xtv, st>>>(x, nullptr, gout, N, cin, cout, droot);
+    NNC_CHECK_LAUNCH();
+    k_g_rootT<<<(unsigned)ceil_div64(N * cin, 256), 256, smem_rootT, st>>>(gout, root, N, cin, cout, dx);
+    NNC_CHECK_LAUNCH();
+    *launches += 2;
+  } else if (dx != nullptr) {
+    NNC_CHECK_CUDA(cudaMemsetAsync(dx, 0, sizeof(float) * N * cin, st));
+  }
+  return NNCONV_OK;
+}
+
 size_t backward_apply_ws_bytes(const Plan* P, const Weights* W, size_t want_bytes, int64_t E_res, size_t chunk_ws_bytes) {
   ApplyBwdLayout L = apply_bwd_layout(P, W);
   const size_t S = P->n_src > 0 ? P->n_src : 1;
@@ -965,13 +989,15 @@ int backward_apply_tc(const Plan* P, const Weights* W, const float* edge_attr, c
                       int64_t* launches, const int* argmax) {
   NNC_REQUIRE(backward_tc_supported(W), NNCONV_ERR_UNSUPPORTED, "tensor-core backward: unsupported shape / precision");
   const int cin = W->cin, cout = W->cout, Kp = W->Kp, cin_p = W->cin_p;
-  const int64_t N = P->N;
+  const int64_t N = P->N_dst;   // rows of gout; dx has N_src rows (square plans: the same)
   const int bf = W->prec == PREC_BF16;
   const int sp = W->split;
   const bool streamed = E_res < P->E;
   NNC_REQUIRE(!streamed || edge_attr != nullptr, NNCONV_ERR_ARG, "backward_apply: streamed edge features need edge_attr");
   auto count = [&](int64_t k) { if (launches) *launches += k; };
-  int s = tc_init();
+  int s = check_bipartite_root(P, root, 0);
+  if (s) return s;
+  s = tc_init();
   if (s) return s;
   // ---- node-level terms
   if (dbias) {
@@ -988,7 +1014,7 @@ int backward_apply_tc(const Plan* P, const Weights* W, const float* edge_attr, c
     NNC_CHECK_LAUNCH();
     count(2);
   } else {
-    NNC_CHECK_CUDA(cudaMemsetAsync(dx, 0, sizeof(float) * N * cin, st));
+    NNC_CHECK_CUDA(cudaMemsetAsync(dx, 0, sizeof(float) * P->N_src * cin, st));
   }
   NNC_CHECK_CUDA(cudaMemsetAsync(dbL, 0, sizeof(float) * cin * cout, st));
   const int64_t nWL = static_cast<int64_t>(cin) * cout * W->K;
@@ -1271,7 +1297,7 @@ int backward_mlp_tc(const Plan* P, const Weights* W, const float* edge_attr, con
     float* xs = reinterpret_cast<float*>(base + L.off_xs[t]);
     s = launch_src_prep(W->prec, xs_in[t], P->src_nodes, S, cin, cin_p, cout, W->B3, Xc, cvec, xs, st);
     if (s) return s;
-    k_absmax_rows<<<592, 256, 0, st>>>(gouts[t], inv_deg, nullptr, P->N, cout, scal + t);
+    k_absmax_rows<<<592, 256, 0, st>>>(gouts[t], inv_deg, nullptr, P->N_dst, cout, scal + t);
     NNC_CHECK_LAUNCH();
     k_max_f<<<64, 256, 0, st>>>(xs, S, scal + 8 + t);
     NNC_CHECK_LAUNCH();

@@ -177,15 +177,16 @@ int apply_diag(const Plan* P, const Weights* W, const float* d, const float* x, 
                int aggr, float* out, int* argmax, void* ws, size_t ws_bytes, cudaStream_t st, int64_t* launches) {
   NNC_REQUIRE(W->diag, NNCONV_ERR_ARG, "apply_diag: weights not prepared as a diagonal kernel");
   NNC_REQUIRE(aggr >= 0 && aggr <= 2, NNCONV_ERR_ARG, "apply_diag: unknown aggr %d", aggr);
+  if (int sq = check_square(P, "apply_diag")) return sq;
   const int cout = W->cout;
   unsigned long long* keys = nullptr;
   if (aggr == 2) {
-    NNC_REQUIRE(argmax != nullptr && ws != nullptr && ws_bytes >= max_keys_bytes(P->N, cout), NNCONV_ERR_WORKSPACE,
+    NNC_REQUIRE(argmax != nullptr && ws != nullptr && ws_bytes >= max_keys_bytes(P->N_dst, cout), NNCONV_ERR_WORKSPACE,
                 "apply_diag: aggr max needs argmax and a workspace of nnconv_apply_diag_sizes bytes");
     keys = static_cast<unsigned long long*>(ws);
-    NNC_CHECK_CUDA(cudaMemsetAsync(keys, 0, sizeof(unsigned long long) * P->N * cout, st));
+    NNC_CHECK_CUDA(cudaMemsetAsync(keys, 0, sizeof(unsigned long long) * P->N_dst * cout, st));
   }
-  int s = launch_out_init(x, root, bias, P->N, cout, cout, out, st, 0);
+  int s = launch_out_init(x, root, bias, P->N_dst, cout, cout, out, st, 0);
   if (s) return s;
   int64_t n_l = 1;
   if (P->E > 0 && P->n_tiles > 0) {
@@ -211,7 +212,7 @@ int apply_diag(const Plan* P, const Weights* W, const float* d, const float* x, 
     ++n_l;
   }
   if (aggr == 2) {
-    s = launch_max_finalize(keys, P->N * cout, out, argmax, st);
+    s = launch_max_finalize(keys, P->N_dst * cout, out, argmax, st);
     if (s) return s;
     ++n_l;
   }

@@ -239,23 +239,24 @@ bool gauss_aligned(const void* a, const void* b, const void* c, const void* d = 
 
 }  // namespace
 
-size_t gauss_apply_ws_bytes(const Plan* P, int C, int aggr) { return aggr == 2 ? max_keys_bytes(P->N, C) : 1024; }
+size_t gauss_apply_ws_bytes(const Plan* P, int C, int aggr) { return aggr == 2 ? max_keys_bytes(P->N_dst, C) : 1024; }
 
 int apply_gauss(const Plan* P, const float* edge_attr, int k_in, const float* sigma, int C, const float* x,
                 const float* root, const float* bias, int aggr, float* out, int* argmax, void* ws, size_t ws_bytes,
                 cudaStream_t st, int64_t* launches) {
   NNC_REQUIRE(aggr >= 0 && aggr <= 2, NNCONV_ERR_ARG, "apply_gauss: unknown aggr %d", aggr);
+  if (int sq = check_square(P, "apply_gauss")) return sq;
   NNC_REQUIRE(C >= 1 && C <= kGaussMaxChannels, NNCONV_ERR_UNSUPPORTED, "apply_gauss: channels %d not in [1, %d]", C,
               kGaussMaxChannels);
   NNC_REQUIRE(k_in >= 3, NNCONV_ERR_ARG, "apply_gauss: edge_attr needs at least 3 columns, got %d", k_in);
   unsigned long long* keys = nullptr;
   if (aggr == 2) {
-    NNC_REQUIRE(argmax != nullptr && ws != nullptr && ws_bytes >= max_keys_bytes(P->N, C), NNCONV_ERR_WORKSPACE,
+    NNC_REQUIRE(argmax != nullptr && ws != nullptr && ws_bytes >= max_keys_bytes(P->N_dst, C), NNCONV_ERR_WORKSPACE,
                 "apply_gauss: aggr max needs argmax and a workspace of nnconv_gauss_apply_sizes bytes");
     keys = static_cast<unsigned long long*>(ws);
-    NNC_CHECK_CUDA(cudaMemsetAsync(keys, 0, sizeof(unsigned long long) * P->N * C, st));
+    NNC_CHECK_CUDA(cudaMemsetAsync(keys, 0, sizeof(unsigned long long) * P->N_dst * C, st));
   }
-  int s = launch_out_init(x, root, bias, P->N, C, C, out, st, 0);
+  int s = launch_out_init(x, root, bias, P->N_dst, C, C, out, st, 0);
   if (s) return s;
   int64_t n_l = 1;
   if (P->E > 0 && P->n_tiles > 0) {
@@ -280,7 +281,7 @@ int apply_gauss(const Plan* P, const float* edge_attr, int k_in, const float* si
     ++n_l;
   }
   if (aggr == 2) {
-    s = launch_max_finalize(keys, P->N * C, out, argmax, st);
+    s = launch_max_finalize(keys, P->N_dst * C, out, argmax, st);
     if (s) return s;
     ++n_l;
   }
@@ -293,11 +294,12 @@ int backward_gauss(const Plan* P, const float* edge_attr, int k_in, const float*
                    float* dbias, float* dsigma, float* dea, cudaStream_t st, int64_t* launches) {
   NNC_REQUIRE(aggr >= 0 && aggr <= 2 && (aggr != 2 || argmax != nullptr), NNCONV_ERR_ARG,
               "backward_gauss: aggr %d (max needs the forward's argmax)", aggr);
+  if (int sq = check_square(P, "backward_gauss")) return sq;
   NNC_REQUIRE(C >= 1 && C <= kGaussMaxChannels, NNCONV_ERR_UNSUPPORTED, "backward_gauss: channels %d not in [1, %d]", C,
               kGaussMaxChannels);
   NNC_REQUIRE(k_in >= 3, NNCONV_ERR_ARG, "backward_gauss: edge_attr needs at least 3 columns, got %d", k_in);
   int64_t n_l = 0;
-  int s = backward_node_terms(x, root, gout, P->N, C, dx, droot, dbias, st, &n_l);
+  int s = backward_node_terms(x, root, gout, P->N_dst, C, C, dx, droot, dbias, st, &n_l);
   if (s) return s;
   if (dsigma) NNC_CHECK_CUDA(cudaMemsetAsync(dsigma, 0, sizeof(float) * C, st));
   if (P->E > 0 && P->n_tiles > 0) {

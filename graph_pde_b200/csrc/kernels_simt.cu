@@ -353,6 +353,25 @@ __global__ void k_out_init(const float* __restrict__ x, const float* __restrict_
   out_init_rows(x, root, bias, N, cin, cout, out, node_flags, blockIdx.x, sx);
 }
 
+// out[n, o] += bias[o] + sum_i x[n, i] root[i, o]: the root term of a bipartite application (x = x_dst), added after
+// its messages.  The sum is out_init_rows' (same order), so a probe exact in fp32 gets the square conv's bits.
+__global__ void k_root_add(const float* __restrict__ x, const float* __restrict__ root, const float* __restrict__ bias,
+                           int64_t N, int cin, int cout, float* __restrict__ out) {
+  extern __shared__ float sx[];   // [nodes_per_block][cin]
+  const int64_t n = static_cast<int64_t>(blockIdx.x) * blockDim.y + threadIdx.y;
+  float* myx = sx + threadIdx.y * cin;
+  if (root != nullptr && n < N)
+    for (int i = threadIdx.x; i < cin; i += blockDim.x) myx[i] = x[n * cin + i];
+  __syncthreads();
+  if (n >= N) return;
+  for (int o = threadIdx.x; o < cout; o += blockDim.x) {
+    float acc = bias ? bias[o] : 0.f;
+    if (root)
+      for (int i = 0; i < cin; ++i) acc = fmaf(myx[i], root[i * cout + o], acc);
+    out[n * cout + o] += acc;
+  }
+}
+
 // per compact source c: Xc[c, :] = x[src_nodes[c], :] / xs[c] (converted, zero padded to cin_p),
 //                       cvec[c, o] = sum_i x[n, i] * B3[i, o]       (bias of the last Linear, reassociated)
 // xs[c] (16-bit paths only) = the power of two >= max_i |x[n, i]| (1 for an all-zero row): the contraction is
@@ -936,6 +955,16 @@ int launch_out_init(const float* x, const float* root, const float* bias, int64_
   dim3 b(64, 4);
   unsigned g = (unsigned)ceil_div64(N, b.y);
   k_out_init<<<g, b, sizeof(float) * b.y * cin, st>>>(x, root, bias, N, cin, cout, out, node_flags);
+  NNC_CHECK_LAUNCH();
+  return NNCONV_OK;
+}
+
+int root_term(const float* x, const float* root, const float* bias, int64_t N, int cin, int cout, float* out,
+              cudaStream_t st) {
+  if (N <= 0 || (root == nullptr && bias == nullptr)) return NNCONV_OK;
+  dim3 b(64, 4);
+  unsigned g = (unsigned)ceil_div64(N, b.y);
+  k_root_add<<<g, b, root ? sizeof(float) * b.y * cin : 0, st>>>(x, root, bias, N, cin, cout, out);
   NNC_CHECK_LAUNCH();
   return NNCONV_OK;
 }

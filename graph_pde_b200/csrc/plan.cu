@@ -6,7 +6,9 @@
 // Y_src), so the plan (a) verifies / establishes the source grouping (stable radix sort only when the
 // caller's list is not already grouped), (b) compacts the sources that have out-edges, (c) cuts every
 // source group into tiles of <= 128 edges (= one 128-row wgmma tile), (d) stores dst as int32 in sorted order
-// and 1/max(in_degree,1) for the mean aggregation (PyG scatter_('mean'), empty set -> 0).
+// and 1/max(in_degree,1) for the mean aggregation (PyG scatter_('mean'), empty set -> 0).  Sources and targets are
+// counted separately (N_src, N_dst): equal for a square graph, two node sets for a bipartite one (DESIGN 4.10).  Every
+// per-source array runs over N_src, the in-degrees and inv_deg over N_dst.
 #include <cub/cub.cuh>
 
 #include "common.cuh"
@@ -16,13 +18,15 @@ namespace nnc {
 
 namespace {
 
-__global__ void k_count(const int64_t* __restrict__ src, const int64_t* __restrict__ dst, int64_t E, int64_t N,
-                        int* __restrict__ outdeg, int* __restrict__ indeg, int* __restrict__ flags) {
+__global__ void k_count(const int64_t* __restrict__ src, const int64_t* __restrict__ dst, int64_t E, int64_t N_src,
+                        int64_t N_dst, int* __restrict__ outdeg, int* __restrict__ indeg, int* __restrict__ flags) {
   int64_t e = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
   if (e >= E) return;
   int64_t s = src[e], d = dst[e];
-  if (s < 0 || s >= N || d < 0 || d >= N) {
-    atomicOr(&flags[1], 1);   // index out of range
+  const bool bad_s = s < 0 || s >= N_src, bad_d = d < 0 || d >= N_dst;
+  if (bad_s || bad_d) {       // index out of range: flags[1] source row, flags[2] target row
+    if (bad_s) atomicOr(&flags[1], 1);
+    if (bad_d) atomicOr(&flags[2], 1);
     return;
   }
   atomicAdd(&outdeg[s], 1);
@@ -125,10 +129,10 @@ struct PlanLayout {
   size_t ws_bytes;
 };
 
-PlanLayout carve_plan(void* ws, int64_t E, int64_t N) {
+PlanLayout carve_plan(void* ws, int64_t E, int64_t N_src, int64_t N_dst) {
   Carver c(ws, ~size_t(0));
   PlanLayout L;
-  int64_t Smax = (N < E ? N : E) + 1;
+  int64_t Smax = (N_src < E ? N_src : E) + 1;
   int64_t Tmax = E / kTileEdges + Smax + 1;
   L.perm = c.take<int>(E + 1);
   L.dst_sorted = c.take<int>(E + 1);
@@ -141,7 +145,7 @@ PlanLayout carve_plan(void* ws, int64_t E, int64_t N) {
   L.unit_ptr = c.take<int>(Smax + 1);
   L.unit_t = c.take<int>(Tmax);
   L.unit_u = c.take<int>(Tmax);
-  L.inv_deg = c.take<float>(N + 1);
+  L.inv_deg = c.take<float>(N_dst + 1);
   L.ws_bytes = c.off;
   return L;
 }
@@ -153,11 +157,12 @@ struct TmpLayout {
   size_t bytes;
 };
 
-TmpLayout carve_tmp(void* tmp, int64_t E, int64_t N) {
+TmpLayout carve_tmp(void* tmp, int64_t E, int64_t N_src, int64_t N_dst) {
   Carver c(tmp, ~size_t(0));
   TmpLayout L;
+  const int64_t N = N_src;     // the per-source arrays
   L.outdeg = c.take<int>(N + 1);
-  L.indeg = c.take<int>(N + 1);
+  L.indeg = c.take<int>(N_dst + 1);
   L.rowptr = c.take<int>(N + 1);
   L.nz = c.take<int>(N + 1);
   L.nt = c.take<int>(N + 1);
@@ -179,20 +184,22 @@ TmpLayout carve_tmp(void* tmp, int64_t E, int64_t N) {
 
 }  // namespace
 
-void plan_sizes(int64_t E, int64_t N, size_t* ws_bytes, size_t* tmp_bytes) {
-  *ws_bytes = carve_plan(nullptr, E, N).ws_bytes;
-  *tmp_bytes = carve_tmp(nullptr, E, N).bytes;
+void plan_sizes(int64_t E, int64_t N_src, int64_t N_dst, size_t* ws_bytes, size_t* tmp_bytes) {
+  *ws_bytes = carve_plan(nullptr, E, N_src, N_dst).ws_bytes;
+  *tmp_bytes = carve_tmp(nullptr, E, N_src, N_dst).bytes;
 }
 
-int plan_build(Plan* P, const int64_t* row0, const int64_t* row1, int64_t E, int64_t N, int flow, void* ws, size_t ws_bytes,
-               void* tmp, size_t tmp_bytes, cudaStream_t st) {
-  NNC_REQUIRE(E >= 0 && N >= 1, NNCONV_ERR_ARG, "plan: need E >= 0 and N >= 1 (got E=%lld N=%lld)",
-              (long long)E, (long long)N);
-  NNC_REQUIRE(E < (int64_t(1) << 31) - 256 && N < (int64_t(1) << 31) - 256, NNCONV_ERR_UNSUPPORTED,
-              "plan: E and N must fit int32");
+int plan_build(Plan* P, const int64_t* row0, const int64_t* row1, int64_t E, int64_t N_src, int64_t N_dst, int flow, void* ws,
+               size_t ws_bytes, void* tmp, size_t tmp_bytes, cudaStream_t st) {
+  NNC_REQUIRE(E >= 0 && N_src >= 1 && N_dst >= 1, NNCONV_ERR_ARG,
+              "plan: need E >= 0, n_src >= 1 and n_dst >= 1 (got E=%lld n_src=%lld n_dst=%lld)", (long long)E,
+              (long long)N_src, (long long)N_dst);
+  NNC_REQUIRE(E < (int64_t(1) << 31) - 256 && N_src < (int64_t(1) << 31) - 256 && N_dst < (int64_t(1) << 31) - 256,
+              NNCONV_ERR_UNSUPPORTED, "plan: E and N must fit int32");
   NNC_REQUIRE(flow == 0 || flow == 1, NNCONV_ERR_ARG, "plan: flow must be 0 (source_to_target) or 1");
-  PlanLayout L = carve_plan(ws, E, N);
-  TmpLayout T = carve_tmp(tmp, E, N);
+  const int64_t N = N_src;     // every per-source array and kernel below
+  PlanLayout L = carve_plan(ws, E, N_src, N_dst);
+  TmpLayout T = carve_tmp(tmp, E, N_src, N_dst);
   NNC_REQUIRE(ws != nullptr && tmp != nullptr, NNCONV_ERR_ARG, "plan: null workspace");
   NNC_REQUIRE(L.ws_bytes <= ws_bytes && T.bytes <= tmp_bytes, NNCONV_ERR_WORKSPACE,
               "plan: workspace too small (need %zu + %zu bytes)", L.ws_bytes, T.bytes);
@@ -201,7 +208,8 @@ int plan_build(Plan* P, const int64_t* row0, const int64_t* row1, int64_t E, int
   const int64_t* dst = flow == 0 ? row1 : row0;
 
   P->E = E;
-  P->N = N;
+  P->N_src = N_src;
+  P->N_dst = N_dst;
   P->flow = flow;
   P->perm = nullptr;
   P->dst_sorted = L.dst_sorted;
@@ -223,17 +231,21 @@ int plan_build(Plan* P, const int64_t* row0, const int64_t* row1, int64_t E, int
 
   const int TB = 256;
   NNC_CHECK_CUDA(cudaMemsetAsync(T.outdeg, 0, (N + 1) * sizeof(int), st));
-  NNC_CHECK_CUDA(cudaMemsetAsync(T.indeg, 0, (N + 1) * sizeof(int), st));
+  NNC_CHECK_CUDA(cudaMemsetAsync(T.indeg, 0, (N_dst + 1) * sizeof(int), st));
   NNC_CHECK_CUDA(cudaMemsetAsync(T.flags, 0, 8 * sizeof(int), st));
   NNC_CHECK_CUDA(cudaMemsetAsync(T.counts, 0, 8 * sizeof(int), st));
   if (E > 0) {
-    k_count<<<(unsigned)ceil_div64(E, TB), TB, 0, st>>>(src, dst, E, N, T.outdeg, T.indeg, T.flags);
+    k_count<<<(unsigned)ceil_div64(E, TB), TB, 0, st>>>(src, dst, E, N_src, N_dst, T.outdeg, T.indeg, T.flags);
     NNC_CHECK_LAUNCH();
   }
-  int h_flags[2] = {0, 0};
-  NNC_CHECK_CUDA(cudaMemcpyAsync(h_flags, T.flags, 2 * sizeof(int), cudaMemcpyDeviceToHost, st));
+  int h_flags[3] = {0, 0, 0};
+  NNC_CHECK_CUDA(cudaMemcpyAsync(h_flags, T.flags, 3 * sizeof(int), cudaMemcpyDeviceToHost, st));
   NNC_CHECK_CUDA(cudaStreamSynchronize(st));
-  NNC_REQUIRE(h_flags[1] == 0, NNCONV_ERR_ARG, "plan: edge_index has entries outside [0, N)");
+  // the rows are named as the caller passes them: flow 0 gathers from row 0, flow 1 from row 1
+  NNC_REQUIRE(h_flags[1] == 0, NNCONV_ERR_ARG, "plan: edge_index row %d (source row) has entries outside [0, %lld)",
+              flow == 0 ? 0 : 1, (long long)N_src);
+  NNC_REQUIRE(h_flags[2] == 0, NNCONV_ERR_ARG, "plan: edge_index row %d (target row) has entries outside [0, %lld)",
+              flow == 0 ? 1 : 0, (long long)N_dst);
   if (h_flags[0] != 0 && E > 0) {   // not grouped by source: stable sort by source, keep the permutation
     P->src_sorted = 0;
     P->perm = L.perm;
@@ -265,7 +277,7 @@ int plan_build(Plan* P, const int64_t* row0, const int64_t* row1, int64_t E, int
     k_sorted_dst<<<(unsigned)ceil_div64(E, TB), TB, 0, st>>>(dst, P->perm, E, L.dst_sorted);
     NNC_CHECK_LAUNCH();
   }
-  k_inv_deg<<<(unsigned)ceil_div64(N, TB), TB, 0, st>>>(T.indeg, N, L.inv_deg);
+  k_inv_deg<<<(unsigned)ceil_div64(N_dst, TB), TB, 0, st>>>(T.indeg, N_dst, L.inv_deg);
   NNC_CHECK_LAUNCH();
   int h_counts[4] = {0, 0, 0, 0};
   NNC_CHECK_CUDA(cudaMemcpyAsync(h_counts, T.counts, 4 * sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -274,6 +286,19 @@ int plan_build(Plan* P, const int64_t* row0, const int64_t* row1, int64_t E, int
   P->n_tiles = h_counts[1];
   P->max_out_deg = h_counts[2];
   P->n_units = h_counts[3];
+  return NNCONV_OK;
+}
+
+int check_bipartite_root(const Plan* P, const float* root, unsigned node_flags) {
+  NNC_REQUIRE(P->N_src == P->N_dst || (root == nullptr && (node_flags & NNCONV_APPLY_RESIDUAL) == 0), NNCONV_ERR_ARG,
+              "bipartite plan (n_src %lld, n_dst %lld): pass root = NULL and add x_dst root + bias with "
+              "nnconv_root_term; NNCONV_APPLY_RESIDUAL needs a square plan", (long long)P->N_src, (long long)P->N_dst);
+  return NNCONV_OK;
+}
+
+int check_square(const Plan* P, const char* what) {
+  NNC_REQUIRE(P->N_src == P->N_dst, NNCONV_ERR_UNSUPPORTED, "%s needs a square plan (got n_src %lld, n_dst %lld)", what,
+              (long long)P->N_src, (long long)P->N_dst);
   return NNCONV_OK;
 }
 

@@ -16,7 +16,10 @@ inline bool prec_is_bf16(int prec) { return prec == PREC_BF16; }
 inline bool prec_is_split(int prec) { return prec == PREC_F16X2; }
 
 struct Plan {
-  int64_t E, N;
+  int64_t E;
+  // node counts of the two roles: sources (x rows gathered by the messages) and targets (rows of out).  A square plan
+  // has N_src == N_dst; a bipartite one (DESIGN 4.10) maps x_src [N_src, in] to out [N_dst, out]
+  int64_t N_src, N_dst;
   int flow;
   int n_src;        // S: sources with at least one out-edge (compact index c in [0,S))
   int n_tiles;      // T: tiles of <= 128 edges, never spanning two sources
@@ -34,15 +37,20 @@ struct Plan {
   const int* unit_t;      // [U] first tile of the unit
   const int* unit_u;      // [U] tiles in the unit (1 or 2)
   int n_units;
-  const float* inv_deg;   // [N] 1/max(in_degree,1)
+  const float* inv_deg;   // [N_dst] 1/max(in_degree,1)
   const int* h_tile_ptr;  // HOST mirror of tile_ptr ([S+1]) owned by the C handle
   const int* h_group_ptr; // HOST mirror of group_ptr ([S+1]) owned by the C handle
   const int* h_unit_ptr;  // HOST copy of unit_ptr ([S+1]) owned by the C handle
 };
 
-void plan_sizes(int64_t E, int64_t N, size_t* ws_bytes, size_t* tmp_bytes);
-int plan_build(Plan* P, const int64_t* row0, const int64_t* row1, int64_t E, int64_t N, int flow, void* ws, size_t ws_bytes,
-               void* tmp, size_t tmp_bytes, cudaStream_t st);
+void plan_sizes(int64_t E, int64_t N_src, int64_t N_dst, size_t* ws_bytes, size_t* tmp_bytes);
+int plan_build(Plan* P, const int64_t* row0, const int64_t* row1, int64_t E, int64_t N_src, int64_t N_dst, int flow, void* ws,
+               size_t ws_bytes, void* tmp, size_t tmp_bytes, cudaStream_t st);
+// a bipartite plan (N_src != N_dst) takes root = NULL and no NNCONV_APPLY_RESIDUAL in the message entry points: the root
+// term reads x_dst, not x_src (root_term / backward_node_terms)
+int check_bipartite_root(const Plan* P, const float* root, unsigned node_flags);
+// the convs without a bipartite form (DiagNNConv, GaussianNNConv) refuse a plan with N_src != N_dst
+int check_square(const Plan* P, const char* what);
 
 // hidden activation of the edge MLP: kind = NNCONV_ACT_* (0 = ReLU), param = LeakyReLU slope / ELU alpha
 struct Act {
@@ -181,10 +189,18 @@ size_t backward_mlp_diag_ws_bytes(const Plan* P, const Weights* W, size_t want_b
 int backward_mlp_diag(const Plan* P, const Weights* W, const float* edge_attr, const float* dd, float* const* dWs,
                       float* const* dbs, void* ws, size_t ws_bytes, cudaStream_t st, float* grad_ea);
 
-// node-level gradients of an application whose message is channel by channel (in == out == C), backward.cu:
-// dbias = sum_n g_n (dbias nullable), droot = x^T g and dx = g root^T (root NULL: dx = 0)
-int backward_node_terms(const float* x, const float* root, const float* gout, int64_t N, int C, float* dx, float* droot,
-                        float* dbias, cudaStream_t st, int64_t* launches);
+// node-level gradients of the root term x root + bias over N rows (x [N, cin], g [N, cout]), backward.cu:
+// dbias = sum_n g_n (dbias nullable), droot = x^T g and dx = g root^T (root NULL: dx = 0, dx nullable then)
+int backward_node_terms(const float* x, const float* root, const float* gout, int64_t N, int cin, int cout, float* dx,
+                        float* droot, float* dbias, cudaStream_t st, int64_t* launches);
+// the same terms with the tensor-core backward's node-level kernels (k_colsum, k_xtv, k_g_rootT: parallel over the
+// rows) when their shared memory fits, else backward_node_terms (backward_tc.cu)
+int node_terms_rows(const float* x, const float* root, const float* gout, int64_t N, int cin, int cout, float* dx,
+                    float* droot, float* dbias, cudaStream_t st, int64_t* launches);
+// out[n, :] += bias + x[n, :] root over N rows (kernels_simt.cu): the root term of a bipartite application, added
+// after the messages (root or bias nullable)
+int root_term(const float* x, const float* root, const float* bias, int64_t N, int cin, int cout, float* out,
+              cudaStream_t st);
 
 // Gaussian-kernel conv (gauss.cu, DESIGN 4.9): d_ec = exp(-p_e0^2 / sigma_c^2) / sqrt(|p_e1 p_e2|) computed in registers
 //   out_n = aggr_{e: dst_e = n} x_src(e) * d_e + x_n root + bias          (C == in == out, 1 <= C <= kGaussMaxChannels)

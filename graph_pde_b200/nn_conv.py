@@ -131,15 +131,31 @@ def _require_cuda(t, name):
                            % (name, t.device))
 
 
+def _node_pair(n_nodes):
+    """(N_src, N_dst) of a node count: an int N is the square graph (N, N), a pair a bipartite one."""
+    if isinstance(n_nodes, (tuple, list)):
+        return int(n_nodes[0]), int(n_nodes[1])
+    return int(n_nodes), int(n_nodes)
+
+
+def _in_pair(in_channels):
+    """(in_src, in_dst) of ``in_channels``: an int means the same width on both sides."""
+    if isinstance(in_channels, (tuple, list)):
+        return int(in_channels[0]), int(in_channels[1])
+    return in_channels, in_channels
+
+
 class _Plan(object):
-    """Per-edge_index preprocessing owned by the C library (nnconv_plan_t) + the buffers it lives in."""
+    """Per-edge_index preprocessing owned by the C library (nnconv_plan_t) + the buffers it lives in.  ``n_nodes``: N
+    (square graph) or (N_src, N_dst) (bipartite: sources index x_src, targets the rows of out)."""
 
     def __init__(self, edge_index, n_nodes, flow):
         L = _lib.lib()
         _lib.check(L.nnconv_init())
         e = edge_index.size(1)
+        n_src, n_dst = _node_pair(n_nodes)
         ws_b, tmp_b = ctypes.c_size_t(), ctypes.c_size_t()
-        _lib.check(L.nnconv_plan_sizes(e, n_nodes, ctypes.byref(ws_b), ctypes.byref(tmp_b)))
+        _lib.check(L.nnconv_plan_sizes_bipartite(e, n_src, n_dst, ctypes.byref(ws_b), ctypes.byref(tmp_b)))
         dev = edge_index.device
         self.ws = torch.empty(ws_b.value, dtype=torch.uint8, device=dev)
         tmp = torch.empty(tmp_b.value, dtype=torch.uint8, device=dev)
@@ -151,14 +167,16 @@ class _Plan(object):
         self._rows = (row0, row1)
         self.edge_index = edge_index          # keeps the storage (and so the cache key) alive
         h = ctypes.c_void_p()
-        _lib.check(L.nnconv_plan_create(_ptr(row0), _ptr(row1), e, n_nodes, _lib.FLOW[flow], _ptr(self.ws),
-                                        ws_b.value, _ptr(tmp), tmp_b.value, _stream_ptr(dev), ctypes.byref(h)))
+        _lib.check(L.nnconv_plan_create_bipartite(_ptr(row0), _ptr(row1), e, n_src, n_dst, _lib.FLOW[flow],
+                                                  _ptr(self.ws), ws_b.value, _ptr(tmp), tmp_b.value, _stream_ptr(dev),
+                                                  ctypes.byref(h)))
         self.handle = h
         self.key = _plan_key(edge_index, n_nodes, flow)
         self.nbytes = self.ws.numel() + edge_index.numel() * edge_index.element_size()
         info = (ctypes.c_int64 * 8)()
         _lib.check(L.nnconv_plan_info(h, info, 8))
         self.E, self.N, self.n_src, self.n_tiles, self.max_out_deg, self.src_sorted = [int(v) for v in info[:6]]
+        self.N_dst = int(info[7])        # rows of out (= N, the source count, on a square plan)
         stats['plans_built'] += 1
         self._finalizer = weakref.finalize(self, L.nnconv_plan_destroy, h)
 
@@ -196,7 +214,7 @@ def _streamed_chunks(plan, prepared, e_res, n_apps, ws_bytes):
 
 def _plan_key(edge_index, n_nodes, flow):
     return (edge_index.data_ptr(), tuple(edge_index.shape), tuple(edge_index.stride()), edge_index._version,
-            edge_index.device.index, int(n_nodes), flow)
+            edge_index.device.index, _node_pair(n_nodes), flow)
 
 
 def get_plan(edge_index, n_nodes, flow='source_to_target'):
@@ -335,14 +353,17 @@ class _Prepared(object):
 class _NNConvFunction(torch.autograd.Function):
     """Differentiable wrapper, CUDA-core variant: forward = the configured precision path, backward =
     nnconv_backward_ex (fp32 CUDA-core kernels, csrc/backward.cu; any shape, activations recomputed).  Gradients flow
-    to x, edge_attr, the edge-MLP Linear weights/biases, root and bias; edge_index gets none."""
+    to x, edge_attr, the edge-MLP Linear weights/biases, root and bias; edge_index gets none.  A bipartite call
+    (``n_dst`` not None) takes x = x_src and the nullable x_dst, and its gradient also flows to x_dst."""
 
     @staticmethod
-    def forward(ctx, module, x, edge_index, edge_attr, *params):
+    def forward(ctx, module, x, edge_index, edge_attr, x_dst, n_dst, *params):
         ctx.module = module
         ctx.edge_index = edge_index
+        ctx.pair = None if n_dst is None else _Pair(_f32(x_dst), n_dst)
+        ctx.x_dst_dtype = x_dst.dtype if x_dst is not None else None
         ctx.save_for_backward(x, edge_attr)
-        out, ctx.argmax = module._forward_impl(x, edge_index, edge_attr, for_grad=True, with_argmax=True)
+        out, ctx.argmax = module._forward_impl(x, edge_index, edge_attr, for_grad=True, with_argmax=True, pair=ctx.pair)
         return out
 
     @staticmethod
@@ -350,11 +371,20 @@ class _NNConvFunction(torch.autograd.Function):
         module = ctx.module
         x, edge_attr = ctx.saved_tensors
         grads = module._backward_impl(x, ctx.edge_index, edge_attr, grad_out, want_ea=ctx.needs_input_grad[3],
-                                      argmax=ctx.argmax)
+                                      argmax=ctx.argmax, pair=ctx.pair)
         # order of *params in forward(): list(module.parameters())
         by_id = {id(p): g for p, g in grads['params']}
-        return (None, grads['x'] if ctx.needs_input_grad[1] else None, None, grads.get('edge_attr')) + tuple(
+        gxd = grads.get('x_dst')
+        gxd = gxd.to(ctx.x_dst_dtype) if gxd is not None and ctx.needs_input_grad[4] else None
+        return (None, grads['x'] if ctx.needs_input_grad[1] else None, None, grads.get('edge_attr'), gxd, None) + tuple(
             by_id.get(id(p)) for p in module.parameters())
+
+
+class _Pair(object):
+    """The target side of a bipartite call: x_dst (fp32, or None: no root term) and the target count N_dst."""
+
+    def __init__(self, x_dst, n_dst):
+        self.x_dst, self.n_dst = x_dst, n_dst
 
 
 class _TrainState(object):
@@ -399,15 +429,18 @@ class _EdgeFeaturesFn(torch.autograd.Function):
 
 
 class _ApplyFn(torch.autograd.Function):
-    """One NNConv application given the edge features (tensor-core forward and backward)."""
+    """One NNConv application given the edge features (tensor-core forward and backward).  A bipartite call (``n_dst``
+    not None) takes x = x_src and the nullable x_dst; a square one passes None for both."""
 
     @staticmethod
-    def forward(ctx, module, state, x, token, w_last, b_last, root, bias):
+    def forward(ctx, module, state, x, token, w_last, b_last, root, bias, x_dst, n_dst):
         ctx.module, ctx.state = module, state
         x32 = _f32(x)
         ctx.save_for_backward(x32)
         ctx.x_dtype = x.dtype
-        out, ctx.argmax = module._apply_impl(state.plan, state.prepared, state.ef, x32)
+        ctx.pair = None if n_dst is None else _Pair(_f32(x_dst), n_dst)
+        ctx.x_dst_dtype = x_dst.dtype if x_dst is not None else None
+        out, ctx.argmax = module._apply_impl(state.plan, state.prepared, state.ef, x32, pair=ctx.pair)
         return out
 
     @staticmethod
@@ -415,10 +448,11 @@ class _ApplyFn(torch.autograd.Function):
         (x32,) = ctx.saved_tensors
         module, state = ctx.module, ctx.state
         g32 = _f32(grad_out)
-        dx, dwl, dbl, droot, dbias = module._backward_apply_impl(state, x32, g32, ctx.argmax)
+        dx, dwl, dbl, droot, dbias, dxd = module._backward_apply_impl(state, x32, g32, ctx.argmax, ctx.pair)
         state.apps.append((g32, x32, ctx.argmax))
+        dxd = dxd.to(ctx.x_dst_dtype) if dxd is not None and ctx.needs_input_grad[8] else None
         return (None, None, dx.to(ctx.x_dtype) if ctx.needs_input_grad[2] else None, torch.zeros_like(state.token),
-                dwl, dbl, droot, dbias)
+                dwl, dbl, droot, dbias, dxd, None)
 
 
 class NNConv_old(torch.nn.Module):
@@ -445,6 +479,15 @@ class NNConv_old(torch.nn.Module):
     features raises.  When the budget comes from the free device memory, the resident prefix leaves room for the
     backward's workspace.
 
+    Bipartite input (PyG's form, DESIGN 4.10): ``in_channels`` may be a pair ``(in_src, in_dst)`` (an int means
+    ``(in, in)``); the edge network then maps to ``in_src * out_channels``, ``root`` is ``[in_dst, out_channels]``, and
+    ``reset_parameters`` draws root and bias from U(-1/sqrt(in_src), 1/sqrt(in_src)), the reference's rule applied to
+    the message side.  ``forward(x, edge_index, edge_attr, size=None)`` accepts ``x = (x_src [N_src, in_src], x_dst
+    [N_dst, in_dst] or None)``: ``out[i] = x_dst[i] root + bias + aggr_{e: dst_e = i} x_src[src_e] . nn(e)``, with
+    N_dst rows; edge_index row 0 indexes x_src, row 1 x_dst.  ``x_dst = None`` drops the root term and needs ``size =
+    (N_src, N_dst)``; a ``size`` that disagrees with the tensors raises ValueError, as do a pair under
+    flow='target_to_source' and a pair passed to ``residual_step``.
+
     Caches: the down-converted weights and the x-independent edge features are cached per (parameter versions,
     edge_attr version).  Optimizer steps, ``load_state_dict`` and ``train()/eval()`` invalidate them; writes that
     bypass autograd's version counter (``p.data.copy_()``, ``p.data.clamp_()``) do NOT -- call ``invalidate()``
@@ -463,12 +506,12 @@ class NNConv_old(torch.nn.Module):
             raise ValueError("aggr must be 'add', 'mean' or 'max'")
         if self.flow not in _lib.FLOW:
             raise ValueError('flow must be source_to_target or target_to_source')
-        self.in_channels = in_channels
+        self.in_channels = tuple(in_channels) if isinstance(in_channels, (tuple, list)) else in_channels
         self.out_channels = out_channels
         self.nn = nn
         self.aggr = aggr
         if root_weight:
-            self.root = Parameter(torch.Tensor(in_channels, out_channels))
+            self.root = Parameter(torch.Tensor(_in_pair(self.in_channels)[1], out_channels))
         else:
             self.register_parameter('root', None)
         if bias:
@@ -491,25 +534,69 @@ class NNConv_old(torch.nn.Module):
             elif hasattr(m, 'reset_parameters'):
                 m.reset_parameters()
         _reset(self.nn)
-        bound = 1.0 / math.sqrt(self.in_channels)
+        bound = 1.0 / math.sqrt(_in_pair(self.in_channels)[0])
         if self.root is not None:
             self.root.data.uniform_(-bound, bound)
         if self.bias is not None:
             self.bias.data.uniform_(-bound, bound)
 
     # -- reference: nn_conv.py:267-271 ------------------------------------------------------------------
-    def forward(self, x, edge_index, edge_attr):
-        x = x.unsqueeze(-1) if x.dim() == 1 else x
+    def forward(self, x, edge_index, edge_attr, size=None):
         pseudo = edge_attr.unsqueeze(-1) if edge_attr.dim() == 1 else edge_attr
+        if isinstance(x, (tuple, list)):
+            x, x_dst, n_dst = self._bipartite_inputs(x, size)
+        else:
+            x = x.unsqueeze(-1) if x.dim() == 1 else x
+            if size is not None and any(n is not None and int(n) != x.size(0) for n in size):
+                raise ValueError('size %s disagrees with x of %d rows (a Tensor x is one node set)'
+                                 % (tuple(size), x.size(0)))
+            x_dst = n_dst = None
+        nodes = x.size(0) if n_dst is None else (x.size(0), n_dst)
         needs_grad = torch.is_grad_enabled() and (
-            x.requires_grad or pseudo.requires_grad or any(p.requires_grad for p in self.parameters()))
+            x.requires_grad or pseudo.requires_grad or any(p.requires_grad for p in self.parameters()) or
+            (x_dst is not None and x_dst.requires_grad))
         if needs_grad:
-            state = self._train_state(x, edge_index, pseudo)
+            state = self._train_state(x, edge_index, pseudo, nodes)
             if state is not None:            # tensor-core backward (csrc/backward_tc.cu)
                 lin = _edge_network(self.nn)[0][-1]
-                return _ApplyFn.apply(self, state, x, state.token, lin.weight, lin.bias, self.root, self.bias)
-            return _NNConvFunction.apply(self, x, edge_index, pseudo, *list(self.parameters()))
-        return self._forward_impl(x, edge_index, pseudo)
+                return _ApplyFn.apply(self, state, x, state.token, lin.weight, lin.bias, self.root, self.bias, x_dst,
+                                      n_dst)
+            return _NNConvFunction.apply(self, x, edge_index, pseudo, x_dst, n_dst, *list(self.parameters()))
+        pair = None if n_dst is None else _Pair(_f32(x_dst), n_dst)
+        return self._forward_impl(x, edge_index, pseudo, pair=pair)
+
+    def _bipartite_inputs(self, x, size):
+        """(x_src, x_dst or None, N_dst) of a pair ``x``, checked on the host before any launch."""
+        if len(x) != 2:
+            raise ValueError('x must be a Tensor or a pair (x_src, x_dst), got a sequence of %d' % len(x))
+        if self.flow != 'source_to_target':
+            raise ValueError("a pair (x_src, x_dst) needs flow='source_to_target': under 'target_to_source' PyG takes "
+                             'both the messages and the root term from x[1], which is not a bipartite map')
+        x_src, x_dst = x
+        x_src = x_src.unsqueeze(-1) if x_src.dim() == 1 else x_src
+        if x_dst is not None:
+            x_dst = x_dst.unsqueeze(-1) if x_dst.dim() == 1 else x_dst
+        if size is not None:
+            if len(size) != 2:
+                raise ValueError('size must be (N_src, N_dst), got %s' % (tuple(size),))
+            if size[0] is not None and int(size[0]) != x_src.size(0):
+                raise ValueError('size[0] = %d disagrees with x_src of %d rows' % (int(size[0]), x_src.size(0)))
+            if size[1] is not None and x_dst is not None and int(size[1]) != x_dst.size(0):
+                raise ValueError('size[1] = %d disagrees with x_dst of %d rows' % (int(size[1]), x_dst.size(0)))
+        if x_dst is not None:
+            n_dst = x_dst.size(0)
+        elif size is not None and size[1] is not None:
+            n_dst = int(size[1])
+        else:
+            raise ValueError('x_dst = None needs size = (N_src, N_dst) to give the number of targets')
+        if n_dst < 1:
+            raise ValueError('a bipartite call needs at least one target, got N_dst = %d' % n_dst)
+        if x_dst is not None:
+            _require_cuda(x_dst, 'x_dst')
+            in_dst = _in_pair(self.in_channels)[1]
+            if x_dst.dim() != 2 or x_dst.size(1) != in_dst:
+                raise ValueError('x_dst has shape %s, expected [N_dst, %d]' % (tuple(x_dst.shape), in_dst))
+        return x_src, x_dst, n_dst
 
     def __repr__(self):
         return '{}({}, {})'.format(self.__class__.__name__, self.in_channels, self.out_channels)
@@ -539,7 +626,8 @@ class NNConv_old(torch.nn.Module):
                                        for l in linears)
         hit = self._prepared.get(slot)
         if hit is None or hit[0] != key:
-            hit = self._prepared[slot] = (key, _Prepared(linears, self.in_channels, self.out_channels, precision, act))
+            hit = self._prepared[slot] = (key, _Prepared(linears, _in_pair(self.in_channels)[0], self.out_channels,
+                                                         precision, act))
             if slot == 'forward':
                 self._h_cache.clear()
         return hit[1]
@@ -728,16 +816,18 @@ class NNConv_old(torch.nn.Module):
         _require_cuda(pseudo, 'edge_attr')
         if edge_index.dtype != torch.int64 or edge_index.dim() != 2 or edge_index.size(0) != 2:
             raise ValueError('edge_index must be an int64 tensor of shape [2, E]')
-        if x.size(1) != self.in_channels:
-            raise ValueError('x has %d channels, expected %d' % (x.size(1), self.in_channels))
+        in_src = _in_pair(self.in_channels)[0]
+        if x.size(1) != in_src:
+            raise ValueError('x has %d channels, expected %d' % (x.size(1), in_src))
         if pseudo.size(0) != edge_index.size(1):
             raise ValueError('edge_attr has %d rows for %d edges' % (pseudo.size(0), edge_index.size(1)))
 
-    def _prepare(self, x, edge_index, pseudo, keep_acts=False, for_grad=False):
-        """plan, prepared weights, fp32 edge_attr and the (cached) edge features for this call."""
+    def _prepare(self, x, edge_index, pseudo, keep_acts=False, for_grad=False, nodes=None):
+        """plan, prepared weights, fp32 edge_attr and the (cached) edge features for this call; nodes: N_src or
+        (N_src, N_dst), default x's rows."""
         precision = self.precision or default_precision()
         ea32 = _f32(pseudo)
-        plan = get_plan(edge_index, x.size(0), self.flow)
+        plan = get_plan(edge_index, x.size(0) if nodes is None else nodes, self.flow)
         prepared = self._get_prepared(precision)
         ef = self._features(plan, prepared, ea32, keep_acts and prepared.bwd_tc, for_grad)
         return plan, prepared, ea32, ef
@@ -748,7 +838,8 @@ class NNConv_old(torch.nn.Module):
             return False
         return _EDGE_KERNELS == 'on' or ((plan.E <= _EDGE_KERNELS_MAX_DEG * max(plan.n_src, 1) or
                                           plan.E <= _EDGE_KERNELS_MAX_EDGES) and
-                                         plan.E * self.in_channels * self.out_channels * 2 <= _EDGE_KERNELS_MAX_BYTES)
+                                         plan.E * _in_pair(self.in_channels)[0] * self.out_channels * 2 <=
+                                         _EDGE_KERNELS_MAX_BYTES)
 
     def _edge_kernels(self, plan, prepared, ef):
         """K_e = W_L h_e + b_L for every edge (formulation B) when the graph has few out-edges per source, else None.
@@ -777,13 +868,14 @@ class NNConv_old(torch.nn.Module):
         ef.kmat = kmat
         return kmat
 
-    def _apply_impl(self, plan, prepared, ef, x32, flags=0):
+    def _apply_impl(self, plan, prepared, ef, x32, flags=0, pair=None):
         """One application: on the per-edge kernel matrices (formulation B, nnconv_apply_edge_ex), else on the whole h
         (nnconv_apply_ex), else on the resident prefix with the other edges' h recomputed in chunks
         (nnconv_apply_streamed: no allocation inside the library and, besides the optional overflow check, no host
         sync -- capturable by capture.GraphedForward).  aggr='max' takes nnconv_apply_max for either residency.
         Returns (out, argmax): argmax [N, out] int32 holds the winning caller edge of every (node, channel) under
-        aggr='max' (-1: no in-edge), else None."""
+        aggr='max' (-1: no in-edge), else None.  A bipartite call (pair: the _Pair of x_dst) runs the message part on
+        x32 = x_src with no root or bias and then adds x_dst root + bias (nnconv_root_term); out has N_dst rows."""
         L = _lib.lib()
         dev = x32.device
         kmat = self._edge_kernels(plan, prepared, ef)
@@ -798,12 +890,12 @@ class NNConv_old(torch.nn.Module):
                 keys_b = max_b.value - ws_b.value
                 ws_b = max_b
             ws = torch.empty(ws_b.value, dtype=torch.uint8, device=dev)
-        out = torch.empty(x32.size(0), self.out_channels, dtype=torch.float32, device=dev)
-        root, bias = _f32(self.root), _f32(self.bias)
+        out = torch.empty(plan.N_dst, self.out_channels, dtype=torch.float32, device=dev)
+        root, bias = (_f32(self.root), _f32(self.bias)) if pair is None else (None, None)
         aggr = _lib.AGGR[self.aggr]
         argmax = None
         if self.aggr == 'max':
-            argmax = torch.empty(x32.size(0), self.out_channels, dtype=torch.int32, device=dev)
+            argmax = torch.empty(plan.N_dst, self.out_channels, dtype=torch.int32, device=dev)
             n_l = ctypes.c_int64(0)
             _lib.check(L.nnconv_apply_max(plan.handle, prepared.handle, _ptr(ef.ea32), _ptr(ef.h), ef.E_res, _ptr(x32),
                                           _ptr(root), _ptr(bias), flags, _ptr(out), _ptr(argmax), _ptr(ws), ws.numel(),
@@ -824,19 +916,51 @@ class NNConv_old(torch.nn.Module):
                                              aggr, flags, _ptr(out), _ptr(ws), ws.numel(), _stream_ptr(dev),
                                              ctypes.byref(n_l)))
             stats['launches'] += n_l.value
+        if pair is not None:
+            self._root_term(pair, out)
         stats['applies'] += 1
         if ef.n_chunks:
             stats['streamed_chunk_passes'] += ef.n_chunks
             self._check_overflow(prepared, ws[keys_b:], dev)    # its first word: fp16 overflows of the chunks
         return out, argmax
 
-    def _forward_impl(self, x, edge_index, pseudo, flags=0, for_grad=False, with_argmax=False):
+    def _root_term(self, pair, out):
+        """out += x_dst root + bias of a bipartite call (no root term without x_dst)."""
+        root = _f32(self.root) if pair.x_dst is not None else None
+        bias = _f32(self.bias)
+        if root is None and bias is None:
+            return
+        _lib.check(_lib.lib().nnconv_root_term(_ptr(pair.x_dst if root is not None else None), _ptr(root), _ptr(bias),
+                                               out.size(0), _in_pair(self.in_channels)[1], self.out_channels, _ptr(out),
+                                               _stream_ptr(out.device)))
+        stats['launches'] += 1
+
+    def _root_backward(self, pair, g32):
+        """(grad x_dst or None, grad root or None, grad bias or None) of a bipartite call's root term."""
+        dev = g32.device
+        root = _f32(self.root) if pair.x_dst is not None else None
+        dxd = torch.empty_like(pair.x_dst) if root is not None else None
+        droot = torch.empty_like(self.root, dtype=torch.float32) if root is not None else None
+        dbias = torch.empty_like(self.bias, dtype=torch.float32) if self.bias is not None else None
+        if root is not None or dbias is not None:
+            n_l = ctypes.c_int64(0)
+            _lib.check(_lib.lib().nnconv_root_term_backward(
+                _ptr(pair.x_dst if root is not None else None), _ptr(root), _ptr(g32), g32.size(0),
+                _in_pair(self.in_channels)[1], self.out_channels, _ptr(dxd), _ptr(droot), _ptr(dbias),
+                _stream_ptr(dev), ctypes.byref(n_l)))
+            stats['launches'] += n_l.value
+        if self.root is not None and droot is None:     # x_dst = None: root takes no part in the result
+            droot = torch.zeros_like(self.root, dtype=torch.float32)
+        return dxd, droot, dbias
+
+    def _forward_impl(self, x, edge_index, pseudo, flags=0, for_grad=False, with_argmax=False, pair=None):
         """One application on the cached edge features; with_argmax: returns (out, argmax) (see _apply_impl)."""
         self._check_inputs(x, edge_index, pseudo)
         with torch.cuda.device(x.device):
             x32 = _f32(x)
-            plan, prepared, _, ef = self._prepare(x32, edge_index, pseudo, for_grad=for_grad)
-            out, argmax = self._apply_impl(plan, prepared, ef, x32, flags)
+            nodes = None if pair is None else (x32.size(0), pair.n_dst)
+            plan, prepared, _, ef = self._prepare(x32, edge_index, pseudo, for_grad=for_grad, nodes=nodes)
+            out, argmax = self._apply_impl(plan, prepared, ef, x32, flags, pair)
             return (out, argmax) if with_argmax else out
 
     def residual_step(self, z, edge_index, edge_attr, relu_in=True):
@@ -845,7 +969,9 @@ class NNConv_old(torch.nn.Module):
         ``z' = x + conv(x)``; the caller chains ``z'`` into the next step and applies the last ReLU itself.  The ReLU
         and the residual live in the node-prep launch of the application (``nnconv_apply_ex``), so a chain of steps
         has no elementwise kernels between its applications."""
-        if self.in_channels != self.out_channels:
+        if isinstance(z, (tuple, list)):
+            raise ValueError('residual_step needs one node set: x + conv(x) has no meaning for a pair (x_src, x_dst)')
+        if _in_pair(self.in_channels) != (self.out_channels, self.out_channels):
             raise ValueError('residual_step needs in_channels == out_channels')
         if torch.is_grad_enabled() and (z.requires_grad or edge_attr.requires_grad or
                                         any(p.requires_grad for p in self.parameters())):
@@ -855,7 +981,7 @@ class NNConv_old(torch.nn.Module):
         return self._forward_impl(z, edge_index, pseudo, flags)
 
     # -- tensor-core training path ----------------------------------------------------------------------
-    def _train_state(self, x, edge_index, pseudo):
+    def _train_state(self, x, edge_index, pseudo, nodes=None):
         """State shared by the applications of this conv on (edge_attr, parameters), or None when the tensor-core
         backward does not cover the configuration (the fp32 CUDA-core backward is used then)."""
         mode = _BWD_MODE
@@ -863,7 +989,7 @@ class NNConv_old(torch.nn.Module):
             return None
         self._check_inputs(x, edge_index, pseudo)
         with torch.cuda.device(x.device):
-            plan, prepared, ea32, ef = self._prepare(x, edge_index, pseudo, keep_acts=True, for_grad=True)
+            plan, prepared, ea32, ef = self._prepare(x, edge_index, pseudo, keep_acts=True, for_grad=True, nodes=nodes)
             if not prepared.bwd_tc:
                 if mode == 'tc':
                     raise NotImplementedError('NNCONV_B200_BACKWARD=tc: shape / precision not covered by the tensor-core backward')
@@ -881,10 +1007,12 @@ class NNConv_old(torch.nn.Module):
                 self._tstate = st
             return st
 
-    def _backward_apply_impl(self, state, x32, g32, argmax=None):
+    def _backward_apply_impl(self, state, x32, g32, argmax=None, pair=None):
         """Tensor-core backward of one application over the resident rows [0, E_res) of h; the other edges' h is
         recomputed per source batch.  With E_res = E this is the call nnconv_backward_apply makes.  argmax: the
-        forward's, under aggr='max' (nnconv_backward_apply_max routes every gradient to its winning edge)."""
+        forward's, under aggr='max' (nnconv_backward_apply_max routes every gradient to its winning edge).  Returns
+        (dx, dW_L, db_L, droot, dbias, dx_dst); a bipartite call (pair) takes droot, dbias and dx_dst from the root
+        term's backward, else dx_dst is None."""
         L = _lib.lib()
         dev = x32.device
         plan, prep, ef = state.plan, state.prepared, state.ef
@@ -893,9 +1021,10 @@ class NNConv_old(torch.nn.Module):
             dx = torch.empty_like(x32)
             dwl = torch.empty_like(lin.weight, dtype=torch.float32)
             dbl = torch.empty_like(lin.bias, dtype=torch.float32)
-            droot = torch.empty_like(self.root, dtype=torch.float32) if self.root is not None else None
-            dbias = torch.empty_like(self.bias, dtype=torch.float32) if self.bias is not None else None
-            root = _f32(self.root)
+            square = pair is None
+            droot = torch.empty_like(self.root, dtype=torch.float32) if self.root is not None and square else None
+            dbias = torch.empty_like(self.bias, dtype=torch.float32) if self.bias is not None and square else None
+            root = _f32(self.root) if square else None
             ws = ef.bwd_ws
             if ws is None:
                 b = ctypes.c_size_t()
@@ -917,8 +1046,11 @@ class NNConv_old(torch.nn.Module):
             stats['launches'] += n_l.value
             if ef.streamed:
                 stats['streamed_backward_chunk_passes'] += _streamed_chunks(plan, prep, ef.E_res, 0, ws.numel())
+            dxd = None
+            if not square:
+                dxd, droot, dbias = self._root_backward(pair, g32)
             stats['backwards'] += 1
-        return dx, dwl, dbl, droot, dbias
+        return dx, dwl, dbl, droot, dbias, dxd
 
     def _backward_mlp_impl(self, state, want_ea=False):
         """Gradients of the hidden Linear layers, one pass for all applications recorded in the state (in groups
@@ -974,17 +1106,19 @@ class NNConv_old(torch.nn.Module):
                 gea_total = torch.zeros(ef.ea32.shape, dtype=torch.float32, device=dev)
         return total, gea_total
 
-    def _backward_impl(self, x, edge_index, pseudo, grad_out, want_ea=False, argmax=None):
+    def _backward_impl(self, x, edge_index, pseudo, grad_out, want_ea=False, argmax=None, pair=None):
         """fp32 CUDA-core backward of one application; with ``want_ea`` also the gradient w.r.t. edge_attr
         (returned under 'edge_attr' in pseudo's dtype).  argmax: the forward's, under aggr='max' (whatever precision
-        that forward ran at, the gradients follow its winning edges)."""
+        that forward ran at, the gradients follow its winning edges).  A bipartite call (pair) also returns the
+        fp32 gradient w.r.t. x_dst under 'x_dst' (None without x_dst)."""
         L = _lib.lib()
+        square = pair is None
         with torch.cuda.device(x.device):
             x32 = _f32(x)
             ea32 = _f32(pseudo)
             g32 = _f32(grad_out)
             n = x32.size(0)
-            plan = get_plan(edge_index, n, self.flow)
+            plan = get_plan(edge_index, n if square else (n, pair.n_dst), self.flow)
             linears = _edge_network(self.nn)[0]
             prep = self._get_prepared('fp32', 'backward')
             ws_b = ctypes.c_size_t()
@@ -993,12 +1127,12 @@ class NNConv_old(torch.nn.Module):
             dx = torch.empty_like(x32)
             dws = [torch.empty_like(l.weight, dtype=torch.float32) for l in linears]
             dbs = [torch.empty_like(l.bias, dtype=torch.float32) for l in linears]
-            droot = torch.empty_like(self.root, dtype=torch.float32) if self.root is not None else None
-            dbias = torch.empty_like(self.bias, dtype=torch.float32) if self.bias is not None else None
+            droot = torch.empty_like(self.root, dtype=torch.float32) if self.root is not None and square else None
+            dbias = torch.empty_like(self.bias, dtype=torch.float32) if self.bias is not None and square else None
             nl = len(linears)
             wp = (ctypes.c_void_p * nl)(*[t.data_ptr() for t in dws])
             bp = (ctypes.c_void_p * nl)(*[t.data_ptr() for t in dbs])
-            root = _f32(self.root)
+            root = _f32(self.root) if square else None
             gea = torch.empty_like(ea32) if want_ea else None
             if self.aggr == 'max':
                 _lib.check(L.nnconv_backward_max(plan.handle, prep.handle, _ptr(ea32), _ptr(x32), _ptr(root), _ptr(argmax),
@@ -1008,13 +1142,16 @@ class NNConv_old(torch.nn.Module):
                 _lib.check(L.nnconv_backward_ex(plan.handle, prep.handle, _ptr(ea32), _ptr(x32), _ptr(root),
                                                 _lib.AGGR[self.aggr], _ptr(g32), _ptr(dx), wp, bp, _ptr(droot),
                                                 _ptr(dbias), _ptr(ws), ws_b.value, _stream_ptr(x.device), _ptr(gea)))
+            dxd = None
+            if not square:
+                dxd, droot, dbias = self._root_backward(pair, g32)
             stats['backwards'] += 1
         params = [(l.weight, dw) for l, dw in zip(linears, dws)] + [(l.bias, db) for l, db in zip(linears, dbs)]
         if self.root is not None:
             params.append((self.root, droot))
         if self.bias is not None:
             params.append((self.bias, dbias))
-        grads = {'x': dx.to(x.dtype), 'params': params}
+        grads = {'x': dx.to(x.dtype), 'params': params, 'x_dst': dxd}
         if gea is not None:
             grads['edge_attr'] = gea.to(pseudo.dtype)
         return grads

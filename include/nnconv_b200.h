@@ -92,8 +92,31 @@ int nnconv_plan_sizes(int64_t E, int64_t N, size_t* ws_bytes, size_t* tmp_bytes)
 int nnconv_plan_create(const int64_t* row0, const int64_t* row1, int64_t E, int64_t N, int flow, void* ws, size_t ws_bytes,
                        void* tmp, size_t tmp_bytes, void* stream, nnconv_plan_t** out);
 void nnconv_plan_destroy(nnconv_plan_t* plan);
-/* info[0..6] = E, N, #sources with out-edges, #tiles, max out-degree, already-grouped flag, flow */
+/* info[0..6] = E, N (the source count n_src), #sources with out-edges, #tiles, max out-degree, already-grouped flag,
+ * flow; with n_info >= 8 also info[7] = n_dst, the target count (= N on a square plan) */
 int nnconv_plan_info(const nnconv_plan_t* plan, int64_t* info, int n_info);
+/* bipartite plan (DESIGN 4.10): messages from n_src source nodes into n_dst target nodes, PyG's (x_src, x_dst) input.
+ * The source row of edge_index (row 0 for flow 0, row 1 for flow 1) indexes [0, n_src), the target row [0, n_dst); an
+ * entry outside its range fails the create with a message naming the row.  nnconv_plan_create is the case
+ * n_src == n_dst == N.  On a plan with n_src != n_dst the apply and backward entry points of NNConv (nnconv_apply*,
+ * nnconv_backward*) take x = x_src [n_src, in] and compute only the message part into out / grad_out [n_dst, out]: they
+ * need root = NULL and no NNCONV_APPLY_RESIDUAL, and the root term comes from nnconv_root_term below (bias may go to
+ * either; nnconv_root_term adds it after the messages).  The diagonal and Gaussian convs refuse such a plan. */
+int nnconv_plan_sizes_bipartite(int64_t E, int64_t n_src, int64_t n_dst, size_t* ws_bytes, size_t* tmp_bytes);
+int nnconv_plan_create_bipartite(const int64_t* row0, const int64_t* row1, int64_t E, int64_t n_src, int64_t n_dst,
+                                 int flow, void* ws, size_t ws_bytes, void* tmp, size_t tmp_bytes, void* stream,
+                                 nnconv_plan_t** out);
+/* root term of a bipartite application, fp32 on the CUDA cores, over n rows (x [n, in_channels], root
+ * [in_channels, out_channels], bias [out_channels], both nullable):
+ *   nnconv_root_term:          out[i] += x[i] root + bias         (ADDED into the message part)
+ *   nnconv_root_term_backward: grad_x = grad_out root^T, grad_root = x^T grad_out, grad_bias = sum_i grad_out[i]
+ *                              (WRITTEN; grad_x and grad_root with root only, grad_bias with bias only: NULL otherwise)
+ * No allocation; no host synchronisation. */
+int nnconv_root_term(const float* x, const float* root, const float* bias, int64_t n, int in_channels, int out_channels,
+                     float* out, void* stream);
+int nnconv_root_term_backward(const float* x, const float* root, const float* grad_out, int64_t n, int in_channels,
+                              int out_channels, float* grad_x, float* grad_root, float* grad_bias, void* stream,
+                              int64_t* launches);
 
 /* ---- weights: snapshot of the edge MLP ("nn" argument of NNConv_old.__init__, nn_conv.py:234-246) -- */
 /* dims[0..n_layers] = k_in, k_1, ..., in_channels*out_channels;  W[l]: [dims[l+1], dims[l]] fp32
