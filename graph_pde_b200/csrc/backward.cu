@@ -605,8 +605,6 @@ int backward_node_terms(const float* x, const float* root, const float* gout, in
     s = gemm_any(gout, cout, 1, root, 1, cout, dx, cin, static_cast<int>(N), cin, cout, 0.f, st);       // dx = g root^T
     if (s) return s;
     *launches += 2;
-  } else if (dx != nullptr) {
-    NNC_CHECK_CUDA(cudaMemsetAsync(dx, 0, sizeof(float) * N * cin, st));
   }
   return NNCONV_OK;
 }
@@ -619,9 +617,10 @@ int backward_apply_diag(const Plan* P, const Weights* W, const float* d, const f
               "backward_apply_diag: aggr %d (max needs the forward's argmax)", aggr);
   const int C = W->cout;
   int64_t n_l = 0;
-  if (int sq = check_square(P, "backward_apply_diag")) return sq;
-  const int s = backward_node_terms(x, root, gout, P->N_dst, C, C, dx, droot, dbias, st, &n_l);
+  if (int sb = check_bipartite_root(P, root, 0)) return sb;
+  const int s = backward_node_terms(x, root, gout, P->N_dst, C, C, root ? dx : nullptr, droot, dbias, st, &n_l);
   if (s) return s;
+  if (root == nullptr) NNC_CHECK_CUDA(cudaMemsetAsync(dx, 0, sizeof(float) * P->N_src * C, st));   // dx: the sources
   if (P->E > 0 && P->n_tiles > 0) {
     const unsigned grid = static_cast<unsigned>(ceil_div64(static_cast<int64_t>(P->n_tiles) * 32, 256));
 #define NNC_DIAG_BWD(A)                                                                                               \

@@ -177,7 +177,7 @@ int apply_diag(const Plan* P, const Weights* W, const float* d, const float* x, 
                int aggr, float* out, int* argmax, void* ws, size_t ws_bytes, cudaStream_t st, int64_t* launches) {
   NNC_REQUIRE(W->diag, NNCONV_ERR_ARG, "apply_diag: weights not prepared as a diagonal kernel");
   NNC_REQUIRE(aggr >= 0 && aggr <= 2, NNCONV_ERR_ARG, "apply_diag: unknown aggr %d", aggr);
-  if (int sq = check_square(P, "apply_diag")) return sq;
+  if (int sb = check_bipartite_root(P, root, 0)) return sb;
   const int cout = W->cout;
   unsigned long long* keys = nullptr;
   if (aggr == 2) {

@@ -245,7 +245,7 @@ int apply_gauss(const Plan* P, const float* edge_attr, int k_in, const float* si
                 const float* root, const float* bias, int aggr, float* out, int* argmax, void* ws, size_t ws_bytes,
                 cudaStream_t st, int64_t* launches) {
   NNC_REQUIRE(aggr >= 0 && aggr <= 2, NNCONV_ERR_ARG, "apply_gauss: unknown aggr %d", aggr);
-  if (int sq = check_square(P, "apply_gauss")) return sq;
+  if (int sb = check_bipartite_root(P, root, 0)) return sb;
   NNC_REQUIRE(C >= 1 && C <= kGaussMaxChannels, NNCONV_ERR_UNSUPPORTED, "apply_gauss: channels %d not in [1, %d]", C,
               kGaussMaxChannels);
   NNC_REQUIRE(k_in >= 3, NNCONV_ERR_ARG, "apply_gauss: edge_attr needs at least 3 columns, got %d", k_in);
@@ -294,13 +294,14 @@ int backward_gauss(const Plan* P, const float* edge_attr, int k_in, const float*
                    float* dbias, float* dsigma, float* dea, cudaStream_t st, int64_t* launches) {
   NNC_REQUIRE(aggr >= 0 && aggr <= 2 && (aggr != 2 || argmax != nullptr), NNCONV_ERR_ARG,
               "backward_gauss: aggr %d (max needs the forward's argmax)", aggr);
-  if (int sq = check_square(P, "backward_gauss")) return sq;
+  if (int sb = check_bipartite_root(P, root, 0)) return sb;
   NNC_REQUIRE(C >= 1 && C <= kGaussMaxChannels, NNCONV_ERR_UNSUPPORTED, "backward_gauss: channels %d not in [1, %d]", C,
               kGaussMaxChannels);
   NNC_REQUIRE(k_in >= 3, NNCONV_ERR_ARG, "backward_gauss: edge_attr needs at least 3 columns, got %d", k_in);
   int64_t n_l = 0;
-  int s = backward_node_terms(x, root, gout, P->N_dst, C, C, dx, droot, dbias, st, &n_l);
+  int s = backward_node_terms(x, root, gout, P->N_dst, C, C, root ? dx : nullptr, droot, dbias, st, &n_l);
   if (s) return s;
+  if (root == nullptr) NNC_CHECK_CUDA(cudaMemsetAsync(dx, 0, sizeof(float) * P->N_src * C, st));   // dx: the sources
   if (dsigma) NNC_CHECK_CUDA(cudaMemsetAsync(dsigma, 0, sizeof(float) * C, st));
   if (P->E > 0 && P->n_tiles > 0) {
     const unsigned grid = static_cast<unsigned>(ceil_div64(static_cast<int64_t>(P->n_tiles) * 32, 256));

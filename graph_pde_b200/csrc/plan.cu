@@ -296,10 +296,4 @@ int check_bipartite_root(const Plan* P, const float* root, unsigned node_flags) 
   return NNCONV_OK;
 }
 
-int check_square(const Plan* P, const char* what) {
-  NNC_REQUIRE(P->N_src == P->N_dst, NNCONV_ERR_UNSUPPORTED, "%s needs a square plan (got n_src %lld, n_dst %lld)", what,
-              (long long)P->N_src, (long long)P->N_dst);
-  return NNCONV_OK;
-}
-
 }  // namespace nnc

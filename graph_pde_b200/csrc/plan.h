@@ -46,11 +46,9 @@ struct Plan {
 void plan_sizes(int64_t E, int64_t N_src, int64_t N_dst, size_t* ws_bytes, size_t* tmp_bytes);
 int plan_build(Plan* P, const int64_t* row0, const int64_t* row1, int64_t E, int64_t N_src, int64_t N_dst, int flow, void* ws,
                size_t ws_bytes, void* tmp, size_t tmp_bytes, cudaStream_t st);
-// a bipartite plan (N_src != N_dst) takes root = NULL and no NNCONV_APPLY_RESIDUAL in the message entry points: the root
-// term reads x_dst, not x_src (root_term / backward_node_terms)
+// a bipartite plan (N_src != N_dst) takes root = NULL and no NNCONV_APPLY_RESIDUAL in the message entry points of every
+// conv (NNConv, diagonal, Gaussian): the root term reads x_dst, not x_src (root_term / node_terms_rows)
 int check_bipartite_root(const Plan* P, const float* root, unsigned node_flags);
-// the convs without a bipartite form (DiagNNConv, GaussianNNConv) refuse a plan with N_src != N_dst
-int check_square(const Plan* P, const char* what);
 
 // hidden activation of the edge MLP: kind = NNCONV_ACT_* (0 = ReLU), param = LeakyReLU slope / ELU alpha
 struct Act {
@@ -175,7 +173,8 @@ int apply_edge(const Plan* P, const Weights* W, const void* Kmat, const float* x
 // diag_build computes d chunk by chunk from edge_attr (only d is kept); ws: diag_ws_bytes, its header holds the fp16
 // range counter of the chunks' hidden activations (nnconv_edge_features_overflow).  apply_diag: aggr 0 add, 1 mean,
 // 2 max (ws: max_keys_bytes of keys, argmax written).  backward_apply_diag: dx, droot, dbias of one application, and
-// dd_e += x_src(e) * G_e accumulated over the applications; backward_mlp_diag (weights prepared at fp32): every
+// dd_e += x_src(e) * G_e accumulated over the applications (bipartite plans: root NULL; out, argmax and gout have N_dst
+// rows, x and dx N_src, and dx is zeroed over them); backward_mlp_diag (weights prepared at fp32): every
 // Linear's gradient from dd, the activations recomputed in fp32 batch by batch.
 size_t diag_ws_bytes(const Plan* P, const Weights* W, size_t want_bytes);
 int diag_build(const Plan* P, const Weights* W, const float* edge_attr, float* d, void* ws, size_t ws_bytes, cudaStream_t st,
@@ -190,7 +189,7 @@ int backward_mlp_diag(const Plan* P, const Weights* W, const float* edge_attr, c
                       float* const* dbs, void* ws, size_t ws_bytes, cudaStream_t st, float* grad_ea);
 
 // node-level gradients of the root term x root + bias over N rows (x [N, cin], g [N, cout]), backward.cu:
-// dbias = sum_n g_n (dbias nullable), droot = x^T g and dx = g root^T (root NULL: dx = 0, dx nullable then)
+// dbias = sum_n g_n (dbias nullable), droot = x^T g and dx = g root^T (root NULL: dx untouched, dx nullable then)
 int backward_node_terms(const float* x, const float* root, const float* gout, int64_t N, int cin, int cout, float* dx,
                         float* droot, float* dbias, cudaStream_t st, int64_t* launches);
 // the same terms with the tensor-core backward's node-level kernels (k_colsum, k_xtv, k_g_rootT: parallel over the
@@ -206,7 +205,7 @@ int root_term(const float* x, const float* root, const float* bias, int64_t N, i
 //   out_n = aggr_{e: dst_e = n} x_src(e) * d_e + x_n root + bias          (C == in == out, 1 <= C <= kGaussMaxChannels)
 // edge_attr [E, k_in] (k_in >= 3) in the caller's order, sigma [C].  apply_gauss: aggr 0 add, 1 mean, 2 max (ws:
 // max_keys_bytes of keys, argmax written).  backward_gauss: dx, droot, dbias, and the nullable dsigma [C] and dea
-// [E, k_in] (written, columns 3 and up 0) of one application.
+// [E, k_in] (written, columns 3 and up 0) of one application.  Bipartite plans as for apply_diag / backward_apply_diag.
 constexpr int kGaussMaxChannels = 4096;
 size_t gauss_apply_ws_bytes(const Plan* P, int C, int aggr);
 int apply_gauss(const Plan* P, const float* edge_attr, int k_in, const float* sigma, int C, const float* x,

@@ -145,6 +145,47 @@ def _in_pair(in_channels):
     return in_channels, in_channels
 
 
+def _node_sets(x, size, flow, in_dst):
+    """(x, x_dst, N_dst) of a conv's ``x`` and ``size``, checked on the host before any launch.  A Tensor ``x`` is one
+    node set: x_dst and N_dst are None, and a ``size`` must agree with its rows.  A pair ``(x_src, x_dst or None)`` is
+    PyG's bipartite input (DESIGN 4.10): x = x_src, and x_dst must be [N_dst, in_dst]."""
+    if not isinstance(x, (tuple, list)):
+        x = x.unsqueeze(-1) if x.dim() == 1 else x
+        if size is not None and any(n is not None and int(n) != x.size(0) for n in size):
+            raise ValueError('size %s disagrees with x of %d rows (a Tensor x is one node set)'
+                             % (tuple(size), x.size(0)))
+        return x, None, None
+    if len(x) != 2:
+        raise ValueError('x must be a Tensor or a pair (x_src, x_dst), got a sequence of %d' % len(x))
+    if flow != 'source_to_target':
+        raise ValueError("a pair (x_src, x_dst) needs flow='source_to_target': under 'target_to_source' PyG takes "
+                         'both the messages and the root term from x[1], which is not a bipartite map')
+    x_src, x_dst = x
+    x_src = x_src.unsqueeze(-1) if x_src.dim() == 1 else x_src
+    if x_dst is not None:
+        x_dst = x_dst.unsqueeze(-1) if x_dst.dim() == 1 else x_dst
+    if size is not None:
+        if len(size) != 2:
+            raise ValueError('size must be (N_src, N_dst), got %s' % (tuple(size),))
+        if size[0] is not None and int(size[0]) != x_src.size(0):
+            raise ValueError('size[0] = %d disagrees with x_src of %d rows' % (int(size[0]), x_src.size(0)))
+        if size[1] is not None and x_dst is not None and int(size[1]) != x_dst.size(0):
+            raise ValueError('size[1] = %d disagrees with x_dst of %d rows' % (int(size[1]), x_dst.size(0)))
+    if x_dst is not None:
+        n_dst = x_dst.size(0)
+    elif size is not None and size[1] is not None:
+        n_dst = int(size[1])
+    else:
+        raise ValueError('x_dst = None needs size = (N_src, N_dst) to give the number of targets')
+    if n_dst < 1:
+        raise ValueError('a bipartite call needs at least one target, got N_dst = %d' % n_dst)
+    if x_dst is not None:
+        _require_cuda(x_dst, 'x_dst')
+        if x_dst.dim() != 2 or x_dst.size(1) != in_dst:
+            raise ValueError('x_dst has shape %s, expected [N_dst, %d]' % (tuple(x_dst.shape), in_dst))
+    return x_src, x_dst, n_dst
+
+
 class _Plan(object):
     """Per-edge_index preprocessing owned by the C library (nnconv_plan_t) + the buffers it lives in.  ``n_nodes``: N
     (square graph) or (N_src, N_dst) (bipartite: sources index x_src, targets the rows of out)."""
@@ -543,14 +584,7 @@ class NNConv_old(torch.nn.Module):
     # -- reference: nn_conv.py:267-271 ------------------------------------------------------------------
     def forward(self, x, edge_index, edge_attr, size=None):
         pseudo = edge_attr.unsqueeze(-1) if edge_attr.dim() == 1 else edge_attr
-        if isinstance(x, (tuple, list)):
-            x, x_dst, n_dst = self._bipartite_inputs(x, size)
-        else:
-            x = x.unsqueeze(-1) if x.dim() == 1 else x
-            if size is not None and any(n is not None and int(n) != x.size(0) for n in size):
-                raise ValueError('size %s disagrees with x of %d rows (a Tensor x is one node set)'
-                                 % (tuple(size), x.size(0)))
-            x_dst = n_dst = None
+        x, x_dst, n_dst = _node_sets(x, size, self.flow, _in_pair(self.in_channels)[1])
         nodes = x.size(0) if n_dst is None else (x.size(0), n_dst)
         needs_grad = torch.is_grad_enabled() and (
             x.requires_grad or pseudo.requires_grad or any(p.requires_grad for p in self.parameters()) or
@@ -564,39 +598,6 @@ class NNConv_old(torch.nn.Module):
             return _NNConvFunction.apply(self, x, edge_index, pseudo, x_dst, n_dst, *list(self.parameters()))
         pair = None if n_dst is None else _Pair(_f32(x_dst), n_dst)
         return self._forward_impl(x, edge_index, pseudo, pair=pair)
-
-    def _bipartite_inputs(self, x, size):
-        """(x_src, x_dst or None, N_dst) of a pair ``x``, checked on the host before any launch."""
-        if len(x) != 2:
-            raise ValueError('x must be a Tensor or a pair (x_src, x_dst), got a sequence of %d' % len(x))
-        if self.flow != 'source_to_target':
-            raise ValueError("a pair (x_src, x_dst) needs flow='source_to_target': under 'target_to_source' PyG takes "
-                             'both the messages and the root term from x[1], which is not a bipartite map')
-        x_src, x_dst = x
-        x_src = x_src.unsqueeze(-1) if x_src.dim() == 1 else x_src
-        if x_dst is not None:
-            x_dst = x_dst.unsqueeze(-1) if x_dst.dim() == 1 else x_dst
-        if size is not None:
-            if len(size) != 2:
-                raise ValueError('size must be (N_src, N_dst), got %s' % (tuple(size),))
-            if size[0] is not None and int(size[0]) != x_src.size(0):
-                raise ValueError('size[0] = %d disagrees with x_src of %d rows' % (int(size[0]), x_src.size(0)))
-            if size[1] is not None and x_dst is not None and int(size[1]) != x_dst.size(0):
-                raise ValueError('size[1] = %d disagrees with x_dst of %d rows' % (int(size[1]), x_dst.size(0)))
-        if x_dst is not None:
-            n_dst = x_dst.size(0)
-        elif size is not None and size[1] is not None:
-            n_dst = int(size[1])
-        else:
-            raise ValueError('x_dst = None needs size = (N_src, N_dst) to give the number of targets')
-        if n_dst < 1:
-            raise ValueError('a bipartite call needs at least one target, got N_dst = %d' % n_dst)
-        if x_dst is not None:
-            _require_cuda(x_dst, 'x_dst')
-            in_dst = _in_pair(self.in_channels)[1]
-            if x_dst.dim() != 2 or x_dst.size(1) != in_dst:
-                raise ValueError('x_dst has shape %s, expected [N_dst, %d]' % (tuple(x_dst.shape), in_dst))
-        return x_src, x_dst, n_dst
 
     def __repr__(self):
         return '{}({}, {})'.format(self.__class__.__name__, self.in_channels, self.out_channels)
@@ -1168,6 +1169,15 @@ class NNConv(NNConv_old):
 ECConv = NNConv
 
 
+def _require_int_channels(conv, in_channels, out_channels):
+    """The channel-wise convs (DiagNNConv, GaussianNNConv) have one width on both sides of a bipartite map: a pair
+    ``in_channels`` raises NotImplementedError, as a non-square shape does."""
+    if isinstance(in_channels, (tuple, list)):
+        raise NotImplementedError(
+            '%s: the channel-wise kernel needs one width C = in_channels = out_channels for x_src, x_dst and the output; '
+            'got in_channels %s, out_channels %d' % (type(conv).__name__, tuple(in_channels), out_channels))
+
+
 # ---------------------------------------------------------------------------------------------------------------------
 # diagonal-kernel conv (formulation D, DESIGN 4.7)
 # ---------------------------------------------------------------------------------------------------------------------
@@ -1245,24 +1255,28 @@ class _DiagMlpFn(torch.autograd.Function):
 
 
 class _DiagApplyFn(torch.autograd.Function):
-    """One DiagNNConv application given d."""
+    """One DiagNNConv application given d.  A bipartite call (``n_dst`` not None) takes x = x_src and the nullable
+    x_dst; a square one passes None for both."""
 
     @staticmethod
-    def forward(ctx, module, state, x, token, root, bias):
+    def forward(ctx, module, state, x, token, root, bias, x_dst, n_dst):
         ctx.module, ctx.state = module, state
         x32 = _f32(x)
         ctx.save_for_backward(x32)
         ctx.x_dtype = x.dtype
-        out, ctx.argmax = module._apply_impl(state.plan, state.feats, x32)
+        ctx.pair = None if n_dst is None else _Pair(_f32(x_dst), n_dst)
+        ctx.x_dst_dtype = x_dst.dtype if x_dst is not None else None
+        out, ctx.argmax = module._apply_impl(state.plan, state.feats, x32, ctx.pair)
         return out
 
     @staticmethod
     def backward(ctx, grad_out):
         (x32,) = ctx.saved_tensors
         state = ctx.state
-        dx, droot, dbias = ctx.module._backward_apply_impl(state, x32, _f32(grad_out), ctx.argmax)
+        dx, droot, dbias, dxd = ctx.module._backward_apply_impl(state, x32, _f32(grad_out), ctx.argmax, ctx.pair)
+        dxd = dxd.to(ctx.x_dst_dtype) if dxd is not None and ctx.needs_input_grad[6] else None
         return (None, None, dx.to(ctx.x_dtype) if ctx.needs_input_grad[2] else None,
-                torch.zeros_like(state.token) if state.token is not None else None, droot, dbias)
+                torch.zeros_like(state.token) if state.token is not None else None, droot, dbias, dxd, None)
 
 
 class DiagNNConv(torch.nn.Module):
@@ -1282,6 +1296,12 @@ class DiagNNConv(torch.nn.Module):
     Each application is one pass over d.  The backward computes every gradient on the CUDA cores in fp32, recomputing
     the edge network's activations from edge_attr once per backward pass for all applications of a shared conv.  Cache
     rules are NNConv_old's: ``invalidate()`` after parameter writes that bypass autograd's version counter.
+
+    Bipartite input (PyG's form, DESIGN 4.10): ``forward(x, edge_index, edge_attr, size=None)`` also accepts ``x =
+    (x_src [N_src, C], x_dst [N_dst, C] or None)`` and returns ``out[i] = x_dst[i] root + bias + aggr_{e: dst_e = i}
+    x_src[src_e] * nn(e)`` over N_dst rows, with NNConv_old's rules for ``size``, ``x_dst = None``, the aggregations and
+    the refusals.  ``in_channels`` stays an int: the diagonal kernel has one width C on both sides, and a pair raises
+    NotImplementedError.
     """
 
     def __init__(self, in_channels, out_channels, nn, aggr='add', root_weight=True, bias=True, **kwargs):
@@ -1294,6 +1314,7 @@ class DiagNNConv(torch.nn.Module):
             raise ValueError("aggr must be 'add', 'mean' or 'max'")
         if self.flow not in _lib.FLOW:
             raise ValueError('flow must be source_to_target or target_to_source')
+        _require_int_channels(self, in_channels, out_channels)
         self.in_channels = in_channels
         self.out_channels = out_channels
         self.nn = nn
@@ -1313,6 +1334,8 @@ class DiagNNConv(torch.nn.Module):
 
     reset_parameters = NNConv_old.reset_parameters
     __repr__ = NNConv_old.__repr__
+    _root_term = NNConv_old._root_term
+    _root_backward = NNConv_old._root_backward
 
     def invalidate(self):
         """Drop the prepared-weight snapshots and the cached d."""
@@ -1337,19 +1360,21 @@ class DiagNNConv(torch.nn.Module):
         return lin
 
     # -- reference: nn_conv.py:79-84 -----------------------------------------------------------------------------
-    def forward(self, x, edge_index, edge_attr):
-        x = x.unsqueeze(-1) if x.dim() == 1 else x
+    def forward(self, x, edge_index, edge_attr, size=None):
+        x, x_dst, n_dst = _node_sets(x, size, self.flow, self.in_channels)
         pseudo = edge_attr.unsqueeze(-1) if edge_attr.dim() == 1 else edge_attr
         lin = self._check_shape()
         NNConv_old._check_inputs(self, x, edge_index, pseudo)
         needs_grad = torch.is_grad_enabled() and (
-            x.requires_grad or pseudo.requires_grad or any(p.requires_grad for p in self.parameters()))
+            x.requires_grad or pseudo.requires_grad or any(p.requires_grad for p in self.parameters()) or
+            (x_dst is not None and x_dst.requires_grad))
         with torch.cuda.device(x.device):
-            plan = get_plan(edge_index, x.size(0), self.flow)
+            plan = get_plan(edge_index, x.size(0) if n_dst is None else (x.size(0), n_dst), self.flow)
             ea32 = _f32(pseudo)
             feats = self._features(plan, ea32)
             if not needs_grad:
-                return self._apply_impl(plan, feats, _f32(x))[0]
+                pair = None if n_dst is None else _Pair(_f32(x_dst), n_dst)
+                return self._apply_impl(plan, feats, _f32(x), pair)[0]
             params = [t for l in lin for t in (l.weight, l.bias)]
             for_mlp = pseudo.requires_grad or any(p.requires_grad for p in params)
             key = (plan.key, ea32.data_ptr(), tuple(ea32.shape), ea32._version, id(feats), pseudo.requires_grad, for_mlp)
@@ -1359,7 +1384,7 @@ class DiagNNConv(torch.nn.Module):
                 if for_mlp:
                     st.token = _DiagMlpFn.apply(self, st, pseudo, *params)
                 self._tstate = st
-            return _DiagApplyFn.apply(self, st, x, st.token, self.root, self.bias)
+            return _DiagApplyFn.apply(self, st, x, st.token, self.root, self.bias, x_dst, n_dst)
 
     # -- host-side sequencing ------------------------------------------------------------------------------------
     def _get_prepared(self, precision, slot='forward'):
@@ -1398,40 +1423,51 @@ class DiagNNConv(torch.nn.Module):
         self._d_cache[key] = feats
         return feats
 
-    def _apply_impl(self, plan, feats, x32):
-        """One application (nnconv_apply_diag); returns (out, argmax), argmax None unless aggr='max'."""
+    def _apply_impl(self, plan, feats, x32, pair=None):
+        """One application (nnconv_apply_diag); returns (out, argmax), argmax None unless aggr='max'.  A bipartite call
+        (pair: the _Pair of x_dst) runs the messages from x32 = x_src with no root or bias, then adds x_dst root + bias
+        (nnconv_root_term); out has N_dst rows."""
         L = _lib.lib()
         dev = x32.device
         aggr = _lib.AGGR[self.aggr]
         ws_b = ctypes.c_size_t()
         _lib.check(L.nnconv_apply_diag_sizes(plan.handle, feats.prepared.handle, aggr, ctypes.byref(ws_b)))
         ws = torch.empty(ws_b.value, dtype=torch.uint8, device=dev)
-        out = torch.empty(x32.size(0), self.out_channels, dtype=torch.float32, device=dev)
-        argmax = torch.empty(x32.size(0), self.out_channels, dtype=torch.int32, device=dev) if self.aggr == 'max' else None
+        out = torch.empty(plan.N_dst, self.out_channels, dtype=torch.float32, device=dev)
+        argmax = torch.empty(plan.N_dst, self.out_channels, dtype=torch.int32, device=dev) if self.aggr == 'max' else None
+        root, bias = (_f32(self.root), _f32(self.bias)) if pair is None else (None, None)
         n_l = ctypes.c_int64(0)
-        _lib.check(L.nnconv_apply_diag(plan.handle, feats.prepared.handle, _ptr(feats.d), _ptr(x32), _ptr(_f32(self.root)),
-                                       _ptr(_f32(self.bias)), aggr, _ptr(out), _ptr(argmax), _ptr(ws), ws_b.value,
+        _lib.check(L.nnconv_apply_diag(plan.handle, feats.prepared.handle, _ptr(feats.d), _ptr(x32), _ptr(root),
+                                       _ptr(bias), aggr, _ptr(out), _ptr(argmax), _ptr(ws), ws_b.value,
                                        _stream_ptr(dev), ctypes.byref(n_l)))
         stats['launches'] += n_l.value
+        if pair is not None:
+            self._root_term(pair, out)
         stats['applies'] += 1
         return out, argmax
 
-    def _backward_apply_impl(self, state, x32, g32, argmax):
-        """dx, droot, dbias of one application; adds its share into state.dd (when the edge network needs it)."""
+    def _backward_apply_impl(self, state, x32, g32, argmax, pair=None):
+        """dx, droot, dbias, dx_dst of one application; adds its share into state.dd (when the edge network needs it).
+        A bipartite call (pair) takes droot, dbias and dx_dst from the root term's backward, else dx_dst is None."""
         L = _lib.lib()
         dev = x32.device
         with torch.cuda.device(dev):
+            square = pair is None
             dx = torch.empty_like(x32)
-            droot = torch.empty_like(self.root, dtype=torch.float32) if self.root is not None else None
-            dbias = torch.empty_like(self.bias, dtype=torch.float32) if self.bias is not None else None
+            droot = torch.empty_like(self.root, dtype=torch.float32) if self.root is not None and square else None
+            dbias = torch.empty_like(self.bias, dtype=torch.float32) if self.bias is not None and square else None
+            root = _f32(self.root) if square else None
             n_l = ctypes.c_int64(0)
             _lib.check(L.nnconv_backward_apply_diag(state.plan.handle, state.feats.prepared.handle, _ptr(state.feats.d),
-                                                    _ptr(x32), _ptr(_f32(self.root)), _lib.AGGR[self.aggr], _ptr(argmax),
+                                                    _ptr(x32), _ptr(root), _lib.AGGR[self.aggr], _ptr(argmax),
                                                     _ptr(g32), _ptr(dx), _ptr(droot), _ptr(dbias), _ptr(state.dd),
                                                     _stream_ptr(dev), ctypes.byref(n_l)))
             stats['launches'] += n_l.value
+            dxd = None
+            if not square:
+                dxd, droot, dbias = self._root_backward(pair, g32)
             stats['backwards'] += 1
-        return dx, droot, dbias
+        return dx, droot, dbias, dxd
 
     def _backward_mlp_impl(self, state, want_ea=False):
         """Gradients of every Linear of the edge network (weight, bias, in order) from the summed grad_d, and with

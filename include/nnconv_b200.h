@@ -101,7 +101,9 @@ int nnconv_plan_info(const nnconv_plan_t* plan, int64_t* info, int n_info);
  * n_src == n_dst == N.  On a plan with n_src != n_dst the apply and backward entry points of NNConv (nnconv_apply*,
  * nnconv_backward*) take x = x_src [n_src, in] and compute only the message part into out / grad_out [n_dst, out]: they
  * need root = NULL and no NNCONV_APPLY_RESIDUAL, and the root term comes from nnconv_root_term below (bias may go to
- * either; nnconv_root_term adds it after the messages).  The diagonal and Gaussian convs refuse such a plan. */
+ * either; nnconv_root_term adds it after the messages).  The diagonal and Gaussian convs (nnconv_apply_diag,
+ * nnconv_backward_apply_diag, nnconv_gauss_apply, nnconv_gauss_backward) follow the same rule: x and grad_x have n_src
+ * rows, out, argmax and grad_out n_dst, and the root term is nnconv_root_term's with in_channels = channels. */
 int nnconv_plan_sizes_bipartite(int64_t E, int64_t n_src, int64_t n_dst, size_t* ws_bytes, size_t* tmp_bytes);
 int nnconv_plan_create_bipartite(const int64_t* row0, const int64_t* row1, int64_t E, int64_t n_src, int64_t n_dst,
                                  int flow, void* ws, size_t ws_bytes, void* tmp, size_t tmp_bytes, void* stream,
