@@ -18,7 +18,8 @@ AGGR = {'add': 0, 'mean': 1, 'max': 2}     # max: through the nnconv_*_max entry
 APPLY_RELU_IN, APPLY_RESIDUAL = 1, 2        # include/nnconv_b200.h NNCONV_APPLY_*
 FLOW = {'source_to_target': 0, 'target_to_source': 1}
 # hidden activation of the edge MLP, include/nnconv_b200.h NNCONV_ACT_*
-ACT = {'relu': 0, 'leaky_relu': 1, 'elu': 2, 'tanh': 3, 'sigmoid': 4}
+ACT = {'relu': 0, 'leaky_relu': 1, 'elu': 2, 'tanh': 3, 'sigmoid': 4, 'clamp': 5, 'scaled_elu': 6, 'softsign': 7,
+       'logsigmoid': 8}
 
 # every symbol include/nnconv_b200.h declares (tests/test_cabi_symbols.py checks the .so exports them)
 SYMBOLS = [
@@ -50,6 +51,7 @@ SYMBOLS = [
     'nnconv_weights_create_act', 'nnconv_diag_weights_create_act',
     'nnconv_gauss_apply_sizes', 'nnconv_gauss_apply', 'nnconv_gauss_backward',
     'nnconv_plan_sizes_bipartite', 'nnconv_plan_create_bipartite', 'nnconv_root_term', 'nnconv_root_term_backward',
+    'nnconv_weights_create_act_params', 'nnconv_diag_weights_create_act_params',
 ]
 GCN_IMPROVED, GCN_NO_SELF_LOOPS, GCN_NO_NORMALIZE = 1, 2, 4   # include/nnconv_b200.h NNCONV_GCN_*
 
@@ -102,6 +104,8 @@ def lib():
                                         P(c_vp)]
     L.nnconv_weights_create_act.argtypes = [c_int, P(c_int), c_int, c_int, c_int, c_int, ctypes.c_float, P(c_vp), P(c_vp),
                                             c_vp, c_sz, c_vp, P(c_vp)]
+    L.nnconv_weights_create_act_params.argtypes = [c_int, P(c_int), c_int, c_int, c_int, c_int, P(ctypes.c_float), c_int,
+                                                   P(c_vp), P(c_vp), c_vp, c_sz, c_vp, P(c_vp)]
     L.nnconv_weights_destroy.argtypes = [c_vp]
     L.nnconv_weights_destroy.restype = None
     L.nnconv_weights_tc_supported.argtypes = [c_vp]
@@ -177,6 +181,8 @@ def lib():
     L.nnconv_diag_weights_create.argtypes = [c_int, P(c_int), c_int, c_int, P(c_vp), P(c_vp), c_vp, c_sz, c_vp, P(c_vp)]
     L.nnconv_diag_weights_create_act.argtypes = [c_int, P(c_int), c_int, c_int, c_int, ctypes.c_float, P(c_vp), P(c_vp),
                                                  c_vp, c_sz, c_vp, P(c_vp)]
+    L.nnconv_diag_weights_create_act_params.argtypes = [c_int, P(c_int), c_int, c_int, c_int, P(ctypes.c_float), c_int,
+                                                        P(c_vp), P(c_vp), c_vp, c_sz, c_vp, P(c_vp)]
     L.nnconv_diag_weights_destroy.argtypes = [c_vp]
     L.nnconv_diag_weights_destroy.restype = None
     L.nnconv_diag_sizes.argtypes = [c_vp, c_vp, c_sz, P(c_sz), P(c_sz)]

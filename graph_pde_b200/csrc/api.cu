@@ -1,12 +1,16 @@
 // C-ABI of libnnconv_b200 (declared in include/nnconv_b200.h) and the host-side sequencing of the
 // kernels.  No device allocation and no device synchronisation happens here except in
 // nnconv_plan_create (one-time per graph, returns counts to the host).
+#include <cmath>
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
 #include <new>
 #include <vector>
+
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
 
 #include "common.cuh"
 #include "kernels.h"
@@ -935,13 +939,49 @@ struct nnconv_diag_weights {
   Weights w;
 };
 
-// the backward takes f'(z) from the output y = f(z): for a negative LeakyReLU slope or ELU alpha y no longer tells the
-// sign of z
-static int check_act(int activation, float act_param) {
-  NNC_REQUIRE(activation >= NNCONV_ACT_RELU && activation <= NNCONV_ACT_SIGMOID, NNCONV_ERR_ARG,
+// the backward takes f'(z) from the output y = f(z): for a negative LeakyReLU slope or ELU alpha, a CLAMP with lo >= hi
+// or a <= 0, or a SCALED_ELU with lambda <= 0, alpha < 0 or c <= 0, y no longer determines f'.  Fills the handle's
+// activation fields (the bounds' images of CLAMP in the storage format of `prec`, see act.cuh) without touching the
+// device, so that every refusal comes before any allocation or launch.
+static float bound_image(int prec, float v) {
+  if (prec == PREC_F16) return __half2float(__float2half_rn(v));
+  if (prec == PREC_BF16) return __bfloat162float(__float2bfloat16_rn(v));
+  if (prec == PREC_F16X2) {   // (hi, lo) widened as the readers widen it: fp32 hi + lo
+    const float hi = __half2float(__float2half_rn(v));
+    return hi + __half2float(__float2half_rn(v - hi));
+  }
+  return v;
+}
+
+static int check_act(int activation, const float* p, int n, int prec, int* kind, float* param, ActParams* q) {
+  NNC_REQUIRE(activation >= NNCONV_ACT_RELU && activation <= NNCONV_ACT_LOGSIGMOID, NNCONV_ERR_ARG,
               "unknown edge-network activation %d", activation);
-  NNC_REQUIRE(!(activation == NNCONV_ACT_LEAKY_RELU || activation == NNCONV_ACT_ELU) || act_param >= 0.f, NNCONV_ERR_UNSUPPORTED,
-              "edge-network activation: a negative LeakyReLU slope / ELU alpha (%g) is not supported", act_param);
+  const int want = activation == NNCONV_ACT_LEAKY_RELU || activation == NNCONV_ACT_ELU ? 1
+                   : activation == NNCONV_ACT_CLAMP ? 4 : activation == NNCONV_ACT_SCALED_ELU ? 3 : 0;
+  NNC_REQUIRE(n == want || (n == 1 && want == 0), NNCONV_ERR_ARG,
+              "edge-network activation %d takes %d parameters, got %d", activation, want, n);
+  NNC_REQUIRE(n == 0 || p != nullptr, NNCONV_ERR_ARG, "null pointer");
+  for (int i = 0; i < n && want > 1; ++i)   // (LEAKY_RELU and ELU keep the checks they always had)
+    NNC_REQUIRE(std::isfinite(p[i]), NNCONV_ERR_ARG, "edge-network activation: parameter %d is not finite", i);
+  NNC_REQUIRE(!(activation == NNCONV_ACT_LEAKY_RELU || activation == NNCONV_ACT_ELU) || p[0] >= 0.f, NNCONV_ERR_UNSUPPORTED,
+              "edge-network activation: a negative LeakyReLU slope / ELU alpha (%g) is not supported", p[0]);
+  if (activation == NNCONV_ACT_CLAMP) {
+    NNC_REQUIRE(p[0] > 0.f, NNCONV_ERR_ARG, "edge-network activation: clamp slope a = %g must be > 0", p[0]);
+    NNC_REQUIRE(p[2] < p[3], NNCONV_ERR_ARG, "edge-network activation: clamp bounds lo = %g >= hi = %g", p[2], p[3]);
+  }
+  if (activation == NNCONV_ACT_SCALED_ELU) {
+    NNC_REQUIRE(p[0] > 0.f && p[1] >= 0.f && p[2] > 0.f, NNCONV_ERR_ARG,
+                "edge-network activation: scaled ELU needs lambda > 0, alpha >= 0 and c > 0 (got %g, %g, %g)", p[0], p[1],
+                p[2]);
+  }
+  *kind = activation;
+  *param = want == 1 ? p[0] : 0.f;
+  *q = ActParams{};
+  if (activation == NNCONV_ACT_CLAMP) {
+    *q = ActParams{{p[0], bound_image(prec, p[2]), bound_image(prec, p[3]), p[1], p[2], p[3]}};
+  } else if (activation == NNCONV_ACT_SCALED_ELU) {
+    *q = ActParams{{p[0], p[2], p[0] * p[1], p[1], 0.f, 0.f}};
+  }
   return NNCONV_OK;
 }
 
@@ -1099,17 +1139,29 @@ int nnconv_weights_create(int n_layers, const int* dims, int in_channels, int ou
 int nnconv_weights_create_act(int n_layers, const int* dims, int in_channels, int out_channels, int precision,
                               int activation, float act_param, const float* const* W, const float* const* b, void* buf,
                               size_t buf_bytes, void* stream, nnconv_weights_t** out) {
+  return nnconv_weights_create_act_params(n_layers, dims, in_channels, out_channels, precision, activation, &act_param, 1,
+                                          W, b, buf, buf_bytes, stream, out);
+}
+
+int nnconv_weights_create_act_params(int n_layers, const int* dims, int in_channels, int out_channels, int precision,
+                                     int activation, const float* act_params, int n_act_params, const float* const* W,
+                                     const float* const* b, void* buf, size_t buf_bytes, void* stream,
+                                     nnconv_weights_t** out) {
   NNC_REQUIRE(out && dims && W && b, NNCONV_ERR_ARG, "null pointer");
   *out = nullptr;
-  int s = check_act(activation, act_param);
+  int kind;
+  float param;
+  ActParams q;
+  int s = check_act(activation, act_params, n_act_params, precision, &kind, &param, &q);
   if (s) return s;
   nnconv_weights* h = new (std::nothrow) nnconv_weights();
   NNC_REQUIRE(h != nullptr, NNCONV_ERR_ARG, "out of host memory");
   s = weights_prepare(&h->w, n_layers, dims, in_channels, out_channels, precision, W, b, buf, buf_bytes,
                       static_cast<cudaStream_t>(stream));
   if (s != NNCONV_OK) { delete h; return s; }
-  h->w.act = activation;
-  h->w.act_param = act_param;
+  h->w.act = kind;
+  h->w.act_param = param;
+  h->w.act_p = q;
   *out = h;
   return NNCONV_OK;
 }
@@ -1437,17 +1489,29 @@ int nnconv_diag_weights_create(int n_layers, const int* dims, int channels, int 
 int nnconv_diag_weights_create_act(int n_layers, const int* dims, int channels, int precision, int activation,
                                    float act_param, const float* const* W, const float* const* b, void* buf,
                                    size_t buf_bytes, void* stream, nnconv_diag_weights_t** out) {
+  return nnconv_diag_weights_create_act_params(n_layers, dims, channels, precision, activation, &act_param, 1, W, b, buf,
+                                               buf_bytes, stream, out);
+}
+
+int nnconv_diag_weights_create_act_params(int n_layers, const int* dims, int channels, int precision, int activation,
+                                          const float* act_params, int n_act_params, const float* const* W,
+                                          const float* const* b, void* buf, size_t buf_bytes, void* stream,
+                                          nnconv_diag_weights_t** out) {
   NNC_REQUIRE(out && dims && W && b, NNCONV_ERR_ARG, "null pointer");
   *out = nullptr;
-  int s = check_act(activation, act_param);
+  int kind;
+  float param;
+  ActParams q;
+  int s = check_act(activation, act_params, n_act_params, precision, &kind, &param, &q);
   if (s) return s;
   nnconv_diag_weights* h = new (std::nothrow) nnconv_diag_weights();
   NNC_REQUIRE(h != nullptr, NNCONV_ERR_ARG, "out of host memory");
   s = weights_prepare(&h->w, n_layers, dims, channels, channels, precision, W, b, buf, buf_bytes,
                       static_cast<cudaStream_t>(stream), 1);
   if (s != NNCONV_OK) { delete h; return s; }
-  h->w.act = activation;
-  h->w.act_param = act_param;
+  h->w.act = kind;
+  h->w.act_param = param;
+  h->w.act_p = q;
   *out = h;
   return NNCONV_OK;
 }

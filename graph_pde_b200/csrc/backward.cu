@@ -145,17 +145,18 @@ __global__ void k_group_sum(const float* __restrict__ G, const int* __restrict__
 }
 
 // dz = dh * (act > 0), in place; column sums accumulate into db (one block per 32 columns).  k_act_grad_colsum<ACT>
-// multiplies by f'(act) of another hidden activation (act.cuh) instead.
+// multiplies by f'(act) of another hidden activation (act.cuh) instead; the kinds with a parameter block (CLAMP,
+// SCALED_ELU) take it in the overload whose last argument is the block.
 template <int ACT>
 __device__ __forceinline__ void act_grad_colsum(float* __restrict__ dh, const float* __restrict__ act, int ne, int kp,
-                                                float* __restrict__ db, float act_param) {
+                                                float* __restrict__ db, float act_param, const ActParams& act_p) {
   __shared__ float red[8][33];
   const int col = blockIdx.x * 32 + threadIdx.x;
   float s = 0.f;
   for (int p = threadIdx.y; p < ne; p += 8) {
     if (col < kp) {
       const int64_t i = static_cast<int64_t>(p) * kp + col;
-      const float v = ACT == ACT_RELU ? (act[i] > 0.f ? dh[i] : 0.f) : dh[i] * act_grad<ACT>(act[i], act_param);
+      const float v = ACT == ACT_RELU ? (act[i] > 0.f ? dh[i] : 0.f) : dh[i] * act_grad<ACT>(act[i], act_param, act_p);
       dh[i] = v;
       s += v;
     }
@@ -171,13 +172,19 @@ __device__ __forceinline__ void act_grad_colsum(float* __restrict__ dh, const fl
 
 __global__ void k_relu_mask_colsum(float* __restrict__ dh, const float* __restrict__ act, int ne, int kp,
                                    float* __restrict__ db) {
-  act_grad_colsum<ACT_RELU>(dh, act, ne, kp, db, 0.f);
+  act_grad_colsum<ACT_RELU>(dh, act, ne, kp, db, 0.f, ActParams{});
 }
 
 template <int ACT>
 __global__ void k_act_grad_colsum(float* __restrict__ dh, const float* __restrict__ act, int ne, int kp,
                                   float* __restrict__ db, float act_param) {
-  act_grad_colsum<ACT>(dh, act, ne, kp, db, act_param);
+  act_grad_colsum<ACT>(dh, act, ne, kp, db, act_param, ActParams{});
+}
+
+template <int ACT>
+__global__ void k_act_grad_colsum(float* __restrict__ dh, const float* __restrict__ act, int ne, int kp,
+                                  float* __restrict__ db, ActParams act_p) {
+  act_grad_colsum<ACT>(dh, act, ne, kp, db, 0.f, act_p);
 }
 
 __global__ void k_gather_ea(const float* __restrict__ edge_attr, const int* __restrict__ perm, int e0, int ne,
@@ -268,8 +275,12 @@ int mlp_backward_rows(const Plan* P, const Weights* W, const float* edge_attr, i
       k_relu_mask_colsum<<<ceil_div(W->kp[l], 32), dim3(32, 8), 0, st>>>(cur, act[l], ne, W->kp[l], db[l]);
     else
       act_dispatch(W->act, [&](auto k) {
-        k_act_grad_colsum<decltype(k)::value><<<ceil_div(W->kp[l], 32), dim3(32, 8), 0, st>>>(cur, act[l], ne, W->kp[l],
-                                                                                              db[l], W->act_param);
+        constexpr int A = decltype(k)::value;
+        if constexpr (A == ACT_CLAMP || A == ACT_SCALED_ELU)
+          k_act_grad_colsum<A><<<ceil_div(W->kp[l], 32), dim3(32, 8), 0, st>>>(cur, act[l], ne, W->kp[l], db[l], W->act_p);
+        else
+          k_act_grad_colsum<A><<<ceil_div(W->kp[l], 32), dim3(32, 8), 0, st>>>(cur, act[l], ne, W->kp[l], db[l],
+                                                                               W->act_param);
       });
     NNC_CHECK_LAUNCH();
     const float* prev = l == 1 ? ea : act[l - 1];

@@ -539,6 +539,9 @@ struct DhArgs {
   float* colsum;
   int colsum_stride;
   float act_param;          // LeakyReLU slope / ELU alpha of MODE's activation
+  // act_grad's part of the parameter block of a CLAMP / SCALED_ELU MODE activation (ActParams v[0 .. 2]; three scalars
+  // rather than the whole block, which leaves the code of the other instantiations as it was)
+  float act_q0, act_q1, act_q2;
 };
 
 constexpr int kDhScratch = 4 * acc_scratch_bytes<32>();
@@ -704,8 +707,9 @@ k_dh(const __grid_constant__ Maps8 tmA, const __grid_constant__ CUtensorMap tmB,
                     y.x += yl.x;
                     y.y += yl.y;
                   }
-                  f0 = __uint_as_float(v[8 * q + 2 * j]) * act_grad<kAct>(y.x, a.act_param);
-                  f1 = __uint_as_float(v[8 * q + 2 * j + 1]) * act_grad<kAct>(y.y, a.act_param);
+                  const ActParams aq{{a.act_q0, a.act_q1, a.act_q2}};
+                  f0 = __uint_as_float(v[8 * q + 2 * j]) * act_grad<kAct>(y.x, a.act_param, aq);
+                  f1 = __uint_as_float(v[8 * q + 2 * j + 1]) * act_grad<kAct>(y.y, a.act_param, aq);
                 }
                 if (SPLIT) pack2_split(f0, f1, pk[4 * q + j], pl[4 * q + j]);
                 else pk[4 * q + j] = pack2<FMT>(f0, f1);
@@ -1442,6 +1446,7 @@ int backward_mlp_tc(const Plan* P, const Weights* W, const float* edge_attr, con
       const int tiles = a.tile1 - a.tile0;
       const int grid = tiles < tc_num_sms() ? tiles : tc_num_sms();
       a.act_param = W->act_param;
+      a.act_q0 = W->act_p.v[0]; a.act_q1 = W->act_p.v[1]; a.act_q2 = W->act_p.v[2];
       if (W->act != ACT_RELU) {
         s = act_dispatch(W->act, [&](auto k) {
           constexpr int M = decltype(k)::value << 1;

@@ -65,6 +65,7 @@ struct GemmTcArgs {
   TraceBuf trace;
   unsigned int trace_seq;
   float act_param;     // LeakyReLU slope / ELU alpha of the activation epi_act(EPI)
+  ActParams act_p;     // parameter block of a CLAMP / SCALED_ELU epi_act(EPI)
 };
 
 // EPI selects the epilogue at COMPILE time (runtime flags inside the 32-column inner loop cut it into dozens of
@@ -76,7 +77,8 @@ struct GemmTcArgs {
 // The hidden activation (act.cuh) rides in the bits above: EPI = base | ACT << 3.  ReLU is ACT 0, so the ReLU
 // instantiations keep their names and code; for the other activations the forward epilogues apply act_fwd<ACT> where
 // ReLU applies the max, and the mask epilogues multiply by act_grad<ACT>(y) of the stored activation y (the split
-// form reads y = hi + lo, the lo half at column c + N of the mask row).
+// form reads y = hi + lo, the lo half at column c + N of the mask row).  For CLAMP the forward epilogues also apply the
+// store rule of act.cuh (act_store16, act_split_lo), so that no interior entry is stored on a bound's image.
 // The forward epilogues (PLAIN, NOCHECK, SPLIT) work on the accumulator fragments and write the 16-bit staging with
 // stmatrix; the backward ones first transpose the fragments through a per-warp fp32 scratch (acc_rows: lane = row),
 // because their mask is read and their fp32 output written a row at a time.
@@ -310,11 +312,12 @@ k_gemm_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
                 } else {
                   float r0 = fabsf(f0), r1 = fabsf(f1);
                   if (a.relu) {
-                    const float y0 = act_fwd<kAct>(f0, a.act_param), y1 = act_fwd<kAct>(f1, a.act_param);
+                    const float y0 = act_fwd<kAct>(f0, a.act_param, a.act_p);
+                    const float y1 = act_fwd<kAct>(f1, a.act_param, a.act_p);
                     r0 = act_range<kAct>(f0, y0);
                     r1 = act_range<kAct>(f1, y1);
-                    f0 = y0;
-                    f1 = y1;
+                    f0 = kSplitOut ? y0 : act_store16<kAct, FMT>(y0, a.act_p);
+                    f1 = kSplitOut ? y1 : act_store16<kAct, FMT>(y1, a.act_p);
                   }
                   if (kRangeCheck && ok) vmax[j & 1] = fmaxf(vmax[j & 1], fmaxf(r0, r1));
                 }
@@ -323,7 +326,11 @@ k_gemm_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
                   hi[h][g][j] = *reinterpret_cast<const uint32_t*>(&hv);
                   if (kSplitOut) {
                     const float2 hf = __half22float2(hv);
-                    const __half2 lv = __floats2half2_rn(f0 - hf.x, f1 - hf.y);
+                    __half2 lv = __floats2half2_rn(f0 - hf.x, f1 - hf.y);
+                    if (kAct == ACT_CLAMP && a.relu) {
+                      lv.x = act_split_lo<kAct>(f0, hv.x, lv.x, a.act_p);
+                      lv.y = act_split_lo<kAct>(f1, hv.y, lv.y, a.act_p);
+                    }
                     lo[h][g][j] = *reinterpret_cast<const uint32_t*>(&lv);
                   }
                 } else {
@@ -379,7 +386,7 @@ k_gemm_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
             }
             if (a.relu) {
 #pragma unroll
-              for (int q = 0; q < 4; ++q) f[q] = act_fwd<kAct>(f[q], a.act_param);
+              for (int q = 0; q < 4; ++q) f[q] = act_fwd<kAct>(f[q], a.act_param, a.act_p);
             }
             if (kMask && kAct != ACT_RELU) {
               // f'(y) from the stored activation: y = hi (+ lo at column c + N for the split form)
@@ -398,8 +405,8 @@ k_gemm_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
                     y.x += yl.x;
                     y.y += yl.y;
                   }
-                  f[2 * q] *= act_grad<kAct>(y.x, a.act_param);
-                  f[2 * q + 1] *= act_grad<kAct>(y.y, a.act_param);
+                  f[2 * q] *= act_grad<kAct>(y.x, a.act_param, a.act_p);
+                  f[2 * q + 1] *= act_grad<kAct>(y.y, a.act_param, a.act_p);
                 }
               }
             } else if (kMask) {
@@ -625,6 +632,7 @@ int launch_gemm_tc(int prec, const void* A_base, int64_t a_rows_total, int64_t a
   // the activation matters only where it is applied (relu) or differentiated (mask); every other launch is the ReLU
   // instantiation, as it always was
   a.act_param = act.param;
+  a.act_p = act.p;
   if (act.kind == ACT_RELU || (!relu && mask == nullptr)) return dispatch_gemm<ACT_RELU>(tmA, tmB, tmC, a, st, pdl, BN, bf, small, out_f32, mask_split, mask != nullptr, c_split);
   NNC_REQUIRE(!out_f32 && !small, NNCONV_ERR_ARG, "gemm_tc: the activation excludes fp32 output / the small-footprint configuration");
   return act_dispatch(act.kind, [&](auto k) {

@@ -50,10 +50,20 @@ int plan_build(Plan* P, const int64_t* row0, const int64_t* row1, int64_t E, int
 // conv (NNConv, diagonal, Gaussian): the root term reads x_dst, not x_src (root_term / node_terms_rows)
 int check_bipartite_root(const Plan* P, const float* root, unsigned node_flags);
 
-// hidden activation of the edge MLP: kind = NNCONV_ACT_* (0 = ReLU), param = LeakyReLU slope / ELU alpha
+// parameter block of the activations with more than one parameter (act.cuh); act_grad reads v[0 .. 2] only:
+//   NNCONV_ACT_CLAMP       v = a, lo_img, hi_img, b, lo, hi   (the bounds' images in the weights' storage format)
+//   NNCONV_ACT_SCALED_ELU  v = lambda, c, lambda * alpha, alpha
+constexpr int kActParams = 6;
+struct ActParams {
+  float v[kActParams];
+};
+
+// hidden activation of the edge MLP: kind = NNCONV_ACT_* (0 = ReLU), param = LeakyReLU slope / ELU alpha, p = the
+// parameter block of the other kinds
 struct Act {
   int kind;
   float param;
+  ActParams p;
 };
 
 // Prepared (padded / permuted / down-converted) snapshot of the edge-MLP parameters.
@@ -91,9 +101,10 @@ struct Weights {
   // hidden activation of the edge MLP (NNCONV_ACT_*) and its parameter (LeakyReLU slope / ELU alpha), see act.cuh
   int act;
   float act_param;
+  ActParams act_p;              // NNCONV_ACT_CLAMP and NNCONV_ACT_SCALED_ELU, see ActParams
 };
 
-inline Act act_of(const Weights* W) { return Act{W->act, W->act_param}; }
+inline Act act_of(const Weights* W) { return Act{W->act, W->act_param, W->act_p}; }
 
 size_t weights_bytes(int n_layers, const int* dims, int cin, int cout, int prec, int diag = 0);
 int weights_prepare(Weights* W, int n_layers, const int* dims, int cin, int cout, int prec,

@@ -277,9 +277,14 @@ def get_plan(edge_index, n_nodes, flow='source_to_target'):
 
 # hidden activations the library runs: each has a derivative that is a function of its output (include/nnconv_b200.h
 # NNCONV_ACT_*), so the backward needs nothing beyond the activations it keeps for ReLU
+_SELU_SCALE, _SELU_ALPHA = 1.0507009873554805, 1.6732632423543772    # torch.nn.SELU's constants
+
+
 def _act_spec(m):
-    """('relu' | 'leaky_relu' | 'elu' | 'tanh' | 'sigmoid', parameter) of an activation module, None for any other
-    module; raises NotImplementedError for an activation the library does not run, naming the reason."""
+    """('relu' | 'leaky_relu' | 'elu' | 'tanh' | 'sigmoid', parameter) of an activation module, or for the kinds with
+    a parameter block ('clamp' | 'scaled_elu' | 'softsign' | 'logsigmoid', tuple of parameters); None for any other
+    module.  Raises NotImplementedError for an activation the library does not run, naming the reason.  Two specs are
+    equal exactly when they are the same function: ReLU6() and Hardtanh(0, 6) are both ('clamp', (1, 0, 0, 6))."""
     if isinstance(m, torch.nn.ReLU):
         return ('relu', 0.0)
     if isinstance(m, torch.nn.LeakyReLU):
@@ -296,6 +301,21 @@ def _act_spec(m):
         return ('tanh', 0.0)
     if isinstance(m, torch.nn.Sigmoid):
         return ('sigmoid', 0.0)
+    if isinstance(m, torch.nn.Hardtanh):           # ReLU6 is Hardtanh(0, 6); torch requires min_val < max_val
+        return ('clamp', (1.0, 0.0, float(m.min_val), float(m.max_val)))
+    if isinstance(m, torch.nn.Hardsigmoid):
+        return ('clamp', (1.0 / 6.0, 0.5, 0.0, 1.0))
+    if isinstance(m, torch.nn.SELU):
+        return ('scaled_elu', (_SELU_SCALE, _SELU_ALPHA, 1.0))
+    if isinstance(m, torch.nn.CELU):
+        if not m.alpha > 0:
+            raise NotImplementedError('edge network: CELU with alpha <= 0 (%g) is not supported: CELU divides by '
+                                      'alpha, and its derivative is not a function of its output' % m.alpha)
+        return ('scaled_elu', (1.0, float(m.alpha), 1.0 / float(m.alpha)))
+    if isinstance(m, torch.nn.Softsign):
+        return ('softsign', ())
+    if isinstance(m, torch.nn.LogSigmoid):
+        return ('logsigmoid', ())
     if isinstance(m, (torch.nn.GELU, torch.nn.SiLU, torch.nn.Softplus, torch.nn.Mish, torch.nn.Hardswish)):
         raise NotImplementedError('edge network: %s is not supported: its derivative is not a function of its '
                                   'output, so the backward would have to recompute the pre-activations'
@@ -309,8 +329,9 @@ def _act_spec(m):
 def _edge_network(nn_module):
     """The edge network must be the reference's DenseNet shape (graph-neural-operator/utilities.py:201-227):
     Linear (act Linear)* with one hidden activation ``act`` in {ReLU, LeakyReLU(s >= 0), ELU(alpha >= 0), Tanh,
-    Sigmoid} after every Linear but the last, no output nonlinearity and normalize=False.  Returns (the Linear
-    layers, the activation spec (kind, parameter)); a single Linear has the spec ('relu', 0.0), which it never uses."""
+    Sigmoid, Hardtanh, ReLU6, Hardsigmoid, SELU, CELU(alpha > 0), Softsign, LogSigmoid} after every Linear but the last,
+    no output nonlinearity and normalize=False.  Returns (the Linear layers, the activation spec (kind, parameter));
+    a single Linear has the spec ('relu', 0.0), which it never uses."""
     if type(nn_module).__name__ == 'DenseNet_sin':
         raise NotImplementedError('edge network: DenseNet_sin (torch.sin between the layers) is not supported: the '
                                   'derivative of sin is not a function of its output')
@@ -330,8 +351,9 @@ def _edge_network(nn_module):
             continue
         spec = _act_spec(m)
         if spec is None:
-            raise NotImplementedError('edge network: only Linear chains with ReLU, LeakyReLU, ELU, Tanh or Sigmoid '
-                                      'between them (DenseNet) are supported, found %s' % type(m).__name__)
+            raise NotImplementedError('edge network: only Linear chains with ReLU, LeakyReLU, ELU, Tanh, Sigmoid, '
+                                      'Hardtanh, ReLU6, Hardsigmoid, SELU, CELU, Softsign or LogSigmoid between them '
+                                      '(DenseNet) are supported, found %s' % type(m).__name__)
         if expect_linear:
             if lin:
                 raise NotImplementedError('edge network: two activations in a row (%s after an activation)'
@@ -358,6 +380,13 @@ def _linear_chain(nn_module):
     return lin
 
 
+def _act_params(act):
+    """(float array, count) of an activation spec for nnconv_*weights_create_act_params: the tuple of a spec with a
+    parameter block, the single parameter of the others."""
+    p = act[1] if isinstance(act[1], tuple) else (act[1],)
+    return (ctypes.c_float * max(len(p), 1))(*p), len(p)
+
+
 class _Prepared(object):
     """nnconv_weights_t: padded / permuted / down-converted snapshot of the edge-MLP parameters."""
 
@@ -377,8 +406,9 @@ class _Prepared(object):
         wp = (ctypes.c_void_p * n)(*[w.data_ptr() for w in ws])
         bp = (ctypes.c_void_p * n)(*[b.data_ptr() for b in bs])
         h = ctypes.c_void_p()
-        _lib.check(L.nnconv_weights_create_act(n, c_dims, cin, cout, prec, _lib.ACT[act[0]], act[1], wp, bp,
-                                               _ptr(self.buf), nbytes.value, _stream_ptr(dev), ctypes.byref(h)))
+        q, nq = _act_params(act)
+        _lib.check(L.nnconv_weights_create_act_params(n, c_dims, cin, cout, prec, _lib.ACT[act[0]], q, nq, wp, bp,
+                                                      _ptr(self.buf), nbytes.value, _stream_ptr(dev), ctypes.byref(h)))
         self._keep = (ws, bs)
         self.handle = h
         self.dims = dims
@@ -1203,8 +1233,10 @@ class _DiagWeights(object):
         wp = (ctypes.c_void_p * n)(*[w.data_ptr() for w in ws])
         bp = (ctypes.c_void_p * n)(*[b.data_ptr() for b in bs])
         h = ctypes.c_void_p()
-        _lib.check(L.nnconv_diag_weights_create_act(n, c_dims, channels, prec, _lib.ACT[act[0]], act[1], wp, bp,
-                                                    _ptr(self.buf), nbytes.value, _stream_ptr(dev), ctypes.byref(h)))
+        q, nq = _act_params(act)
+        _lib.check(L.nnconv_diag_weights_create_act_params(n, c_dims, channels, prec, _lib.ACT[act[0]], q, nq, wp,
+                                                           bp, _ptr(self.buf), nbytes.value, _stream_ptr(dev),
+                                                           ctypes.byref(h)))
         self._keep = (ws, bs)
         self.handle = h
         self.precision = precision

@@ -139,17 +139,36 @@ int nnconv_weights_tc_supported(const nnconv_weights_t* w);
  *   ELU         z > 0 ? z : a (e^z - 1) (a>=0) f' = y > 0 ? 1 : y + a
  *   TANH        tanh z                        f' = 1 - y^2
  *   SIGMOID     1 / (1 + e^-z)                f' = y (1 - y)
+ *   CLAMP       clamp(a z + b, lo, hi)        f' = lo < y < hi ? a : 0     (Hardtanh, ReLU6, Hardsigmoid)
+ *   SCALED_ELU  l (z > 0 ? z : al (e^(c z) - 1))  f' = y > 0 ? l : c (y + l al)   (SELU, CELU)
+ *   SOFTSIGN    z / (1 + |z|)                 f' = (1 - |y|)^2
+ *   LOGSIGMOID  min(z, 0) - log(1 + e^-|z|)   f' = -(e^y - 1)
  * act_param is s (LEAKY_RELU) or a (ELU) and is ignored otherwise.  The activation is stored in the handle and every
  * entry point that runs or differentiates the edge MLP reads it from there; nnconv_weights_create is
- * nnconv_weights_create_act with NNCONV_ACT_RELU. */
+ * nnconv_weights_create_act with NNCONV_ACT_RELU.
+ * nnconv_weights_create_act_params takes the parameters as an array of n_act_params floats: 1 for LEAKY_RELU and ELU
+ * (nnconv_weights_create_act is that case), 4 for CLAMP (a, b, lo, hi), 3 for SCALED_ELU (l, al, c), 0 otherwise.
+ * A parameter that is not finite, lo >= hi or a <= 0 (CLAMP), l <= 0, al < 0 or c <= 0 (SCALED_ELU), a negative s or
+ * a (LEAKY_RELU, ELU: NNCONV_ERR_UNSUPPORTED) or a wrong n_act_params is refused: y would no longer determine f'.
+ * CLAMP decides "saturated" from the STORED activation: an entry is saturated exactly when its stored image (16-bit at
+ * f16 / bf16, hi + lo at f16x2) equals a bound's image, and the writers store an interior value that would round onto
+ * a bound's image one 16-bit step inward. */
 #define NNCONV_ACT_RELU 0
 #define NNCONV_ACT_LEAKY_RELU 1
 #define NNCONV_ACT_ELU 2
 #define NNCONV_ACT_TANH 3
 #define NNCONV_ACT_SIGMOID 4
+#define NNCONV_ACT_CLAMP 5
+#define NNCONV_ACT_SCALED_ELU 6
+#define NNCONV_ACT_SOFTSIGN 7
+#define NNCONV_ACT_LOGSIGMOID 8
 int nnconv_weights_create_act(int n_layers, const int* dims, int in_channels, int out_channels, int precision,
                               int activation, float act_param, const float* const* W, const float* const* b, void* buf,
                               size_t buf_bytes, void* stream, nnconv_weights_t** out);
+int nnconv_weights_create_act_params(int n_layers, const int* dims, int in_channels, int out_channels, int precision,
+                                     int activation, const float* act_params, int n_act_params, const float* const* W,
+                                     const float* const* b, void* buf, size_t buf_bytes, void* stream,
+                                     nnconv_weights_t** out);
 
 /* ---- hoisted, x-independent part of message(): h_e for every edge (utilities.py:223-227 minus the
  * last Linear).  Valid as long as edge_attr and the weights are unchanged, i.e. for all T applications
@@ -371,6 +390,10 @@ int nnconv_diag_weights_create(int n_layers, const int* dims, int channels, int 
 int nnconv_diag_weights_create_act(int n_layers, const int* dims, int channels, int precision, int activation,
                                    float act_param, const float* const* W, const float* const* b, void* buf,
                                    size_t buf_bytes, void* stream, nnconv_diag_weights_t** out);
+int nnconv_diag_weights_create_act_params(int n_layers, const int* dims, int channels, int precision, int activation,
+                                          const float* act_params, int n_act_params, const float* const* W,
+                                          const float* const* b, void* buf, size_t buf_bytes, void* stream,
+                                          nnconv_diag_weights_t** out);
 void nnconv_diag_weights_destroy(nnconv_diag_weights_t* w);
 int nnconv_diag_sizes(const nnconv_plan_t* plan, const nnconv_diag_weights_t* w, size_t want_ws_bytes, size_t* d_bytes,
                       size_t* ws_bytes);

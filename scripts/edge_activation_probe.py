@@ -26,7 +26,9 @@ from graph_pde_b200.models import DenseNet, KernelNN  # noqa: E402
 from scripts.train_probe import _power_limit, _timed  # noqa: E402
 
 ACTS = [('relu', torch.nn.ReLU), ('leaky_relu', lambda: torch.nn.LeakyReLU(0.01)), ('elu', torch.nn.ELU),
-        ('tanh', torch.nn.Tanh), ('sigmoid', torch.nn.Sigmoid)]
+        ('tanh', torch.nn.Tanh), ('sigmoid', torch.nn.Sigmoid), ('relu6', torch.nn.ReLU6),
+        ('hardtanh', lambda: torch.nn.Hardtanh(-0.3, 0.7)), ('hardsigmoid', torch.nn.Hardsigmoid), ('selu', torch.nn.SELU),
+        ('celu', lambda: torch.nn.CELU(0.5)), ('softsign', torch.nn.Softsign), ('logsigmoid', torch.nn.LogSigmoid)]
 
 
 class _Data(object):
@@ -151,14 +153,15 @@ def _forward_241(dev, rounds):
 
 
 def _accuracy():
-    from tests import test_gpu_edge_activation as G
+    from tests import test_gpu_edge_activation as G0
+    from tests import test_gpu_edge_activation_more as G1
     from tests.helpers import rel_err
     nn_conv._EDGE_KERNELS = 'off'
-    ei, n = G._hub_graph()
-    ea, xs, gs = G._inputs(ei, n, T=2)
+    ei, n = G0._hub_graph()
+    ea, xs, gs = G0._inputs(ei, n, T=2)
     print('max|err| / max|ref| against fp64 (forward; worst parameter / x gradient; edge_attr gradient), aggr mean, '
           'E=%d, T=2, [6, 128, 128, 64 * 64]:' % ei.size(1))
-    for kind, p in G.ACTS:
+    for G, kind, p in [(G, kind, p) for G in (G0, G1) for kind, p in G.ACTS]:   # G1: first layer scaled by 4
         for precision in ('f16', 'bf16', 'f16x2', 'fp32'):
             conv = G._conv(kind, p, precision, 'mean')
             with torch.no_grad():
