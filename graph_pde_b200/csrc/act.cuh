@@ -1,8 +1,8 @@
 // Hidden activation of the edge MLP (include/nnconv_b200.h NNCONV_ACT_*), as a compile-time template argument of the
 // kernels that fuse it.  act_fwd is f(z); act_grad is f'(z) written as a function of the output y = f(z), which is all
 // the backward keeps or recomputes (the stored activation, never the pre-activation).  At y = 0 it follows torch's
-// backward: LeakyReLU gives the slope, ELU gives alpha, ReLU gives 0.  p is the single parameter of LEAKY_RELU / ELU,
-// q the parameter block of CLAMP and SCALED_ELU (plan.h ActParams).
+// backward: LeakyReLU gives the slope, ELU gives alpha, ReLU gives 0.  q is the kind's parameter block (plan.h
+// ActParams).
 //
 // Every function is fp32-accurate to a few ulp (tanhf, expf, expm1f, log1pf; the reciprocals of the sigmoid and of
 // softsign's 1 + |z| are refined by one Newton step), so f16x2 and fp32 keep their tolerances; at f16 / bf16 the
@@ -28,10 +28,10 @@ enum { ACT_RELU = NNCONV_ACT_RELU, ACT_LEAKY_RELU = NNCONV_ACT_LEAKY_RELU, ACT_E
        ACT_SCALED_ELU = NNCONV_ACT_SCALED_ELU, ACT_SOFTSIGN = NNCONV_ACT_SOFTSIGN, ACT_LOGSIGMOID = NNCONV_ACT_LOGSIGMOID };
 
 template <int ACT>
-__device__ __forceinline__ float act_fwd(float z, float p, const ActParams& q) {
+__device__ __forceinline__ float act_fwd(float z, const ActParams& q) {
   if (ACT == ACT_RELU) return fmaxf(z, 0.f);
-  if (ACT == ACT_LEAKY_RELU) return z > 0.f ? z : p * z;
-  if (ACT == ACT_ELU) return z > 0.f ? z : p * expm1f(z);
+  if (ACT == ACT_LEAKY_RELU) return z > 0.f ? z : q.v[0] * z;
+  if (ACT == ACT_ELU) return z > 0.f ? z : q.v[0] * expm1f(z);
   if (ACT == ACT_TANH) return tanhf(z);
   // clamp(a z + b, lo, hi)
   if (ACT == ACT_CLAMP) return fminf(fmaxf(fmaf(q.v[0], z, q.v[3]), q.v[4]), q.v[5]);
@@ -53,10 +53,10 @@ __device__ __forceinline__ float act_fwd(float z, float p, const ActParams& q) {
 }
 
 template <int ACT>
-__device__ __forceinline__ float act_grad(float y, float p, const ActParams& q) {
+__device__ __forceinline__ float act_grad(float y, const ActParams& q) {
   if (ACT == ACT_RELU) return y > 0.f ? 1.f : 0.f;
-  if (ACT == ACT_LEAKY_RELU) return y > 0.f ? 1.f : p;
-  if (ACT == ACT_ELU) return y > 0.f ? 1.f : y + p;
+  if (ACT == ACT_LEAKY_RELU) return y > 0.f ? 1.f : q.v[0];
+  if (ACT == ACT_ELU) return y > 0.f ? 1.f : y + q.v[0];
   if (ACT == ACT_TANH) return 1.f - y * y;
   if (ACT == ACT_CLAMP) return y > q.v[1] && y < q.v[2] ? q.v[0] : 0.f;   // strictly between the bounds' images
   if (ACT == ACT_SCALED_ELU) return y > 0.f ? q.v[0] : q.v[1] * (y + q.v[2]);

@@ -299,7 +299,7 @@ int edge_features_rows(const Plan* P, const Weights* W, const float* edge_attr, 
   if (rowb == 0) {   // CUDA-core first layer straight into h (2-layer MLP: fp32, or k_in > 20 in 16 bits)
     ProfScope ps(PK_LAYER1, st);
     s = launch_edge_layer1(W->prec, edge_attr, P->perm, e_begin, E, W->dims[0], W->W1, W->b1, W->kp[1], 0, h, st, hpad, 0,
-                           overflow, act_of(W));
+                           overflow, W->act);
     if (launches) ++*launches;
     return s;
   }
@@ -324,11 +324,11 @@ int edge_features_rows(const Plan* P, const Weights* W, const float* edge_attr, 
         if (s) return s;
         s = launch_gemm_tc(W->prec, a1, n, 0, static_cast<int>(n), 64, W->W1aug, W->kp[1], nullptr, 1, dst1,
                            static_cast<int64_t>(amul) * W->kp[1], st, nullptr, h_pad_l1, e0,
-                           W->split ? GEMM_C_SPLIT : 0, overflow, nullptr, 0, 0, 0, nullptr, act_of(W));
+                           W->split ? GEMM_C_SPLIT : 0, overflow, nullptr, 0, 0, 0, nullptr, W->act);
         if (launches) ++*launches;
       } else {
         s = launch_edge_layer1(W->prec, edge_attr, P->perm, e_begin + e0, n, W->dims[0], W->W1, W->b1, W->kp[1], 0, dst1,
-                               st, h_pad_l1, e0, overflow, act_of(W));
+                               st, h_pad_l1, e0, overflow, W->act);
       }
     }
     if (s) return s;
@@ -343,12 +343,12 @@ int edge_features_rows(const Plan* P, const Weights* W, const float* edge_attr, 
       if (W->prec == PREC_FP32) {
         s = launch_sgemm_store(reinterpret_cast<const float*>(cur), W->kp[l - 1],
                                reinterpret_cast<const float*>(W->Wh[l]), W->kp[l - 1], static_cast<float*>(dst),
-                               W->kp[l], static_cast<int>(n), W->kp[l], W->kp[l - 1], W->bh[l], st, act_of(W));
+                               W->kp[l], static_cast<int>(n), W->kp[l], W->kp[l - 1], W->bh[l], st, W->act);
       } else {
         s = launch_gemm_tc(W->prec, cur, n, 0, static_cast<int>(n), kmul * W->kp[l - 1], W->Wh[l], W->kp[l], W->bh[l], 1,
                            dst, static_cast<int64_t>(amul) * W->kp[l], st, nullptr, last ? hpad : 0, e0,
                            W->split ? (GEMM_A_SPLIT | GEMM_C_SPLIT) : 0, overflow, nullptr, 0, 0, 0,
-                           W->split ? W->wscale + 2 * l + 1 : nullptr, act_of(W));
+                           W->split ? W->wscale + 2 * l + 1 : nullptr, W->act);
       }
       if (s) return s;
       if (launches) ++*launches;
@@ -940,8 +940,8 @@ struct nnconv_diag_weights {
 };
 
 // the backward takes f'(z) from the output y = f(z): for a negative LeakyReLU slope or ELU alpha, a CLAMP with lo >= hi
-// or a <= 0, or a SCALED_ELU with lambda <= 0, alpha < 0 or c <= 0, y no longer determines f'.  Fills the handle's
-// activation fields (the bounds' images of CLAMP in the storage format of `prec`, see act.cuh) without touching the
+// or a <= 0, or a SCALED_ELU with lambda <= 0, alpha < 0 or c <= 0, y no longer determines f'.  Builds the handle's
+// activation (plan.h Act; the bounds' images of CLAMP in the storage format of `prec`, see act.cuh) without touching the
 // device, so that every refusal comes before any allocation or launch.
 static float bound_image(int prec, float v) {
   if (prec == PREC_F16) return __half2float(__float2half_rn(v));
@@ -953,7 +953,7 @@ static float bound_image(int prec, float v) {
   return v;
 }
 
-static int check_act(int activation, const float* p, int n, int prec, int* kind, float* param, ActParams* q) {
+static int check_act(int activation, const float* p, int n, int prec, Act* act) {
   NNC_REQUIRE(activation >= NNCONV_ACT_RELU && activation <= NNCONV_ACT_LOGSIGMOID, NNCONV_ERR_ARG,
               "unknown edge-network activation %d", activation);
   const int want = activation == NNCONV_ACT_LEAKY_RELU || activation == NNCONV_ACT_ELU ? 1
@@ -974,13 +974,13 @@ static int check_act(int activation, const float* p, int n, int prec, int* kind,
                 "edge-network activation: scaled ELU needs lambda > 0, alpha >= 0 and c > 0 (got %g, %g, %g)", p[0], p[1],
                 p[2]);
   }
-  *kind = activation;
-  *param = want == 1 ? p[0] : 0.f;
-  *q = ActParams{};
-  if (activation == NNCONV_ACT_CLAMP) {
-    *q = ActParams{{p[0], bound_image(prec, p[2]), bound_image(prec, p[3]), p[1], p[2], p[3]}};
+  *act = Act{activation, ActParams{}};
+  if (want == 1) {   // LEAKY_RELU slope / ELU alpha
+    act->p = ActParams{{p[0]}};
+  } else if (activation == NNCONV_ACT_CLAMP) {
+    act->p = ActParams{{p[0], bound_image(prec, p[2]), bound_image(prec, p[3]), p[1], p[2], p[3]}};
   } else if (activation == NNCONV_ACT_SCALED_ELU) {
-    *q = ActParams{{p[0], p[2], p[0] * p[1], p[1], 0.f, 0.f}};
+    act->p = ActParams{{p[0], p[2], p[0] * p[1], p[1], 0.f, 0.f}};
   }
   return NNCONV_OK;
 }
@@ -1149,19 +1149,15 @@ int nnconv_weights_create_act_params(int n_layers, const int* dims, int in_chann
                                      nnconv_weights_t** out) {
   NNC_REQUIRE(out && dims && W && b, NNCONV_ERR_ARG, "null pointer");
   *out = nullptr;
-  int kind;
-  float param;
-  ActParams q;
-  int s = check_act(activation, act_params, n_act_params, precision, &kind, &param, &q);
+  Act act;
+  int s = check_act(activation, act_params, n_act_params, precision, &act);
   if (s) return s;
   nnconv_weights* h = new (std::nothrow) nnconv_weights();
   NNC_REQUIRE(h != nullptr, NNCONV_ERR_ARG, "out of host memory");
   s = weights_prepare(&h->w, n_layers, dims, in_channels, out_channels, precision, W, b, buf, buf_bytes,
                       static_cast<cudaStream_t>(stream));
   if (s != NNCONV_OK) { delete h; return s; }
-  h->w.act = kind;
-  h->w.act_param = param;
-  h->w.act_p = q;
+  h->w.act = act;
   *out = h;
   return NNCONV_OK;
 }
@@ -1499,19 +1495,15 @@ int nnconv_diag_weights_create_act_params(int n_layers, const int* dims, int cha
                                           nnconv_diag_weights_t** out) {
   NNC_REQUIRE(out && dims && W && b, NNCONV_ERR_ARG, "null pointer");
   *out = nullptr;
-  int kind;
-  float param;
-  ActParams q;
-  int s = check_act(activation, act_params, n_act_params, precision, &kind, &param, &q);
+  Act act;
+  int s = check_act(activation, act_params, n_act_params, precision, &act);
   if (s) return s;
   nnconv_diag_weights* h = new (std::nothrow) nnconv_diag_weights();
   NNC_REQUIRE(h != nullptr, NNCONV_ERR_ARG, "out of host memory");
   s = weights_prepare(&h->w, n_layers, dims, channels, channels, precision, W, b, buf, buf_bytes,
                       static_cast<cudaStream_t>(stream), 1);
   if (s != NNCONV_OK) { delete h; return s; }
-  h->w.act = kind;
-  h->w.act_param = param;
-  h->w.act_p = q;
+  h->w.act = act;
   *out = h;
   return NNCONV_OK;
 }

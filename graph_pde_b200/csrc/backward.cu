@@ -145,18 +145,17 @@ __global__ void k_group_sum(const float* __restrict__ G, const int* __restrict__
 }
 
 // dz = dh * (act > 0), in place; column sums accumulate into db (one block per 32 columns).  k_act_grad_colsum<ACT>
-// multiplies by f'(act) of another hidden activation (act.cuh) instead; the kinds with a parameter block (CLAMP,
-// SCALED_ELU) take it in the overload whose last argument is the block.
+// multiplies by f'(act) of another hidden activation (act.cuh) instead, with its parameter block as the last argument.
 template <int ACT>
 __device__ __forceinline__ void act_grad_colsum(float* __restrict__ dh, const float* __restrict__ act, int ne, int kp,
-                                                float* __restrict__ db, float act_param, const ActParams& act_p) {
+                                                float* __restrict__ db, const ActParams& act_p) {
   __shared__ float red[8][33];
   const int col = blockIdx.x * 32 + threadIdx.x;
   float s = 0.f;
   for (int p = threadIdx.y; p < ne; p += 8) {
     if (col < kp) {
       const int64_t i = static_cast<int64_t>(p) * kp + col;
-      const float v = ACT == ACT_RELU ? (act[i] > 0.f ? dh[i] : 0.f) : dh[i] * act_grad<ACT>(act[i], act_param, act_p);
+      const float v = ACT == ACT_RELU ? (act[i] > 0.f ? dh[i] : 0.f) : dh[i] * act_grad<ACT>(act[i], act_p);
       dh[i] = v;
       s += v;
     }
@@ -172,19 +171,13 @@ __device__ __forceinline__ void act_grad_colsum(float* __restrict__ dh, const fl
 
 __global__ void k_relu_mask_colsum(float* __restrict__ dh, const float* __restrict__ act, int ne, int kp,
                                    float* __restrict__ db) {
-  act_grad_colsum<ACT_RELU>(dh, act, ne, kp, db, 0.f, ActParams{});
-}
-
-template <int ACT>
-__global__ void k_act_grad_colsum(float* __restrict__ dh, const float* __restrict__ act, int ne, int kp,
-                                  float* __restrict__ db, float act_param) {
-  act_grad_colsum<ACT>(dh, act, ne, kp, db, act_param, ActParams{});
+  act_grad_colsum<ACT_RELU>(dh, act, ne, kp, db, ActParams{});
 }
 
 template <int ACT>
 __global__ void k_act_grad_colsum(float* __restrict__ dh, const float* __restrict__ act, int ne, int kp,
                                   float* __restrict__ db, ActParams act_p) {
-  act_grad_colsum<ACT>(dh, act, ne, kp, db, 0.f, act_p);
+  act_grad_colsum<ACT>(dh, act, ne, kp, db, act_p);
 }
 
 __global__ void k_gather_ea(const float* __restrict__ edge_attr, const int* __restrict__ perm, int e0, int ne,
@@ -271,16 +264,12 @@ int mlp_backward_rows(const Plan* P, const Weights* W, const float* edge_attr, i
     NNC_CHECK_LAUNCH();
   }
   for (int l = nl - 1; l >= 1; --l) {
-    if (W->act == ACT_RELU)
+    if (W->act.kind == ACT_RELU)
       k_relu_mask_colsum<<<ceil_div(W->kp[l], 32), dim3(32, 8), 0, st>>>(cur, act[l], ne, W->kp[l], db[l]);
     else
-      act_dispatch(W->act, [&](auto k) {
-        constexpr int A = decltype(k)::value;
-        if constexpr (A == ACT_CLAMP || A == ACT_SCALED_ELU)
-          k_act_grad_colsum<A><<<ceil_div(W->kp[l], 32), dim3(32, 8), 0, st>>>(cur, act[l], ne, W->kp[l], db[l], W->act_p);
-        else
-          k_act_grad_colsum<A><<<ceil_div(W->kp[l], 32), dim3(32, 8), 0, st>>>(cur, act[l], ne, W->kp[l], db[l],
-                                                                               W->act_param);
+      act_dispatch(W->act.kind, [&](auto k) {
+        k_act_grad_colsum<decltype(k)::value><<<ceil_div(W->kp[l], 32), dim3(32, 8), 0, st>>>(cur, act[l], ne, W->kp[l],
+                                                                                              db[l], W->act.p);
       });
     NNC_CHECK_LAUNCH();
     const float* prev = l == 1 ? ea : act[l - 1];
@@ -317,10 +306,10 @@ const float* recompute_acts_fp32(const Plan* P, const Weights* W, const float* e
     return hid;
   }
   s = launch_edge_layer1(PREC_FP32, edge_attr, P->perm, e0, ne, W->dims[0], W->W1, W->b1, W->kp[1], 0, act[1], st, 0, 0,
-                         nullptr, act_of(W));
+                         nullptr, W->act);
   for (int l = 2; l <= nl - 1 && s == NNCONV_OK; ++l)
     s = launch_sgemm_store(act[l - 1], W->kp[l - 1], reinterpret_cast<const float*>(W->Wh[l]), W->kp[l - 1], act[l],
-                           W->kp[l], ne, W->kp[l], W->kp[l - 1], W->bh[l], st, act_of(W));
+                           W->kp[l], ne, W->kp[l], W->kp[l - 1], W->bh[l], st, W->act);
   *status = s;
   return act[nl - 1];
 }

@@ -538,10 +538,7 @@ struct DhArgs {
   // transpose and accumulated in a per-warp shared array; needs 4 * (4224 + 4 * Kp) extra bytes of shared memory.
   float* colsum;
   int colsum_stride;
-  float act_param;          // LeakyReLU slope / ELU alpha of MODE's activation
-  // act_grad's part of the parameter block of a CLAMP / SCALED_ELU MODE activation (ActParams v[0 .. 2]; three scalars
-  // rather than the whole block, which leaves the code of the other instantiations as it was)
-  float act_q0, act_q1, act_q2;
+  float act_q0, act_q1, act_q2;   // v[0 .. 2] of MODE's activation parameter block (ActParams), all act_grad reads
 };
 
 constexpr int kDhScratch = 4 * acc_scratch_bytes<32>();
@@ -708,8 +705,8 @@ k_dh(const __grid_constant__ Maps8 tmA, const __grid_constant__ CUtensorMap tmB,
                     y.y += yl.y;
                   }
                   const ActParams aq{{a.act_q0, a.act_q1, a.act_q2}};
-                  f0 = __uint_as_float(v[8 * q + 2 * j]) * act_grad<kAct>(y.x, a.act_param, aq);
-                  f1 = __uint_as_float(v[8 * q + 2 * j + 1]) * act_grad<kAct>(y.y, a.act_param, aq);
+                  f0 = __uint_as_float(v[8 * q + 2 * j]) * act_grad<kAct>(y.x, aq);
+                  f1 = __uint_as_float(v[8 * q + 2 * j + 1]) * act_grad<kAct>(y.y, aq);
                 }
                 if (SPLIT) pack2_split(f0, f1, pk[4 * q + j], pl[4 * q + j]);
                 else pk[4 * q + j] = pack2<FMT>(f0, f1);
@@ -1373,12 +1370,12 @@ int backward_mlp_tc(const Plan* P, const Weights* W, const float* edge_attr, con
       if (r) return r;
       if (nl >= 3 && acts == nullptr) {
         r = launch_gemm_tc(W->prec, A1, n, 0, n, 64, W->W1aug, W->kp[1], nullptr, 1, act[1], pm * W->kp[1], st, nullptr, 0, 0,
-                           sp ? GEMM_C_SPLIT : 0, nullptr, nullptr, 0, 0, 0, nullptr, act_of(W));
+                           sp ? GEMM_C_SPLIT : 0, nullptr, nullptr, 0, 0, 0, nullptr, W->act);
         if (r) return r;
         for (int l = 2; l <= nl - 2; ++l) {
           r = launch_gemm_tc(W->prec, act[l - 1], n, 0, n, kmul * W->kp[l - 1], W->Wh[l], W->kp[l], W->bh[l], 1, act[l],
                              pm * W->kp[l], st, nullptr, 0, 0, sp ? (GEMM_A_SPLIT | GEMM_C_SPLIT) : 0, nullptr, nullptr, 0, 0,
-                             0, sp ? W->wscale + 2 * l + 1 : nullptr, act_of(W));
+                             0, sp ? W->wscale + 2 * l + 1 : nullptr, W->act);
           if (r) return r;
         }
       }
@@ -1391,11 +1388,11 @@ int backward_mlp_tc(const Plan* P, const Weights* W, const float* edge_attr, con
       const int64_t hpad = round_up64(n, 128);
       if (nl == 2)
         s = launch_gemm_tc(W->prec, A1, n, 0, n, 64, W->W1aug, W->kp[1], nullptr, 1, hb, pm * W->kp[1], st, nullptr, hpad, 0,
-                           sp ? GEMM_C_SPLIT : 0, nullptr, nullptr, 0, 0, 0, nullptr, act_of(W));
+                           sp ? GEMM_C_SPLIT : 0, nullptr, nullptr, 0, 0, 0, nullptr, W->act);
       else
         s = launch_gemm_tc(W->prec, act[nl - 2], n, 0, n, kmul * W->kp[nl - 2], W->Wh[nl - 1], W->kp[nl - 1], W->bh[nl - 1], 1,
                            hb, pm * W->kp[nl - 1], st, nullptr, hpad, 0, sp ? (GEMM_A_SPLIT | GEMM_C_SPLIT) : 0, nullptr,
-                           nullptr, 0, 0, 0, sp ? W->wscale + 2 * (nl - 1) + 1 : nullptr, act_of(W));
+                           nullptr, 0, 0, 0, sp ? W->wscale + 2 * (nl - 1) + 1 : nullptr, W->act);
       if (s) return s;
     }
     // ---- Y^T of the batch for every application: Yt[t][(c, k), o] = sum_i Xc_t[c, i] W_L[i*out + o, k]
@@ -1445,10 +1442,9 @@ int backward_mlp_tc(const Plan* P, const Weights* W, const float* edge_attr, con
       a.colsum_stride = 64;
       const int tiles = a.tile1 - a.tile0;
       const int grid = tiles < tc_num_sms() ? tiles : tc_num_sms();
-      a.act_param = W->act_param;
-      a.act_q0 = W->act_p.v[0]; a.act_q1 = W->act_p.v[1]; a.act_q2 = W->act_p.v[2];
-      if (W->act != ACT_RELU) {
-        s = act_dispatch(W->act, [&](auto k) {
+      a.act_q0 = W->act.p.v[0]; a.act_q1 = W->act.p.v[1]; a.act_q2 = W->act.p.v[2];
+      if (W->act.kind != ACT_RELU) {
+        s = act_dispatch(W->act.kind, [&](auto k) {
           constexpr int M = decltype(k)::value << 1;
           if (sp) return BN == 128 ? launch_dh<0, 128, M | 1>(tmA, tmB, a, grid, dh_smem, st)
                                    : launch_dh<0, 64, M | 1>(tmA, tmB, a, grid, dh_smem, st);
@@ -1493,7 +1489,7 @@ int backward_mlp_tc(const Plan* P, const Weights* W, const float* edge_attr, con
         // activation multiplies by f'(h_{l-1}) instead (PREC_F16X2: of hi + lo)
         s = launch_gemm_tc(W->prec, cur, n, 0, n, kmul * W->kp[l], W->WhT[l], W->kp[l - 1], nullptr, 0, nxt,
                            pm * W->kp[l - 1], st, nullptr, 0, 0, sp ? (GEMM_A_SPLIT | GEMM_C_SPLIT) : 0, nullptr, act[l - 1],
-                           pm * W->kp[l - 1], 0, 0, sp ? W->wscale + 2 * l + 1 : nullptr, act_of(W));
+                           pm * W->kp[l - 1], 0, 0, sp ? W->wscale + 2 * l + 1 : nullptr, W->act);
         if (s) return s;
         uint16_t* tmp = cur; cur = nxt; nxt = tmp;
       }

@@ -64,8 +64,7 @@ struct GemmTcArgs {
   int out_f32;
   TraceBuf trace;
   unsigned int trace_seq;
-  float act_param;     // LeakyReLU slope / ELU alpha of the activation epi_act(EPI)
-  ActParams act_p;     // parameter block of a CLAMP / SCALED_ELU epi_act(EPI)
+  ActParams act_p;     // parameter block of the activation epi_act(EPI)
 };
 
 // EPI selects the epilogue at COMPILE time (runtime flags inside the 32-column inner loop cut it into dozens of
@@ -312,8 +311,8 @@ k_gemm_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
                 } else {
                   float r0 = fabsf(f0), r1 = fabsf(f1);
                   if (a.relu) {
-                    const float y0 = act_fwd<kAct>(f0, a.act_param, a.act_p);
-                    const float y1 = act_fwd<kAct>(f1, a.act_param, a.act_p);
+                    const float y0 = act_fwd<kAct>(f0, a.act_p);
+                    const float y1 = act_fwd<kAct>(f1, a.act_p);
                     r0 = act_range<kAct>(f0, y0);
                     r1 = act_range<kAct>(f1, y1);
                     f0 = kSplitOut ? y0 : act_store16<kAct, FMT>(y0, a.act_p);
@@ -386,7 +385,7 @@ k_gemm_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
             }
             if (a.relu) {
 #pragma unroll
-              for (int q = 0; q < 4; ++q) f[q] = act_fwd<kAct>(f[q], a.act_param, a.act_p);
+              for (int q = 0; q < 4; ++q) f[q] = act_fwd<kAct>(f[q], a.act_p);
             }
             if (kMask && kAct != ACT_RELU) {
               // f'(y) from the stored activation: y = hi (+ lo at column c + N for the split form)
@@ -405,8 +404,8 @@ k_gemm_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
                     y.x += yl.x;
                     y.y += yl.y;
                   }
-                  f[2 * q] *= act_grad<kAct>(y.x, a.act_param, a.act_p);
-                  f[2 * q + 1] *= act_grad<kAct>(y.y, a.act_param, a.act_p);
+                  f[2 * q] *= act_grad<kAct>(y.x, a.act_p);
+                  f[2 * q + 1] *= act_grad<kAct>(y.y, a.act_p);
                 }
               }
             } else if (kMask) {
@@ -631,7 +630,6 @@ int launch_gemm_tc(int prec, const void* A_base, int64_t a_rows_total, int64_t a
   const bool pdl = pf && pf->pdl;
   // the activation matters only where it is applied (relu) or differentiated (mask); every other launch is the ReLU
   // instantiation, as it always was
-  a.act_param = act.param;
   a.act_p = act.p;
   if (act.kind == ACT_RELU || (!relu && mask == nullptr)) return dispatch_gemm<ACT_RELU>(tmA, tmB, tmC, a, st, pdl, BN, bf, small, out_f32, mask_split, mask != nullptr, c_split);
   NNC_REQUIRE(!out_f32 && !small, NNCONV_ERR_ARG, "gemm_tc: the activation excludes fp32 output / the small-footprint configuration");

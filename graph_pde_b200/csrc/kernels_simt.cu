@@ -172,16 +172,15 @@ __global__ void k_transpose_pad_split3(const float* __restrict__ src, int R, int
 // overflow (fp16 output, nullable): +1 per block that wrote a value beyond the fp16 range or NaN.  Counted here, at the
 // writer: the next layer's GEMM would turn an inf into NaN, which its ReLU turns into 0 before its own range check.
 // k_edge_layer1 is the ReLU kernel; k_edge_layer1_act<ACT> applies another hidden activation (act.cuh, act_range for
-// the range check) in its place.  The kinds with a parameter block (CLAMP, SCALED_ELU) take it in an overload of
-// k_edge_layer1_act whose last argument is the block, so the single-parameter kernels keep their signatures; a 16-bit
-// CLAMP output follows the store rule of act.cuh (act_store16).
+// the range check) in its place, with its parameter block as the last argument; a 16-bit CLAMP output follows the
+// store rule of act.cuh (act_store16).
 constexpr int kL1Edges = 32;
 template <int ACT, typename T>
 __device__ __forceinline__ void edge_layer1(const float* __restrict__ edge_attr, const int* __restrict__ perm,
                                             int64_t e_begin, int64_t e_count, int k_in, const float* __restrict__ W1,
                                             const float* __restrict__ b1, int kp1, int identity, T* __restrict__ out,
                                             int64_t chunk_rows_pad, int64_t out_row0, int* __restrict__ overflow,
-                                            float act_param, const ActParams& act_p) {
+                                            const ActParams& act_p) {
   constexpr bool kRangeCheck = std::is_same<T, __half>::value;
   bool bad = false;
   extern __shared__ float sm[];
@@ -231,7 +230,7 @@ __device__ __forceinline__ void edge_layer1(const float* __restrict__ edge_attr,
         if (kRangeCheck) bad |= !(v <= 65504.f);
         out[oidx(e, j)] = cvt<T>(v);
       } else {
-        float v = act_fwd<ACT>(acc, act_param, act_p);
+        float v = act_fwd<ACT>(acc, act_p);
         if (kRangeCheck) bad |= !(act_range<ACT>(acc, v) <= 65504.f);
         if (std::is_same<T, __half>::value) v = act_store16<ACT, 0>(v, act_p);
         if (std::is_same<T, __nv_bfloat16>::value) v = act_store16<ACT, 1>(v, act_p);
@@ -250,16 +249,7 @@ k_edge_layer1(const float* __restrict__ edge_attr, const int* __restrict__ perm,
               int k_in, const float* __restrict__ W1, const float* __restrict__ b1, int kp1, int identity,
               T* __restrict__ out, int64_t chunk_rows_pad, int64_t out_row0, int* __restrict__ overflow) {
   edge_layer1<ACT_RELU>(edge_attr, perm, e_begin, e_count, k_in, W1, b1, kp1, identity, out, chunk_rows_pad, out_row0,
-                        overflow, 0.f, ActParams{});
-}
-
-template <int ACT, typename T>
-__global__ void __launch_bounds__(256)
-k_edge_layer1_act(const float* __restrict__ edge_attr, const int* __restrict__ perm, int64_t e_begin, int64_t e_count,
-                  int k_in, const float* __restrict__ W1, const float* __restrict__ b1, int kp1, T* __restrict__ out,
-                  int64_t chunk_rows_pad, int64_t out_row0, int* __restrict__ overflow, float act_param) {
-  edge_layer1<ACT>(edge_attr, perm, e_begin, e_count, k_in, W1, b1, kp1, 0, out, chunk_rows_pad, out_row0, overflow,
-                   act_param, ActParams{});
+                        overflow, ActParams{});
 }
 
 template <int ACT, typename T>
@@ -268,7 +258,7 @@ k_edge_layer1_act(const float* __restrict__ edge_attr, const int* __restrict__ p
                   int k_in, const float* __restrict__ W1, const float* __restrict__ b1, int kp1, T* __restrict__ out,
                   int64_t chunk_rows_pad, int64_t out_row0, int* __restrict__ overflow, ActParams act_p) {
   edge_layer1<ACT>(edge_attr, perm, e_begin, e_count, k_in, W1, b1, kp1, 0, out, chunk_rows_pad, out_row0, overflow,
-                   0.f, act_p);
+                   act_p);
 }
 
 // ---- first edge-MLP layer on the tensor cores with fp32-grade inputs -------------------------------
@@ -505,8 +495,7 @@ struct SgemmArgs {
   // EPI_SCATTER_MAX (aggr = max): the rows reduce keys (common.cuh max_key) into keys [N, ldc] instead of adding to C
   unsigned long long* keys;
   const int* perm;
-  float act_param;     // EPI_BIAS_ACT + ACT
-  ActParams act_p;     // EPI_BIAS_ACT + ACT of a CLAMP / SCALED_ELU
+  ActParams act_p;     // EPI_BIAS_ACT + ACT
 };
 
 template <int EPI>
@@ -587,7 +576,7 @@ __global__ void __launch_bounds__(256) k_sgemm_nt(SgemmArgs a) {
         if (gn < a.N) {
           float v = acc[i][j];
           if (EPI == EPI_BIAS_RELU) v = fmaxf(v + a.bias[gn], 0.f);
-          if constexpr (EPI > EPI_BIAS_ACT) v = act_fwd<EPI - EPI_BIAS_ACT>(v + a.bias[gn], a.act_param, a.act_p);
+          if constexpr (EPI > EPI_BIAS_ACT) v = act_fwd<EPI - EPI_BIAS_ACT>(v + a.bias[gn], a.act_p);
           a.C[static_cast<int64_t>(gm) * a.ldc + gn] = v;
         }
       }
@@ -917,23 +906,18 @@ int launch_edge_layer1(int prec, const float* edge_attr, const int* perm, int64_
   if (!identity && act.kind != ACT_RELU) {
     act_dispatch(act.kind, [&](auto k) {
       constexpr int A = decltype(k)::value;
-      // the single-parameter kinds pass act.param, the others the parameter block (the k_edge_layer1_act overloads)
-      auto param = [&]() {
-        if constexpr (A == ACT_CLAMP || A == ACT_SCALED_ELU) return act.p;
-        else return act.param;
-      };
       if (prec == PREC_FP32)
         k_edge_layer1_act<A, float><<<g, 256, sm, st>>>(edge_attr, perm, e_begin, e_count, k_in, W1, b1, kp1,
                                                          static_cast<float*>(out), chunk_rows_pad, out_row0, nullptr,
-                                                         param());
+                                                         act.p);
       else if (prec == PREC_F16 || prec == PREC_F16X2)
         k_edge_layer1_act<A, __half><<<g, 256, sm, st>>>(edge_attr, perm, e_begin, e_count, k_in, W1, b1, kp1,
                                                           static_cast<__half*>(out), chunk_rows_pad, out_row0, overflow,
-                                                          param());
+                                                          act.p);
       else
         k_edge_layer1_act<A, __nv_bfloat16><<<g, 256, sm, st>>>(edge_attr, perm, e_begin, e_count, k_in, W1, b1, kp1,
                                                                  static_cast<__nv_bfloat16*>(out), chunk_rows_pad,
-                                                                 out_row0, nullptr, param());
+                                                                 out_row0, nullptr, act.p);
     });
   } else if (prec == PREC_FP32)
     k_edge_layer1<float><<<g, 256, sm, st>>>(edge_attr, perm, e_begin, e_count, k_in, W1, b1, kp1, identity,
@@ -1093,7 +1077,6 @@ int launch_sgemm_store(const float* A, int64_t lda, const float* B, int64_t ldb,
   if (M <= 0 || N <= 0) return NNCONV_OK;
   SgemmArgs a{};
   a.A = A; a.lda = lda; a.B = B; a.ldb = ldb; a.C = C; a.ldc = ldc; a.M = M; a.N = N; a.K = K; a.bias = bias_relu;
-  a.act_param = act.param;
   a.act_p = act.p;
   dim3 g(ceil_div(M, 64), ceil_div(N, 64));
   if (bias_relu && act.kind != ACT_RELU)

@@ -50,7 +50,9 @@ int plan_build(Plan* P, const int64_t* row0, const int64_t* row1, int64_t E, int
 // conv (NNConv, diagonal, Gaussian): the root term reads x_dst, not x_src (root_term / node_terms_rows)
 int check_bipartite_root(const Plan* P, const float* root, unsigned node_flags);
 
-// parameter block of the activations with more than one parameter (act.cuh); act_grad reads v[0 .. 2] only:
+// parameter block of the edge MLP's hidden activation (act.cuh); act_grad reads v[0 .. 2] only, unused entries are 0:
+//   NNCONV_ACT_LEAKY_RELU  v[0] = slope
+//   NNCONV_ACT_ELU         v[0] = alpha
 //   NNCONV_ACT_CLAMP       v = a, lo_img, hi_img, b, lo, hi   (the bounds' images in the weights' storage format)
 //   NNCONV_ACT_SCALED_ELU  v = lambda, c, lambda * alpha, alpha
 constexpr int kActParams = 6;
@@ -58,11 +60,9 @@ struct ActParams {
   float v[kActParams];
 };
 
-// hidden activation of the edge MLP: kind = NNCONV_ACT_* (0 = ReLU), param = LeakyReLU slope / ELU alpha, p = the
-// parameter block of the other kinds
+// hidden activation of the edge MLP: kind = NNCONV_ACT_* (0 = ReLU) and its parameter block
 struct Act {
   int kind;
-  float param;
   ActParams p;
 };
 
@@ -98,13 +98,8 @@ struct Weights {
   // b_L with cin == cout == dims[L].  Only the hidden layers, W3n and B3 are prepared: W3n = W_L [cout, Kp] zero padded,
   // 16-bit at f16 / bf16 (tensor-core build of d), fp32 at f16x2 and fp32 (CUDA-core build); B3 = b_L [cout] fp32.
   int diag;
-  // hidden activation of the edge MLP (NNCONV_ACT_*) and its parameter (LeakyReLU slope / ELU alpha), see act.cuh
-  int act;
-  float act_param;
-  ActParams act_p;              // NNCONV_ACT_CLAMP and NNCONV_ACT_SCALED_ELU, see ActParams
+  Act act;                      // hidden activation of the edge MLP, see act.cuh
 };
-
-inline Act act_of(const Weights* W) { return Act{W->act, W->act_param, W->act_p}; }
 
 size_t weights_bytes(int n_layers, const int* dims, int cin, int cout, int prec, int diag = 0);
 int weights_prepare(Weights* W, int n_layers, const int* dims, int cin, int cout, int prec,
