@@ -710,6 +710,16 @@ static int contract_range(const Plan* P, const Weights* W, const UnitRange& R, i
     return launch_conv_tc(W->prec, P, h, W->Kp, Ybuf[b % 3], nb, W->cout, tb, te, static_cast<int>(c0), A.cvec, A.xs,
                           aggr_mean, out, st, S.pipe ? &pf : nullptr, R.e_base, R.h_rows, max_keys);
   };
+  if (!S.pipe) {   // one Y buffer: batch b's contraction reads it before batch b + 1's Y GEMM overwrites it
+    for (int64_t b = 0; b < n_batches; ++b) {
+      int s = launch_y(b);
+      if (s) return s;
+      s = launch_c(b);
+      if (s) return s;
+    }
+    if (launches) *launches += 2 * n_batches;
+    return NNCONV_OK;
+  }
   int s = launch_y(0);
   if (s) return s;
   for (int64_t b = 0; b < n_batches; ++b) {

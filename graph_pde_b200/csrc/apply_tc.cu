@@ -599,7 +599,8 @@ struct ApplyShape {
 
 // num_kx: 64-column boxes of the Y GEMM's K (the Xc tile of a 128-source m-block is num_kx * 16 KiB)
 // staging: the scatter staging is needed whatever scatter_mode says (aggr = max stages its key rows there)
-bool apply_shape(int cout, int Kp, int ybn, int num_kx, ApplyShape* as, bool staging = false) {
+// forced: the only pass count to consider (0 = any)
+static bool apply_shape_passes(int cout, int Kp, int ybn, int num_kx, ApplyShape* as, bool staging, int forced) {
   const int w_bytes = ybn * 64 * 2;
   if (cout % 16 != 0 || cout < 16 || cout > 64 || Kp % 64 != 0) return false;
   const int num_kc = Kp / 64;
@@ -607,7 +608,6 @@ bool apply_shape(int cout, int Kp, int ybn, int num_kx, ApplyShape* as, bool sta
   const int bar_bytes = 1024 + kYStagingBytes + (options().scatter_mode == 1 || staging ? kScatterBytes : 0);
   // fewest passes that leave >= 7 A stages (the h stream needs the bytes in flight), else >= 5, else >= 3; at each
   // level a resident Xc tile (loaded once per m-block instead of once per n-block) first, where it fits
-  const int forced = options().apply_passes;
   for (int min_stages = 7; min_stages >= 3; min_stages -= 2) {
     for (int xres = num_kx * kATileBytes <= kMaxXBytes ? 1 : 0; xres >= 0; --xres) {
       const int y_bytes = xres ? num_kx * kATileBytes + kYStages * w_bytes : kYStages * (kATileBytes + w_bytes);
@@ -633,6 +633,15 @@ bool apply_shape(int cout, int Kp, int ybn, int num_kx, ApplyShape* as, bool sta
     }
   }
   return false;
+}
+
+// The apply_passes option forces the pass count where that count has a shape.  A count that leaves none (fewer than
+// 4 B slots per pass, or too few A stages) is ignored like one that does not divide Kp / 64: the option never makes a
+// shape unsupported, so it cannot turn the fused kernel into the per-batch one or refuse precision f16x2.
+bool apply_shape(int cout, int Kp, int ybn, int num_kx, ApplyShape* as, bool staging = false) {
+  const int forced = options().apply_passes;
+  if (forced > 0 && apply_shape_passes(cout, Kp, ybn, num_kx, as, staging, forced)) return true;
+  return apply_shape_passes(cout, Kp, ybn, num_kx, as, staging, 0);
 }
 
 }  // namespace
